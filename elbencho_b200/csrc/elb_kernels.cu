@@ -28,14 +28,14 @@
  * result copy, no init launch. These launches are PCIe-bound, the resident forms are HBM-bound.
  *
  * One launch processes an array of block descriptors {devPtr, len, fileOffset, blockCounter}.
- * Tiles are ELB_TILE_BYTES slices of a block's 16-byte-aligned body; unaligned head/tail bytes
- * (device address not 16-byte aligned, or odd lengths) are handled byte-wise by tile 0 of the
- * block. Mismatch counts are reduced per warp (redux.sync) before touching global atomics.
+ * Three launch shapes (tiled, persistent, warp per block) share one per-mode core and one walker:
+ * a thread group (a CTA or a warp) walks a block's 16-byte-aligned body in unrolled spans (a CTA
+ * span is an ELB_TILE_BYTES tile); unaligned head/tail bytes (device address not 16-byte aligned,
+ * or odd lengths) are handled byte-wise by the group that owns the start of the body. Mismatch
+ * counts are reduced per warp (redux.sync) before touching global atomics.
  */
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdio.h>
-#include <stdlib.h>
 
 #include <atomic>
 #include <mutex>
@@ -53,8 +53,9 @@
 #define ELB_UNROLL 8
 #define ELB_TILE_BYTES (ELB_THREADS * ELB_VEC_BYTES * ELB_UNROLL) /* 32 KiB */
 /* verify holds all ELB_UNROLL vectors of a thread in registers before it compares them: 3 CTAs per
-   SM (85 registers) instead of 4 (64) keep them out of local memory, and 3 x 256 threads with 128 B
-   in flight each are still far more than the H100's HBM latency needs */
+   SM (ptxas of CUDA 12.9 allocates 80 registers) instead of 4 (64) keep them out of local memory
+   (only the persistent stage-in + verify form spills, 20 B), and 3 x 256 threads with 128 B in
+   flight each are still far more than the H100's HBM latency needs */
 #define ELB_MIN_CTAS_PER_SM(mode) ( ( (mode) == 1 /* MODE_VERIFY_PATTERN */) ? 3 : 4)
 
 struct __align__(16) u64x2
@@ -89,6 +90,7 @@ __device__ __forceinline__ unsigned first_diff_byte64(uint64_t x, uint64_t y)
 {
 	return (unsigned)(__ffsll( (long long)(x ^ y) ) - 1) >> 3;
 }
+
 
 /* ---- generators ------------------------------------------------------------------------- */
 
@@ -170,7 +172,51 @@ struct RandomGen
 		{ return elb_rand_byte(pos, blockKey, varFillLen, remainderVal); }
 };
 
-/* ---- block geometry --------------------------------------------------------------------- */
+struct NoGen {}; // the stage copies generate nothing
+
+/* the expected element at block position pos: a 16-byte vector or a byte */
+template<bool FAST, class T, class Gen>
+__device__ __forceinline__ T generate(const Gen& gen, uint64_t pos)
+{
+	if constexpr(sizeof(T) == ELB_VEC_BYTES)
+		return gen.template vec16<FAST>(pos);
+	else
+		return gen.byte(pos);
+}
+
+/* ---- launch arguments and block geometry ------------------------------------------------ */
+
+/* STAGE_NONE: work on the device slot only (kernel level ABI, resident windows). STAGE_PUBLISH:
+ * device slot only, but the last CTA of a verify launch publishes the results to pinned host
+ * memory (copy-engine staging). STAGE_FULL: the kernel also moves the block between the rings. */
+enum { STAGE_NONE = 0, STAGE_PUBLISH = 1, STAGE_FULL = 2 };
+
+enum { MODE_FILL_PATTERN = 0, MODE_VERIFY_PATTERN = 1, MODE_FILL_RANDOM = 2,
+	MODE_COPY_IN = 3 /* host slot -> device slot */, MODE_COPY_OUT = 4 /* device -> host */,
+	NUM_MODES = 5 };
+
+struct KernelArgs
+{
+	const elb_block_desc* descs; // device-readable array, or NULL to use inlineDesc
+	elb_block_desc inlineDesc;   // single-block launches pass the descriptor by value
+	uint32_t numDescs;
+	uint64_t salt;         // pattern
+	uint64_t seed;         // random
+	unsigned pct;          // random
+	elb_verify_result* results; // verify
+	unsigned long long* counters; // optional device counter block
+
+	// staging (see the header comment); hostDelta == 0: work on the device slot only
+	int64_t hostDelta;              // host slot address = device slot address + hostDelta
+	elb_verify_result* hostResults; // verify: pinned copy of results, written by the last CTA
+	unsigned* doneTicket;           // device counter behind the last-CTA detection (stays 0)
+};
+
+/* descriptor descIdx of the launch (the only reader of inlineDesc) */
+__device__ __forceinline__ elb_block_desc load_desc(const KernelArgs& args, uint32_t descIdx)
+{
+	return args.descs ? args.descs[descIdx] : args.inlineDesc;
+}
 
 struct BlockGeom
 {
@@ -203,348 +249,249 @@ __device__ __forceinline__ BlockGeom make_geom(const elb_block_desc& desc)
 	return g;
 }
 
-/* ---- fill ------------------------------------------------------------------------------- */
+/* ---- verify accumulation ---------------------------------------------------------------- */
 
-template<bool FAST, bool STAGED, class Gen>
-__device__ __forceinline__ void fill_tile(const BlockGeom& g, const Gen& gen, uint64_t tileIdx,
-	int64_t hostDelta)
+/* a thread's mismatching bytes so far: count and first block position (~0: none) */
+struct VerifyAcc
 {
-	const uint64_t tileStart = tileIdx * ELB_TILE_BYTES; // within body
-	uint8_t* bodyPtr = g.ptr + g.headLen;
-
-	if( (tileStart + ELB_TILE_BYTES) <= g.bodyLen)
-	{ // full tile: no bounds checks, all stores independent
-		#pragma unroll
-		for(int u = 0; u < ELB_UNROLL; u++)
-		{
-			const uint64_t bodyOff = tileStart +
-				(uint64_t)(u * ELB_THREADS + threadIdx.x) * ELB_VEC_BYTES;
-			const uint64_t pos = g.headLen + bodyOff;
-			const u64x2 v = gen.template vec16<FAST>(pos);
-			st_na_128(bodyPtr + bodyOff, v);
-			if(STAGED)
-				st_na_128(bodyPtr + hostDelta + bodyOff, v);
-		}
-	}
-	else
-	{
-		#pragma unroll
-		for(int u = 0; u < ELB_UNROLL; u++)
-		{
-			const uint64_t bodyOff = tileStart +
-				(uint64_t)(u * ELB_THREADS + threadIdx.x) * ELB_VEC_BYTES;
-			if(bodyOff < g.bodyLen)
-			{
-				const uint64_t pos = g.headLen + bodyOff;
-				const u64x2 v = gen.template vec16<FAST>(pos);
-				st_na_128(bodyPtr + bodyOff, v);
-				if(STAGED)
-					st_na_128(bodyPtr + hostDelta + bodyOff, v);
-			}
-		}
-	}
-
-	if(!tileIdx && (g.headLen | g.tailLen) )
-	{ // unaligned head/tail bytes (at most 15 each)
-		if(threadIdx.x < g.headLen)
-		{
-			const uint8_t b = gen.byte(threadIdx.x);
-			g.ptr[threadIdx.x] = b;
-			if(STAGED)
-				g.ptr[hostDelta + (int64_t)threadIdx.x] = b;
-		}
-
-		const uint64_t tailStart = g.headLen + g.bodyLen;
-		if(threadIdx.x < g.tailLen)
-		{
-			const uint8_t b = gen.byte(tailStart + threadIdx.x);
-			g.ptr[tailStart + threadIdx.x] = b;
-			if(STAGED)
-				g.ptr[hostDelta + (int64_t)(tailStart + threadIdx.x)] = b;
-		}
-	}
-}
-
-/* plain slot copy between the rings: IN = host slot -> device slot, else device -> host */
-template<bool IN>
-__device__ __forceinline__ void copy_tile(const BlockGeom& g, uint64_t tileIdx, int64_t hostDelta)
-{
-	const uint64_t tileStart = tileIdx * ELB_TILE_BYTES;
-	uint8_t* devBody = g.ptr + g.headLen;
-	uint8_t* hostBody = devBody + hostDelta;
-	const uint8_t* src = IN ? hostBody : devBody;
-	uint8_t* dst = IN ? devBody : hostBody;
-
-	if( (tileStart + ELB_TILE_BYTES) <= g.bodyLen)
-	{
-		u64x2 v[ELB_UNROLL];
-
-		#pragma unroll
-		for(int u = 0; u < ELB_UNROLL; u++)
-			v[u] = ld_nc_na_128(src + tileStart +
-				(uint64_t)(u * ELB_THREADS + threadIdx.x) * ELB_VEC_BYTES);
-
-		#pragma unroll
-		for(int u = 0; u < ELB_UNROLL; u++)
-			st_na_128(dst + tileStart +
-				(uint64_t)(u * ELB_THREADS + threadIdx.x) * ELB_VEC_BYTES, v[u] );
-	}
-	else
-	{
-		#pragma unroll
-		for(int u = 0; u < ELB_UNROLL; u++)
-		{
-			const uint64_t bodyOff = tileStart +
-				(uint64_t)(u * ELB_THREADS + threadIdx.x) * ELB_VEC_BYTES;
-			if(bodyOff < g.bodyLen)
-				st_na_128(dst + bodyOff, ld_nc_na_128(src + bodyOff) );
-		}
-	}
-
-	if(!tileIdx && (g.headLen | g.tailLen) )
-	{
-		const uint8_t* srcBlock = IN ? (g.ptr + hostDelta) : g.ptr;
-		uint8_t* dstBlock = IN ? g.ptr : (g.ptr + hostDelta);
-
-		if(threadIdx.x < g.headLen)
-			dstBlock[threadIdx.x] = srcBlock[threadIdx.x];
-
-		const uint64_t tailStart = g.headLen + g.bodyLen;
-		if(threadIdx.x < g.tailLen)
-			dstBlock[tailStart + threadIdx.x] = srcBlock[tailStart + threadIdx.x];
-	}
-}
-
-/* ---- verify ----------------------------------------------------------------------------- */
-
-/* compare one 16-byte vector; update thread-local count and first mismatch position */
-__device__ __forceinline__ void verify_vec(const u64x2& got, const u64x2& exp, uint64_t pos,
-	unsigned& numBad, uint64_t& firstBad)
-{
-	const uint64_t anyDiff = (got.a ^ exp.a) | (got.b ^ exp.b);
-
-	if(__builtin_expect(anyDiff != 0, 0) )
-	{
-		numBad += diff_bytes64(got.a, exp.a) + diff_bytes64(got.b, exp.b);
-
-		uint64_t first;
-		if(got.a != exp.a)
-			first = pos + first_diff_byte64(got.a, exp.a);
-		else
-			first = pos + 8 + first_diff_byte64(got.b, exp.b);
-
-		if(first < firstBad)
-			firstBad = first;
-	}
-}
-
-template<bool FAST, bool STAGED, class Gen>
-__device__ __forceinline__ void verify_tile(const BlockGeom& g, const Gen& gen,
-	uint64_t tileIdx, elb_verify_result* result, unsigned long long* counters, int64_t hostDelta)
-{
-	const uint64_t tileStart = tileIdx * ELB_TILE_BYTES;
-	uint8_t* devBody = g.ptr + g.headLen;
-	const uint8_t* bodyPtr = STAGED ? (devBody + hostDelta) : devBody; // where the data is read
-
 	unsigned numBad = 0;
 	uint64_t firstBad = ~0ULL;
 
-	if( (tileStart + ELB_TILE_BYTES) <= g.bodyLen)
-	{ // full tile: issue all loads first, then compare
-		u64x2 got[ELB_UNROLL];
+	__device__ __forceinline__ void check(const u64x2& got, const u64x2& exp, uint64_t pos)
+	{
+		const uint64_t anyDiff = (got.a ^ exp.a) | (got.b ^ exp.b);
 
+		if(__builtin_expect(anyDiff != 0, 0) )
+		{
+			numBad += diff_bytes64(got.a, exp.a) + diff_bytes64(got.b, exp.b);
+
+			uint64_t first;
+			if(got.a != exp.a)
+				first = pos + first_diff_byte64(got.a, exp.a);
+			else
+				first = pos + 8 + first_diff_byte64(got.b, exp.b);
+
+			if(first < firstBad)
+				firstBad = first;
+		}
+	}
+
+	__device__ __forceinline__ void check(uint8_t got, uint8_t exp, uint64_t pos)
+	{
+		if(got != exp)
+		{
+			numBad++;
+			if(pos < firstBad)
+				firstBad = pos;
+		}
+	}
+
+	/* warp-reduced count and first position into the block's result and the mismatch counter;
+	   global atomics only on the (rare) mismatch path. Must be reached by all lanes of the warp.
+	   (The atomics let several launches accumulate into one result.) */
+	__device__ __forceinline__ void flush(elb_verify_result* result,
+		unsigned long long* counters) const
+	{
+		const unsigned warpBad = __reduce_add_sync(0xffffffffu, numBad);
+
+		if(__builtin_expect(warpBad != 0, 0) )
+		{
+			// 64-bit min via two 32-bit redux steps
+			const unsigned firstHi = (unsigned)(firstBad >> 32);
+			const unsigned minHi = __reduce_min_sync(0xffffffffu, firstHi);
+			const unsigned firstLo = (firstHi == minHi) ? (unsigned)firstBad : 0xffffffffu;
+			const unsigned minLo = __reduce_min_sync(0xffffffffu, firstLo);
+
+			if( (threadIdx.x & 31) == 0)
+			{
+				atomicAdd( (unsigned long long*)&result->numMismatchBytes,
+					(unsigned long long)warpBad);
+				atomicMin( (unsigned long long*)&result->firstMismatchIdx,
+					( (unsigned long long)minHi << 32) | minLo);
+				if(counters)
+					atomicAdd(&counters[ELB_DEVCTR_VERIFY_MISMATCH_BYTES],
+						(unsigned long long)warpBad);
+			}
+		}
+	}
+};
+
+/* ---- the per-mode core ------------------------------------------------------------------ */
+
+template<class T>
+__device__ __forceinline__ T load_elem(const uint8_t* ptr)
+{
+	if constexpr(sizeof(T) == ELB_VEC_BYTES)
+		return ld_nc_na_128(ptr);
+	else
+		return *ptr;
+}
+
+__device__ __forceinline__ void store_elem(uint8_t* ptr, const u64x2& v) { st_na_128(ptr, v); }
+__device__ __forceinline__ void store_elem(uint8_t* ptr, uint8_t v) { *ptr = v; }
+
+/**
+ * What a mode does with one element of a block: a 16-byte vector of the body or a head/tail byte.
+ * It reads the element from the device slot or the host slot, or generates it; it writes it to
+ * the device slot, the host slot or both; verify compares it with the pattern. STAGED (STAGE_FULL)
+ * adds the host-slot side; the stage copies exist in their staged form only.
+ */
+template<int MODE, bool STAGED>
+struct ModeCore
+{
+	static constexpr bool COPY = (MODE == MODE_COPY_IN) || (MODE == MODE_COPY_OUT);
+	static constexpr bool VERIFY = (MODE == MODE_VERIFY_PATTERN);
+	static constexpr bool READS = COPY || VERIFY; // (else generates)
+	static constexpr bool READS_HOST = (MODE == MODE_COPY_IN) || (VERIFY && STAGED);
+	static constexpr bool WRITES_DEV = !READS || (MODE == MODE_COPY_IN) || (VERIFY && STAGED);
+	static constexpr bool WRITES_HOST = (!READS && STAGED) || (MODE == MODE_COPY_OUT);
+
+	/* devPtr: device slot address of the element */
+	template<class T>
+	static __device__ __forceinline__ T read(const uint8_t* devPtr, int64_t hostDelta)
+		{ return load_elem<T>(READS_HOST ? (devPtr + hostDelta) : devPtr); }
+
+	/* got: what read() returned (not used by the modes that generate) */
+	template<bool FAST, class T, class Gen>
+	static __device__ __forceinline__ void apply(uint8_t* devPtr, int64_t hostDelta, uint64_t pos,
+		const Gen& gen, const T& got, VerifyAcc& acc)
+	{
+		T val;
+
+		if constexpr(READS)
+			val = got;
+		else
+			val = generate<FAST, T>(gen, pos);
+
+		if constexpr(WRITES_DEV)
+			store_elem(devPtr, val);
+		if constexpr(WRITES_HOST)
+			store_elem(devPtr + hostDelta, val);
+		if constexpr(VERIFY)
+			acc.check(val, generate<FAST, T>(gen, pos), pos);
+	}
+};
+
+/* ---- walking a block, for any thread group ------------------------------------------------
+ *
+ * A group of GROUP threads (a CTA of 256 for the tile kernels, a warp for the warp kernel) walks
+ * the 16-byte aligned body of a block in spans of GROUP x ELB_UNROLL vectors: the thread of rank r
+ * takes vectors r, r + GROUP, ..., so that every warp access covers 512 contiguous bytes and each
+ * thread has ELB_UNROLL independent accesses in flight. A CTA span is one 32 KiB tile. */
+
+template<int MODE, bool STAGED, int GROUP, bool FAST, bool FULL, class Gen>
+__device__ __forceinline__ void walk_span(const BlockGeom& g, const Gen& gen, int64_t hostDelta,
+	uint64_t spanStart, unsigned rank, VerifyAcc& acc)
+{
+	using Core = ModeCore<MODE, STAGED>;
+	uint8_t* body = g.ptr + g.headLen;
+	u64x2 got[ELB_UNROLL];
+
+	if constexpr(Core::READS && FULL)
+	{ // all loads first, then the rest
 		#pragma unroll
 		for(int u = 0; u < ELB_UNROLL; u++)
-		{
-			const uint64_t bodyOff = tileStart +
-				(uint64_t)(u * ELB_THREADS + threadIdx.x) * ELB_VEC_BYTES;
-			got[u] = ld_nc_na_128(bodyPtr + bodyOff);
-		}
+			got[u] = Core::template read<u64x2>(
+				body + spanStart + (uint64_t)(u * GROUP + rank) * ELB_VEC_BYTES, hostDelta);
+	}
 
-		#pragma unroll
-		for(int u = 0; u < ELB_UNROLL; u++)
+	#pragma unroll
+	for(int u = 0; u < ELB_UNROLL; u++)
+	{
+		const uint64_t off = spanStart + (uint64_t)(u * GROUP + rank) * ELB_VEC_BYTES;
+
+		if(FULL || (off < g.bodyLen) )
 		{
-			const uint64_t bodyOff = tileStart +
-				(uint64_t)(u * ELB_THREADS + threadIdx.x) * ELB_VEC_BYTES;
-			const uint64_t pos = g.headLen + bodyOff;
-			if(STAGED)
-				st_na_128(devBody + bodyOff, got[u] );
-			verify_vec(got[u], gen.template vec16<FAST>(pos), pos, numBad, firstBad);
+			if constexpr(Core::READS && !FULL) // (the last span of a block: one bounds check each)
+				got[u] = Core::template read<u64x2>(body + off, hostDelta);
+
+			Core::template apply<FAST>(body + off, hostDelta, g.headLen + off, gen, got[u], acc);
 		}
+	}
+}
+
+/* unaligned head and tail bytes (< 16 each): rank r < 16 takes head byte r, rank 16 + r takes
+   tail byte r */
+template<int MODE, bool STAGED, bool FAST, class Gen>
+__device__ __forceinline__ void walk_head_tail(const BlockGeom& g, const Gen& gen,
+	int64_t hostDelta, unsigned rank, VerifyAcc& acc)
+{
+	using Core = ModeCore<MODE, STAGED>;
+	const bool isTail = (rank >= ELB_VEC_BYTES);
+	const uint64_t idx = isTail ? (rank - ELB_VEC_BYTES) : rank;
+
+	if( (rank >= 2 * ELB_VEC_BYTES) || (idx >= (isTail ? g.tailLen : g.headLen) ) )
+		return;
+
+	const uint64_t pos = isTail ? (g.headLen + g.bodyLen + idx) : idx;
+	uint8_t got;
+
+	if constexpr(Core::READS)
+		got = Core::template read<uint8_t>(g.ptr + pos, hostDelta);
+
+	Core::template apply<FAST>(g.ptr + pos, hostDelta, pos, gen, got, acc);
+}
+
+/* body bytes [bodyBegin, bodyEnd) of one block; the group that starts at body byte 0 also takes
+   the head/tail bytes, before the spans (after them, ptxas spills the verify kernels). Verify
+   flushes its count once per call. */
+template<int MODE, bool STAGED, int GROUP, bool FAST, class Gen>
+__device__ __forceinline__ void walk_block(const KernelArgs& args, const BlockGeom& g,
+	const Gen& gen, uint32_t descIdx, uint64_t bodyBegin, uint64_t bodyEnd, unsigned rank)
+{
+	constexpr uint64_t SPAN_BYTES = (uint64_t)GROUP * ELB_VEC_BYTES * ELB_UNROLL;
+	const uint64_t end = (bodyEnd < g.bodyLen) ? bodyEnd : g.bodyLen;
+	VerifyAcc acc;
+
+	if(!bodyBegin)
+		walk_head_tail<MODE, STAGED, FAST>(g, gen, args.hostDelta, rank, acc);
+
+	for(uint64_t spanStart = bodyBegin; spanStart < end; spanStart += SPAN_BYTES)
+	{
+		if( (spanStart + SPAN_BYTES) <= g.bodyLen)
+			walk_span<MODE, STAGED, GROUP, FAST, true>(g, gen, args.hostDelta, spanStart, rank, acc);
+		else
+			walk_span<MODE, STAGED, GROUP, FAST, false>(g, gen, args.hostDelta, spanStart, rank,
+				acc);
+	}
+
+	if constexpr(MODE == MODE_VERIFY_PATTERN)
+		acc.flush(&args.results[descIdx], args.counters);
+}
+
+/* the generator of a fill or verify mode for one block */
+template<int MODE>
+__device__ __forceinline__ auto make_gen(const KernelArgs& args, const elb_block_desc& desc)
+{
+	if constexpr(MODE == MODE_FILL_RANDOM)
+	{
+		const uint64_t blockKey = elb_rand_block_key(args.seed, desc.blockCounter);
+		return RandomGen{blockKey, elb_rand_var_fill_len(desc.len, args.pct),
+			elb_rand_remainder_val(blockKey)};
 	}
 	else
+		return PatternGen{desc.fileOffset, args.salt};
+}
+
+/* builds the mode's generator for the block and picks its FAST or unaligned path */
+template<int MODE, bool STAGED, int GROUP>
+__device__ __forceinline__ void process_block(const KernelArgs& args, const elb_block_desc& desc,
+	uint32_t descIdx, const BlockGeom& g, uint64_t bodyBegin, uint64_t bodyEnd, unsigned rank)
+{
+	if constexpr(ModeCore<MODE, STAGED>::COPY)
+		walk_block<MODE, STAGED, GROUP, true>(args, g, NoGen{}, descIdx, bodyBegin, bodyEnd, rank);
+	else
 	{
-		#pragma unroll
-		for(int u = 0; u < ELB_UNROLL; u++)
-		{
-			const uint64_t bodyOff = tileStart +
-				(uint64_t)(u * ELB_THREADS + threadIdx.x) * ELB_VEC_BYTES;
-			if(bodyOff < g.bodyLen)
-			{
-				const uint64_t pos = g.headLen + bodyOff;
-				const u64x2 got = ld_nc_na_128(bodyPtr + bodyOff);
-				if(STAGED)
-					st_na_128(devBody + bodyOff, got);
-				verify_vec(got, gen.template vec16<FAST>(pos), pos, numBad, firstBad);
-			}
-		}
-	}
+		const auto gen = make_gen<MODE>(args, desc);
 
-	if(!tileIdx && (g.headLen | g.tailLen) )
-	{
-		const uint8_t* srcBlock = STAGED ? (g.ptr + hostDelta) : g.ptr;
-
-		if(threadIdx.x < g.headLen)
-		{
-			const uint8_t got = srcBlock[threadIdx.x];
-			if(STAGED)
-				g.ptr[threadIdx.x] = got;
-			if(got != gen.byte(threadIdx.x) )
-			{
-				numBad++;
-				if(threadIdx.x < firstBad)
-					firstBad = threadIdx.x;
-			}
-		}
-
-		const uint64_t tailStart = g.headLen + g.bodyLen;
-		if(threadIdx.x < g.tailLen)
-		{
-			const uint64_t pos = tailStart + threadIdx.x;
-			const uint8_t got = srcBlock[pos];
-			if(STAGED)
-				g.ptr[pos] = got;
-			if(got != gen.byte(pos) )
-			{
-				numBad++;
-				if(pos < firstBad)
-					firstBad = pos;
-			}
-		}
-	}
-
-	// warp-reduced mismatch count; global atomics only on the (rare) mismatch path
-	const unsigned warpBad = __reduce_add_sync(0xffffffffu, numBad);
-
-	if(__builtin_expect(warpBad != 0, 0) )
-	{
-		// 64-bit min via two 32-bit redux steps
-		const unsigned firstHi = (unsigned)(firstBad >> 32);
-		const unsigned minHi = __reduce_min_sync(0xffffffffu, firstHi);
-		const unsigned firstLo = (firstHi == minHi) ? (unsigned)firstBad : 0xffffffffu;
-		const unsigned minLo = __reduce_min_sync(0xffffffffu, firstLo);
-
-		if( (threadIdx.x & 31) == 0)
-		{
-			atomicAdd( (unsigned long long*)&result->numMismatchBytes,
-				(unsigned long long)warpBad);
-			atomicMin( (unsigned long long*)&result->firstMismatchIdx,
-				( (unsigned long long)minHi << 32) | minLo);
-			if(counters)
-				atomicAdd(&counters[ELB_DEVCTR_VERIFY_MISMATCH_BYTES],
-					(unsigned long long)warpBad);
-		}
+		if(gen.canUseFast(g.headLen) )
+			walk_block<MODE, STAGED, GROUP, true>(args, g, gen, descIdx, bodyBegin, bodyEnd, rank);
+		else
+			walk_block<MODE, STAGED, GROUP, false>(args, g, gen, descIdx, bodyBegin, bodyEnd, rank);
 	}
 }
 
 /* ---- kernels: walk all tiles of all descriptors, round-robin over the grid --------------- */
-
-/* STAGE_NONE: work on the device slot only (kernel level ABI, resident windows). STAGE_PUBLISH:
- * device slot only, but the last CTA of a verify launch publishes the results to pinned host
- * memory (copy-engine staging). STAGE_FULL: the kernel also moves the block between the rings. */
-enum { STAGE_NONE = 0, STAGE_PUBLISH = 1, STAGE_FULL = 2 };
-
-enum { MODE_FILL_PATTERN = 0, MODE_VERIFY_PATTERN = 1, MODE_FILL_RANDOM = 2,
-	MODE_COPY_IN = 3 /* host slot -> device slot */, MODE_COPY_OUT = 4 /* device -> host */,
-	NUM_MODES = 5 };
-
-struct KernelArgs
-{
-	const elb_block_desc* descs; // device-readable array, or NULL to use inlineDesc
-	elb_block_desc inlineDesc;   // single-block launches pass the descriptor by value
-	uint32_t numDescs;
-	uint64_t salt;         // pattern
-	uint64_t seed;         // random
-	unsigned pct;          // random
-	elb_verify_result* results; // verify
-	unsigned long long* counters; // optional device counter block
-
-	// staging (see the header comment); hostDelta == 0: work on the device slot only
-	int64_t hostDelta;              // host slot address = device slot address + hostDelta
-	elb_verify_result* hostResults; // verify: pinned copy of results, written by the last CTA
-	unsigned* doneTicket;           // device counter behind the last-CTA detection (stays 0)
-};
-
-/* number of tiles of a block; same rule as make_geom() */
-__device__ __forceinline__ uint64_t num_tiles_of(const elb_block_desc& desc)
-{
-	const uint64_t misalign = (uint64_t)(uintptr_t)desc.devPtr & (ELB_VEC_BYTES - 1);
-	uint64_t headLen = misalign ? (ELB_VEC_BYTES - misalign) : 0;
-	if(headLen > desc.len)
-		headLen = desc.len;
-
-	const uint64_t bodyLen = (desc.len - headLen) & ~(uint64_t)(ELB_VEC_BYTES - 1);
-	const uint64_t numTiles = (bodyLen + ELB_TILE_BYTES - 1) / ELB_TILE_BYTES;
-
-	return (!numTiles && desc.len) ? 1 : numTiles;
-}
-
-/* process tiles [tileBegin, tileEnd) of one block */
-template<int MODE, bool STAGED>
-__device__ __forceinline__ void process_block_tiles(const KernelArgs& args,
-	const elb_block_desc& desc, uint32_t descIdx, const BlockGeom& g, uint64_t tileBegin,
-	uint64_t tileEnd)
-{
-	const int64_t hostDelta = args.hostDelta;
-
-	if(MODE == MODE_FILL_PATTERN)
-	{
-		PatternGen gen;
-		gen.fileOffset = desc.fileOffset;
-		gen.salt = args.salt;
-
-		if(gen.canUseFast(g.headLen) )
-			for(uint64_t tileIdx = tileBegin; tileIdx < tileEnd; tileIdx++)
-				fill_tile<true, STAGED>(g, gen, tileIdx, hostDelta);
-		else
-			for(uint64_t tileIdx = tileBegin; tileIdx < tileEnd; tileIdx++)
-				fill_tile<false, STAGED>(g, gen, tileIdx, hostDelta);
-	}
-	else if(MODE == MODE_VERIFY_PATTERN)
-	{
-		PatternGen gen;
-		gen.fileOffset = desc.fileOffset;
-		gen.salt = args.salt;
-
-		if(gen.canUseFast(g.headLen) )
-			for(uint64_t tileIdx = tileBegin; tileIdx < tileEnd; tileIdx++)
-				verify_tile<true, STAGED>(g, gen, tileIdx, &args.results[descIdx], args.counters,
-					hostDelta);
-		else
-			for(uint64_t tileIdx = tileBegin; tileIdx < tileEnd; tileIdx++)
-				verify_tile<false, STAGED>(g, gen, tileIdx, &args.results[descIdx], args.counters,
-					hostDelta);
-	}
-	else if(MODE == MODE_FILL_RANDOM)
-	{
-		RandomGen gen;
-		gen.blockKey = elb_rand_block_key(args.seed, desc.blockCounter);
-		gen.varFillLen = elb_rand_var_fill_len(desc.len, args.pct);
-		gen.remainderVal = elb_rand_remainder_val(gen.blockKey);
-
-		if(gen.canUseFast(g.headLen) )
-			for(uint64_t tileIdx = tileBegin; tileIdx < tileEnd; tileIdx++)
-				fill_tile<true, STAGED>(g, gen, tileIdx, hostDelta);
-		else
-			for(uint64_t tileIdx = tileBegin; tileIdx < tileEnd; tileIdx++)
-				fill_tile<false, STAGED>(g, gen, tileIdx, hostDelta);
-	}
-	else
-	{
-		for(uint64_t tileIdx = tileBegin; tileIdx < tileEnd; tileIdx++)
-			copy_tile<MODE == MODE_COPY_IN>(g, tileIdx, hostDelta);
-	}
-}
 
 /* which device counter a mode accumulates block lengths into (-1: none) */
 template<int MODE>
@@ -644,16 +591,12 @@ elb_blocks_kernel(const KernelArgs args)
 	__shared__ uint32_t sStartDesc;
 
 	const uint32_t numDescs = args.numDescs;
-	const elb_block_desc* descs = args.descs;
 
 	// pass 1: total number of tiles
 	uint64_t myTiles = 0;
 
-	if(!descs)
-		myTiles = threadIdx.x ? 0 : num_tiles_of(args.inlineDesc);
-	else
-		for(uint32_t descIdx = threadIdx.x; descIdx < numDescs; descIdx += ELB_THREADS)
-			myTiles += num_tiles_of(descs[descIdx] );
+	for(uint32_t descIdx = threadIdx.x; descIdx < numDescs; descIdx += ELB_THREADS)
+		myTiles += make_geom(load_desc(args, descIdx) ).numTiles;
 
 	const uint64_t totalTiles = block_sum(myTiles, sScratch);
 	const uint64_t chunkTiles = (totalTiles + gridDim.x - 1) / gridDim.x;
@@ -670,71 +613,65 @@ elb_blocks_kernel(const KernelArgs args)
 		(chunkBegin + chunkTiles) : totalTiles;
 
 	// pass 2: locate the block that contains tile chunkBegin
-	uint32_t descIdx = 0;
-	uint64_t tileIdx = chunkBegin;
+	uint64_t segmentBase = 0; // tiles of all previous segments (uniform)
 
-	if(descs)
+	for(uint32_t segment = 0; segment < numDescs; segment += ELB_THREADS)
 	{
-		uint64_t segmentBase = 0; // tiles of all previous segments (uniform)
+		const uint32_t myDesc = segment + threadIdx.x;
+		const uint64_t tiles = (myDesc < numDescs) ? make_geom(load_desc(args, myDesc) ).numTiles : 0;
 
-		for(uint32_t segment = 0; segment < numDescs; segment += ELB_THREADS)
+		// inclusive scan inside the warp
+		uint64_t inclusive = tiles;
+		for(int offset = 1; offset < 32; offset <<= 1)
 		{
-			const uint32_t myDesc = segment + threadIdx.x;
-			const uint64_t tiles = (myDesc < numDescs) ? num_tiles_of(descs[myDesc] ) : 0;
-
-			// inclusive scan inside the warp
-			uint64_t inclusive = tiles;
-			for(int offset = 1; offset < 32; offset <<= 1)
-			{
-				const uint64_t other = __shfl_up_sync(0xffffffffu, inclusive, offset);
-				if( (threadIdx.x & 31) >= offset)
-					inclusive += other;
-			}
-
-			__syncthreads();
-
-			if( (threadIdx.x & 31) == 31)
-				sScratch[threadIdx.x >> 5] = inclusive;
-
-			__syncthreads();
-
-			uint64_t warpBase = 0;
-			uint64_t segmentTotal = 0;
-
-			#pragma unroll
-			for(int warp = 0; warp < (ELB_THREADS / 32); warp++)
-			{
-				if(warp < (int)(threadIdx.x >> 5) )
-					warpBase += sScratch[warp];
-				segmentTotal += sScratch[warp];
-			}
-
-			const uint64_t exclusive = segmentBase + warpBase + inclusive - tiles;
-
-			if(tiles && (chunkBegin >= exclusive) && (chunkBegin < (exclusive + tiles) ) )
-			{
-				sStartDesc = myDesc;
-				sStartTile = chunkBegin - exclusive;
-			}
-
-			segmentBase += segmentTotal;
-
-			if(segmentBase > chunkBegin)
-				break; // found (uniform)
+			const uint64_t other = __shfl_up_sync(0xffffffffu, inclusive, offset);
+			if( (threadIdx.x & 31) >= offset)
+				inclusive += other;
 		}
 
 		__syncthreads();
 
-		descIdx = sStartDesc;
-		tileIdx = sStartTile;
+		if( (threadIdx.x & 31) == 31)
+			sScratch[threadIdx.x >> 5] = inclusive;
+
+		__syncthreads();
+
+		uint64_t warpBase = 0;
+		uint64_t segmentTotal = 0;
+
+		#pragma unroll
+		for(int warp = 0; warp < (ELB_THREADS / 32); warp++)
+		{
+			if(warp < (int)(threadIdx.x >> 5) )
+				warpBase += sScratch[warp];
+			segmentTotal += sScratch[warp];
+		}
+
+		const uint64_t exclusive = segmentBase + warpBase + inclusive - tiles;
+
+		if(tiles && (chunkBegin >= exclusive) && (chunkBegin < (exclusive + tiles) ) )
+		{
+			sStartDesc = myDesc;
+			sStartTile = chunkBegin - exclusive;
+		}
+
+		segmentBase += segmentTotal;
+
+		if(segmentBase > chunkBegin)
+			break; // found (uniform)
 	}
+
+	__syncthreads();
+
+	uint32_t descIdx = sStartDesc;
+	uint64_t tileIdx = sStartTile;
 
 	// walk the chunk: consecutive tiles, block after block
 	uint64_t tilesLeft = chunkEnd - chunkBegin;
 
 	while(tilesLeft)
 	{
-		const elb_block_desc desc = descs ? descs[descIdx] : args.inlineDesc;
+		const elb_block_desc desc = load_desc(args, descIdx);
 		const BlockGeom g = make_geom(desc);
 
 		const uint64_t tileEnd = (g.numTiles - tileIdx < tilesLeft) ?
@@ -742,7 +679,8 @@ elb_blocks_kernel(const KernelArgs args)
 
 		if(tileIdx < tileEnd)
 		{
-			process_block_tiles<MODE, STAGED>(args, desc, descIdx, g, tileIdx, tileEnd);
+			process_block<MODE, STAGED, ELB_THREADS>(args, desc, descIdx, g,
+				tileIdx * ELB_TILE_BYTES, tileEnd * ELB_TILE_BYTES, threadIdx.x);
 
 			// device-resident stats: one atomic per block, by the CTA that owns its first tile
 			if( (counter_slot_of<MODE>() >= 0) && args.counters && !tileIdx && !threadIdx.x)
@@ -780,7 +718,7 @@ elb_blocks_tiled_kernel(const KernelArgs args, const uint32_t ctasPerBlock,
 	const uint32_t ctaInBlock = blockIdx.x - descIdx * ctasPerBlock;
 	const uint64_t tileIdx = (uint64_t)ctaInBlock * tilesPerCTA;
 
-	const elb_block_desc desc = args.descs ? args.descs[descIdx] : args.inlineDesc;
+	const elb_block_desc desc = load_desc(args, descIdx);
 	const BlockGeom g = make_geom(desc);
 
 	if(tileIdx >= g.numTiles)
@@ -795,7 +733,8 @@ elb_blocks_tiled_kernel(const KernelArgs args, const uint32_t ctasPerBlock,
 	const uint64_t tileEnd = ( (ctaInBlock + 1 == ctasPerBlock) ||
 		(tileIdx + tilesPerCTA >= g.numTiles) ) ? g.numTiles : (tileIdx + tilesPerCTA);
 
-	process_block_tiles<MODE, STAGED>(args, desc, descIdx, g, tileIdx, tileEnd);
+	process_block<MODE, STAGED, ELB_THREADS>(args, desc, descIdx, g, tileIdx * ELB_TILE_BYTES,
+		tileEnd * ELB_TILE_BYTES, threadIdx.x);
 
 	// device-resident stats: one atomic per block, by the CTA that owns its first tile
 	if( (counter_slot_of<MODE>() >= 0) && args.counters && !tileIdx && !threadIdx.x)
@@ -809,146 +748,11 @@ elb_blocks_tiled_kernel(const KernelArgs args, const uint32_t ctasPerBlock,
  *
  * For 4 KiB .. 8 KiB blocks (BASELINE configs[2]: 4 KiB random reads) a CTA per block leaves half
  * of its threads without a vector and pays the descriptor fetch and the block setup once per
- * 4 KiB. Here a CTA takes ELB_WARPS blocks, warp w works on block (cta * ELB_WARPS + w): a lane
- * handles the 16-byte vectors lane, lane+32, ... of the block body (a warp access covers 512 B,
- * 8 independent accesses in flight per lane), the verify reduction is the warp's own redux, the
- * device counter gets one atomic per CTA. */
+ * 4 KiB. Here a CTA takes ELB_WARPS blocks, warp w works on block (cta * ELB_WARPS + w) as a group
+ * of 32 (4 KiB spans), the verify reduction is the warp's own redux, the device counter gets one
+ * atomic per CTA. */
 
 #define ELB_WARPS (ELB_THREADS / 32)
-#define ELB_WARP_SPAN (32 * ELB_VEC_BYTES * ELB_UNROLL) /* 4 KiB per unrolled warp iteration */
-
-template<int MODE, bool STAGED, bool FAST, class Gen>
-__device__ __forceinline__ void process_block_warp(const KernelArgs& args, const BlockGeom& g,
-	const Gen& gen, elb_verify_result* result)
-{
-	const unsigned lane = threadIdx.x & 31;
-	const int64_t hostDelta = args.hostDelta;
-	uint8_t* devBody = g.ptr + g.headLen;
-	uint8_t* hostBody = devBody + hostDelta;
-
-	unsigned numBad = 0;
-	uint64_t firstBad = ~0ULL;
-
-	for(uint64_t spanStart = 0; spanStart < g.bodyLen; spanStart += ELB_WARP_SPAN)
-	{
-		if( (MODE == MODE_VERIFY_PATTERN) || (MODE == MODE_COPY_IN) || (MODE == MODE_COPY_OUT) )
-		{ // loads first, then the rest
-			const uint8_t* src = (MODE == MODE_COPY_OUT) ? devBody :
-				( ( (MODE == MODE_COPY_IN) || STAGED) ? hostBody : devBody);
-			u64x2 got[ELB_UNROLL];
-			bool valid[ELB_UNROLL];
-
-			#pragma unroll
-			for(int u = 0; u < ELB_UNROLL; u++)
-			{
-				const uint64_t bodyOff = spanStart + (uint64_t)(u * 32 + lane) * ELB_VEC_BYTES;
-				valid[u] = (bodyOff < g.bodyLen);
-				if(valid[u] )
-					got[u] = ld_nc_na_128(src + bodyOff);
-			}
-
-			#pragma unroll
-			for(int u = 0; u < ELB_UNROLL; u++)
-			{
-				const uint64_t bodyOff = spanStart + (uint64_t)(u * 32 + lane) * ELB_VEC_BYTES;
-				if(!valid[u] )
-					continue;
-
-				if(MODE == MODE_COPY_OUT)
-					st_na_128(hostBody + bodyOff, got[u] );
-				else
-				if( (MODE == MODE_COPY_IN) || STAGED)
-					st_na_128(devBody + bodyOff, got[u] );
-
-				if(MODE == MODE_VERIFY_PATTERN)
-				{
-					const uint64_t pos = g.headLen + bodyOff;
-					verify_vec(got[u], gen.template vec16<FAST>(pos), pos, numBad, firstBad);
-				}
-			}
-		}
-		else
-		{ // fill
-			#pragma unroll
-			for(int u = 0; u < ELB_UNROLL; u++)
-			{
-				const uint64_t bodyOff = spanStart + (uint64_t)(u * 32 + lane) * ELB_VEC_BYTES;
-				if(bodyOff < g.bodyLen)
-				{
-					const u64x2 v = gen.template vec16<FAST>(g.headLen + bodyOff);
-					st_na_128(devBody + bodyOff, v);
-					if(STAGED)
-						st_na_128(hostBody + bodyOff, v);
-				}
-			}
-		}
-	}
-
-	if(g.headLen | g.tailLen)
-	{ // unaligned head / tail bytes (at most 15 each): one lane per byte
-		const uint64_t tailStart = g.headLen + g.bodyLen;
-
-		for(int part = 0; part < 2; part++)
-		{
-			const uint64_t partLen = part ? g.tailLen : g.headLen;
-			const uint64_t pos = (part ? tailStart : 0) + lane;
-
-			if(lane >= partLen)
-				continue;
-
-			if( (MODE == MODE_FILL_PATTERN) || (MODE == MODE_FILL_RANDOM) )
-			{
-				const uint8_t b = gen.byte(pos);
-				g.ptr[pos] = b;
-				if(STAGED)
-					g.ptr[hostDelta + (int64_t)pos] = b;
-			}
-			else
-			if(MODE == MODE_COPY_OUT)
-				g.ptr[hostDelta + (int64_t)pos] = g.ptr[pos];
-			else
-			{
-				const bool fromHost = (MODE == MODE_COPY_IN) || STAGED;
-				const uint8_t got = fromHost ? g.ptr[hostDelta + (int64_t)pos] : g.ptr[pos];
-
-				if(fromHost)
-					g.ptr[pos] = got;
-
-				if( (MODE == MODE_VERIFY_PATTERN) && (got != gen.byte(pos) ) )
-				{
-					numBad++;
-					if(pos < firstBad)
-						firstBad = pos;
-				}
-			}
-		}
-	}
-
-	if(MODE == MODE_VERIFY_PATTERN)
-	{
-		const unsigned warpBad = __reduce_add_sync(0xffffffffu, numBad);
-
-		if(__builtin_expect(warpBad != 0, 0) )
-		{
-			const unsigned firstHi = (unsigned)(firstBad >> 32);
-			const unsigned minHi = __reduce_min_sync(0xffffffffu, firstHi);
-			const unsigned firstLo = (firstHi == minHi) ? (unsigned)firstBad : 0xffffffffu;
-			const unsigned minLo = __reduce_min_sync(0xffffffffu, firstLo);
-
-			if(!lane)
-			{ // (the only writer of this block's result: plain stores would do, atomics keep the
-			  //  contract that several launches may accumulate into one result)
-				atomicAdd( (unsigned long long*)&result->numMismatchBytes,
-					(unsigned long long)warpBad);
-				atomicMin( (unsigned long long*)&result->firstMismatchIdx,
-					( (unsigned long long)minHi << 32) | minLo);
-				if(args.counters)
-					atomicAdd(&args.counters[ELB_DEVCTR_VERIFY_MISMATCH_BYTES],
-						(unsigned long long)warpBad);
-			}
-		}
-	}
-}
 
 template<int MODE, int STAGE>
 __global__ void __launch_bounds__(ELB_THREADS, 3)
@@ -968,40 +772,13 @@ elb_blocks_warp_kernel(const KernelArgs args)
 
 	if(descIdx < args.numDescs)
 	{ // (uniform per warp)
-		const elb_block_desc desc = args.descs ? args.descs[descIdx] : args.inlineDesc;
+		const elb_block_desc desc = load_desc(args, descIdx);
 		const BlockGeom g = make_geom(desc);
 
 		if(g.len)
 		{
-			if( (MODE == MODE_FILL_PATTERN) || (MODE == MODE_VERIFY_PATTERN) )
-			{
-				PatternGen gen;
-				gen.fileOffset = desc.fileOffset;
-				gen.salt = args.salt;
-
-				if(gen.canUseFast(g.headLen) )
-					process_block_warp<MODE, STAGED, true>(args, g, gen, &args.results[descIdx] );
-				else
-					process_block_warp<MODE, STAGED, false>(args, g, gen, &args.results[descIdx] );
-			}
-			else
-			if(MODE == MODE_FILL_RANDOM)
-			{
-				RandomGen gen;
-				gen.blockKey = elb_rand_block_key(args.seed, desc.blockCounter);
-				gen.varFillLen = elb_rand_var_fill_len(desc.len, args.pct);
-				gen.remainderVal = elb_rand_remainder_val(gen.blockKey);
-
-				if(gen.canUseFast(g.headLen) )
-					process_block_warp<MODE, STAGED, true>(args, g, gen, NULL);
-				else
-					process_block_warp<MODE, STAGED, false>(args, g, gen, NULL);
-			}
-			else
-			{
-				PatternGen unused{};
-				process_block_warp<MODE, true, true>(args, g, unused, NULL);
-			}
+			process_block<MODE, STAGED, 32>(args, desc, descIdx, g, 0, g.bodyLen,
+				threadIdx.x & 31);
 
 			if( (counter_slot_of<MODE>() >= 0) && args.counters && !(threadIdx.x & 31) )
 				atomicAdd(&sBlockBytes, (unsigned long long)g.len);
@@ -1046,10 +823,11 @@ struct DeviceLaunchInfo
 {
 	int numSMs{0};
 	int ctasPerSM[NUM_MODES]{0, 0, 0, 0, 0};
-	/* 32 KiB tiles per CTA of the hardware-scheduled kernel; 0 = always use the persistent
-	   kernel for this mode. Tuning knob: ELB_TILES_PER_CTA="fill,verify,random". */
-	uint32_t tilesPerCTA[NUM_MODES]{1, 2, 8, 2, 2}; // H100: 1/1/4, 2/4/8, 4/4/16 within 0.6 % (DESIGN.md)
 };
+
+/* 32 KiB tiles per CTA of the hardware-scheduled kernel, per mode. H100: 1/1/4, 2/4/8, 4/4/16 for
+   fill/verify/random were within 0.6 % of 1/2/8 (DESIGN.md). */
+static const uint32_t gTilesPerCTA[NUM_MODES] = {1, 2, 8, 2, 2};
 
 static DeviceLaunchInfo gDevInfo[ELB_MAX_DEVICES];
 static std::once_flag gDevInfoOnce[ELB_MAX_DEVICES];
@@ -1083,15 +861,6 @@ static const DeviceLaunchInfo* getDeviceLaunchInfo()
 		gDevInfo[dev].ctasPerSM[MODE_FILL_RANDOM] = queryOccupancy<MODE_FILL_RANDOM>();
 		gDevInfo[dev].ctasPerSM[MODE_COPY_IN] = queryOccupancy<MODE_COPY_IN>();
 		gDevInfo[dev].ctasPerSM[MODE_COPY_OUT] = queryOccupancy<MODE_COPY_OUT>();
-
-		const char* tilesEnv = getenv("ELB_TILES_PER_CTA");
-		if(tilesEnv)
-		{
-			unsigned vals[3];
-			if(sscanf(tilesEnv, "%u,%u,%u", &vals[0], &vals[1], &vals[2]) == 3)
-				for(int mode = 0; mode < 3; mode++)
-					gDevInfo[dev].tilesPerCTA[mode] = vals[mode];
-		}
 	});
 
 	if(gDevInfo[dev].numSMs <= 0)
@@ -1104,18 +873,6 @@ static const DeviceLaunchInfo* getDeviceLaunchInfo()
 }
 
 #define ELB_WARP_KERNEL_MAX_BLOCK (8 * 1024)
-
-/* tuning / profiling knob: ELB_NO_WARP_KERNEL=1 sends small blocks through the tile kernels */
-static bool smallBlockKernelEnabled()
-{
-	static const bool enabled = []()
-	{
-		const char* env = getenv("ELB_NO_WARP_KERNEL");
-		return !(env && env[0] && (env[0] != '0') );
-	}();
-
-	return enabled;
-}
 
 static const char* modeName(int mode)
 {
@@ -1157,12 +914,11 @@ static int launchBlocksKernelT(const KernelArgs& args, uint64_t totalBytesHint,
 		return -1;
 
 	/* staged launches run at PCIe speed: one tile per CTA keeps the most loads in flight */
-	const uint32_t tilesPerCTA = (STAGE == STAGE_FULL) ? 1 : devInfo->tilesPerCTA[MODE];
+	const uint32_t tilesPerCTA = (STAGE == STAGE_FULL) ? 1 : gTilesPerCTA[MODE];
 
 	/* small blocks: one warp per block (a longer block than the hint said is still processed
 	   completely, the warp loops over its whole body) */
-	if(maxBlockLenHint && (maxBlockLenHint <= ELB_WARP_KERNEL_MAX_BLOCK) && args.descs &&
-		smallBlockKernelEnabled() )
+	if(maxBlockLenHint && (maxBlockLenHint <= ELB_WARP_KERNEL_MAX_BLOCK) && args.descs)
 	{
 		const uint64_t numCTAs = ( (uint64_t)args.numDescs + ELB_WARPS - 1) / ELB_WARPS;
 
@@ -1172,7 +928,7 @@ static int launchBlocksKernelT(const KernelArgs& args, uint64_t totalBytesHint,
 		return checkLaunch(modeName(MODE) );
 	}
 
-	if(maxBlockLenHint && totalBytesHint && tilesPerCTA)
+	if(maxBlockLenHint && totalBytesHint)
 	{
 		const uint64_t ctaBytes = (uint64_t)ELB_TILE_BYTES * tilesPerCTA;
 		const uint64_t ctasPerBlock = (maxBlockLenHint + ctaBytes - 1) / ctaBytes;

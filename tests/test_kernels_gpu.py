@@ -166,12 +166,34 @@ def make_batch(cuda_device, blocks):
     return torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(cuda_device)
 
 
-@pytest.mark.parametrize("max_block_len", [0, 1 << 20, 1 << 26])
+SHAPES = ["persistent", "warp", "tiled"]
+
+
+def shape_hints(shape, lens):
+    """size hints that pick the launch shape of a batch: none -> persistent grid; a block size
+    hint <= 8 KiB -> one warp per block (longer blocks are still processed whole); a larger hint
+    that covers every block -> hardware-scheduled tiles"""
+    if shape == "persistent":
+        return {}
+    hint = 4096 if shape == "warp" else max(max(lens), 32 << 10)
+    return dict(total_bytes=sum(lens), max_block_len=hint)
+
+
+def for_each_shape(check, *args, shapes=SHAPES):
+    """check(*args, shape) for every launch shape; a failure names the shape"""
+    for shape in shapes:
+        try:
+            check(*args, shape)
+        except AssertionError as err:
+            raise AssertionError("shape %s: %s" % (shape, err)) from err
+
+
+@pytest.mark.parametrize("max_block_len", [0, 4096, 1 << 20, 1 << 26])
 def test_batched_window_ragged_blocks(cuda_device, max_block_len):
     """one launch over a ragged window: different lengths, offsets, alignments, empty blocks.
-    max_block_len 0: persistent grid with static tile partition; 1 MiB: hardware-scheduled tiles
-    (CTAs past the end of shorter blocks exit); 64 MiB: bound so loose that the launcher falls
-    back to the persistent grid"""
+    max_block_len 0: persistent grid with static tile partition; 4 KiB: one warp per block, most
+    blocks longer than the hint; 1 MiB: hardware-scheduled tiles (CTAs past the end of shorter
+    blocks exit); 64 MiB: bound so loose that the launcher falls back to the persistent grid"""
     rng = random.Random(77)
     lens = [1 << 20, 4096, 0, 65536 + 3, 1, (1 << 20) - 32, 777, 32768 * 3, 5, 1 << 16]
     arena = dev_bytes(sum(lens) + 64 * len(lens), cuda_device)
@@ -354,7 +376,13 @@ def _pinned_descs(blocks):
 @pytest.mark.parametrize("hinted", [True, False])
 def test_staged_fill_writes_both_rings(cuda_device, misalign, hinted):
     """fill + stage-out: device slot and host slot both hold the oracle's bytes, nothing else is
-    touched; descriptors are read from pinned host memory (ragged lengths, both launch shapes)."""
+    touched; descriptors are read from pinned host memory (ragged lengths; with size hints the
+    tiled and the warp shape, without them the persistent one)."""
+    for_each_shape(_check_staged_fill, cuda_device, misalign,
+                   shapes=["tiled", "warp"] if hinted else ["persistent"])
+
+
+def _check_staged_fill(cuda_device, misalign, shape):
     lens = [1 << 20, (1 << 20) - 13, 4096, 33, 0, 65536 + 5]
     stride = (1 << 20) + 4096
     dev, host, delta = _staged_arena(cuda_device, stride * len(lens) + 64)
@@ -362,7 +390,7 @@ def test_staged_fill_writes_both_rings(cuda_device, misalign, hinted):
     blocks = [(dev.data_ptr() + i * stride + misalign, n, (i << 21) + 3 * i, i)
               for i, n in enumerate(lens)]
     descs = _pinned_descs(blocks)
-    hints = dict(total_bytes=sum(lens), max_block_len=max(lens)) if hinted else {}
+    hints = shape_hints(shape, lens)
     kernels.fill_pattern_staged(descs.data_ptr(), len(blocks), salt, delta, 0, stream_handle(),
                                 **hints)
     torch.cuda.synchronize()
@@ -389,7 +417,12 @@ def test_staged_fill_writes_both_rings(cuda_device, misalign, hinted):
 @pytest.mark.parametrize("misalign", [0, 5])
 def test_staged_verify_reads_host_ring_and_publishes_results(cuda_device, misalign):
     """stage-in + verify: data comes from the pinned host slot, lands in the device slot, the
-    last CTA publishes per-block results to pinned host memory and re-arms the device results."""
+    last CTA publishes per-block results to pinned host memory and re-arms the device results
+    (every launch shape)."""
+    for_each_shape(_check_staged_verify, cuda_device, misalign)
+
+
+def _check_staged_verify(cuda_device, misalign, shape):
     lens = [1 << 20, 70000, 4096, 0, (1 << 20) + 31]
     stride = (1 << 20) + 4096
     dev, host, delta = _staged_arena(cuda_device, stride * len(lens) + 64)
@@ -416,7 +449,7 @@ def test_staged_verify_reads_host_ring_and_publishes_results(cuda_device, misali
         kernels.verify_pattern_staged(descs.data_ptr(), len(blocks), salt, delta,
                                       dev_results.data_ptr(), host_results.data_ptr(),
                                       ticket.data_ptr(), counters.data_ptr(), stream_handle(),
-                                      total_bytes=sum(lens), max_block_len=max(lens))
+                                      **shape_hints(shape, lens))
         torch.cuda.synchronize()
         got = [(int(host_results[2 * i]) & (2 ** 64 - 1), int(host_results[2 * i + 1]) & (2 ** 64 - 1))
                for i in range(len(blocks))]
@@ -435,7 +468,11 @@ def test_staged_verify_reads_host_ring_and_publishes_results(cuda_device, misali
 
 def test_verify_publishes_results_without_staging(cuda_device):
     """host_delta 0: verify on the device slot (copy-engine staging / cuFile), results still
-    published by the last CTA"""
+    published by the last CTA (every launch shape)"""
+    for_each_shape(_check_verify_publishes, cuda_device)
+
+
+def _check_verify_publishes(cuda_device, shape):
     n, salt = (1 << 20) + 17, 3
     dev = dev_bytes(n, cuda_device)
     kernels.fill_pattern(dev.data_ptr(), n, 4096, salt, stream_handle())
@@ -447,13 +484,17 @@ def test_verify_publishes_results_without_staging(cuda_device):
     kernels.verify_results_init(dev_results.data_ptr(), 1, stream_handle())
     kernels.verify_pattern_staged(descs.data_ptr(), 1, salt, 0, dev_results.data_ptr(),
                                   host_results.data_ptr(), ticket.data_ptr(), 0, stream_handle(),
-                                  total_bytes=n, max_block_len=n)
+                                  **shape_hints(shape, [n]))
     torch.cuda.synchronize()
     assert host_results.tolist() == [1, 123456]
 
 
 @pytest.mark.parametrize("to_device", [True, False])
 def test_stage_copy_kernels(cuda_device, to_device):
+    for_each_shape(_check_stage_copy, cuda_device, to_device)
+
+
+def _check_stage_copy(cuda_device, to_device, shape):
     lens = [1 << 20, 12345, 0, 4096]
     stride = (1 << 20) + 4096
     dev, host, delta = _staged_arena(cuda_device, stride * len(lens))
@@ -465,7 +506,7 @@ def test_stage_copy_kernels(cuda_device, to_device):
     else:
         dev.copy_(rnd.to(cuda_device))
     kernels.stage_copy(descs.data_ptr(), len(blocks), to_device, delta, stream_handle(),
-                       total_bytes=sum(lens), max_block_len=max(lens))
+                       **shape_hints(shape, lens))
     torch.cuda.synchronize()
     dev_bytes_, host_bytes, src = to_bytes(dev), host.numpy().tobytes(), rnd.numpy().tobytes()
     for ptr, n, _, _ in blocks:
@@ -486,8 +527,12 @@ SMALL_LENS = [4096, 4096, 1, 31, 32, 33, 0, 1000, 4095, 4097, 8192, 8191, 4096, 
 @pytest.mark.parametrize("misalign", [0, 3, 16])
 def test_small_block_kernels_match_oracle(cuda_device, misalign):
     """hint <= 8 KiB -> one warp per block: ragged lengths, unaligned addresses and file offsets,
-    a block longer than the hint, more blocks than one CTA takes; fill / verify / random fill"""
-    hint = 4096
+    a block longer than the hint, more blocks than one CTA takes; fill / verify / random fill.
+    The same small blocks also go through the tile kernels."""
+    for_each_shape(_check_small_blocks, cuda_device, misalign)
+
+
+def _check_small_blocks(cuda_device, misalign, shape):
     stride = 24 * 1024
     nblocks = len(SMALL_LENS) * 3 + 1  # (not a multiple of the 8 blocks a CTA takes)
     lens = (SMALL_LENS * 4)[:nblocks]
@@ -499,8 +544,9 @@ def test_small_block_kernels_match_oracle(cuda_device, misalign):
     descs = make_batch(cuda_device, blocks)
     results = torch.zeros(2 * nblocks, dtype=torch.int64, device=cuda_device)
     counters = torch.zeros(kernels.DEVCTR_NUM, dtype=torch.int64, device=cuda_device)
+    hints = shape_hints(shape, lens)
     kernels.fill_pattern_batch(descs.data_ptr(), nblocks, salt, counters.data_ptr(),
-                               stream_handle(), total_bytes=sum(lens), max_block_len=hint)
+                               stream_handle(), **hints)
     torch.cuda.synchronize()
     host = to_bytes(arena)
     covered = bytearray(len(host))
@@ -513,8 +559,7 @@ def test_small_block_kernels_match_oracle(cuda_device, misalign):
 
     # verify: clean, then corrupted
     kernels.verify_pattern_batch(descs.data_ptr(), nblocks, salt, results.data_ptr(),
-                                 counters.data_ptr(), stream_handle(), total_bytes=sum(lens),
-                                 max_block_len=hint)
+                                 counters.data_ptr(), stream_handle(), **hints)
     torch.cuda.synchronize()
     assert read_result(results) == [(0, 0xFFFFFFFFFFFFFFFF)] * nblocks
     assert counters.cpu().tolist()[kernels.DEVCTR_VERIFIED_BYTES] == sum(lens)
@@ -529,15 +574,14 @@ def test_small_block_kernels_match_oracle(cuda_device, misalign):
         for pos in positions:
             arena[blocks[idx][0] - base + pos] ^= 0x3C
     kernels.verify_pattern_batch(descs.data_ptr(), nblocks, salt, results.data_ptr(), 0,
-                                 stream_handle(), total_bytes=sum(lens), max_block_len=hint)
+                                 stream_handle(), **hints)
     torch.cuda.synchronize()
     got = read_result(results)
     for idx in range(nblocks):
         exp = (len(bad[idx]), bad[idx][0]) if idx in bad else (0, 0xFFFFFFFFFFFFFFFF)
         assert got[idx] == exp, idx
 
-    kernels.fill_random_batch(descs.data_ptr(), nblocks, 50, 777, 0, stream_handle(),
-                              total_bytes=sum(lens), max_block_len=hint)
+    kernels.fill_random_batch(descs.data_ptr(), nblocks, 50, 777, 0, stream_handle(), **hints)
     torch.cuda.synchronize()
     host = to_bytes(arena)
     for ptr, n, _, ctr in blocks:
@@ -547,8 +591,12 @@ def test_small_block_kernels_match_oracle(cuda_device, misalign):
 
 def test_small_block_staged_kernels(cuda_device):
     """the staged forms of the warp-per-block kernels: fill + stage-out, stage-in + verify with
-    published results, stage copies"""
-    hint, stride = 4096, 8192
+    published results, stage copies (and the same small blocks through the tile kernels)"""
+    for_each_shape(_check_small_blocks_staged, cuda_device)
+
+
+def _check_small_blocks_staged(cuda_device, shape):
+    stride = 8192
     lens = [4096] * 21 + [100, 0, 4095, 8192 - 64]
     nblocks = len(lens)
     dev, host, delta = _staged_arena(cuda_device, stride * nblocks + 64)
@@ -556,7 +604,7 @@ def test_small_block_staged_kernels(cuda_device):
     blocks = [(dev.data_ptr() + i * stride + (8 if i % 4 == 1 else 0), n, 1 << 30 | (i * 4096), i)
               for i, n in enumerate(lens)]
     descs = _pinned_descs(blocks)
-    hints = dict(total_bytes=sum(lens), max_block_len=hint)
+    hints = shape_hints(shape, lens)
     kernels.fill_pattern_staged(descs.data_ptr(), nblocks, salt, delta, 0, stream_handle(), **hints)
     torch.cuda.synchronize()
     dev_b, host_b = to_bytes(dev), host.numpy().tobytes()
