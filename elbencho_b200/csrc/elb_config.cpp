@@ -175,10 +175,21 @@ Config Config::fromABI(const elb_cfg* cfg)
 	if(c.doDirectVerify && !c.integrityCheckSalt) // :1424-1426
 		throw WorkerError("Direct verification requires --verify and --write");
 
-	if(c.doDirectVerify && (c.ioDepth > 1) ) // :1428-1429
+	if(cfg->ioEngine == ELB_IOENGINE_AUTO) // LocalWorker.cpp:1243-1244
+		c.ioEngine = (c.ioDepth > 1) ? ELB_IOENGINE_AIO : ELB_IOENGINE_SYNC;
+	else
+	if( (cfg->ioEngine == ELB_IOENGINE_SYNC) || (cfg->ioEngine == ELB_IOENGINE_AIO) )
+		c.ioEngine = cfg->ioEngine;
+	else
+		throw WorkerError("Invalid I/O engine: " + std::to_string(cfg->ioEngine) );
+
+	// the async engines have no read-back and no direct verification, also at --iodepth 1
+	const bool useAsyncEngine = (c.ioDepth > 1) || (c.ioEngine == ELB_IOENGINE_AIO);
+
+	if(c.doDirectVerify && useAsyncEngine) // :1428-1429
 		throw WorkerError("Direct verification cannot be used together with --iodepth");
 
-	if(c.doReadInline && (c.ioDepth > 1) ) // :1431-1432
+	if(c.doReadInline && useAsyncEngine) // :1431-1432
 		throw WorkerError("Inline read cannot be used together with --iodepth");
 
 	if( (c.doDirectVerify || c.doReadInline) && c.rwMixReadPercent)
@@ -189,14 +200,6 @@ Config Config::fromABI(const elb_cfg* cfg)
 
 	if(c.useCuFile && !c.useDirectIO) // :1315-1322
 		c.useDirectIO = true;
-
-	if(cfg->ioEngine == ELB_IOENGINE_AUTO) // LocalWorker.cpp:1243-1244
-		c.ioEngine = (c.ioDepth > 1) ? ELB_IOENGINE_AIO : ELB_IOENGINE_SYNC;
-	else
-	if( (cfg->ioEngine == ELB_IOENGINE_SYNC) || (cfg->ioEngine == ELB_IOENGINE_AIO) )
-		c.ioEngine = cfg->ioEngine;
-	else
-		throw WorkerError("Invalid I/O engine: " + std::to_string(cfg->ioEngine) );
 
 	// ---- path dependent normalisation (ProgArgs.cpp:1471-1671) ----
 

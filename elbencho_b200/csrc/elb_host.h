@@ -781,7 +781,7 @@ inline void liveOpsAdd(elb_liveops& dst, const elb_liveops& src)
  *
  * Buffered writes to one inode are serialised by the kernel on the inode lock; what a writer can
  * win is a fast hand-over and a source buffer that is still in the last level cache. Tickets give
- * FIFO order. A waiter sleeps on a futex word of its own ticket slot while nearDistance() (2) or more
+ * FIFO order. A waiter sleeps on a futex word of its own ticket slot while NEAR_DISTANCE (2) or more
  * tickets are ahead of it and is woken when it gets near (one targeted wake-up per hand-over,
  * hidden behind the current holder's write); the near ones spin in user space, so the hand-over
  * itself costs a cache line transfer, not a wake-up. Knowing its position lets a worker produce
@@ -792,18 +792,7 @@ inline void liveOpsAdd(elb_liveops& dst, const elb_liveops& src)
 class FileWriteGate
 {
 	public:
-		/* tickets ahead at which a waiter still sleeps (tuning knob: ELB_GATE_NEAR=2..8) */
-		static unsigned nearDistance()
-		{
-			static const unsigned distance = []()
-			{
-				const char* env = getenv("ELB_GATE_NEAR");
-				const int val = env ? atoi(env) : 0;
-				return ( (val >= 2) && (val <= 8) ) ? (unsigned)val : 2u;
-			}();
-
-			return distance;
-		}
+		static const unsigned NEAR_DISTANCE = 2; // tickets ahead at which a waiter still sleeps
 
 		/* tickets ahead of the given one right now (0 = it is its turn) */
 		uint64_t distanceOf(uint64_t ticket) const
@@ -817,7 +806,7 @@ class FileWriteGate
 
 		uint64_t takeTicket() { return nextTicket.fetch_add(1, std::memory_order_relaxed); }
 
-		/* sleeps until fewer than nearDistance() tickets are ahead of this one */
+		/* sleeps until fewer than NEAR_DISTANCE tickets are ahead of this one */
 		void waitUntilNear(uint64_t ticket)
 		{
 			std::atomic<uint32_t>& mySlot = wakeSeq[ticket % NUM_SLOTS];
@@ -826,7 +815,7 @@ class FileWriteGate
 			{
 				const uint32_t seq = mySlot.load(std::memory_order_acquire);
 
-				if( (ticket - serving.load(std::memory_order_acquire) ) < nearDistance() )
+				if( (ticket - serving.load(std::memory_order_acquire) ) < NEAR_DISTANCE)
 					return;
 
 				futexWait(&mySlot, seq);
@@ -861,9 +850,9 @@ class FileWriteGate
 		{
 			const uint64_t done = serving.fetch_add(1, std::memory_order_release);
 
-			/* ticket done+1 is served now; ticket done+nearDistance() just got near: wake it if it
+			/* ticket done+1 is served now; ticket done+NEAR_DISTANCE just got near: wake it if it
 			   sleeps (a thread that takes that ticket later sees the new serving value) */
-			const uint64_t nearTicket = done + nearDistance();
+			const uint64_t nearTicket = done + NEAR_DISTANCE;
 			std::atomic<uint32_t>& slot = wakeSeq[nearTicket % NUM_SLOTS];
 
 			slot.fetch_add(1, std::memory_order_release);

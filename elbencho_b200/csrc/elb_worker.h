@@ -10,12 +10,14 @@
  * contiguous slice of a pinned host ring and of a device ring, and every batch moves through
  * two stages that overlap across batches:
  *
- *   write:  [GPU: fill kernel over the whole batch -> one staged D2H copy] -> [storage writes]
- *   read:   [storage reads] -> [GPU: one staged H2D copy -> verify kernel over the whole batch]
+ *   write:  [GPU: fill the batch's blocks, stage them out to the host ring] -> [storage writes]
+ *   read:   [storage reads] -> [GPU: stage the batch's blocks in, verify them]
  *
  * so that storage transfers of batch k run while the GPU works on batch k+1 (write) or k-1
- * (read). Results (bytes on disk, counters, verify outcome and message) equal the reference's
- * serial loop.
+ * (read). With kernel staging the GPU stage of a batch is one launch; copy-engine staging pairs
+ * the fill / verify launch with cudaMemcpyAsync; with cuFile the storage I/O uses the device ring
+ * and the fill / verify is all that is left (GpuStage). Results (bytes on disk, counters, verify
+ * outcome and message) equal the reference's serial loop.
  */
 #ifndef ELB_WORKER_H_
 #define ELB_WORKER_H_
@@ -113,6 +115,25 @@ class BlockSource
 		virtual uint64_t getNumBytesTotal() const = 0; // expected bytes of this worker
 };
 
+/* what the GPU stage of a batch does in one direction, resolved from the config once */
+struct GpuStage
+{
+	enum Transfer
+	{
+		TRANSFER_NONE,   // cuFile: the storage I/O uses the device ring
+		TRANSFER_KERNEL, // the fill / verify launch moves the blocks, else the stage-copy kernel
+		TRANSFER_COPY,   // cudaMemcpyAsync between the rings
+	};
+
+	enum Compute { COMPUTE_NONE, COMPUTE_FILL_PATTERN, COMPUTE_FILL_RANDOM, COMPUTE_VERIFY };
+
+	bool isRead;      // host ring -> device ring (read) or device ring -> host ring (write)
+	Transfer transfer;
+	Compute compute;
+	bool useGraph;    // replay full batches from a CUDA graph (one launch per batch anyway under
+	                  // kernel staging)
+};
+
 /* a batch: a contiguous slice of the rings plus everything its GPU stage needs */
 struct Batch
 {
@@ -125,7 +146,7 @@ struct Batch
 	cudaEvent_t gpuDoneEvent{NULL};
 	cudaEvent_t kernelStartEvent{NULL}; // around the fill/verify kernel only
 	cudaEvent_t kernelDoneEvent{NULL};
-	bool hadKernel{false};
+	bool hadKernel{false};              // the last GPU stage recorded the kernel events
 
 	/* descriptors live in pinned host memory and are read by the kernels over PCIe; verify results
 	   are published to pinned host memory by the last CTA of the launch (device-side ticket),
@@ -139,7 +160,6 @@ struct Batch
 	std::vector<struct iocb> iocbs;
 	std::vector<struct iocb*> iocbPtrs;
 	uint32_t numIOPending{0};
-	bool ioSubmitted{false};
 
 	// cuFile batch state (iodepth > 1 with --cufile)
 	CUfileBatchHandle_t cuBatch{NULL};
@@ -230,7 +250,8 @@ class Worker
 		char* hostRing{NULL}; // pinned
 		char* devRing{NULL};
 		int64_t hostDelta{0}; // hostRing - devRing: host slot of a block = device slot + hostDelta
-		bool stageWithKernels{true}; // resolved elb_cfg::stagingEngine
+		GpuStage readStage{};  // resolved elb_cfg::stagingEngine, --cufile, --verify, --blockvarpct
+		GpuStage writeStage{};
 		bool useWriteGate{false};    // resolved elb_cfg::serializeBufferedWrites
 		int boundNumaNode{-1};       // NUMA node this worker bound itself to (-1: none)
 		std::vector<Batch> batches;
@@ -246,7 +267,7 @@ class Worker
 		bool dirModeCountsEntry{true}; // false for a partial slice of a shared tree file
 		void applyNumaAndCoreBinding();     // Worker.cpp:102-146
 		void bindToNumaNode(int zoneNum, bool strict);
-		void enqueueStageCopies(Batch& batch, bool hostToDevice, bool onlyWrites);
+		uint64_t enqueueStageCopies(Batch& batch, bool hostToDevice, bool onlyOwnDirection);
 		void flockBlock(int fd, const BlockRef& block, bool isUnlock); // FileTk::flock
 		void fadviseFile(int fd, const std::string& path);             // FileTk::fadvise
 		void takeCustomTreeShare(); // LocalWorker.cpp:1520-1560
@@ -318,14 +339,13 @@ class Worker
 			bool oneFilePerBatch = false);
 		void verifyWrittenBatch(Batch& batch);
 		void accountBatch(Batch& batch, uint64_t gpuUSecTotal);
-		void gpuLaunchWriteStage(Batch& batch);
-		void gpuLaunchReadStage(Batch& batch);
-		size_t fillWriteDescs(Batch& batch, uint64_t& outNumWriteBytes);
-		void enqueueWriteWork(Batch& batch, size_t numWriteBlocks, uint64_t numWriteBytes,
-			bool timeKernel);
-		void enqueueReadWork(Batch& batch, bool timeKernel);
+		void gpuLaunchStage(Batch& batch, bool isRead);
+		uint32_t fillStageDescs(Batch& batch, bool isRead, uint64_t& outNumBytes);
+		void enqueueStage(Batch& batch, const GpuStage& stage, uint32_t numBlocks,
+			uint64_t numBytes);
 		bool isStandardShapedBatch(const Batch& batch) const;
-		cudaGraphExec_t captureBatchGraph(Batch& batch, bool isRead);
+		cudaGraphExec_t captureBatchGraph(Batch& batch, const GpuStage& stage, uint32_t numBlocks,
+			uint64_t numBytes);
 		void gpuWait(Batch& batch);
 		void retireReadBatch(Batch& batch);
 		void checkVerifyResults(Batch& batch);

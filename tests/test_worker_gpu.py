@@ -332,6 +332,70 @@ def test_plain_write_read_without_verify(workdir, staging_engine):
         assert not os.path.exists(cfg.paths[0])
 
 
+def expected_stage_counters(staging_engine, num_batches, stage_bytes, compute):
+    """GPU stage counters of a phase in which every batch has blocks for its stage: one launch
+    per batch if there is something to compute or the stage-copy kernel moves the blocks"""
+    launches = num_batches if (compute or staging_engine == "kernel") else 0
+    return dict(num_kernel_launches=launches,
+                filled_bytes=stage_bytes if compute == "fill" else 0,
+                verified_bytes=stage_bytes if compute == "verify" else 0,
+                kernel_timed=bool(compute))
+
+
+def check_stage_counters(res, expected, h2d_bytes, d2h_bytes):
+    got = dict(num_kernel_launches=res["num_kernel_launches"], filled_bytes=res["filled_bytes"],
+               verified_bytes=res["verified_bytes"], kernel_timed=res["dev_kernel_usec"] > 0)
+    assert got == expected
+    assert (res["h2d_bytes"], res["d2h_bytes"]) == (h2d_bytes, d2h_bytes)
+
+
+@pytest.mark.parametrize("num_blocks", [12, 10], ids=["standard", "ragged"])
+@pytest.mark.parametrize("fill", ["pattern", "random", "none"])
+def test_stage_counters_per_phase(workdir, staging_engine, fill, num_blocks):
+    """exact launch / byte counters of a write phase (pattern fill, random fill or nothing) and of
+    the read phase after it (with --verify after the pattern fill): 4 blocks per batch, so that
+    12 blocks are full batches (replayed from CUDA graphs under copy-engine staging) and 10 end
+    with a ragged batch"""
+    block, batch_blocks = 256 * KiB, 4
+    size = num_blocks * block
+    num_batches = -(-num_blocks // batch_blocks)
+    cfg = WorkerConfig(paths=[os.path.join(workdir, "ctr")], block_size=block, file_size=size,
+                       pipeline_batch_blocks=batch_blocks,
+                       integrity_check_salt=1 if fill == "pattern" else 0,
+                       block_variance_percent=100 if fill == "random" else 0,
+                       block_variance_seed=5)
+    with WorkerManager(cfg) as mgr:
+        w = mgr.run_phase(BenchPhase.CREATEFILES)
+        r = mgr.run_phase(BenchPhase.READFILES)
+    assert w["ops_total"]["bytes"] == r["ops_total"]["bytes"] == size
+    check_stage_counters(w, expected_stage_counters(
+        staging_engine, num_batches, size, "fill" if fill != "none" else None), 0, size)
+    check_stage_counters(r, expected_stage_counters(
+        staging_engine, num_batches, size, "verify" if fill == "pattern" else None), size, 0)
+
+
+@pytest.mark.parametrize("fill", ["random", "none"])
+@pytest.mark.parametrize("engine,depth", [(IOEngine.SYNC, 1), (IOEngine.AIO, 4)])
+def test_stage_counters_rwmix_write(workdir, staging_engine, engine, depth, fill):
+    """--rwmixpct 6 over 12 blocks of one worker: blocks 0-5 are reads, 6-11 writes. Batch 0
+    (blocks 0-3) has no GPU write stage, batch 1 fills 2 blocks, batch 2 is a full write batch.
+    The reads of the write phase go to the GPU, the writes come from it."""
+    block, batch_blocks, num_blocks = 256 * KiB, 4, 12
+    size = num_blocks * block
+    path = os.path.join(workdir, "mix")
+    with open(path, "wb") as f:
+        f.write(bytes(size))
+    cfg = WorkerConfig(paths=[path], block_size=block, file_size=size,
+                       pipeline_batch_blocks=batch_blocks, rwmix_read_percent=6,
+                       block_variance_percent=100 if fill == "random" else 0,
+                       block_variance_seed=5, io_engine=engine, io_depth=depth)
+    with WorkerManager(cfg) as mgr:
+        w = mgr.run_phase(BenchPhase.CREATEFILES)
+    assert w["ops_total"]["bytes"] == w["ops_readmix_total"]["bytes"] == size // 2
+    check_stage_counters(w, expected_stage_counters(
+        staging_engine, 2, size // 2, "fill" if fill == "random" else None), size // 2, size // 2)
+
+
 def test_short_read_error_text(workdir):
     size, block = 1 * MiB, 256 * KiB
     cfg = WorkerConfig(paths=[os.path.join(workdir, "short")], block_size=block, file_size=size,

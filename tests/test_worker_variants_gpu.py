@@ -173,6 +173,14 @@ def test_variant_option_validation():
     with pytest.raises(WorkerError, match="cannot be used together with --iodepth"):
         WorkerManager(WorkerConfig(paths=["/tmp/x"], file_size=4096, do_read_inline=True,
                                    io_depth=4))
+    # the async engine at iodepth 1 would skip the read-back and the direct verification
+    with pytest.raises(WorkerError, match="Direct verification cannot be used together with "
+                                          "--iodepth"):
+        WorkerManager(WorkerConfig(paths=["/tmp/x"], file_size=4096, do_direct_verify=True,
+                                   integrity_check_salt=1, io_engine=IOEngine.AIO))
+    with pytest.raises(WorkerError, match="Inline read cannot be used together with --iodepth"):
+        WorkerManager(WorkerConfig(paths=["/tmp/x"], file_size=4096, do_read_inline=True,
+                                   io_engine=IOEngine.AIO))
     with pytest.raises(WorkerError, match="rwmixthr"):
         WorkerManager(WorkerConfig(paths=["/tmp/x"], file_size=4096, rwmix_read_percent=10,
                                    num_rwmix_read_threads=1))
