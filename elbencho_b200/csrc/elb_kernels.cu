@@ -292,10 +292,14 @@ struct VerifyAcc
 	__device__ __forceinline__ void flush(elb_verify_result* result,
 		unsigned long long* counters) const
 	{
-		const unsigned warpBad = __reduce_add_sync(0xffffffffu, numBad);
-
-		if(__builtin_expect(warpBad != 0, 0) )
+		if(__builtin_expect(__any_sync(0xffffffffu, numBad != 0), 0) )
 		{
+			/* a warp's count can reach 2^32 (the warp shape walks a whole block with one warp):
+			   sum the high and low 16 bits of the lane counts apart (each sum < 2^21) */
+			const uint64_t warpBad =
+				( (uint64_t)__reduce_add_sync(0xffffffffu, numBad >> 16) << 16) +
+				__reduce_add_sync(0xffffffffu, numBad & 0xffffu);
+
 			// 64-bit min via two 32-bit redux steps
 			const unsigned firstHi = (unsigned)(firstBad >> 32);
 			const unsigned minHi = __reduce_min_sync(0xffffffffu, firstHi);

@@ -510,3 +510,119 @@ def test_mid_size_multi_batch_run_bytes_equal_oracle(workdir, staging_engine):
     assert gr["h2d_bytes"] == size
     assert gr["dev_kernel_usec"] > 0 and gw["dev_kernel_usec"] > 0
     assert sha(gcfg.paths[0]) == sha(ccfg.paths[0])
+
+
+# verify failures in every submission order: (offset order, threads, block size, engine), a
+# pairwise cover of 5 orders x 2 thread counts x 3 block sizes x 2 I/O engines
+ORDERS = {
+    "sequential": {},
+    "reverse": dict(do_reverse_seq_offsets=True),
+    "strided": dict(use_strided_access=True),
+    "random": dict(use_random_offsets=True, rand_offset_seed=31),
+    "random_unaligned": dict(use_random_offsets=True, use_random_unaligned=True,
+                             rand_offset_seed=34),
+}
+ENGINES = {"sync": dict(io_engine=IOEngine.SYNC, io_depth=1),
+           "aio4": dict(io_engine=IOEngine.AIO, io_depth=4)}
+NUM_BLOCKS = {4 * KiB: 600, 64 * KiB: 60, 1000: 1500}
+VERIFY_ORDER_CASES = [
+    ("sequential", 4 * KiB, 1, "sync"), ("sequential", 64 * KiB, 3, "aio4"),
+    ("sequential", 1000, 3, "sync"),
+    ("reverse", 4 * KiB, 3, "aio4"), ("reverse", 64 * KiB, 1, "sync"),
+    ("reverse", 1000, 1, "aio4"),
+    ("strided", 4 * KiB, 3, "sync"), ("strided", 64 * KiB, 1, "aio4"),
+    ("strided", 1000, 3, "aio4"),
+    ("random", 4 * KiB, 1, "aio4"), ("random", 64 * KiB, 3, "sync"),
+    ("random", 1000, 3, "sync"),
+    ("random_unaligned", 4 * KiB, 3, "sync"), ("random_unaligned", 64 * KiB, 1, "aio4"),
+    ("random_unaligned", 1000, 1, "sync"),
+]
+
+
+def verify_order_flips(order, block, threads):
+    """file positions to corrupt, none 8-byte aligned: in three blocks of one worker (the last
+    rank), two of them in the middle block, so that reverse order meets a higher bad block first;
+    for the random orders in five blocks spread over the whole file"""
+    num_blocks = NUM_BLOCKS[block]
+    if order in ("sequential", "reverse"):
+        per_rank = num_blocks // threads
+        blocks = list(range((threads - 1) * per_rank, num_blocks))
+    elif order == "strided":
+        blocks = list(range(threads - 1, num_blocks, threads))
+    else:
+        blocks = list(range(num_blocks))
+        return sorted(b * block + 9 for b in (blocks[len(blocks) * k // 6] for k in range(1, 6)))
+    picked = [blocks[len(blocks) // 5], blocks[len(blocks) // 2], blocks[-2]]
+    positions = [b * block + 9 for b in picked]
+    positions.append(picked[1] * block + block // 2 + 3)
+    return sorted(positions)
+
+
+def flip_bytes(path, positions):
+    with open(path, "r+b") as f:
+        for pos in positions:
+            f.seek(pos)
+            byte = f.read(1)
+            f.seek(pos)
+            f.write(bytes([byte[0] ^ 0x24]))
+
+
+@pytest.mark.parametrize("order,block,threads,engine", VERIFY_ORDER_CASES)
+def test_verify_failure_in_submission_order_matches_oracle(workdir, order, block, threads,
+                                                           engine):
+    """a worker reports the first bad block it submitted, which need not be its lowest bad
+    offset: each worker's error text (offset, expected and actual byte) equals the oracle
+    worker's, in every offset order, with both I/O engines and block sizes that are not a
+    multiple of the pattern word. Where random offsets let several workers meet bad blocks, the
+    manager stops the others at the first error, so which of them still report is timing: each
+    one that does reports the oracle worker's text."""
+    salt = 0x1122334455667788
+    size = NUM_BLOCKS[block] * block
+    gcfg, ccfg = gpu_and_cpu_configs(workdir, ["f"], num_threads=1, block_size=block,
+                                     file_size=size, integrity_check_salt=salt)
+    with WorkerManager(gcfg) as mgr:
+        mgr.run_phase(BenchPhase.CREATEFILES)
+    rc, _, _ = oracle_lib.run_oracle_phase(ccfg, BenchPhase.CREATEFILES)
+    assert rc == 0
+    assert sha(gcfg.paths[0]) == sha(ccfg.paths[0])
+    flips = verify_order_flips(order, block, threads)
+    for path in (gcfg.paths[0], ccfg.paths[0]):
+        flip_bytes(path, flips)
+
+    extra = dict(ORDERS[order])
+    if order == "random_unaligned":
+        extra["random_amount"] = size
+    read = dict(num_threads=threads, block_size=block, file_size=size,
+                integrity_check_salt=salt, **extra)
+    rc, ow, _ = oracle_lib.run_oracle_phase(WorkerConfig(paths=ccfg.paths, **read),
+                                            BenchPhase.READFILES)
+    oracle_msgs = [w.errorMsg.decode() for w in ow]
+    failed = [i for i, msg in enumerate(oracle_msgs) if msg]
+    assert rc != 0 and failed, oracle_msgs
+    assert len(failed) == 1 or order.startswith("random")
+    bad_offsets = [int(oracle_msgs[i].split("Offset: ")[1].split(";")[0]) for i in failed]
+    assert set(bad_offsets) <= set(flips)
+    if threads == 1 and order not in ("sequential", "strided"):
+        assert bad_offsets[0] != min(flips)  # submission order is not file order here
+
+    with WorkerManager(WorkerConfig(paths=gcfg.paths, **read, **ENGINES[engine])) as mgr:
+        with pytest.raises(WorkerError) as excinfo:
+            mgr.run_phase(BenchPhase.READFILES)
+        errors = [mgr.worker(i).last_error for i in range(threads)]
+        num_failed = mgr.phase_results()["num_workers_done_with_error"]
+    assert str(excinfo.value) in oracle_msgs
+    if len(failed) == 1:
+        assert errors == oracle_msgs
+        assert num_failed == 1
+    else:
+        assert all(err in ("", oracle_msgs[i]) for i, err in enumerate(errors)), errors
+        assert num_failed == sum(1 for err in errors if err) >= 1
+
+    if order in ("sequential", "reverse", "strided"):  # every byte is read once
+        collect = WorkerConfig(paths=gcfg.paths, verify_collect_all=True, **read,
+                               **ENGINES[engine])
+        with WorkerManager(collect) as mgr:
+            res = mgr.run_phase(BenchPhase.READFILES)
+        with open(gcfg.paths[0], "rb") as f:
+            expected = oracle_lib.verify_pattern(f.read(), 0, salt)[1]
+        assert res["verify_mismatch_bytes"] == expected == len(flips)
