@@ -93,7 +93,7 @@ class Cfg(ctypes.Structure):
         ("stagingEngine", ctypes.c_int32),
         ("noGPUNumaBinding", ctypes.c_int32),
         ("useNoFDSharing", ctypes.c_int32),
-        ("reserved5", ctypes.c_int32),
+        ("integrityCheckKind", ctypes.c_int32),
     ]
 
 
@@ -188,6 +188,15 @@ SIGNATURES = {
                                               ctypes.c_int64, _VP, c_u64, c_u64, _VP]),
     "elb_verify_pattern_staged": (ctypes.c_int, [_VP, c_u32, c_u64, ctypes.c_int64, _VP, _VP,
                                                  _VP, _VP, c_u64, c_u64, _VP]),
+    "elb_verify_random": (ctypes.c_int, [_VP, c_u64, ctypes.c_uint, c_u64, c_u64, ctypes.c_int,
+                                          _VP, _VP]),
+    "elb_verify_random_batch_sized": (ctypes.c_int, [_VP, c_u32, ctypes.c_uint, c_u64,
+                                                     ctypes.c_int, _VP, _VP, c_u64, c_u64, _VP]),
+    "elb_verify_random_staged": (ctypes.c_int, [_VP, c_u32, ctypes.c_uint, c_u64, ctypes.c_int,
+                                                ctypes.c_int64, _VP, _VP, _VP, _VP, c_u64, c_u64,
+                                                _VP]),
+    "elb_rand_pos_counter": (c_u64, [c_u64, c_u64]),
+    "elb_rand_dir_file_key": (c_u64, [c_u64, c_u64, c_u64]),
     "elb_stage_copy": (ctypes.c_int, [_VP, c_u32, ctypes.c_int, ctypes.c_int64, c_u64, c_u64,
                                       _VP]),
     "elb_verify_results_init": (ctypes.c_int, [_VP, c_u32, _VP]),

@@ -9,6 +9,7 @@
 #include <string>
 
 #include "elb_internal.h"
+#include "elb_patterns.cuh"
 
 extern thread_local std::string elbThreadLastError;
 
@@ -109,6 +110,43 @@ int elb_fill_random(void* devPtr, uint64_t len, unsigned pct, uint64_t seed,
 		(cudaStream_t)stream);
 }
 
+int elb_verify_random(const void* devPtr, uint64_t len, unsigned pct, uint64_t seed,
+	uint64_t blockCounter, int randAlgo, elb_verify_result* devOut, void* stream)
+{
+	if(checkRandArgs(pct, randAlgo) )
+		return -1;
+
+	if(!devOut)
+	{
+		elb_set_last_error("elb_verify_random: NULL result pointer");
+		return -1;
+	}
+
+	if(!len)
+		return elb_launch_verify_init(devOut, 1, (cudaStream_t)stream);
+
+	if(!devPtr)
+	{
+		elb_set_last_error("elb_verify_random: NULL device pointer");
+		return -1;
+	}
+
+	elb_block_desc desc{const_cast<void*>(devPtr), len, 0, blockCounter};
+
+	return elb_launch_verify_random(NULL, &desc, 1, pct, seed, devOut, NULL, len, len,
+		true /*initResults*/, (cudaStream_t)stream);
+}
+
+uint64_t elb_rand_pos_counter(uint64_t fileKey, uint64_t fileOffset)
+{
+	return elb_rand_pos_counter_hd(fileKey, fileOffset);
+}
+
+uint64_t elb_rand_dir_file_key(uint64_t rank, uint64_t dirIndex, uint64_t fileIndex)
+{
+	return elb_rand_dir_file_key_hd(rank, dirIndex, fileIndex);
+}
+
 int elb_fill_pattern_batch_sized(const elb_block_desc* descs, uint32_t numDescs, uint64_t salt,
 	uint64_t* devCounters, uint64_t totalBytes, uint64_t maxBlockLen, void* stream)
 {
@@ -151,6 +189,23 @@ int elb_fill_random_batch_sized(const elb_block_desc* descs, uint32_t numDescs, 
 
 	return elb_launch_fill_random(descs, NULL, numDescs, pct, seed, devCounters, totalBytes,
 		maxBlockLen, (cudaStream_t)stream);
+}
+
+int elb_verify_random_batch_sized(const elb_block_desc* descs, uint32_t numDescs, unsigned pct,
+	uint64_t seed, int randAlgo, elb_verify_result* devResults, uint64_t* devCounters,
+	uint64_t totalBytes, uint64_t maxBlockLen, void* stream)
+{
+	if(checkRandArgs(pct, randAlgo) )
+		return -1;
+
+	if(numDescs && (!descs || !devResults) )
+	{
+		elb_set_last_error("elb_verify_random_batch: NULL descriptor or result array");
+		return -1;
+	}
+
+	return elb_launch_verify_random(descs, NULL, numDescs, pct, seed, devResults, devCounters,
+		totalBytes, maxBlockLen, true /*initResults*/, (cudaStream_t)stream);
 }
 
 int elb_fill_pattern_staged(const elb_block_desc* descs, uint32_t numDescs, uint64_t salt,
@@ -207,6 +262,29 @@ int elb_verify_pattern_staged(const elb_block_desc* descs, uint32_t numDescs, ui
 	stage.doneTicket = devDoneTicket;
 
 	return elb_launch_verify_pattern(descs, NULL, numDescs, salt, devResults, devCounters,
+		totalBytes, maxBlockLen, false /*initResults*/, (cudaStream_t)stream, &stage);
+}
+
+int elb_verify_random_staged(const elb_block_desc* descs, uint32_t numDescs, unsigned pct,
+	uint64_t seed, int randAlgo, int64_t hostDelta, elb_verify_result* devResults,
+	elb_verify_result* hostResults, unsigned* devDoneTicket, uint64_t* devCounters,
+	uint64_t totalBytes, uint64_t maxBlockLen, void* stream)
+{
+	if(checkRandArgs(pct, randAlgo) )
+		return -1;
+
+	if(numDescs && (!descs || !devResults) )
+	{
+		elb_set_last_error("elb_verify_random_staged: NULL descriptor or result array");
+		return -1;
+	}
+
+	elb_stage_args stage;
+	stage.hostDelta = hostDelta;
+	stage.hostResults = hostResults;
+	stage.doneTicket = devDoneTicket;
+
+	return elb_launch_verify_random(descs, NULL, numDescs, pct, seed, devResults, devCounters,
 		totalBytes, maxBlockLen, false /*initResults*/, (cudaStream_t)stream, &stage);
 }
 

@@ -81,6 +81,10 @@ static const OptDef optDefs[] =
 	{"blockvaralgo", 0, Opt_STR, "Random number algorithm for --blockvarpct. Values: fast, balanced, "
 		"balanced_single, strong (all map to the counter based GPU generator)"},
 	{"blockvarseed", 0, Opt_U64, "Seed for reproducible block variance data (0 = self-seed). [b200]"},
+	{"verifyrand", 0, Opt_U64, "Enable data integrity check of random data with the given seed "
+		"(non-zero): writes --blockvarpct random data keyed by seed and block position, checks it on "
+		"the GPU in the read phase. Unlike --verify not block size independent: reads must use the "
+		"block size, file size and --blockvarpct of the write. [b200]"},
 	{"rwmixpct", 0, Opt_U64, "Percentage of blocks that should be read in a write phase."},
 	{"rwmixthr", 0, Opt_U64, "Number of threads that should do reads in a write phase."},
 	// GPU
@@ -577,6 +581,7 @@ ProgArgs::ProgArgs(int argc, char** argv)
 	hasUserSetBlockVariance = num("blockvarpct", blockVariancePercent);
 	str("blockvaralgo", blockVarianceAlgo);
 	num("blockvarseed", blockVarianceSeed);
+	num("verifyrand", randomVerifySeed);
 	hasUserSetRWMixPercent = num("rwmixpct", rwMixReadPercent);
 	hasUserSetRWMixReadThreads = num("rwmixthr", numRWMixReadThreads);
 	num("rwmixthrpct", rwMixThreadsReadPercent);
@@ -935,8 +940,21 @@ void ProgArgs::checkArgs()
 		throw ProgError("Integrity check writes are not supported in combination with random "
 			"offsets.");
 
-	if(doDirectVerify && (!integrityCheckSalt || !runCreateFilesPhase) ) // :1426-1428
-		throw ProgError("Direct verification requires --verify and --write");
+	if(randomVerifySeed && integrityCheckSalt)
+		throw ProgError("Option \"--verifyrand\" cannot be used together with \"--verify\"");
+
+	if(randomVerifySeed && rwMixReadPercent)
+		throw ProgError("Option --rwmixpct cannot be used together with option \"--verifyrand\"");
+
+	if(randomVerifySeed && runCreateFilesPhase && useRandomOffsets)
+		throw ProgError("Integrity check writes are not supported in combination with random "
+			"offsets.");
+
+	if(randomVerifySeed && !treeFilePath.empty() )
+		throw ProgError("Custom tree mode cannot be used together with --verifyrand.");
+
+	if(doDirectVerify && ( (!integrityCheckSalt && !randomVerifySeed) || !runCreateFilesPhase) )
+		throw ProgError("Direct verification requires --verify and --write"); // :1426-1428
 
 	if(doDirectVerify && (ioDepth > 1) ) // :1430-1431
 		throw ProgError("Direct verification cannot be used together with --iodepth");
@@ -1005,7 +1023,8 @@ void ProgArgs::toABIConfig(ABIConfig& out) const
 	cfg.useStridedAccess = useStridedAccess;
 	cfg.randomAmount = randomAmount;
 	cfg.randOffsetSeed = randOffsetSeed;
-	cfg.integrityCheckSalt = integrityCheckSalt;
+	cfg.integrityCheckSalt = randomVerifySeed ? randomVerifySeed : integrityCheckSalt;
+	cfg.integrityCheckKind = randomVerifySeed ? ELB_VERIFY_RANDOM : ELB_VERIFY_PATTERN;
 	cfg.doDirectVerify = doDirectVerify;
 	cfg.doReadInline = doReadInline;
 	cfg.blockVariancePercent = (uint32_t)blockVariancePercent;

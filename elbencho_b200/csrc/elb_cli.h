@@ -82,6 +82,7 @@ class ProgArgs
 		bool hasUserSetBlockVariance{false};
 		std::string blockVarianceAlgo;
 		uint64_t blockVarianceSeed{0};
+		uint64_t randomVerifySeed{0}; // --verifyrand
 		uint64_t rwMixReadPercent{0};
 		bool hasUserSetRWMixPercent{false};
 		uint64_t numRWMixReadThreads{0};

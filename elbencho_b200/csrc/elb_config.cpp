@@ -87,6 +87,7 @@ Config Config::fromABI(const elb_cfg* cfg)
 		throw WorkerError("Option \"--rwmixthrpct\" cannot be used together with "
 			"\"--limitread\" or \"--limitwrite\"");
 	c.integrityCheckSalt = cfg->integrityCheckSalt;
+	c.integrityCheckKind = cfg->integrityCheckKind;
 	c.doDirectVerify = cfg->doDirectVerify;
 	c.doReadInline = cfg->doReadInline;
 	c.blockVariancePercent = cfg->blockVariancePercent;
@@ -166,6 +167,9 @@ Config Config::fromABI(const elb_cfg* cfg)
 		throw WorkerError("Unknown block variance algorithm: " +
 			std::to_string(c.blockVarianceAlgo) );
 
+	if( (c.integrityCheckKind != ELB_VERIFY_PATTERN) && (c.integrityCheckKind != ELB_VERIFY_RANDOM) )
+		throw WorkerError("Invalid integrity check kind: " + std::to_string(c.integrityCheckKind) );
+
 	if(c.integrityCheckSalt && c.rwMixReadPercent) // :1414
 		throw WorkerError("Integrity check cannot be used together with rwmixpct.");
 
@@ -195,7 +199,8 @@ Config Config::fromABI(const elb_cfg* cfg)
 	if( (c.doDirectVerify || c.doReadInline) && c.rwMixReadPercent)
 		throw WorkerError("--verifydirect/--readinline cannot be used together with --rwmixpct");
 
-	if(c.integrityCheckSalt && c.blockVariancePercent) // :1161-1167: verify wins
+	// :1161-1167: verify wins (--verifyrand writes the random data of blockVariancePercent)
+	if(c.integrityCheckSalt && c.blockVariancePercent && !c.useRandomVerify() )
 		c.blockVariancePercent = 0;
 
 	if(c.useCuFile && !c.useDirectIO) // :1315-1322
@@ -213,6 +218,9 @@ Config Config::fromABI(const elb_cfg* cfg)
 
 	if(haveTreeFile && !c.blockSize)
 		throw WorkerError("Custom tree mode requires a block size.");
+
+	if(haveTreeFile && c.useRandomVerify() )
+		throw WorkerError("Custom tree mode cannot be used together with --verifyrand.");
 
 	if(!c.fileShareSize) // :1291-1292
 		c.fileShareSize = 32 * c.blockSize;
@@ -240,6 +248,11 @@ Config Config::fromABI(const elb_cfg* cfg)
 			throw WorkerError("Block size for direct IO is not a multiple of required size. "
 				"Required size: 512");
 	}
+
+	// (the random data of a block is keyed by its offset on the block grid)
+	if(c.useRandomOffsets && c.useRandomUnaligned && c.useRandomVerify() )
+		throw WorkerError("Random data verification (--verifyrand) cannot be used together with "
+			"unaligned random offsets.");
 
 	if(c.useRandomOffsets && !c.useRandomUnaligned && c.blockSize &&
 		(c.randomAmount % c.blockSize) && (c.pathType != ELB_PATH_DIR) ) // :1586-1597

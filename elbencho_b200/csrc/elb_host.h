@@ -983,7 +983,8 @@ struct Config
 	unsigned fadviseFlags{0};   // --fadv
 	bool doStatInline{false};   // --statinline
 	bool noDirectIOCheck{false}; // --nodiocheck
-	uint64_t integrityCheckSalt{0};
+	uint64_t integrityCheckSalt{0}; // --verify salt or --verifyrand seed (0: no integrity check)
+	int integrityCheckKind{ELB_VERIFY_PATTERN}; // enum elb_verify_kind
 	bool doDirectVerify{false};
 	bool doReadInline{false};
 	uint32_t blockVariancePercent{0};
@@ -1003,6 +1004,10 @@ struct Config
 	int stagingEngine{ELB_STAGING_AUTO};
 	bool noGPUNumaBinding{false};
 	bool useNoFDSharing{false}; // --nofdsharing
+
+	/* --verifyrand: random block data keyed by position, checked on reads */
+	bool useRandomVerify() const
+		{ return integrityCheckSalt && (integrityCheckKind == ELB_VERIFY_RANDOM); }
 
 	/* @throw WorkerError on invalid combinations */
 	static Config fromABI(const elb_cfg* cfg);

@@ -38,6 +38,10 @@ int elb_launch_verify_pattern(const elb_block_desc* descs, const elb_block_desc*
 	uint32_t numDescs, uint64_t salt, elb_verify_result* devResults, uint64_t* devCounters,
 	uint64_t totalBytesHint, uint64_t maxBlockLenHint, bool initResults, cudaStream_t stream,
 	const elb_stage_args* stage = NULL);
+int elb_launch_verify_random(const elb_block_desc* descs, const elb_block_desc* inlineDesc,
+	uint32_t numDescs, unsigned pct, uint64_t seed, elb_verify_result* devResults,
+	uint64_t* devCounters, uint64_t totalBytesHint, uint64_t maxBlockLenHint, bool initResults,
+	cudaStream_t stream, const elb_stage_args* stage = NULL);
 int elb_launch_fill_random(const elb_block_desc* descs, const elb_block_desc* inlineDesc,
 	uint32_t numDescs, unsigned pct, uint64_t seed, uint64_t* devCounters,
 	uint64_t totalBytesHint, uint64_t maxBlockLenHint, cudaStream_t stream,

@@ -4,9 +4,10 @@
  *   K1 fill_pattern   <- LocalWorker::preWriteIntegrityCheckFillBuf   (LocalWorker.cpp:2091-2128)
  *   K2 verify_pattern <- LocalWorker::postReadIntegrityCheckVerifyBuf (LocalWorker.cpp:2137-2179)
  *   K3 fill_random    <- LocalWorker::preWriteBufRandRefillCuda + bufFill (:2185-2203, 2236-2277)
+ *   K4 verify_random  (no reference counterpart: --verifyrand checks K3's content on reads)
  *
- * All three are HBM-bound byte/integer kernels (K1/K3: 1 byte written per payload byte, K2: 1 byte
- * read per payload byte), so the design follows the streaming rules: 16-byte (128-bit) vector
+ * All four are HBM-bound byte/integer kernels (K1/K3: 1 byte written per payload byte, K2/K4: 1
+ * byte read per payload byte), so the design follows the streaming rules: 16-byte (128-bit) vector
  * accesses per thread (LDG/STG.E.128, the widest global access of sm_90), fully coalesced (a warp
  * covers 512 contiguous bytes per access), L1 no-allocate hints, several independent accesses in
  * flight per thread, and a grid sized to a multiple of the SM count that walks "tiles" of the whole
@@ -52,11 +53,13 @@
 #define ELB_VEC_BYTES 16
 #define ELB_UNROLL 8
 #define ELB_TILE_BYTES (ELB_THREADS * ELB_VEC_BYTES * ELB_UNROLL) /* 32 KiB */
-/* verify holds all ELB_UNROLL vectors of a thread in registers before it compares them: 3 CTAs per
-   SM (ptxas of CUDA 12.9 allocates 80 registers) instead of 4 (64) keep them out of local memory
-   (only the persistent stage-in + verify form spills, 20 B), and 3 x 256 threads with 128 B in
-   flight each are still far more than the H100's HBM latency needs */
-#define ELB_MIN_CTAS_PER_SM(mode) ( ( (mode) == 1 /* MODE_VERIFY_PATTERN */) ? 3 : 4)
+/* both verify modes hold all ELB_UNROLL vectors of a thread in registers before they compare
+   them: 3 CTAs per SM (ptxas of CUDA 12.9 allocates 80 registers) instead of 4 (64) keep them out
+   of local memory (only the persistent stage-in + verify forms spill: 20 / 28 B stores / loads
+   for verify_pattern, 16 / 24 B for verify_random), and 3 x 256 threads with 128 B in flight each
+   are still far more than the H100's HBM latency needs */
+#define ELB_MIN_CTAS_PER_SM(mode) \
+	( ( (mode) == 1 /* MODE_VERIFY_PATTERN */ || (mode) == 5 /* MODE_VERIFY_RANDOM */) ? 3 : 4)
 
 struct __align__(16) u64x2
 {
@@ -131,6 +134,52 @@ struct PatternGen
 		{ return elb_pattern_byte(fileOffset + pos, salt); }
 };
 
+/* the random part of a random-filled block, for vectors that start on a word boundary */
+struct RandomVarGen
+{
+	uint64_t blockKey;
+
+	template<bool FAST>
+	__device__ __forceinline__ u64x2 vec16(uint64_t pos) const
+	{ // two whole random words (of this vector only: see order_after_loads)
+		uint64_t key = blockKey;
+		asm volatile("" : "+l"(key) );
+
+		const uint64_t wordIdx = pos >> 3;
+		return u64x2{elb_rand_word(key, wordIdx), elb_rand_word(key, wordIdx + 1)};
+	}
+};
+
+/* the constant remainder of a random-filled block, for vectors that start on a word boundary */
+struct RandomRemainderGen
+{
+	uint64_t varFillLen;
+	uint64_t remainderVal;
+
+	template<bool FAST>
+	__device__ __forceinline__ u64x2 vec16(uint64_t pos) const
+	{ // the same rotation of the repeated u64 twice
+		const unsigned rotBits = (unsigned)( (pos - varFillLen) & 7) * 8;
+		const uint64_t val = rotBits ?
+			( (remainderVal >> rotBits) | (remainderVal << (64 - rotBits) ) ) : remainderVal;
+		return u64x2{val, val};
+	}
+};
+
+/* the work after the loads of a loads-first span stays after them: nothing to do, except for the
+   random words, which ptxas would otherwise compute ahead while the loads are in flight and hold
+   next to the loaded vectors together with the span's store addresses (the persistent stage-in +
+   verify form then spills 40/72 B). Empty asm statements that "change" the key and the body
+   pointer after the loads order the two; RandomVarGen::vec16 does the same for each vector. */
+template<class Gen>
+__device__ __forceinline__ void order_after_loads(Gen& gen, uint8_t*& body) {}
+
+__device__ __forceinline__ void order_after_loads(RandomVarGen& gen, uint8_t*& body)
+{
+	asm volatile("" : "+l"(gen.blockKey) );
+	asm volatile("" : "+l"(body) );
+}
+
 struct RandomGen
 {
 	uint64_t blockKey;
@@ -147,18 +196,9 @@ struct RandomGen
 		u64x2 v;
 
 		if(FAST && ( (pos + ELB_VEC_BYTES) <= varFillLen) )
-		{ // two whole random words
-			const uint64_t wordIdx = pos >> 3;
-			v.a = elb_rand_word(blockKey, wordIdx);
-			v.b = elb_rand_word(blockKey, wordIdx + 1);
-		}
+			v = RandomVarGen{blockKey}.vec16<true>(pos);
 		else if(FAST && (pos >= varFillLen) )
-		{ // constant remainder: the same rotation of the repeated u64 twice
-			const unsigned rotBits = (unsigned)( (pos - varFillLen) & 7) * 8;
-			const uint64_t val = rotBits ?
-				( (remainderVal >> rotBits) | (remainderVal << (64 - rotBits) ) ) : remainderVal;
-			v.a = v.b = val;
-		}
+			v = RandomRemainderGen{varFillLen, remainderVal}.vec16<true>(pos);
 		else
 		{ // boundary vector or unaligned block start
 			v.a = elb_rand_bytes8(pos, blockKey, varFillLen, remainderVal);
@@ -193,7 +233,11 @@ enum { STAGE_NONE = 0, STAGE_PUBLISH = 1, STAGE_FULL = 2 };
 
 enum { MODE_FILL_PATTERN = 0, MODE_VERIFY_PATTERN = 1, MODE_FILL_RANDOM = 2,
 	MODE_COPY_IN = 3 /* host slot -> device slot */, MODE_COPY_OUT = 4 /* device -> host */,
-	NUM_MODES = 5 };
+	MODE_VERIFY_RANDOM = 5, NUM_MODES = 6 };
+
+/* the modes that compare the block with a generator and record per-block results */
+__host__ __device__ constexpr bool is_verify_mode(int mode)
+	{ return (mode == MODE_VERIFY_PATTERN) || (mode == MODE_VERIFY_RANDOM); }
 
 struct KernelArgs
 {
@@ -201,8 +245,8 @@ struct KernelArgs
 	elb_block_desc inlineDesc;   // single-block launches pass the descriptor by value
 	uint32_t numDescs;
 	uint64_t salt;         // pattern
-	uint64_t seed;         // random
-	unsigned pct;          // random
+	uint64_t seed;         // random (fill and verify)
+	unsigned pct;          // random (fill and verify)
 	elb_verify_result* results; // verify
 	unsigned long long* counters; // optional device counter block
 
@@ -344,7 +388,7 @@ template<int MODE, bool STAGED>
 struct ModeCore
 {
 	static constexpr bool COPY = (MODE == MODE_COPY_IN) || (MODE == MODE_COPY_OUT);
-	static constexpr bool VERIFY = (MODE == MODE_VERIFY_PATTERN);
+	static constexpr bool VERIFY = is_verify_mode(MODE);
 	static constexpr bool READS = COPY || VERIFY; // (else generates)
 	static constexpr bool READS_HOST = (MODE == MODE_COPY_IN) || (VERIFY && STAGED);
 	static constexpr bool WRITES_DEV = !READS || (MODE == MODE_COPY_IN) || (VERIFY && STAGED);
@@ -399,6 +443,9 @@ __device__ __forceinline__ void walk_span(const BlockGeom& g, const Gen& gen, in
 				body + spanStart + (uint64_t)(u * GROUP + rank) * ELB_VEC_BYTES, hostDelta);
 	}
 
+	Gen genAfterLoads = gen;
+	order_after_loads(genAfterLoads, body);
+
 	#pragma unroll
 	for(int u = 0; u < ELB_UNROLL; u++)
 	{
@@ -409,7 +456,8 @@ __device__ __forceinline__ void walk_span(const BlockGeom& g, const Gen& gen, in
 			if constexpr(Core::READS && !FULL) // (the last span of a block: one bounds check each)
 				got[u] = Core::template read<u64x2>(body + off, hostDelta);
 
-			Core::template apply<FAST>(body + off, hostDelta, g.headLen + off, gen, got[u], acc);
+			Core::template apply<FAST>(body + off, hostDelta, g.headLen + off, genAfterLoads,
+				got[u], acc);
 		}
 	}
 }
@@ -436,6 +484,33 @@ __device__ __forceinline__ void walk_head_tail(const BlockGeom& g, const Gen& ge
 	Core::template apply<FAST>(g.ptr + pos, hostDelta, pos, gen, got, acc);
 }
 
+/**
+ * A whole span of verify_random. The loads-first walk holds all ELB_UNROLL vectors in registers,
+ * so its generator must not branch per vector: a span that lies wholly in the random part or
+ * wholly in the constant remainder takes the generator of that part alone. The one span of a
+ * block that straddles the boundary, and blocks whose vectors do not start on word boundaries
+ * (!FAST: the byte-wise path, device addresses that are not 8-byte aligned), take the
+ * bounds-checked walk of a block's last span, which loads each vector right before its compare.
+ * (The per-vector branches of RandomGen in the loads-first walk spill up to 184 B.)
+ */
+template<int MODE, bool STAGED, int GROUP, bool FAST>
+__device__ __forceinline__ void walk_random_verify_span(const BlockGeom& g, const RandomGen& gen,
+	int64_t hostDelta, uint64_t spanStart, unsigned rank, VerifyAcc& acc)
+{
+	constexpr uint64_t SPAN_BYTES = (uint64_t)GROUP * ELB_VEC_BYTES * ELB_UNROLL;
+	const uint64_t posBegin = g.headLen + spanStart; // (uniform for the group)
+
+	if(FAST && ( (posBegin + SPAN_BYTES) <= gen.varFillLen) )
+		walk_span<MODE, STAGED, GROUP, true, true>(g, RandomVarGen{gen.blockKey}, hostDelta,
+			spanStart, rank, acc);
+	else
+	if(FAST && (posBegin >= gen.varFillLen) )
+		walk_span<MODE, STAGED, GROUP, true, true>(g,
+			RandomRemainderGen{gen.varFillLen, gen.remainderVal}, hostDelta, spanStart, rank, acc);
+	else
+		walk_span<MODE, STAGED, GROUP, FAST, false>(g, gen, hostDelta, spanStart, rank, acc);
+}
+
 /* body bytes [bodyBegin, bodyEnd) of one block; the group that starts at body byte 0 also takes
    the head/tail bytes, before the spans (after them, ptxas spills the verify kernels). Verify
    flushes its count once per call. */
@@ -453,13 +528,20 @@ __device__ __forceinline__ void walk_block(const KernelArgs& args, const BlockGe
 	for(uint64_t spanStart = bodyBegin; spanStart < end; spanStart += SPAN_BYTES)
 	{
 		if( (spanStart + SPAN_BYTES) <= g.bodyLen)
-			walk_span<MODE, STAGED, GROUP, FAST, true>(g, gen, args.hostDelta, spanStart, rank, acc);
+		{
+			if constexpr(MODE == MODE_VERIFY_RANDOM)
+				walk_random_verify_span<MODE, STAGED, GROUP, FAST>(g, gen, args.hostDelta,
+					spanStart, rank, acc);
+			else
+				walk_span<MODE, STAGED, GROUP, FAST, true>(g, gen, args.hostDelta, spanStart, rank,
+					acc);
+		}
 		else
 			walk_span<MODE, STAGED, GROUP, FAST, false>(g, gen, args.hostDelta, spanStart, rank,
 				acc);
 	}
 
-	if constexpr(MODE == MODE_VERIFY_PATTERN)
+	if constexpr(is_verify_mode(MODE) )
 		acc.flush(&args.results[descIdx], args.counters);
 }
 
@@ -467,7 +549,7 @@ __device__ __forceinline__ void walk_block(const KernelArgs& args, const BlockGe
 template<int MODE>
 __device__ __forceinline__ auto make_gen(const KernelArgs& args, const elb_block_desc& desc)
 {
-	if constexpr(MODE == MODE_FILL_RANDOM)
+	if constexpr( (MODE == MODE_FILL_RANDOM) || (MODE == MODE_VERIFY_RANDOM) )
 	{
 		const uint64_t blockKey = elb_rand_block_key(args.seed, desc.blockCounter);
 		return RandomGen{blockKey, elb_rand_var_fill_len(desc.len, args.pct),
@@ -501,7 +583,7 @@ __device__ __forceinline__ void process_block(const KernelArgs& args, const elb_
 template<int MODE>
 __device__ __forceinline__ int counter_slot_of()
 {
-	return (MODE == MODE_VERIFY_PATTERN) ? ELB_DEVCTR_VERIFIED_BYTES :
+	return is_verify_mode(MODE) ? ELB_DEVCTR_VERIFIED_BYTES :
 		( (MODE == MODE_FILL_PATTERN) || (MODE == MODE_FILL_RANDOM) ) ? ELB_DEVCTR_FILLED_BYTES : -1;
 }
 
@@ -588,7 +670,7 @@ __global__ void __launch_bounds__(ELB_THREADS, ELB_MIN_CTAS_PER_SM(MODE) )
 elb_blocks_kernel(const KernelArgs args)
 {
 	constexpr bool STAGED = (STAGE == STAGE_FULL);
-	constexpr bool PUBLISH = (MODE == MODE_VERIFY_PATTERN) && (STAGE != STAGE_NONE);
+	constexpr bool PUBLISH = is_verify_mode(MODE) && (STAGE != STAGE_NONE);
 
 	__shared__ uint64_t sScratch[ELB_THREADS / 32];
 	__shared__ uint64_t sStartTile;
@@ -716,7 +798,7 @@ elb_blocks_tiled_kernel(const KernelArgs args, const uint32_t ctasPerBlock,
 	const uint32_t tilesPerCTA)
 {
 	constexpr bool STAGED = (STAGE == STAGE_FULL);
-	constexpr bool PUBLISH = (MODE == MODE_VERIFY_PATTERN) && (STAGE != STAGE_NONE);
+	constexpr bool PUBLISH = is_verify_mode(MODE) && (STAGE != STAGE_NONE);
 
 	const uint32_t descIdx = blockIdx.x / ctasPerBlock;
 	const uint32_t ctaInBlock = blockIdx.x - descIdx * ctasPerBlock;
@@ -763,7 +845,7 @@ __global__ void __launch_bounds__(ELB_THREADS, 3)
 elb_blocks_warp_kernel(const KernelArgs args)
 {
 	constexpr bool STAGED = (STAGE == STAGE_FULL);
-	constexpr bool PUBLISH = (MODE == MODE_VERIFY_PATTERN) && (STAGE != STAGE_NONE);
+	constexpr bool PUBLISH = is_verify_mode(MODE) && (STAGE != STAGE_NONE);
 
 	__shared__ unsigned long long sBlockBytes;
 
@@ -826,12 +908,12 @@ void elb_set_last_error(const std::string& msg)
 struct DeviceLaunchInfo
 {
 	int numSMs{0};
-	int ctasPerSM[NUM_MODES]{0, 0, 0, 0, 0};
+	int ctasPerSM[NUM_MODES]{};
 };
 
 /* 32 KiB tiles per CTA of the hardware-scheduled kernel, per mode. H100: 1/1/4, 2/4/8, 4/4/16 for
-   fill/verify/random were within 0.6 % of 1/2/8 (DESIGN.md). */
-static const uint32_t gTilesPerCTA[NUM_MODES] = {1, 2, 8, 2, 2};
+   fill/verify/random were within 0.6 % of 1/2/8 (DESIGN.md). verify_random takes verify's 2. */
+static const uint32_t gTilesPerCTA[NUM_MODES] = {1, 2, 8, 2, 2, 2};
 
 static DeviceLaunchInfo gDevInfo[ELB_MAX_DEVICES];
 static std::once_flag gDevInfoOnce[ELB_MAX_DEVICES];
@@ -865,6 +947,7 @@ static const DeviceLaunchInfo* getDeviceLaunchInfo()
 		gDevInfo[dev].ctasPerSM[MODE_FILL_RANDOM] = queryOccupancy<MODE_FILL_RANDOM>();
 		gDevInfo[dev].ctasPerSM[MODE_COPY_IN] = queryOccupancy<MODE_COPY_IN>();
 		gDevInfo[dev].ctasPerSM[MODE_COPY_OUT] = queryOccupancy<MODE_COPY_OUT>();
+		gDevInfo[dev].ctasPerSM[MODE_VERIFY_RANDOM] = queryOccupancy<MODE_VERIFY_RANDOM>();
 	});
 
 	if(gDevInfo[dev].numSMs <= 0)
@@ -881,7 +964,8 @@ static const DeviceLaunchInfo* getDeviceLaunchInfo()
 static const char* modeName(int mode)
 {
 	static const char* names[NUM_MODES] =
-		{"fill_pattern", "verify_pattern", "fill_random", "stage_copy_in", "stage_copy_out"};
+		{"fill_pattern", "verify_pattern", "fill_random", "stage_copy_in", "stage_copy_out",
+		"verify_random"};
 	return names[mode];
 }
 
@@ -977,7 +1061,7 @@ static int launchBlocksKernel(const KernelArgs& args, uint64_t totalBytesHint,
 		return -1; // (not reached: the copy kernels exist in their staged form only)
 	else
 	{
-		if constexpr(MODE == MODE_VERIFY_PATTERN)
+		if constexpr(is_verify_mode(MODE) )
 			if(args.hostResults)
 				return launchBlocksKernelT<MODE, STAGE_PUBLISH>(args, totalBytesHint,
 					maxBlockLenHint, stream);
@@ -1026,38 +1110,64 @@ int elb_launch_verify_init(elb_verify_result* devResults, uint32_t numDescs,
 }
 
 /**
+ * Both verify modes; args carries the generator's parameters.
  * @initResults false if the caller knows devResults still holds {0, ~0} entries (true after any
  *    launch that found no mismatch, and always after a launch with stage->hostResults, which
  *    re-arms the entries itself), which saves the init launch.
  */
-int elb_launch_verify_pattern(const elb_block_desc* descs, const elb_block_desc* inlineDesc,
-	uint32_t numDescs, uint64_t salt, elb_verify_result* devResults, uint64_t* devCounters,
-	uint64_t totalBytesHint, uint64_t maxBlockLenHint, bool initResults, cudaStream_t stream,
-	const elb_stage_args* stage)
+template<int MODE>
+static int launchVerify(KernelArgs& args, const elb_block_desc* descs,
+	const elb_block_desc* inlineDesc, uint32_t numDescs, elb_verify_result* devResults,
+	uint64_t* devCounters, uint64_t totalBytesHint, uint64_t maxBlockLenHint, bool initResults,
+	cudaStream_t stream, const elb_stage_args* stage)
 {
 	if(!numDescs)
 		return 0;
 
 	if(stage && stage->hostResults && !stage->doneTicket)
 	{
-		elb_set_last_error("verify_pattern: host results need a device ticket counter");
+		elb_set_last_error(std::string(modeName(MODE) ) +
+			": host results need a device ticket counter");
 		return -1;
 	}
 
 	if(initResults && elb_launch_verify_init(devResults, numDescs, stream) )
 		return -1;
 
-	KernelArgs args{};
 	args.descs = descs;
 	if(inlineDesc)
 		args.inlineDesc = *inlineDesc;
 	args.numDescs = numDescs;
-	args.salt = salt;
 	args.results = devResults;
 	args.counters = (unsigned long long*)devCounters;
 	applyStage(args, stage);
 
-	return launchBlocksKernel<MODE_VERIFY_PATTERN>(args, totalBytesHint, maxBlockLenHint, stream);
+	return launchBlocksKernel<MODE>(args, totalBytesHint, maxBlockLenHint, stream);
+}
+
+int elb_launch_verify_pattern(const elb_block_desc* descs, const elb_block_desc* inlineDesc,
+	uint32_t numDescs, uint64_t salt, elb_verify_result* devResults, uint64_t* devCounters,
+	uint64_t totalBytesHint, uint64_t maxBlockLenHint, bool initResults, cudaStream_t stream,
+	const elb_stage_args* stage)
+{
+	KernelArgs args{};
+	args.salt = salt;
+
+	return launchVerify<MODE_VERIFY_PATTERN>(args, descs, inlineDesc, numDescs, devResults,
+		devCounters, totalBytesHint, maxBlockLenHint, initResults, stream, stage);
+}
+
+int elb_launch_verify_random(const elb_block_desc* descs, const elb_block_desc* inlineDesc,
+	uint32_t numDescs, unsigned pct, uint64_t seed, elb_verify_result* devResults,
+	uint64_t* devCounters, uint64_t totalBytesHint, uint64_t maxBlockLenHint, bool initResults,
+	cudaStream_t stream, const elb_stage_args* stage)
+{
+	KernelArgs args{};
+	args.seed = seed;
+	args.pct = pct;
+
+	return launchVerify<MODE_VERIFY_RANDOM>(args, descs, inlineDesc, numDescs, devResults,
+		devCounters, totalBytesHint, maxBlockLenHint, initResults, stream, stage);
 }
 
 int elb_launch_fill_random(const elb_block_desc* descs, const elb_block_desc* inlineDesc,

@@ -12,6 +12,13 @@
  *   word k      = splitmix64_mix(blockKey + (k+1) * GOLDEN)   (k = byte position / 8 in block)
  *   remainder v = splitmix64_mix(blockKey)                    (the one repeated u64, :2228)
  * i.e. word k is output k of a standard SplitMix64 stream seeded with blockKey.
+ *
+ * --verifyrand keys the random fill by the block's place in the data set instead of by the worker
+ * that wrote it, so that a later read can recompute it:
+ *   blockCounter = elb_rand_pos_counter_hd(fileKey, file offset of block byte 0)
+ * fileKey is the file's index in the bench path list (file / blockdev mode) or
+ * elb_rand_dir_file_key_hd() of the numbers in its dir mode name. (The C ABI exports both as
+ * elb_rand_pos_counter / elb_rand_dir_file_key.)
  */
 #ifndef ELB_PATTERNS_CUH_
 #define ELB_PATTERNS_CUH_
@@ -37,6 +44,21 @@ ELB_HD uint64_t elb_splitmix64_mix(uint64_t z)
 ELB_HD uint64_t elb_rand_block_key(uint64_t seed, uint64_t blockCounter)
 {
 	return elb_splitmix64_mix(seed + blockCounter * ELB_CTR_MULT);
+}
+
+/* fileKey of the dir mode file r<rank>/d<dirIndex>/r<rank>-f<fileIndex> (with --dirsharing:
+ * r0/d<dirIndex>/r<rank>-f<fileIndex>; the rank in the file name tells the two apart) */
+ELB_HD uint64_t elb_rand_dir_file_key_hd(uint64_t rank, uint64_t dirIndex, uint64_t fileIndex)
+{
+	return elb_splitmix64_mix(elb_splitmix64_mix(elb_splitmix64_mix(rank) + dirIndex) +
+		fileIndex);
+}
+
+/* position counter of the block at fileOffset of the file with fileKey: for one file a bijection
+ * of the offset, so no two blocks of a file share a key */
+ELB_HD uint64_t elb_rand_pos_counter_hd(uint64_t fileKey, uint64_t fileOffset)
+{
+	return elb_splitmix64_mix(elb_splitmix64_mix(fileKey + ELB_GOLDEN) ^ fileOffset);
 }
 
 ELB_HD uint64_t elb_rand_word(uint64_t blockKey, uint64_t wordIdx)

@@ -98,7 +98,7 @@ struct BlockRef
 	bool lastOfFile{false};   // dir mode: close the file after this block
 	bool ioIsRead{false};     // direction of this block's storage call (rwmix: read in a write phase)
 	bool statsReadMix{false}; // account into the *ReadMix counters (Worker.h:52,56,58)
-	uint64_t blockCounter{0}; // keys the random fill
+	uint64_t blockCounter{0}; // keys the random fill (--verifyrand: the position counter instead)
 	uint64_t ioUSec{0};       // measured storage time of this block
 	Clock::time_point submitT; // aio: time of submission
 	bool ioDone{false};        // aio: completion seen
@@ -125,7 +125,8 @@ struct GpuStage
 		TRANSFER_COPY,   // cudaMemcpyAsync between the rings
 	};
 
-	enum Compute { COMPUTE_NONE, COMPUTE_FILL_PATTERN, COMPUTE_FILL_RANDOM, COMPUTE_VERIFY };
+	enum Compute { COMPUTE_NONE, COMPUTE_FILL_PATTERN, COMPUTE_FILL_RANDOM, COMPUTE_VERIFY,
+		COMPUTE_VERIFY_RANDOM };
 
 	bool isRead;      // host ring -> device ring (read) or device ring -> host ring (write)
 	Transfer transfer;
@@ -250,7 +251,7 @@ class Worker
 		char* hostRing{NULL}; // pinned
 		char* devRing{NULL};
 		int64_t hostDelta{0}; // hostRing - devRing: host slot of a block = device slot + hostDelta
-		GpuStage readStage{};  // resolved elb_cfg::stagingEngine, --cufile, --verify, --blockvarpct
+		GpuStage readStage{};  // resolved elb_cfg::stagingEngine, --cufile, --verify(rand), --blockvarpct
 		GpuStage writeStage{};
 		bool useWriteGate{false};    // resolved elb_cfg::serializeBufferedWrites
 		int boundNumaNode{-1};       // NUMA node this worker bound itself to (-1: none)
@@ -341,6 +342,7 @@ class Worker
 		void accountBatch(Batch& batch, uint64_t gpuUSecTotal);
 		void gpuLaunchStage(Batch& batch, bool isRead);
 		uint32_t fillStageDescs(Batch& batch, bool isRead, uint64_t& outNumBytes);
+		uint64_t randBlockCounter(const BlockRef& block) const;
 		void enqueueStage(Batch& batch, const GpuStage& stage, uint32_t numBlocks,
 			uint64_t numBytes);
 		bool isStandardShapedBatch(const Batch& batch) const;

@@ -11,6 +11,9 @@ from ._native import BlockDesc, VerifyResult, DEVCTR_NUM  # noqa: F401
 
 RANDALGO_SPLITMIX64 = 0
 
+VERIFY_PATTERN = 0  # elb_verify_kind
+VERIFY_RANDOM = 1
+
 DEVCTR_VERIFY_MISMATCH_BYTES = 0
 DEVCTR_VERIFIED_BYTES = 1
 DEVCTR_FILLED_BYTES = 2
@@ -47,6 +50,24 @@ def fill_random(dev_ptr, length, pct, seed, block_counter, stream=0, algo=RANDAL
            "elb_fill_random")
 
 
+def verify_random(dev_ptr, length, pct, seed, block_counter, dev_result_ptr, stream=0,
+                  algo=RANDALGO_SPLITMIX64):
+    """K4: compare with the K3 content of the same (length, pct, seed, block_counter).
+    dev_result_ptr: device address of 16 bytes {numMismatchBytes, firstMismatchIdx}."""
+    _check(_native.load().elb_verify_random(dev_ptr, length, pct, seed, block_counter, algo,
+                                            dev_result_ptr, stream), "elb_verify_random")
+
+
+def rand_pos_counter(file_key, file_offset):
+    """block counter of --verifyrand for the block at file_offset of the file with file_key"""
+    return int(_native.load().elb_rand_pos_counter(file_key, file_offset))
+
+
+def rand_dir_file_key(rank, dir_index, file_index):
+    """file_key of the dir mode file r<rank>/d<dir_index>/r<rank>-f<file_index>"""
+    return int(_native.load().elb_rand_dir_file_key(rank, dir_index, file_index))
+
+
 def fill_pattern_batch(dev_descs_ptr, num_descs, salt, dev_counters_ptr=0, stream=0,
                        total_bytes=0, max_block_len=0):
     """total_bytes / max_block_len: size hints (0 = unknown) that pick the launch shape: both
@@ -72,6 +93,15 @@ def fill_random_batch(dev_descs_ptr, num_descs, pct, seed, dev_counters_ptr=0, s
                                                       dev_counters_ptr or None, total_bytes,
                                                       max_block_len, stream),
            "elb_fill_random_batch")
+
+
+def verify_random_batch(dev_descs_ptr, num_descs, pct, seed, dev_results_ptr, dev_counters_ptr=0,
+                        stream=0, total_bytes=0, max_block_len=0, algo=RANDALGO_SPLITMIX64):
+    _check(_native.load().elb_verify_random_batch_sized(dev_descs_ptr, num_descs, pct, seed, algo,
+                                                        dev_results_ptr,
+                                                        dev_counters_ptr or None, total_bytes,
+                                                        max_block_len, stream),
+           "elb_verify_random_batch")
 
 
 def fill_pattern_staged(descs_ptr, num_descs, salt, host_delta, dev_counters_ptr=0, stream=0,
@@ -103,6 +133,19 @@ def verify_pattern_staged(descs_ptr, num_descs, salt, host_delta, dev_results_pt
                                                     dev_counters_ptr or None, total_bytes,
                                                     max_block_len, stream),
            "elb_verify_pattern_staged")
+
+
+def verify_random_staged(descs_ptr, num_descs, pct, seed, host_delta, dev_results_ptr,
+                         host_results_ptr=0, dev_ticket_ptr=0, dev_counters_ptr=0, stream=0,
+                         total_bytes=0, max_block_len=0, algo=RANDALGO_SPLITMIX64):
+    """stage-in + K4, with the conventions of verify_pattern_staged"""
+    _check(_native.load().elb_verify_random_staged(descs_ptr, num_descs, pct, seed, algo,
+                                                   host_delta, dev_results_ptr,
+                                                   host_results_ptr or None,
+                                                   dev_ticket_ptr or None,
+                                                   dev_counters_ptr or None, total_bytes,
+                                                   max_block_len, stream),
+           "elb_verify_random_staged")
 
 
 def stage_copy(descs_ptr, num_descs, host_to_device, host_delta, stream=0, total_bytes=0,

@@ -94,7 +94,8 @@ class WorkerConfig:
     fadvise_flags: int = 0            # --fadv (1 seq, 2 rand, 4 willneed, 8 dontneed, 16 noreuse)
     do_stat_inline: bool = False      # --statinline
     no_direct_io_check: bool = False  # --nodiocheck
-    integrity_check_salt: int = 0     # --verify
+    integrity_check_salt: int = 0     # --verify salt, or --verifyrand seed with VERIFY_RANDOM
+    integrity_check_kind: int = 0     # elb_verify_kind: 0 pattern (--verify), 1 random (--verifyrand)
     do_direct_verify: bool = False    # --verifydirect
     do_read_inline: bool = False      # --readinline
     block_variance_percent: int = 0   # --blockvarpct
@@ -147,6 +148,7 @@ class WorkerConfig:
         cfg.randomAmount = self.random_amount
         cfg.randOffsetSeed = self.rand_offset_seed
         cfg.integrityCheckSalt = self.integrity_check_salt
+        cfg.integrityCheckKind = self.integrity_check_kind
         cfg.doDirectVerify = int(self.do_direct_verify)
         cfg.doReadInline = int(self.do_read_inline)
         cfg.blockVariancePercent = self.block_variance_percent

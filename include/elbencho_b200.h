@@ -141,6 +141,18 @@ int elb_verify_pattern(const void* devPtr, uint64_t len, uint64_t fileOffset, ui
 int elb_fill_random(void* devPtr, uint64_t len, unsigned pct, uint64_t seed,
 	uint64_t blockCounter, int randAlgo, void* stream);
 
+/* K4: compare device buffer with the K3 content of the same (len, pct, seed, blockCounter); *devOut
+ * (device memory, 16 bytes) receives the result. No reference counterpart: the reference's random
+ * fill cannot be recomputed, this one can (--verifyrand). */
+int elb_verify_random(const void* devPtr, uint64_t len, unsigned pct, uint64_t seed,
+	uint64_t blockCounter, int randAlgo, elb_verify_result* devOut, void* stream);
+
+/* The block counter that --verifyrand gives the block at fileOffset of the file with fileKey, and
+ * the fileKey of a dir mode file (the numbers in its name r<rank>/d<dirIndex>/r<rank>-f<fileIndex>;
+ * in file / blockdev mode fileKey is the file's index in the bench path list). */
+uint64_t elb_rand_pos_counter(uint64_t fileKey, uint64_t fileOffset);
+uint64_t elb_rand_dir_file_key(uint64_t rank, uint64_t dirIndex, uint64_t fileIndex);
+
 /* Batched forms: one launch over the whole in-flight window. `descs` must be readable by the
  * device (device memory or pinned mapped host memory); `numDescs` blocks. `devResults` has one
  * entry per descriptor. `devCounters` (may be NULL) points to ELB_DEVCTR_NUM u64 in device memory
@@ -166,6 +178,9 @@ int elb_verify_pattern_batch_sized(const elb_block_desc* descs, uint32_t numDesc
 int elb_fill_random_batch_sized(const elb_block_desc* descs, uint32_t numDescs, unsigned pct,
 	uint64_t seed, int randAlgo, uint64_t* devCounters, uint64_t totalBytes, uint64_t maxBlockLen,
 	void* stream);
+int elb_verify_random_batch_sized(const elb_block_desc* descs, uint32_t numDescs, unsigned pct,
+	uint64_t seed, int randAlgo, elb_verify_result* devResults, uint64_t* devCounters,
+	uint64_t totalBytes, uint64_t maxBlockLen, void* stream);
 
 /* Staged forms: the kernels also move each block between a pinned host buffer and its device
  * buffer while they work on it (the worker's kernel staging engine; replaces
@@ -190,6 +205,10 @@ int elb_verify_pattern_staged(const elb_block_desc* descs, uint32_t numDescs, ui
 	int64_t hostDelta, elb_verify_result* devResults, elb_verify_result* hostResults,
 	unsigned* devDoneTicket, uint64_t* devCounters, uint64_t totalBytes, uint64_t maxBlockLen,
 	void* stream);
+int elb_verify_random_staged(const elb_block_desc* descs, uint32_t numDescs, unsigned pct,
+	uint64_t seed, int randAlgo, int64_t hostDelta, elb_verify_result* devResults,
+	elb_verify_result* hostResults, unsigned* devDoneTicket, uint64_t* devCounters,
+	uint64_t totalBytes, uint64_t maxBlockLen, void* stream);
 int elb_stage_copy(const elb_block_desc* descs, uint32_t numDescs, int hostToDevice,
 	int64_t hostDelta, uint64_t totalBytes, uint64_t maxBlockLen, void* stream);
 /* devResults[0..numDescs) <- {0, ~0} */
@@ -252,7 +271,8 @@ typedef struct elb_cfg
 	uint64_t randomAmount; /* 0 = default (ProgArgs.cpp:1558-1561) */
 	uint64_t randOffsetSeed; /* 0 = self-seed (std::random_device) like the reference */
 
-	/* --verify <salt> / --verifydirect / --readinline */
+	/* --verify <salt> or --verifyrand <seed> (see integrityCheckKind) / --verifydirect /
+	 * --readinline */
 	uint64_t integrityCheckSalt;
 	int32_t doDirectVerify;
 	int32_t doReadInline;
@@ -342,8 +362,19 @@ typedef struct elb_cfg
 	/* --nofdsharing: every worker opens its own file descriptors in file / blockdev mode instead
 	 * of using the manager's (ProgArgs.h useNoFDSharing, LocalWorker.cpp:1088-1117) */
 	int32_t useNoFDSharing;
-	int32_t reserved5;
+	/* enum elb_verify_kind: what a nonzero integrityCheckSalt writes and checks */
+	int32_t integrityCheckKind;
 } elb_cfg;
+
+/* elb_cfg::integrityCheckKind values */
+enum elb_verify_kind
+{
+	ELB_VERIFY_PATTERN = 0, /* --verify: the reference's pattern, integrityCheckSalt is the salt */
+	/* --verifyrand: the random fill of blockVariancePercent, keyed by integrityCheckSalt as the seed
+	 * and by each block's position counter (elb_rand_pos_counter); the read must use the write's
+	 * block size, file size and blockVariancePercent */
+	ELB_VERIFY_RANDOM = 1,
+};
 
 enum elb_staging_engine
 {
