@@ -80,7 +80,7 @@ class Cfg(ctypes.Structure):
         ("treeRoundUpSize", c_u64),
         ("fileShareSize", c_u64),
         ("useCustomTreeRandomize", ctypes.c_int32),
-        ("reserved4", ctypes.c_int32),
+        ("randomVerifyGrainShift", ctypes.c_int32),
         ("treeRandomizeSeed", c_u64),
         ("cpuCores", ctypes.POINTER(ctypes.c_int32)),
         ("numaZones", ctypes.POINTER(ctypes.c_int32)),
@@ -195,6 +195,21 @@ SIGNATURES = {
     "elb_verify_random_staged": (ctypes.c_int, [_VP, c_u32, ctypes.c_uint, c_u64, ctypes.c_int,
                                                 ctypes.c_int64, _VP, _VP, _VP, _VP, c_u64, c_u64,
                                                 _VP]),
+    "elb_fill_random_grain": (ctypes.c_int, [_VP, c_u64, c_u64, ctypes.c_uint, ctypes.c_uint,
+                                             c_u64, c_u64, _VP]),
+    "elb_verify_random_grain": (ctypes.c_int, [_VP, c_u64, c_u64, ctypes.c_uint, ctypes.c_uint,
+                                               c_u64, c_u64, _VP, _VP]),
+    "elb_fill_random_grain_batch_sized": (ctypes.c_int, [_VP, c_u32, ctypes.c_uint, ctypes.c_uint,
+                                                         c_u64, _VP, c_u64, c_u64, _VP]),
+    "elb_verify_random_grain_batch_sized": (ctypes.c_int, [_VP, c_u32, ctypes.c_uint,
+                                                           ctypes.c_uint, c_u64, _VP, _VP, c_u64,
+                                                           c_u64, _VP]),
+    "elb_fill_random_grain_staged": (ctypes.c_int, [_VP, c_u32, ctypes.c_uint, ctypes.c_uint,
+                                                    c_u64, ctypes.c_int64, _VP, c_u64, c_u64,
+                                                    _VP]),
+    "elb_verify_random_grain_staged": (ctypes.c_int, [_VP, c_u32, ctypes.c_uint, ctypes.c_uint,
+                                                      c_u64, ctypes.c_int64, _VP, _VP, _VP, _VP,
+                                                      c_u64, c_u64, _VP]),
     "elb_rand_pos_counter": (c_u64, [c_u64, c_u64]),
     "elb_rand_dir_file_key": (c_u64, [c_u64, c_u64, c_u64]),
     "elb_stage_copy": (ctypes.c_int, [_VP, c_u32, ctypes.c_int, ctypes.c_int64, c_u64, c_u64,

@@ -31,6 +31,18 @@ static int checkRandArgs(unsigned pct, int randAlgo)
 	return 0;
 }
 
+static int checkGrainArgs(unsigned grainShift, unsigned pct)
+{
+	if( (grainShift < 12) || (grainShift > 30) )
+	{
+		elb_set_last_error("Random verify grain shift must be in range 12..30. Given: " +
+			std::to_string(grainShift) );
+		return -1;
+	}
+
+	return checkRandArgs(pct, ELB_RANDALGO_SPLITMIX64);
+}
+
 extern "C" {
 
 int elb_abi_version(void)
@@ -286,6 +298,134 @@ int elb_verify_random_staged(const elb_block_desc* descs, uint32_t numDescs, uns
 
 	return elb_launch_verify_random(descs, NULL, numDescs, pct, seed, devResults, devCounters,
 		totalBytes, maxBlockLen, false /*initResults*/, (cudaStream_t)stream, &stage);
+}
+
+int elb_fill_random_grain(void* devPtr, uint64_t len, uint64_t fileOffset, unsigned grainShift,
+	unsigned pct, uint64_t seed, uint64_t fileKey, void* stream)
+{
+	if(checkGrainArgs(grainShift, pct) )
+		return -1;
+
+	if(!len)
+		return 0;
+
+	if(!devPtr)
+	{
+		elb_set_last_error("elb_fill_random_grain: NULL device pointer");
+		return -1;
+	}
+
+	elb_block_desc desc{devPtr, len, fileOffset, fileKey};
+
+	return elb_launch_fill_random_grain(NULL, &desc, 1, grainShift, pct, seed, NULL, len, len,
+		(cudaStream_t)stream);
+}
+
+int elb_verify_random_grain(const void* devPtr, uint64_t len, uint64_t fileOffset,
+	unsigned grainShift, unsigned pct, uint64_t seed, uint64_t fileKey, elb_verify_result* devOut,
+	void* stream)
+{
+	if(checkGrainArgs(grainShift, pct) )
+		return -1;
+
+	if(!devOut)
+	{
+		elb_set_last_error("elb_verify_random_grain: NULL result pointer");
+		return -1;
+	}
+
+	if(!len)
+		return elb_launch_verify_init(devOut, 1, (cudaStream_t)stream);
+
+	if(!devPtr)
+	{
+		elb_set_last_error("elb_verify_random_grain: NULL device pointer");
+		return -1;
+	}
+
+	elb_block_desc desc{const_cast<void*>(devPtr), len, fileOffset, fileKey};
+
+	return elb_launch_verify_random_grain(NULL, &desc, 1, grainShift, pct, seed, devOut, NULL,
+		len, len, true /*initResults*/, (cudaStream_t)stream);
+}
+
+int elb_fill_random_grain_batch_sized(const elb_block_desc* descs, uint32_t numDescs,
+	unsigned grainShift, unsigned pct, uint64_t seed, uint64_t* devCounters, uint64_t totalBytes,
+	uint64_t maxBlockLen, void* stream)
+{
+	if(checkGrainArgs(grainShift, pct) )
+		return -1;
+
+	if(numDescs && !descs)
+	{
+		elb_set_last_error("elb_fill_random_grain_batch: NULL descriptor array");
+		return -1;
+	}
+
+	return elb_launch_fill_random_grain(descs, NULL, numDescs, grainShift, pct, seed, devCounters,
+		totalBytes, maxBlockLen, (cudaStream_t)stream);
+}
+
+int elb_verify_random_grain_batch_sized(const elb_block_desc* descs, uint32_t numDescs,
+	unsigned grainShift, unsigned pct, uint64_t seed, elb_verify_result* devResults,
+	uint64_t* devCounters, uint64_t totalBytes, uint64_t maxBlockLen, void* stream)
+{
+	if(checkGrainArgs(grainShift, pct) )
+		return -1;
+
+	if(numDescs && (!descs || !devResults) )
+	{
+		elb_set_last_error("elb_verify_random_grain_batch: NULL descriptor or result array");
+		return -1;
+	}
+
+	return elb_launch_verify_random_grain(descs, NULL, numDescs, grainShift, pct, seed,
+		devResults, devCounters, totalBytes, maxBlockLen, true /*initResults*/,
+		(cudaStream_t)stream);
+}
+
+int elb_fill_random_grain_staged(const elb_block_desc* descs, uint32_t numDescs,
+	unsigned grainShift, unsigned pct, uint64_t seed, int64_t hostDelta, uint64_t* devCounters,
+	uint64_t totalBytes, uint64_t maxBlockLen, void* stream)
+{
+	if(checkGrainArgs(grainShift, pct) )
+		return -1;
+
+	if(numDescs && !descs)
+	{
+		elb_set_last_error("elb_fill_random_grain_staged: NULL descriptor array");
+		return -1;
+	}
+
+	elb_stage_args stage;
+	stage.hostDelta = hostDelta;
+
+	return elb_launch_fill_random_grain(descs, NULL, numDescs, grainShift, pct, seed, devCounters,
+		totalBytes, maxBlockLen, (cudaStream_t)stream, &stage);
+}
+
+int elb_verify_random_grain_staged(const elb_block_desc* descs, uint32_t numDescs,
+	unsigned grainShift, unsigned pct, uint64_t seed, int64_t hostDelta,
+	elb_verify_result* devResults, elb_verify_result* hostResults, unsigned* devDoneTicket,
+	uint64_t* devCounters, uint64_t totalBytes, uint64_t maxBlockLen, void* stream)
+{
+	if(checkGrainArgs(grainShift, pct) )
+		return -1;
+
+	if(numDescs && (!descs || !devResults) )
+	{
+		elb_set_last_error("elb_verify_random_grain_staged: NULL descriptor or result array");
+		return -1;
+	}
+
+	elb_stage_args stage;
+	stage.hostDelta = hostDelta;
+	stage.hostResults = hostResults;
+	stage.doneTicket = devDoneTicket;
+
+	return elb_launch_verify_random_grain(descs, NULL, numDescs, grainShift, pct, seed,
+		devResults, devCounters, totalBytes, maxBlockLen, false /*initResults*/,
+		(cudaStream_t)stream, &stage);
 }
 
 int elb_stage_copy(const elb_block_desc* descs, uint32_t numDescs, int hostToDevice,

@@ -85,6 +85,10 @@ static const OptDef optDefs[] =
 		"(non-zero): writes --blockvarpct random data keyed by seed and block position, checks it on "
 		"the GPU in the read phase. Unlike --verify not block size independent: reads must use the "
 		"block size, file size and --blockvarpct of the write. [b200]"},
+	{"verifyrandgrain", 0, Opt_BYTES, "Grain mode of --verifyrand: the random data is keyed by file "
+		"position in grains of this size (a power of two from 4K to 1G) instead of by block, so that "
+		"reads of any block size and offset (also --rand --norandalign) can check it. Writes and "
+		"reads must use the same value, seed and --blockvarpct. (Default: 0 = per block) [b200]"},
 	{"rwmixpct", 0, Opt_U64, "Percentage of blocks that should be read in a write phase."},
 	{"rwmixthr", 0, Opt_U64, "Number of threads that should do reads in a write phase."},
 	// GPU
@@ -582,6 +586,7 @@ ProgArgs::ProgArgs(int argc, char** argv)
 	str("blockvaralgo", blockVarianceAlgo);
 	num("blockvarseed", blockVarianceSeed);
 	num("verifyrand", randomVerifySeed);
+	num("verifyrandgrain", randomVerifyGrain);
 	hasUserSetRWMixPercent = num("rwmixpct", rwMixReadPercent);
 	hasUserSetRWMixReadThreads = num("rwmixthr", numRWMixReadThreads);
 	num("rwmixthrpct", rwMixThreadsReadPercent);
@@ -953,6 +958,13 @@ void ProgArgs::checkArgs()
 	if(randomVerifySeed && !treeFilePath.empty() )
 		throw ProgError("Custom tree mode cannot be used together with --verifyrand.");
 
+	if(randomVerifyGrain && !randomVerifySeed)
+		throw ProgError("Option \"--verifyrandgrain\" requires \"--verifyrand\"");
+
+	if(randomVerifyGrain && ( (randomVerifyGrain & (randomVerifyGrain - 1) ) ||
+		(randomVerifyGrain < (4ULL << 10) ) || (randomVerifyGrain > (1ULL << 30) ) ) )
+		throw ProgError("Option \"--verifyrandgrain\" must be a power of two from 4K to 1G");
+
 	if(doDirectVerify && ( (!integrityCheckSalt && !randomVerifySeed) || !runCreateFilesPhase) )
 		throw ProgError("Direct verification requires --verify and --write"); // :1426-1428
 
@@ -1025,6 +1037,9 @@ void ProgArgs::toABIConfig(ABIConfig& out) const
 	cfg.randOffsetSeed = randOffsetSeed;
 	cfg.integrityCheckSalt = randomVerifySeed ? randomVerifySeed : integrityCheckSalt;
 	cfg.integrityCheckKind = randomVerifySeed ? ELB_VERIFY_RANDOM : ELB_VERIFY_PATTERN;
+	cfg.randomVerifyGrainShift = 0;
+	for(uint64_t grain = randomVerifyGrain; grain > 1; grain >>= 1) // (a power of two, checked)
+		cfg.randomVerifyGrainShift++;
 	cfg.doDirectVerify = doDirectVerify;
 	cfg.doReadInline = doReadInline;
 	cfg.blockVariancePercent = (uint32_t)blockVariancePercent;

@@ -170,6 +170,17 @@ Config Config::fromABI(const elb_cfg* cfg)
 	if( (c.integrityCheckKind != ELB_VERIFY_PATTERN) && (c.integrityCheckKind != ELB_VERIFY_RANDOM) )
 		throw WorkerError("Invalid integrity check kind: " + std::to_string(c.integrityCheckKind) );
 
+	if( (cfg->randomVerifyGrainShift != 0) &&
+		( (cfg->randomVerifyGrainShift < 12) || (cfg->randomVerifyGrainShift > 30) ) )
+		throw WorkerError("Invalid random verify grain shift: " +
+			std::to_string(cfg->randomVerifyGrainShift) + " (0 or 12..30)");
+
+	c.randomVerifyGrainShift = (unsigned)cfg->randomVerifyGrainShift;
+
+	if(c.randomVerifyGrainShift && !c.useRandomVerify() )
+		throw WorkerError("A random verify grain (--verifyrandgrain) requires random data "
+			"verification (--verifyrand).");
+
 	if(c.integrityCheckSalt && c.rwMixReadPercent) // :1414
 		throw WorkerError("Integrity check cannot be used together with rwmixpct.");
 
@@ -249,8 +260,10 @@ Config Config::fromABI(const elb_cfg* cfg)
 				"Required size: 512");
 	}
 
-	// (the random data of a block is keyed by its offset on the block grid)
-	if(c.useRandomOffsets && c.useRandomUnaligned && c.useRandomVerify() )
+	// (the random data of a block is keyed by its offset on the block grid; grain mode by the file
+	// position alone)
+	if(c.useRandomOffsets && c.useRandomUnaligned && c.useRandomVerify() &&
+		!c.useRandomVerifyGrain() )
 		throw WorkerError("Random data verification (--verifyrand) cannot be used together with "
 			"unaligned random offsets.");
 

@@ -1009,6 +1009,13 @@ struct Config
 	bool useRandomVerify() const
 		{ return integrityCheckSalt && (integrityCheckKind == ELB_VERIFY_RANDOM); }
 
+	/* --verifyrandgrain: 0 = per-block random data, else grains of 2^shift bytes keyed by the file
+	   position alone (elb_patterns.cuh) */
+	unsigned randomVerifyGrainShift{0};
+
+	bool useRandomVerifyGrain() const
+		{ return useRandomVerify() && randomVerifyGrainShift; }
+
 	/* @throw WorkerError on invalid combinations */
 	static Config fromABI(const elb_cfg* cfg);
 };

@@ -46,6 +46,16 @@ int elb_launch_fill_random(const elb_block_desc* descs, const elb_block_desc* in
 	uint32_t numDescs, unsigned pct, uint64_t seed, uint64_t* devCounters,
 	uint64_t totalBytesHint, uint64_t maxBlockLenHint, cudaStream_t stream,
 	const elb_stage_args* stage = NULL);
+// grain modes: descriptor blockCounter = fileKey, fileOffset = file position of block byte 0
+int elb_launch_fill_random_grain(const elb_block_desc* descs, const elb_block_desc* inlineDesc,
+	uint32_t numDescs, unsigned grainShift, unsigned pct, uint64_t seed, uint64_t* devCounters,
+	uint64_t totalBytesHint, uint64_t maxBlockLenHint, cudaStream_t stream,
+	const elb_stage_args* stage = NULL);
+int elb_launch_verify_random_grain(const elb_block_desc* descs, const elb_block_desc* inlineDesc,
+	uint32_t numDescs, unsigned grainShift, unsigned pct, uint64_t seed,
+	elb_verify_result* devResults, uint64_t* devCounters, uint64_t totalBytesHint,
+	uint64_t maxBlockLenHint, bool initResults, cudaStream_t stream,
+	const elb_stage_args* stage = NULL);
 int elb_launch_stage_copy(const elb_block_desc* descs, uint32_t numDescs, bool hostToDevice,
 	int64_t hostDelta, uint64_t totalBytesHint, uint64_t maxBlockLenHint, cudaStream_t stream);
 int elb_kernels_warmup();

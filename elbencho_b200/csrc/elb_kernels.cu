@@ -5,9 +5,11 @@
  *   K2 verify_pattern <- LocalWorker::postReadIntegrityCheckVerifyBuf (LocalWorker.cpp:2137-2179)
  *   K3 fill_random    <- LocalWorker::preWriteBufRandRefillCuda + bufFill (:2185-2203, 2236-2277)
  *   K4 verify_random  (no reference counterpart: --verifyrand checks K3's content on reads)
+ *   K5 fill_random_grain, K6 verify_random_grain (no reference counterpart: --verifyrandgrain,
+ *      K3's content per grain of the file, keyed by the grain's file position)
  *
- * All four are HBM-bound byte/integer kernels (K1/K3: 1 byte written per payload byte, K2/K4: 1
- * byte read per payload byte), so the design follows the streaming rules: 16-byte (128-bit) vector
+ * All six are HBM-bound byte/integer kernels (K1/K3/K5: 1 byte written per payload byte, K2/K4/K6:
+ * 1 byte read per payload byte), so the design follows the streaming rules: 16-byte (128-bit) vector
  * accesses per thread (LDG/STG.E.128, the widest global access of sm_90), fully coalesced (a warp
  * covers 512 contiguous bytes per access), L1 no-allocate hints, several independent accesses in
  * flight per thread, and a grid sized to a multiple of the SM count that walks "tiles" of the whole
@@ -57,9 +59,12 @@
    them: 3 CTAs per SM (ptxas of CUDA 12.9 allocates 80 registers) instead of 4 (64) keep them out
    of local memory (only the persistent stage-in + verify forms spill: 20 / 28 B stores / loads
    for verify_pattern, 16 / 24 B for verify_random), and 3 x 256 threads with 128 B in flight each
-   are still far more than the H100's HBM latency needs */
+   are still far more than the H100's HBM latency needs. verify_random_grain is a verify mode too.
+   fill_random_grain would take all 64 registers of 4 CTAs per SM; 5 (48 registers, no spills)
+   keep it at least in fill_random's occupancy (48 / 50 registers: 5 / 4 CTAs per SM). */
 #define ELB_MIN_CTAS_PER_SM(mode) \
-	( ( (mode) == 1 /* MODE_VERIFY_PATTERN */ || (mode) == 5 /* MODE_VERIFY_RANDOM */) ? 3 : 4)
+	( ( (mode) == 1 /* MODE_VERIFY_PATTERN */ || (mode) == 5 /* MODE_VERIFY_RANDOM */ || \
+	(mode) == 7 /* MODE_VERIFY_RANDOM_GRAIN */) ? 3 : (mode) == 6 /* MODE_FILL_RANDOM_GRAIN */ ? 5 : 4)
 
 struct __align__(16) u64x2
 {
@@ -212,6 +217,46 @@ struct RandomGen
 		{ return elb_rand_byte(pos, blockKey, varFillLen, remainderVal); }
 };
 
+/* grain-mode content (--verifyrandgrain) of a block at fileOffset: the random fill of the grain
+   that holds each file position. Spans inside one grain take RandomVarGen / RandomRemainderGen
+   (walk_grain_span); this per-vector form is for the spans that cross a grain or part boundary. */
+struct GrainGen
+{
+	uint64_t seed;
+	uint64_t fileBase;   // elb_rand_file_base(fileKey)
+	uint64_t fileOffset; // file position of block byte 0
+	uint64_t grainMask;  // grain size - 1
+	uint64_t varFillLen; // random part of a grain
+
+	/* fast path is valid when every 16-byte vector starts on a word boundary of the file */
+	__device__ __forceinline__ bool canUseFast(uint64_t headLen) const
+		{ return ( (fileOffset + headLen) & 7) == 0; }
+
+	template<bool FAST>
+	__device__ __forceinline__ u64x2 vec16(uint64_t pos) const
+	{
+		/* (of this vector only, as in RandomVarGen: computed ahead for all vectors of a span, the
+		   grain keys and words would take registers that the counterpart K3 / K4 forms do not) */
+		uint64_t base = fileBase;
+		asm volatile("" : "+l"(base) );
+
+		const uint64_t filePos = fileOffset + pos;
+		const uint64_t q = filePos & grainMask;
+
+		if(FAST && ( (q + ELB_VEC_BYTES) <= varFillLen) )
+		{ // two whole random words of one grain
+			const uint64_t grainKey = elb_rand_grain_key(seed, base, filePos - q);
+			return u64x2{elb_rand_word(grainKey, q >> 3), elb_rand_word(grainKey, (q >> 3) + 1)};
+		}
+
+		return u64x2{elb_rand_grain_bytes8(filePos, seed, base, grainMask, varFillLen),
+			elb_rand_grain_bytes8(filePos + 8, seed, base, grainMask, varFillLen)};
+	}
+
+	__device__ __forceinline__ uint8_t byte(uint64_t pos) const
+		{ return elb_rand_grain_byte(fileOffset + pos, seed, fileBase, grainMask, varFillLen); }
+};
+
 struct NoGen {}; // the stage copies generate nothing
 
 /* the expected element at block position pos: a 16-byte vector or a byte */
@@ -233,11 +278,19 @@ enum { STAGE_NONE = 0, STAGE_PUBLISH = 1, STAGE_FULL = 2 };
 
 enum { MODE_FILL_PATTERN = 0, MODE_VERIFY_PATTERN = 1, MODE_FILL_RANDOM = 2,
 	MODE_COPY_IN = 3 /* host slot -> device slot */, MODE_COPY_OUT = 4 /* device -> host */,
-	MODE_VERIFY_RANDOM = 5, NUM_MODES = 6 };
+	MODE_VERIFY_RANDOM = 5, MODE_FILL_RANDOM_GRAIN = 6, MODE_VERIFY_RANDOM_GRAIN = 7,
+	NUM_MODES = 8 };
 
 /* the modes that compare the block with a generator and record per-block results */
 __host__ __device__ constexpr bool is_verify_mode(int mode)
-	{ return (mode == MODE_VERIFY_PATTERN) || (mode == MODE_VERIFY_RANDOM); }
+{
+	return (mode == MODE_VERIFY_PATTERN) || (mode == MODE_VERIFY_RANDOM) ||
+		(mode == MODE_VERIFY_RANDOM_GRAIN);
+}
+
+/* the modes whose content is keyed by file position grains (descriptor blockCounter: fileKey) */
+__host__ __device__ constexpr bool is_grain_mode(int mode)
+	{ return (mode == MODE_FILL_RANDOM_GRAIN) || (mode == MODE_VERIFY_RANDOM_GRAIN); }
 
 struct KernelArgs
 {
@@ -247,6 +300,8 @@ struct KernelArgs
 	uint64_t salt;         // pattern
 	uint64_t seed;         // random (fill and verify)
 	unsigned pct;          // random (fill and verify)
+	uint64_t grainMask;    // random grain: grain size - 1
+	uint64_t grainVarFillLen; // random grain: elb_rand_var_fill_len(grain size, pct)
 	elb_verify_result* results; // verify
 	unsigned long long* counters; // optional device counter block
 
@@ -511,6 +566,48 @@ __device__ __forceinline__ void walk_random_verify_span(const BlockGeom& g, cons
 		walk_span<MODE, STAGED, GROUP, FAST, false>(g, gen, hostDelta, spanStart, rank, acc);
 }
 
+/**
+ * A whole span of the grain modes. A span that lies wholly in one grain's random part is
+ * RandomVarGen of the grain key, with the key advanced so that its word index of block position
+ * pos is (file position mod grain size) / 8; one wholly in a grain's remainder is
+ * RandomRemainderGen of the grain. Both take the loads-first walk without a branch per vector, as
+ * verify_random does. Spans that cross a grain or part boundary (also every span of a grain
+ * smaller than the span), and spans whose file positions are not word aligned (!FAST), take the
+ * bounds-checked walk with GrainGen.
+ */
+template<int MODE, bool STAGED, int GROUP, bool FAST>
+__device__ __forceinline__ void walk_grain_span(const BlockGeom& g, const GrainGen& gen,
+	int64_t hostDelta, uint64_t spanStart, unsigned rank, VerifyAcc& acc)
+{
+	constexpr uint64_t SPAN_BYTES = (uint64_t)GROUP * ELB_VEC_BYTES * ELB_UNROLL;
+	const uint64_t posBegin = g.headLen + spanStart; // (uniform for the group)
+	const uint64_t filePos = gen.fileOffset + posBegin;
+	const uint64_t q = filePos & gen.grainMask;
+
+	if(FAST && ( (q + SPAN_BYTES - 1) <= gen.grainMask) )
+	{
+		const uint64_t grainKey = elb_rand_grain_key(gen.seed, gen.fileBase, filePos - q);
+
+		if( (q + SPAN_BYTES) <= gen.varFillLen)
+		{ // (vectors are 16 bytes apart: pos >> 3 advances with (q + pos - posBegin) >> 3)
+			const uint64_t wordShift = (q >> 3) - (posBegin >> 3);
+			walk_span<MODE, STAGED, GROUP, true, true>(g,
+				RandomVarGen{grainKey + wordShift * ELB_GOLDEN}, hostDelta, spanStart, rank, acc);
+			return;
+		}
+
+		if(q >= gen.varFillLen)
+		{
+			walk_span<MODE, STAGED, GROUP, true, true>(g,
+				RandomRemainderGen{posBegin - q + gen.varFillLen, elb_rand_remainder_val(grainKey)},
+				hostDelta, spanStart, rank, acc);
+			return;
+		}
+	}
+
+	walk_span<MODE, STAGED, GROUP, FAST, false>(g, gen, hostDelta, spanStart, rank, acc);
+}
+
 /* body bytes [bodyBegin, bodyEnd) of one block; the group that starts at body byte 0 also takes
    the head/tail bytes, before the spans (after them, ptxas spills the verify kernels). Verify
    flushes its count once per call. */
@@ -532,6 +629,10 @@ __device__ __forceinline__ void walk_block(const KernelArgs& args, const BlockGe
 			if constexpr(MODE == MODE_VERIFY_RANDOM)
 				walk_random_verify_span<MODE, STAGED, GROUP, FAST>(g, gen, args.hostDelta,
 					spanStart, rank, acc);
+			else
+			if constexpr(is_grain_mode(MODE) )
+				walk_grain_span<MODE, STAGED, GROUP, FAST>(g, gen, args.hostDelta, spanStart, rank,
+					acc);
 			else
 				walk_span<MODE, STAGED, GROUP, FAST, true>(g, gen, args.hostDelta, spanStart, rank,
 					acc);
@@ -555,6 +656,10 @@ __device__ __forceinline__ auto make_gen(const KernelArgs& args, const elb_block
 		return RandomGen{blockKey, elb_rand_var_fill_len(desc.len, args.pct),
 			elb_rand_remainder_val(blockKey)};
 	}
+	else
+	if constexpr(is_grain_mode(MODE) )
+		return GrainGen{args.seed, elb_rand_file_base(desc.blockCounter /* fileKey */),
+			desc.fileOffset, args.grainMask, args.grainVarFillLen};
 	else
 		return PatternGen{desc.fileOffset, args.salt};
 }
@@ -584,7 +689,8 @@ template<int MODE>
 __device__ __forceinline__ int counter_slot_of()
 {
 	return is_verify_mode(MODE) ? ELB_DEVCTR_VERIFIED_BYTES :
-		( (MODE == MODE_FILL_PATTERN) || (MODE == MODE_FILL_RANDOM) ) ? ELB_DEVCTR_FILLED_BYTES : -1;
+		( (MODE == MODE_FILL_PATTERN) || (MODE == MODE_FILL_RANDOM) ||
+		(MODE == MODE_FILL_RANDOM_GRAIN) ) ? ELB_DEVCTR_FILLED_BYTES : -1;
 }
 
 /**
@@ -839,9 +945,12 @@ elb_blocks_tiled_kernel(const KernelArgs args, const uint32_t ctasPerBlock,
  * atomic per CTA. */
 
 #define ELB_WARPS (ELB_THREADS / 32)
+/* fill_random_grain would take all 80 registers that 3 CTAs per SM allow (the other modes need
+   no bound below that); 5 keep it in fill_random's occupancy, which uses 41 / 43 */
+#define ELB_WARP_MIN_CTAS_PER_SM(mode) ( (mode) == 6 /* MODE_FILL_RANDOM_GRAIN */ ? 5 : 3)
 
 template<int MODE, int STAGE>
-__global__ void __launch_bounds__(ELB_THREADS, 3)
+__global__ void __launch_bounds__(ELB_THREADS, ELB_WARP_MIN_CTAS_PER_SM(MODE) )
 elb_blocks_warp_kernel(const KernelArgs args)
 {
 	constexpr bool STAGED = (STAGE == STAGE_FULL);
@@ -912,8 +1021,9 @@ struct DeviceLaunchInfo
 };
 
 /* 32 KiB tiles per CTA of the hardware-scheduled kernel, per mode. H100: 1/1/4, 2/4/8, 4/4/16 for
-   fill/verify/random were within 0.6 % of 1/2/8 (DESIGN.md). verify_random takes verify's 2. */
-static const uint32_t gTilesPerCTA[NUM_MODES] = {1, 2, 8, 2, 2, 2};
+   fill/verify/random were within 0.6 % of 1/2/8 (DESIGN.md). verify_random takes verify's 2; the
+   grain modes take those of their per-block counterparts, 8 and 2. */
+static const uint32_t gTilesPerCTA[NUM_MODES] = {1, 2, 8, 2, 2, 2, 8, 2};
 
 static DeviceLaunchInfo gDevInfo[ELB_MAX_DEVICES];
 static std::once_flag gDevInfoOnce[ELB_MAX_DEVICES];
@@ -948,6 +1058,9 @@ static const DeviceLaunchInfo* getDeviceLaunchInfo()
 		gDevInfo[dev].ctasPerSM[MODE_COPY_IN] = queryOccupancy<MODE_COPY_IN>();
 		gDevInfo[dev].ctasPerSM[MODE_COPY_OUT] = queryOccupancy<MODE_COPY_OUT>();
 		gDevInfo[dev].ctasPerSM[MODE_VERIFY_RANDOM] = queryOccupancy<MODE_VERIFY_RANDOM>();
+		gDevInfo[dev].ctasPerSM[MODE_FILL_RANDOM_GRAIN] = queryOccupancy<MODE_FILL_RANDOM_GRAIN>();
+		gDevInfo[dev].ctasPerSM[MODE_VERIFY_RANDOM_GRAIN] =
+			queryOccupancy<MODE_VERIFY_RANDOM_GRAIN>();
 	});
 
 	if(gDevInfo[dev].numSMs <= 0)
@@ -965,7 +1078,7 @@ static const char* modeName(int mode)
 {
 	static const char* names[NUM_MODES] =
 		{"fill_pattern", "verify_pattern", "fill_random", "stage_copy_in", "stage_copy_out",
-		"verify_random"};
+		"verify_random", "fill_random_grain", "verify_random_grain"};
 	return names[mode];
 }
 
@@ -1186,6 +1299,45 @@ int elb_launch_fill_random(const elb_block_desc* descs, const elb_block_desc* in
 	applyStage(args, stage);
 
 	return launchBlocksKernel<MODE_FILL_RANDOM>(args, totalBytesHint, maxBlockLenHint, stream);
+}
+
+/* the generator parameters of the grain modes (grainShift checked by the caller) */
+static void applyGrain(KernelArgs& args, unsigned grainShift, unsigned pct, uint64_t seed)
+{
+	args.seed = seed;
+	args.pct = pct;
+	args.grainMask = (1ULL << grainShift) - 1;
+	args.grainVarFillLen = elb_rand_var_fill_len(1ULL << grainShift, pct);
+}
+
+int elb_launch_fill_random_grain(const elb_block_desc* descs, const elb_block_desc* inlineDesc,
+	uint32_t numDescs, unsigned grainShift, unsigned pct, uint64_t seed, uint64_t* devCounters,
+	uint64_t totalBytesHint, uint64_t maxBlockLenHint, cudaStream_t stream,
+	const elb_stage_args* stage)
+{
+	KernelArgs args{};
+	args.descs = descs;
+	if(inlineDesc)
+		args.inlineDesc = *inlineDesc;
+	args.numDescs = numDescs;
+	applyGrain(args, grainShift, pct, seed);
+	args.counters = (unsigned long long*)devCounters;
+	applyStage(args, stage);
+
+	return launchBlocksKernel<MODE_FILL_RANDOM_GRAIN>(args, totalBytesHint, maxBlockLenHint,
+		stream);
+}
+
+int elb_launch_verify_random_grain(const elb_block_desc* descs, const elb_block_desc* inlineDesc,
+	uint32_t numDescs, unsigned grainShift, unsigned pct, uint64_t seed,
+	elb_verify_result* devResults, uint64_t* devCounters, uint64_t totalBytesHint,
+	uint64_t maxBlockLenHint, bool initResults, cudaStream_t stream, const elb_stage_args* stage)
+{
+	KernelArgs args{};
+	applyGrain(args, grainShift, pct, seed);
+
+	return launchVerify<MODE_VERIFY_RANDOM_GRAIN>(args, descs, inlineDesc, numDescs, devResults,
+		devCounters, totalBytesHint, maxBlockLenHint, initResults, stream, stage);
 }
 
 /* plain copy of the blocks between the rings (runs without --verify / without fill) */

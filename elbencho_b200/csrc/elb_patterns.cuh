@@ -19,6 +19,13 @@
  * fileKey is the file's index in the bench path list (file / blockdev mode) or
  * elb_rand_dir_file_key_hd() of the numbers in its dir mode name. (The C ABI exports both as
  * elb_rand_pos_counter / elb_rand_dir_file_key.)
+ *
+ * --verifyrandgrain G (G = 2^grainShift) defines the content by the absolute file position alone,
+ * so that reads of any block size and offset can check it: grain g (file bytes [g*G, (g+1)*G),
+ * positions mod 2^64) holds the random fill of a block of length G whose block counter is
+ * elb_rand_pos_counter_hd(fileKey, g*G). A file written with --verifyrand -b G in sequential full
+ * blocks is therefore the same file. A grain key costs two SplitMix64 mixes once the per-file base
+ * elb_rand_file_base(fileKey) is known.
  */
 #ifndef ELB_PATTERNS_CUH_
 #define ELB_PATTERNS_CUH_
@@ -56,9 +63,21 @@ ELB_HD uint64_t elb_rand_dir_file_key_hd(uint64_t rank, uint64_t dirIndex, uint6
 
 /* position counter of the block at fileOffset of the file with fileKey: for one file a bijection
  * of the offset, so no two blocks of a file share a key */
+ELB_HD uint64_t elb_rand_file_base(uint64_t fileKey)
+{
+	return elb_splitmix64_mix(fileKey + ELB_GOLDEN);
+}
+
 ELB_HD uint64_t elb_rand_pos_counter_hd(uint64_t fileKey, uint64_t fileOffset)
 {
-	return elb_splitmix64_mix(elb_splitmix64_mix(fileKey + ELB_GOLDEN) ^ fileOffset);
+	return elb_splitmix64_mix(elb_rand_file_base(fileKey) ^ fileOffset);
+}
+
+/* key of the grain at file position grainOffset (a multiple of the grain size) of the file whose
+ * elb_rand_file_base() is fileBase */
+ELB_HD uint64_t elb_rand_grain_key(uint64_t seed, uint64_t fileBase, uint64_t grainOffset)
+{
+	return elb_rand_block_key(seed, elb_splitmix64_mix(fileBase ^ grainOffset) );
 }
 
 ELB_HD uint64_t elb_rand_word(uint64_t blockKey, uint64_t wordIdx)
@@ -132,6 +151,49 @@ ELB_HD uint64_t elb_rand_bytes8(uint64_t pos, uint64_t blockKey, uint64_t varFil
 #endif
 	for(unsigned i = 0; i < 8; i++)
 		val |= (uint64_t)elb_rand_byte(pos + i, blockKey, varFillLen, remainderVal) << (i * 8);
+
+	return val;
+}
+
+/* single grain-mode byte at file position filePos; grainMask = G - 1, grainVarFillLen =
+ * elb_rand_var_fill_len(G, pct) */
+ELB_HD uint8_t elb_rand_grain_byte(uint64_t filePos, uint64_t seed, uint64_t fileBase,
+	uint64_t grainMask, uint64_t grainVarFillLen)
+{
+	const uint64_t q = filePos & grainMask;
+	const uint64_t grainKey = elb_rand_grain_key(seed, fileBase, filePos - q);
+
+	if(q < grainVarFillLen)
+		return elb_rand_byte(q, grainKey, grainVarFillLen, 0);
+
+	return elb_rand_byte(q, grainKey, grainVarFillLen, elb_rand_remainder_val(grainKey) );
+}
+
+/* 8 grain-mode bytes starting at (arbitrary) file position filePos, as a little-endian u64 */
+ELB_HD uint64_t elb_rand_grain_bytes8(uint64_t filePos, uint64_t seed, uint64_t fileBase,
+	uint64_t grainMask, uint64_t grainVarFillLen)
+{
+	const uint64_t q = filePos & grainMask;
+
+	if(q <= (grainMask - 7) )
+	{ // inside one grain
+		const uint64_t grainKey = elb_rand_grain_key(seed, fileBase, filePos - q);
+
+		if( !(q & 7) && ( (q + 8) <= grainVarFillLen) )
+			return elb_rand_word(grainKey, q >> 3);
+
+		return elb_rand_bytes8(q, grainKey, grainVarFillLen, elb_rand_remainder_val(grainKey) );
+	}
+
+	// crosses a grain boundary (rare path: keep its code small)
+	uint64_t val = 0;
+
+#if defined(__CUDA_ARCH__)
+	#pragma unroll 1
+#endif
+	for(unsigned i = 0; i < 8; i++)
+		val |= (uint64_t)elb_rand_grain_byte(filePos + i, seed, fileBase, grainMask,
+			grainVarFillLen) << (i * 8);
 
 	return val;
 }

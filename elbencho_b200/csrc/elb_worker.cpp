@@ -824,14 +824,18 @@ void Worker::allocRings()
 
 	/* write: pattern fill if salt != 0, else random refill if blockvarpct, else nothing
 	   (initPhaseFunctionPointers, LocalWorker.cpp:1249-1265); read: verify if salt != 0 (:1311).
-	   --verifyrand: random refill and its verify, keyed by the seed and the block positions */
+	   --verifyrand: random refill and its verify, keyed by the seed and the block positions;
+	   --verifyrandgrain: those of the grain mode, keyed by the seed and the file positions */
 	const bool useRandomVerify = cfg.useRandomVerify();
+	const bool useGrain = cfg.useRandomVerifyGrain();
 
 	writeStage = GpuStage{false, transfer,
+		useGrain ? GpuStage::COMPUTE_FILL_RANDOM_GRAIN :
 		useRandomVerify ? GpuStage::COMPUTE_FILL_RANDOM :
 		cfg.integrityCheckSalt ? GpuStage::COMPUTE_FILL_PATTERN :
 		cfg.blockVariancePercent ? GpuStage::COMPUTE_FILL_RANDOM : GpuStage::COMPUTE_NONE, useGraph};
 	readStage = GpuStage{true, transfer,
+		useGrain ? GpuStage::COMPUTE_VERIFY_RANDOM_GRAIN :
 		useRandomVerify ? GpuStage::COMPUTE_VERIFY_RANDOM :
 		cfg.integrityCheckSalt ? GpuStage::COMPUTE_VERIFY : GpuStage::COMPUTE_NONE, useGraph};
 
@@ -2073,9 +2077,10 @@ uint32_t Worker::fillStageDescs(Batch& batch, bool isRead, uint64_t& outNumBytes
 		if(!isRead && block.ioIsRead)
 			continue;
 
-		// (the block counter keys the random fill and its verify; pattern verify does not read it)
+		/* (the block counter keys the random fill and its verify, the grain modes take the fileKey
+		   there; pattern verify does not read it) */
 		batch.hostDescs[numDescs++] = elb_block_desc{slotDevPtr(batch, i), block.len,
-			block.offset, randBlockCounter(block)};
+			block.offset, cfg.useRandomVerifyGrain() ? randFileKey(block) : randBlockCounter(block)};
 		outNumBytes += block.len;
 	}
 
@@ -2089,11 +2094,15 @@ uint64_t Worker::randBlockCounter(const BlockRef& block) const
 	if(!cfg.useRandomVerify() )
 		return (rank << 40) + block.blockCounter;
 
-	// (custom tree mode is rejected with --verifyrand)
-	const uint64_t fileKey = (cfg.pathType == ELB_PATH_DIR) ?
-		elb_rand_dir_file_key_hd(rank, block.dirIndex, block.fileIndex) : block.fileIdx;
+	return elb_rand_pos_counter_hd(randFileKey(block), block.offset);
+}
 
-	return elb_rand_pos_counter_hd(fileKey, block.offset);
+/* --verifyrand: the key of the block's file, its index in the path list or the numbers of its dir
+   mode name (custom tree mode is rejected with --verifyrand) */
+uint64_t Worker::randFileKey(const BlockRef& block) const
+{
+	return (cfg.pathType == ELB_PATH_DIR) ?
+		elb_rand_dir_file_key_hd(rank, block.dirIndex, block.fileIndex) : block.fileIdx;
 }
 
 /* a full batch of full-size blocks in a dense run of slots: its GPU stage has fixed pointers and
@@ -2237,6 +2246,11 @@ void Worker::enqueueStage(Batch& batch, const GpuStage& stage, uint32_t numBlock
 				cfg.blockVariancePercent, cfg.useRandomVerify() ? cfg.integrityCheckSalt :
 				blockVarianceSeed, devCounters, numBytes, cfg.blockSize, batch.stream, &args);
 		else
+		if(stage.compute == GpuStage::COMPUTE_FILL_RANDOM_GRAIN)
+			launchRes = elb_launch_fill_random_grain(batch.hostDescs, NULL, numBlocks,
+				cfg.randomVerifyGrainShift, cfg.blockVariancePercent, cfg.integrityCheckSalt,
+				devCounters, numBytes, cfg.blockSize, batch.stream, &args);
+		else
 		{
 			args.hostResults = batch.hostResults;
 			args.doneTicket = batch.devDoneTicket;
@@ -2246,6 +2260,12 @@ void Worker::enqueueStage(Batch& batch, const GpuStage& stage, uint32_t numBlock
 				launchRes = elb_launch_verify_random(batch.hostDescs, NULL, numBlocks,
 					cfg.blockVariancePercent, cfg.integrityCheckSalt, batch.devResults, devCounters,
 					numBytes, cfg.blockSize, false, batch.stream, &args);
+			else
+			if(stage.compute == GpuStage::COMPUTE_VERIFY_RANDOM_GRAIN)
+				launchRes = elb_launch_verify_random_grain(batch.hostDescs, NULL, numBlocks,
+					cfg.randomVerifyGrainShift, cfg.blockVariancePercent, cfg.integrityCheckSalt,
+					batch.devResults, devCounters, numBytes, cfg.blockSize, false, batch.stream,
+					&args);
 			else
 				launchRes = elb_launch_verify_pattern(batch.hostDescs, NULL, numBlocks,
 					cfg.integrityCheckSalt, batch.devResults, devCounters, numBytes, cfg.blockSize,
@@ -2328,6 +2348,15 @@ void Worker::throwVerifyError(Batch& batch, size_t blockIdx)
 	unsigned expectedVal;
 	unsigned actualVal;
 
+	if(cfg.useRandomVerifyGrain() )
+	{
+		const uint64_t grainSize = 1ULL << cfg.randomVerifyGrainShift;
+
+		expectedVal = elb_rand_grain_byte(badOffset, cfg.integrityCheckSalt,
+			elb_rand_file_base(randFileKey(block) ), grainSize - 1,
+			elb_rand_var_fill_len(grainSize, cfg.blockVariancePercent) );
+	}
+	else
 	if(cfg.useRandomVerify() )
 	{
 		const uint64_t blockKey = elb_rand_block_key(cfg.integrityCheckSalt,

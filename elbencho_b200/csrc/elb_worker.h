@@ -126,7 +126,7 @@ struct GpuStage
 	};
 
 	enum Compute { COMPUTE_NONE, COMPUTE_FILL_PATTERN, COMPUTE_FILL_RANDOM, COMPUTE_VERIFY,
-		COMPUTE_VERIFY_RANDOM };
+		COMPUTE_VERIFY_RANDOM, COMPUTE_FILL_RANDOM_GRAIN, COMPUTE_VERIFY_RANDOM_GRAIN };
 
 	bool isRead;      // host ring -> device ring (read) or device ring -> host ring (write)
 	Transfer transfer;
@@ -343,6 +343,7 @@ class Worker
 		void gpuLaunchStage(Batch& batch, bool isRead);
 		uint32_t fillStageDescs(Batch& batch, bool isRead, uint64_t& outNumBytes);
 		uint64_t randBlockCounter(const BlockRef& block) const;
+		uint64_t randFileKey(const BlockRef& block) const;
 		void enqueueStage(Batch& batch, const GpuStage& stage, uint32_t numBlocks,
 			uint64_t numBytes);
 		bool isStandardShapedBatch(const Batch& batch) const;

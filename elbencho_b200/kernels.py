@@ -148,6 +148,64 @@ def verify_random_staged(descs_ptr, num_descs, pct, seed, host_delta, dev_result
            "elb_verify_random_staged")
 
 
+# ---- grain mode of --verifyrand (--verifyrandgrain): content keyed by file position grains of
+# 2^grain_shift bytes (12..30). Descriptors carry the fileKey in the block counter field and the
+# file position of block byte 0 in file_offset.
+
+def fill_random_grain(dev_ptr, length, file_offset, grain_shift, pct, seed, file_key, stream=0):
+    """K5: the grain-mode content of file bytes [file_offset, file_offset + length)"""
+    _check(_native.load().elb_fill_random_grain(dev_ptr, length, file_offset, grain_shift, pct,
+                                                seed, file_key, stream), "elb_fill_random_grain")
+
+
+def verify_random_grain(dev_ptr, length, file_offset, grain_shift, pct, seed, file_key,
+                        dev_result_ptr, stream=0):
+    """K6: compare with the K5 content; dev_result_ptr as for verify_random"""
+    _check(_native.load().elb_verify_random_grain(dev_ptr, length, file_offset, grain_shift, pct,
+                                                  seed, file_key, dev_result_ptr, stream),
+           "elb_verify_random_grain")
+
+
+def fill_random_grain_batch(dev_descs_ptr, num_descs, grain_shift, pct, seed, dev_counters_ptr=0,
+                            stream=0, total_bytes=0, max_block_len=0):
+    _check(_native.load().elb_fill_random_grain_batch_sized(dev_descs_ptr, num_descs, grain_shift,
+                                                            pct, seed, dev_counters_ptr or None,
+                                                            total_bytes, max_block_len, stream),
+           "elb_fill_random_grain_batch")
+
+
+def verify_random_grain_batch(dev_descs_ptr, num_descs, grain_shift, pct, seed, dev_results_ptr,
+                              dev_counters_ptr=0, stream=0, total_bytes=0, max_block_len=0):
+    _check(_native.load().elb_verify_random_grain_batch_sized(dev_descs_ptr, num_descs,
+                                                              grain_shift, pct, seed,
+                                                              dev_results_ptr,
+                                                              dev_counters_ptr or None,
+                                                              total_bytes, max_block_len, stream),
+           "elb_verify_random_grain_batch")
+
+
+def fill_random_grain_staged(descs_ptr, num_descs, grain_shift, pct, seed, host_delta,
+                             dev_counters_ptr=0, stream=0, total_bytes=0, max_block_len=0):
+    """K5 + stage-out, with the conventions of fill_pattern_staged"""
+    _check(_native.load().elb_fill_random_grain_staged(descs_ptr, num_descs, grain_shift, pct,
+                                                       seed, host_delta, dev_counters_ptr or None,
+                                                       total_bytes, max_block_len, stream),
+           "elb_fill_random_grain_staged")
+
+
+def verify_random_grain_staged(descs_ptr, num_descs, grain_shift, pct, seed, host_delta,
+                               dev_results_ptr, host_results_ptr=0, dev_ticket_ptr=0,
+                               dev_counters_ptr=0, stream=0, total_bytes=0, max_block_len=0):
+    """stage-in + K6, with the conventions of verify_pattern_staged"""
+    _check(_native.load().elb_verify_random_grain_staged(descs_ptr, num_descs, grain_shift, pct,
+                                                         seed, host_delta, dev_results_ptr,
+                                                         host_results_ptr or None,
+                                                         dev_ticket_ptr or None,
+                                                         dev_counters_ptr or None, total_bytes,
+                                                         max_block_len, stream),
+           "elb_verify_random_grain_staged")
+
+
 def stage_copy(descs_ptr, num_descs, host_to_device, host_delta, stream=0, total_bytes=0,
                max_block_len=0):
     _check(_native.load().elb_stage_copy(descs_ptr, num_descs, int(bool(host_to_device)),

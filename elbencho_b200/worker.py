@@ -96,6 +96,7 @@ class WorkerConfig:
     no_direct_io_check: bool = False  # --nodiocheck
     integrity_check_salt: int = 0     # --verify salt, or --verifyrand seed with VERIFY_RANDOM
     integrity_check_kind: int = 0     # elb_verify_kind: 0 pattern (--verify), 1 random (--verifyrand)
+    verify_random_grain: int = 0      # --verifyrandgrain bytes (a power of two; 0 = per block)
     do_direct_verify: bool = False    # --verifydirect
     do_read_inline: bool = False      # --readinline
     block_variance_percent: int = 0   # --blockvarpct
@@ -149,6 +150,10 @@ class WorkerConfig:
         cfg.randOffsetSeed = self.rand_offset_seed
         cfg.integrityCheckSalt = self.integrity_check_salt
         cfg.integrityCheckKind = self.integrity_check_kind
+        grain = self.verify_random_grain
+        # (not a power of two: a shift that the library rejects)
+        cfg.randomVerifyGrainShift = (0 if not grain else grain.bit_length() - 1
+                                      if not grain & (grain - 1) else -1)
         cfg.doDirectVerify = int(self.do_direct_verify)
         cfg.doReadInline = int(self.do_read_inline)
         cfg.blockVariancePercent = self.block_variance_percent

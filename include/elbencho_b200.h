@@ -209,6 +209,31 @@ int elb_verify_random_staged(const elb_block_desc* descs, uint32_t numDescs, uns
 	uint64_t seed, int randAlgo, int64_t hostDelta, elb_verify_result* devResults,
 	elb_verify_result* hostResults, unsigned* devDoneTicket, uint64_t* devCounters,
 	uint64_t totalBytes, uint64_t maxBlockLen, void* stream);
+
+/* K5 / K6, grain mode of --verifyrand (--verifyrandgrain): the content of a file position is that
+ * of its grain of 2^grainShift bytes (12 <= grainShift <= 30), the K3 fill of a block of the grain
+ * size whose block counter is elb_rand_pos_counter(fileKey, grain offset). Independent of how
+ * blocks cut the file. In descriptors, fileOffset is the file position of block byte 0 and
+ * blockCounter carries the fileKey. The forms mirror those of K3 / K4. */
+int elb_fill_random_grain(void* devPtr, uint64_t len, uint64_t fileOffset, unsigned grainShift,
+	unsigned pct, uint64_t seed, uint64_t fileKey, void* stream);
+int elb_verify_random_grain(const void* devPtr, uint64_t len, uint64_t fileOffset,
+	unsigned grainShift, unsigned pct, uint64_t seed, uint64_t fileKey, elb_verify_result* devOut,
+	void* stream);
+int elb_fill_random_grain_batch_sized(const elb_block_desc* descs, uint32_t numDescs,
+	unsigned grainShift, unsigned pct, uint64_t seed, uint64_t* devCounters, uint64_t totalBytes,
+	uint64_t maxBlockLen, void* stream);
+int elb_verify_random_grain_batch_sized(const elb_block_desc* descs, uint32_t numDescs,
+	unsigned grainShift, unsigned pct, uint64_t seed, elb_verify_result* devResults,
+	uint64_t* devCounters, uint64_t totalBytes, uint64_t maxBlockLen, void* stream);
+int elb_fill_random_grain_staged(const elb_block_desc* descs, uint32_t numDescs,
+	unsigned grainShift, unsigned pct, uint64_t seed, int64_t hostDelta, uint64_t* devCounters,
+	uint64_t totalBytes, uint64_t maxBlockLen, void* stream);
+int elb_verify_random_grain_staged(const elb_block_desc* descs, uint32_t numDescs,
+	unsigned grainShift, unsigned pct, uint64_t seed, int64_t hostDelta,
+	elb_verify_result* devResults, elb_verify_result* hostResults, unsigned* devDoneTicket,
+	uint64_t* devCounters, uint64_t totalBytes, uint64_t maxBlockLen, void* stream);
+
 int elb_stage_copy(const elb_block_desc* descs, uint32_t numDescs, int hostToDevice,
 	int64_t hostDelta, uint64_t totalBytes, uint64_t maxBlockLen, void* stream);
 /* devResults[0..numDescs) <- {0, ~0} */
@@ -331,7 +356,10 @@ typedef struct elb_cfg
 	uint64_t fileShareSize;   /* files of at least this size are shared between workers as block
 	                             ranges; 0 = 32 x blockSize (ProgArgs.cpp:52, 1291-1292) */
 	int32_t useCustomTreeRandomize; /* shuffle each worker's file list */
-	int32_t reserved4;
+	/* --verifyrandgrain (with ELB_VERIFY_RANDOM): 0 = per-block random data keyed by each block's
+	 * position, 12..30 = grain mode with grains of 2^shift bytes, keyed by the file position
+	 * alone, so that reads of any block size and offset can check it */
+	int32_t randomVerifyGrainShift;
 	uint64_t treeRandomizeSeed;     /* 0 = self-seed (tests inject one) */
 
 	/* --cores / --zones: worker rank r binds itself to cpuCores[r % n] and / or to the CPUs and
@@ -372,7 +400,8 @@ enum elb_verify_kind
 	ELB_VERIFY_PATTERN = 0, /* --verify: the reference's pattern, integrityCheckSalt is the salt */
 	/* --verifyrand: the random fill of blockVariancePercent, keyed by integrityCheckSalt as the seed
 	 * and by each block's position counter (elb_rand_pos_counter); the read must use the write's
-	 * block size, file size and blockVariancePercent */
+	 * block size, file size and blockVariancePercent (unless randomVerifyGrainShift selects the
+	 * grain mode) */
 	ELB_VERIFY_RANDOM = 1,
 };
 
