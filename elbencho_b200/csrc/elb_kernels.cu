@@ -43,6 +43,7 @@
 #include <atomic>
 #include <mutex>
 #include <string>
+#include <type_traits>
 
 #include "elb_patterns.cuh"
 #include "elb_internal.h"
@@ -1194,20 +1195,65 @@ static void applyStage(KernelArgs& args, const elb_stage_args* stage)
 	args.doneTicket = stage->doneTicket;
 }
 
-int elb_launch_fill_pattern(const elb_block_desc* descs, const elb_block_desc* inlineDesc,
-	uint32_t numDescs, uint64_t salt, uint64_t* devCounters, uint64_t totalBytesHint,
-	uint64_t maxBlockLenHint, cudaStream_t stream, const elb_stage_args* stage)
+/* the generator parameters of the content */
+static void applyContent(KernelArgs& args, const elb_content& content)
+{
+	if(content.kind == elb_content::PATTERN)
+		args.salt = content.key;
+	else
+	{
+		args.seed = content.key;
+		args.pct = content.pct;
+	}
+
+	if(content.kind == elb_content::RANDOM_GRAIN)
+	{
+		args.grainMask = (1ULL << content.grainShift) - 1;
+		args.grainVarFillLen = elb_rand_var_fill_len(1ULL << content.grainShift, content.pct);
+	}
+}
+
+/* calls launch(std::integral_constant<int, MODE>()) with the mode that fills (VERIFY false) or
+   verifies the content */
+template<bool VERIFY, class Launch>
+static int withContentMode(const elb_content& content, Launch launch)
+{
+	switch(content.kind)
+	{
+		case elb_content::PATTERN:
+			return launch(std::integral_constant<int,
+				VERIFY ? MODE_VERIFY_PATTERN : MODE_FILL_PATTERN>() );
+		case elb_content::RANDOM:
+			return launch(std::integral_constant<int,
+				VERIFY ? MODE_VERIFY_RANDOM : MODE_FILL_RANDOM>() );
+		case elb_content::RANDOM_GRAIN:
+			return launch(std::integral_constant<int,
+				VERIFY ? MODE_VERIFY_RANDOM_GRAIN : MODE_FILL_RANDOM_GRAIN>() );
+		default:
+			elb_set_last_error("No block content to fill or verify");
+			return -1;
+	}
+}
+
+int elb_launch_fill(const elb_content& content, const elb_block_desc* descs,
+	const elb_block_desc* inlineDesc, uint32_t numDescs, uint64_t* devCounters,
+	uint64_t totalBytesHint, uint64_t maxBlockLenHint, cudaStream_t stream,
+	const elb_stage_args* stage)
 {
 	KernelArgs args{};
 	args.descs = descs;
 	if(inlineDesc)
 		args.inlineDesc = *inlineDesc;
 	args.numDescs = numDescs;
-	args.salt = salt;
+	applyContent(args, content);
 	args.counters = (unsigned long long*)devCounters;
 	applyStage(args, stage);
 
-	return launchBlocksKernel<MODE_FILL_PATTERN>(args, totalBytesHint, maxBlockLenHint, stream);
+	return withContentMode<false>(content, [&](auto mode)
+	{
+		return launchBlocksKernel<decltype(mode)::value>(args, totalBytesHint, maxBlockLenHint,
+			stream);
+	});
 }
 
 int elb_launch_verify_init(elb_verify_result* devResults, uint32_t numDescs,
@@ -1258,86 +1304,19 @@ static int launchVerify(KernelArgs& args, const elb_block_desc* descs,
 	return launchBlocksKernel<MODE>(args, totalBytesHint, maxBlockLenHint, stream);
 }
 
-int elb_launch_verify_pattern(const elb_block_desc* descs, const elb_block_desc* inlineDesc,
-	uint32_t numDescs, uint64_t salt, elb_verify_result* devResults, uint64_t* devCounters,
-	uint64_t totalBytesHint, uint64_t maxBlockLenHint, bool initResults, cudaStream_t stream,
-	const elb_stage_args* stage)
-{
-	KernelArgs args{};
-	args.salt = salt;
-
-	return launchVerify<MODE_VERIFY_PATTERN>(args, descs, inlineDesc, numDescs, devResults,
-		devCounters, totalBytesHint, maxBlockLenHint, initResults, stream, stage);
-}
-
-int elb_launch_verify_random(const elb_block_desc* descs, const elb_block_desc* inlineDesc,
-	uint32_t numDescs, unsigned pct, uint64_t seed, elb_verify_result* devResults,
+int elb_launch_verify(const elb_content& content, const elb_block_desc* descs,
+	const elb_block_desc* inlineDesc, uint32_t numDescs, elb_verify_result* devResults,
 	uint64_t* devCounters, uint64_t totalBytesHint, uint64_t maxBlockLenHint, bool initResults,
 	cudaStream_t stream, const elb_stage_args* stage)
 {
 	KernelArgs args{};
-	args.seed = seed;
-	args.pct = pct;
+	applyContent(args, content);
 
-	return launchVerify<MODE_VERIFY_RANDOM>(args, descs, inlineDesc, numDescs, devResults,
-		devCounters, totalBytesHint, maxBlockLenHint, initResults, stream, stage);
-}
-
-int elb_launch_fill_random(const elb_block_desc* descs, const elb_block_desc* inlineDesc,
-	uint32_t numDescs, unsigned pct, uint64_t seed, uint64_t* devCounters,
-	uint64_t totalBytesHint, uint64_t maxBlockLenHint, cudaStream_t stream,
-	const elb_stage_args* stage)
-{
-	KernelArgs args{};
-	args.descs = descs;
-	if(inlineDesc)
-		args.inlineDesc = *inlineDesc;
-	args.numDescs = numDescs;
-	args.seed = seed;
-	args.pct = pct;
-	args.counters = (unsigned long long*)devCounters;
-	applyStage(args, stage);
-
-	return launchBlocksKernel<MODE_FILL_RANDOM>(args, totalBytesHint, maxBlockLenHint, stream);
-}
-
-/* the generator parameters of the grain modes (grainShift checked by the caller) */
-static void applyGrain(KernelArgs& args, unsigned grainShift, unsigned pct, uint64_t seed)
-{
-	args.seed = seed;
-	args.pct = pct;
-	args.grainMask = (1ULL << grainShift) - 1;
-	args.grainVarFillLen = elb_rand_var_fill_len(1ULL << grainShift, pct);
-}
-
-int elb_launch_fill_random_grain(const elb_block_desc* descs, const elb_block_desc* inlineDesc,
-	uint32_t numDescs, unsigned grainShift, unsigned pct, uint64_t seed, uint64_t* devCounters,
-	uint64_t totalBytesHint, uint64_t maxBlockLenHint, cudaStream_t stream,
-	const elb_stage_args* stage)
-{
-	KernelArgs args{};
-	args.descs = descs;
-	if(inlineDesc)
-		args.inlineDesc = *inlineDesc;
-	args.numDescs = numDescs;
-	applyGrain(args, grainShift, pct, seed);
-	args.counters = (unsigned long long*)devCounters;
-	applyStage(args, stage);
-
-	return launchBlocksKernel<MODE_FILL_RANDOM_GRAIN>(args, totalBytesHint, maxBlockLenHint,
-		stream);
-}
-
-int elb_launch_verify_random_grain(const elb_block_desc* descs, const elb_block_desc* inlineDesc,
-	uint32_t numDescs, unsigned grainShift, unsigned pct, uint64_t seed,
-	elb_verify_result* devResults, uint64_t* devCounters, uint64_t totalBytesHint,
-	uint64_t maxBlockLenHint, bool initResults, cudaStream_t stream, const elb_stage_args* stage)
-{
-	KernelArgs args{};
-	applyGrain(args, grainShift, pct, seed);
-
-	return launchVerify<MODE_VERIFY_RANDOM_GRAIN>(args, descs, inlineDesc, numDescs, devResults,
-		devCounters, totalBytesHint, maxBlockLenHint, initResults, stream, stage);
+	return withContentMode<true>(content, [&](auto mode)
+	{
+		return launchVerify<decltype(mode)::value>(args, descs, inlineDesc, numDescs, devResults,
+			devCounters, totalBytesHint, maxBlockLenHint, initResults, stream, stage);
+	});
 }
 
 /* plain copy of the blocks between the rings (runs without --verify / without fill) */

@@ -826,18 +826,17 @@ void Worker::allocRings()
 	   (initPhaseFunctionPointers, LocalWorker.cpp:1249-1265); read: verify if salt != 0 (:1311).
 	   --verifyrand: random refill and its verify, keyed by the seed and the block positions;
 	   --verifyrandgrain: those of the grain mode, keyed by the seed and the file positions */
-	const bool useRandomVerify = cfg.useRandomVerify();
-	const bool useGrain = cfg.useRandomVerifyGrain();
+	const uint64_t salt = cfg.integrityCheckSalt;
+	const unsigned pct = cfg.blockVariancePercent;
+	const elb_content writeContent =
+		cfg.useRandomVerifyGrain() ?
+			elb_content{elb_content::RANDOM_GRAIN, salt, pct, cfg.randomVerifyGrainShift} :
+		cfg.useRandomVerify() ? elb_content{elb_content::RANDOM, salt, pct} :
+		salt ? elb_content{elb_content::PATTERN, salt} :
+		pct ? elb_content{elb_content::RANDOM, blockVarianceSeed, pct} : elb_content{};
 
-	writeStage = GpuStage{false, transfer,
-		useGrain ? GpuStage::COMPUTE_FILL_RANDOM_GRAIN :
-		useRandomVerify ? GpuStage::COMPUTE_FILL_RANDOM :
-		cfg.integrityCheckSalt ? GpuStage::COMPUTE_FILL_PATTERN :
-		cfg.blockVariancePercent ? GpuStage::COMPUTE_FILL_RANDOM : GpuStage::COMPUTE_NONE, useGraph};
-	readStage = GpuStage{true, transfer,
-		useGrain ? GpuStage::COMPUTE_VERIFY_RANDOM_GRAIN :
-		useRandomVerify ? GpuStage::COMPUTE_VERIFY_RANDOM :
-		cfg.integrityCheckSalt ? GpuStage::COMPUTE_VERIFY : GpuStage::COMPUTE_NONE, useGraph};
+	writeStage = GpuStage{false, transfer, writeContent, useGraph};
+	readStage = GpuStage{true, transfer, salt ? writeContent : elb_content{}, useGraph};
 
 	if(cfg.pipelineBatchBlocks)
 		batchBlocks = cfg.pipelineBatchBlocks;
@@ -2065,7 +2064,7 @@ void Worker::ioRun(Batch& batch, bool isRead)
 /* pinned descriptors of the blocks the GPU stage works on: every block of a read, the blocks of
  * a write that rwmix did not turn into reads (those get no fill and no staging,
  * LocalWorker.cpp:2213); returns their number and bytes */
-uint32_t Worker::fillStageDescs(Batch& batch, bool isRead, uint64_t& outNumBytes)
+uint32_t Worker::fillStageDescs(Batch& batch, const GpuStage& stage, uint64_t& outNumBytes)
 {
 	uint32_t numDescs = 0;
 	outNumBytes = 0;
@@ -2074,17 +2073,27 @@ uint32_t Worker::fillStageDescs(Batch& batch, bool isRead, uint64_t& outNumBytes
 	{
 		const BlockRef& block = batch.blocks[i];
 
-		if(!isRead && block.ioIsRead)
+		if(!stage.isRead && block.ioIsRead)
 			continue;
 
-		/* (the block counter keys the random fill and its verify, the grain modes take the fileKey
-		   there; pattern verify does not read it) */
 		batch.hostDescs[numDescs++] = elb_block_desc{slotDevPtr(batch, i), block.len,
-			block.offset, cfg.useRandomVerifyGrain() ? randFileKey(block) : randBlockCounter(block)};
+			block.offset, descBlockCounter(stage.content, block)};
 		outNumBytes += block.len;
 	}
 
 	return numDescs;
+}
+
+/* the descriptor's blockCounter field of the block for the content (elb_content) */
+uint64_t Worker::descBlockCounter(const elb_content& content, const BlockRef& block) const
+{
+	if(content.kind == elb_content::RANDOM)
+		return randBlockCounter(block);
+
+	if(content.kind == elb_content::RANDOM_GRAIN)
+		return randFileKey(block);
+
+	return 0;
 }
 
 /* what keys a block's random data: with --verifyrand its place in the data set (the same for the
@@ -2222,7 +2231,7 @@ void Worker::enqueueStage(Batch& batch, const GpuStage& stage, uint32_t numBlock
 	if( (stage.transfer == GpuStage::TRANSFER_COPY) && stage.isRead)
 		enqueueStageCopies(batch, true, false);
 
-	if(stage.compute == GpuStage::COMPUTE_NONE)
+	if(stage.content.kind == elb_content::NONE)
 	{
 		if( (stage.transfer == GpuStage::TRANSFER_KERNEL) && elb_launch_stage_copy(batch.hostDescs,
 			numBlocks, stage.isRead, hostDelta, numBytes, cfg.blockSize, batch.stream) )
@@ -2237,40 +2246,18 @@ void Worker::enqueueStage(Batch& batch, const GpuStage& stage, uint32_t numBlock
 		ELB_CUDA_CHECK(recordKernelEvent(batch.kernelStartEvent, batch.stream),
 			"CUDA event record");
 
-		if(stage.compute == GpuStage::COMPUTE_FILL_PATTERN)
-			launchRes = elb_launch_fill_pattern(batch.hostDescs, NULL, numBlocks,
-				cfg.integrityCheckSalt, devCounters, numBytes, cfg.blockSize, batch.stream, &args);
-		else
-		if(stage.compute == GpuStage::COMPUTE_FILL_RANDOM)
-			launchRes = elb_launch_fill_random(batch.hostDescs, NULL, numBlocks,
-				cfg.blockVariancePercent, cfg.useRandomVerify() ? cfg.integrityCheckSalt :
-				blockVarianceSeed, devCounters, numBytes, cfg.blockSize, batch.stream, &args);
-		else
-		if(stage.compute == GpuStage::COMPUTE_FILL_RANDOM_GRAIN)
-			launchRes = elb_launch_fill_random_grain(batch.hostDescs, NULL, numBlocks,
-				cfg.randomVerifyGrainShift, cfg.blockVariancePercent, cfg.integrityCheckSalt,
-				devCounters, numBytes, cfg.blockSize, batch.stream, &args);
-		else
+		if(stage.isRead)
 		{
 			args.hostResults = batch.hostResults;
 			args.doneTicket = batch.devDoneTicket;
 
 			// (initResults false: armed at setup, re-armed by the kernel)
-			if(stage.compute == GpuStage::COMPUTE_VERIFY_RANDOM)
-				launchRes = elb_launch_verify_random(batch.hostDescs, NULL, numBlocks,
-					cfg.blockVariancePercent, cfg.integrityCheckSalt, batch.devResults, devCounters,
-					numBytes, cfg.blockSize, false, batch.stream, &args);
-			else
-			if(stage.compute == GpuStage::COMPUTE_VERIFY_RANDOM_GRAIN)
-				launchRes = elb_launch_verify_random_grain(batch.hostDescs, NULL, numBlocks,
-					cfg.randomVerifyGrainShift, cfg.blockVariancePercent, cfg.integrityCheckSalt,
-					batch.devResults, devCounters, numBytes, cfg.blockSize, false, batch.stream,
-					&args);
-			else
-				launchRes = elb_launch_verify_pattern(batch.hostDescs, NULL, numBlocks,
-					cfg.integrityCheckSalt, batch.devResults, devCounters, numBytes, cfg.blockSize,
-					false, batch.stream, &args);
+			launchRes = elb_launch_verify(stage.content, batch.hostDescs, NULL, numBlocks,
+				batch.devResults, devCounters, numBytes, cfg.blockSize, false, batch.stream, &args);
 		}
+		else
+			launchRes = elb_launch_fill(stage.content, batch.hostDescs, NULL, numBlocks, devCounters,
+				numBytes, cfg.blockSize, batch.stream, &args);
 
 		if(launchRes)
 			throw WorkerError(std::string(stage.isRead ? "GPU block verification failed. " :
@@ -2293,9 +2280,9 @@ void Worker::gpuLaunchStage(Batch& batch, bool isRead)
 {
 	const GpuStage& stage = isRead ? readStage : writeStage;
 	uint64_t numBytes;
-	const uint32_t numBlocks = fillStageDescs(batch, isRead, numBytes);
+	const uint32_t numBlocks = fillStageDescs(batch, stage, numBytes);
 
-	batch.hadKernel = numBlocks && (stage.compute != GpuStage::COMPUTE_NONE);
+	batch.hadKernel = numBlocks && (stage.content.kind != elb_content::NONE);
 
 	ELB_CUDA_CHECK(cudaEventRecord(batch.gpuStartEvent, batch.stream), "CUDA event record");
 
@@ -2344,30 +2331,11 @@ void Worker::throwVerifyError(Batch& batch, size_t blockIdx)
 	const BlockRef& block = batch.blocks[blockIdx];
 	const uint64_t firstIdx = batch.hostResults[blockIdx].firstMismatchIdx;
 	const uint64_t badOffset = block.offset + firstIdx;
+	const elb_block_desc desc{NULL, block.len, block.offset,
+		descBlockCounter(readStage.content, block)};
 
-	unsigned expectedVal;
+	const unsigned expectedVal = elb_content_byte(readStage.content, desc, firstIdx);
 	unsigned actualVal;
-
-	if(cfg.useRandomVerifyGrain() )
-	{
-		const uint64_t grainSize = 1ULL << cfg.randomVerifyGrainShift;
-
-		expectedVal = elb_rand_grain_byte(badOffset, cfg.integrityCheckSalt,
-			elb_rand_file_base(randFileKey(block) ), grainSize - 1,
-			elb_rand_var_fill_len(grainSize, cfg.blockVariancePercent) );
-	}
-	else
-	if(cfg.useRandomVerify() )
-	{
-		const uint64_t blockKey = elb_rand_block_key(cfg.integrityCheckSalt,
-			randBlockCounter(block) );
-
-		expectedVal = elb_rand_byte(firstIdx, blockKey,
-			elb_rand_var_fill_len(block.len, cfg.blockVariancePercent),
-			elb_rand_remainder_val(blockKey) );
-	}
-	else
-		expectedVal = elb_pattern_byte(badOffset, cfg.integrityCheckSalt);
 
 	if(readStage.transfer != GpuStage::TRANSFER_NONE)
 		actualVal = (unsigned char)slotHostPtr(batch, blockIdx)[firstIdx];

@@ -125,12 +125,9 @@ struct GpuStage
 		TRANSFER_COPY,   // cudaMemcpyAsync between the rings
 	};
 
-	enum Compute { COMPUTE_NONE, COMPUTE_FILL_PATTERN, COMPUTE_FILL_RANDOM, COMPUTE_VERIFY,
-		COMPUTE_VERIFY_RANDOM, COMPUTE_FILL_RANDOM_GRAIN, COMPUTE_VERIFY_RANDOM_GRAIN };
-
 	bool isRead;      // host ring -> device ring (read) or device ring -> host ring (write)
 	Transfer transfer;
-	Compute compute;
+	elb_content content; // what the write fills or the read verifies (NONE: the blocks only move)
 	bool useGraph;    // replay full batches from a CUDA graph (one launch per batch anyway under
 	                  // kernel staging)
 };
@@ -341,7 +338,8 @@ class Worker
 		void verifyWrittenBatch(Batch& batch);
 		void accountBatch(Batch& batch, uint64_t gpuUSecTotal);
 		void gpuLaunchStage(Batch& batch, bool isRead);
-		uint32_t fillStageDescs(Batch& batch, bool isRead, uint64_t& outNumBytes);
+		uint32_t fillStageDescs(Batch& batch, const GpuStage& stage, uint64_t& outNumBytes);
+		uint64_t descBlockCounter(const elb_content& content, const BlockRef& block) const;
 		uint64_t randBlockCounter(const BlockRef& block) const;
 		uint64_t randFileKey(const BlockRef& block) const;
 		void enqueueStage(Batch& batch, const GpuStage& stage, uint32_t numBlocks,
