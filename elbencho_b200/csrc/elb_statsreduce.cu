@@ -211,7 +211,7 @@ LiveStatsReducer::LiveStatsReducer(Manager& manager) : manager(manager)
 			(cudaMalloc( (void**)&gpu.devHistoRecv, histoBytes) == cudaSuccess) &&
 			(cudaHostAlloc( (void**)&gpu.hostHisto, histoBytes, cudaHostAllocDefault) ==
 				cudaSuccess) &&
-			(cudaMemset(gpu.devRecv, 0, slabBytes) == cudaSuccess);
+			(cudaMemsetAsync(gpu.devRecv, 0, slabBytes, gpu.stream) == cudaSuccess);
 
 		if(!deviceStateOK)
 			break;

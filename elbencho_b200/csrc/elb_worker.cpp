@@ -367,14 +367,16 @@ int Worker::snapshotDevCounters(uint64_t out[ELB_DEVCTR_NUM] )
 {
 	memset(out, 0, sizeof(uint64_t) * ELB_DEVCTR_NUM);
 
-	if(!devCounters)
+	if(!devCounters || !auxStream)
 		return -1;
 
 	int oldDev = -1;
 	cudaGetDevice(&oldDev);
 	cudaSetDevice(gpuID);
-	cudaError_t copyRes = cudaMemcpy(out, devCounters, sizeof(uint64_t) * ELB_DEVCTR_NUM,
-		cudaMemcpyDeviceToHost);
+	cudaError_t copyRes = cudaMemcpyAsync(out, devCounters, sizeof(uint64_t) * ELB_DEVCTR_NUM,
+		cudaMemcpyDeviceToHost, auxStream);
+	if(copyRes == cudaSuccess)
+		copyRes = cudaStreamSynchronize(auxStream);
 	if(oldDev >= 0)
 		cudaSetDevice(oldDev);
 
@@ -862,7 +864,9 @@ void Worker::allocRings()
 	ELB_CUDA_CHECK(cudaMalloc( (void**)&devRing, ringBytes), "GPU I/O ring allocation");
 	ELB_CUDA_CHECK(cudaMalloc( (void**)&devCounters, sizeof(uint64_t) * ELB_DEVCTR_NUM),
 		"GPU counter block allocation");
-	ELB_CUDA_CHECK(cudaMemset(devCounters, 0, sizeof(uint64_t) * ELB_DEVCTR_NUM),
+	ELB_CUDA_CHECK(cudaStreamCreateWithFlags(&auxStream, cudaStreamNonBlocking),
+		"CUDA stream creation");
+	ELB_CUDA_CHECK(cudaMemsetAsync(devCounters, 0, sizeof(uint64_t) * ELB_DEVCTR_NUM, auxStream),
 		"GPU counter block init");
 
 	hostDelta = (int64_t)( (intptr_t)hostRing - (intptr_t)devRing);
@@ -876,8 +880,9 @@ void Worker::allocRings()
 			words[i] = initRand.next();
 	}
 
-	ELB_CUDA_CHECK(cudaMemcpy(devRing, hostRing, ringBytes, cudaMemcpyHostToDevice),
-		"Initialization of GPU I/O ring");
+	ELB_CUDA_CHECK(cudaMemcpyAsync(devRing, hostRing, ringBytes, cudaMemcpyHostToDevice,
+		auxStream), "Initialization of GPU I/O ring");
+	ELB_CUDA_CHECK(cudaStreamSynchronize(auxStream), "Initialization of GPU I/O ring");
 
 	if(elb_kernels_warmup() )
 		throw WorkerError(std::string("GPU kernel setup failed. ") + elb_last_error() );
@@ -907,7 +912,7 @@ void Worker::allocRings()
 			"Pinned verify result allocation");
 		ELB_CUDA_CHECK(cudaMalloc( (void**)&batch.devDoneTicket, sizeof(unsigned) ),
 			"GPU ticket counter allocation");
-		ELB_CUDA_CHECK(cudaMemset(batch.devDoneTicket, 0, sizeof(unsigned) ),
+		ELB_CUDA_CHECK(cudaMemsetAsync(batch.devDoneTicket, 0, sizeof(unsigned), batch.stream),
 			"GPU ticket counter init");
 
 		memset(batch.hostResults, 0, sizeof(elb_verify_result) * batchBlocks);
@@ -1027,10 +1032,13 @@ void Worker::freeRings() // LocalWorker::cleanup (:1570-1641)
 		cudaFree(devRing);
 	if(devCounters)
 		cudaFree(devCounters);
+	if(auxStream)
+		cudaStreamDestroy(auxStream);
 
 	hostRing = NULL;
 	devRing = NULL;
 	devCounters = NULL;
+	auxStream = NULL;
 	gpuPrepared = false;
 }
 
@@ -1681,9 +1689,14 @@ void Worker::rwPhase()
 
 	ELB_CUDA_CHECK(cudaSetDevice(gpuID), "Setting CUDA device");
 
-	if(devCounters)
-		ELB_CUDA_CHECK(cudaMemset(devCounters, 0, sizeof(uint64_t) * ELB_DEVCTR_NUM),
-			"GPU counter block reset");
+	if(gpuPrepared)
+	{ /* on a batch stream (all idle between phases) and complete before the first launch: on the
+		 legacy default stream the reset would wait for the caller's work there and could land
+		 after this phase's kernels */
+		ELB_CUDA_CHECK(cudaMemsetAsync(devCounters, 0, sizeof(uint64_t) * ELB_DEVCTR_NUM,
+			batches[0].stream), "GPU counter block reset");
+		ELB_CUDA_CHECK(cudaStreamSynchronize(batches[0].stream), "GPU counter block reset");
+	}
 
 	initPhaseOffsetPlan();
 
@@ -2342,8 +2355,9 @@ void Worker::throwVerifyError(Batch& batch, size_t blockIdx)
 	else
 	{ // the block never touched host memory: fetch the one bad byte
 		unsigned char actualByte = 0;
-		ELB_CUDA_CHECK(cudaMemcpy(&actualByte, slotDevPtr(batch, blockIdx) + firstIdx, 1,
-			cudaMemcpyDeviceToHost), "Copy of mismatching byte from GPU");
+		ELB_CUDA_CHECK(cudaMemcpyAsync(&actualByte, slotDevPtr(batch, blockIdx) + firstIdx, 1,
+			cudaMemcpyDeviceToHost, batch.stream), "Copy of mismatching byte from GPU");
+		ELB_CUDA_CHECK(cudaStreamSynchronize(batch.stream), "Copy of mismatching byte from GPU");
 		actualVal = actualByte;
 	}
 

@@ -254,6 +254,9 @@ class Worker
 		int boundNumaNode{-1};       // NUMA node this worker bound itself to (-1: none)
 		std::vector<Batch> batches;
 		uint64_t* devCounters{NULL};
+		/* non-blocking stream of the ring / counter setup and of counter snapshots: the legacy
+		   default stream would queue them behind the caller's work on it (DESIGN.md) */
+		cudaStream_t auxStream{NULL};
 		bool gpuPrepared{false};
 
 		// offsets

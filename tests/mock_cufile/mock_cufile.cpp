@@ -2,8 +2,8 @@
  * TEST INFRASTRUCTURE — stand-in for libcufile on boxes where GPUDirect Storage cannot be used
  * (on the graft GPU boxes cuFileHandleRegister fails with "internal error" even in compat mode:
  * no nvidia-fs, containerised overlay/tmpfs mounts). It implements the subset of the cuFile API
- * that libelbencho_b200.so binds, with POSIX I/O + cudaMemcpy through an aligned bounce buffer,
- * i.e. what cuFile's own compatibility mode does. The worker loads it through ELB_CUFILE_LIB,
+ * that libelbencho_b200.so binds, with POSIX I/O + synchronized copies through an aligned bounce
+ * buffer, i.e. what cuFile's own compatibility mode does. The worker loads it through ELB_CUFILE_LIB,
  * so the GDS code path of the worker (handle/buffer registration lifecycle, device-ring offsets,
  * sync calls, batch submit/status) runs on a real GPU and is checked bit-exactly.
  *
@@ -18,6 +18,7 @@
 
 #include <atomic>
 #include <deque>
+#include <map>
 #include <mutex>
 #include <set>
 
@@ -36,6 +37,31 @@ struct MockBatch
 
 static int handleToFD(CUfileHandle_t fh) { return (int)(intptr_t)fh - 1; }
 
+/* one non-blocking stream per device for the bounce buffer copies, synchronized before the call
+ * returns: a cudaMemcpy from pageable memory may return before the DMA lands, and on the legacy
+ * default stream the copy would also wait for the application's work there */
+static cudaStream_t copyStream()
+{
+	static std::map<int, cudaStream_t> streams;
+
+	int dev = 0;
+	if(cudaGetDevice(&dev) != cudaSuccess)
+		return NULL;
+
+	std::unique_lock<std::mutex> lock(gMutex);
+	cudaStream_t& stream = streams[dev];
+	if(!stream && (cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking) != cudaSuccess) )
+		stream = NULL;
+	return stream;
+}
+
+static bool copySync(void* dst, const void* src, size_t count, cudaMemcpyKind kind)
+{
+	cudaStream_t stream = copyStream();
+	return stream && (cudaMemcpyAsync(dst, src, count, kind, stream) == cudaSuccess) &&
+		(cudaStreamSynchronize(stream) == cudaSuccess);
+}
+
 static ssize_t doIO(CUfileHandle_t fh, void* devBase, size_t size, off_t fileOffset,
 	off_t devOffset, bool isRead)
 {
@@ -49,12 +75,12 @@ static ssize_t doIO(CUfileHandle_t fh, void* devBase, size_t size, off_t fileOff
 	if(isRead)
 	{
 		res = pread(handleToFD(fh), bounce, size, fileOffset);
-		if( (res > 0) && (cudaMemcpy(devPtr, bounce, res, cudaMemcpyHostToDevice) != cudaSuccess) )
+		if( (res > 0) && !copySync(devPtr, bounce, res, cudaMemcpyHostToDevice) )
 			res = -5011; // CU_FILE_CUDA_DRIVER_ERROR style negative code
 	}
 	else
 	{
-		if(cudaMemcpy(bounce, devPtr, size, cudaMemcpyDeviceToHost) != cudaSuccess)
+		if(!copySync(bounce, devPtr, size, cudaMemcpyDeviceToHost) )
 			res = -5011;
 		else
 			res = pwrite(handleToFD(fh), bounce, size, fileOffset);
