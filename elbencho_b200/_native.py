@@ -60,6 +60,7 @@ class Cfg(ctypes.Structure):
         ("blockVarianceAlgo", c_i32),
         ("blockVarianceSeed", c_u64),
         ("rwMixReadPercent", c_u32),
+        ("dedupePercent", c_u32),
         ("gpuIDs", ctypes.POINTER(c_i32)),
         ("numGPUIDs", c_u32),
         ("useCuFile", c_i32),
@@ -210,6 +211,23 @@ SIGNATURES = {
     "elb_verify_random_grain_staged": (ctypes.c_int, [_VP, c_u32, ctypes.c_uint, ctypes.c_uint,
                                                       c_u64, ctypes.c_int64, _VP, _VP, _VP, _VP,
                                                       c_u64, c_u64, _VP]),
+    "elb_fill_dedupe_grain": (ctypes.c_int, [_VP, c_u64, c_u64, ctypes.c_uint, ctypes.c_uint,
+                                             ctypes.c_uint, c_u64, c_u64, _VP]),
+    "elb_verify_dedupe_grain": (ctypes.c_int, [_VP, c_u64, c_u64, ctypes.c_uint, ctypes.c_uint,
+                                               ctypes.c_uint, c_u64, c_u64, _VP, _VP]),
+    "elb_fill_dedupe_grain_batch_sized": (ctypes.c_int, [_VP, c_u32, ctypes.c_uint, ctypes.c_uint,
+                                                         ctypes.c_uint, c_u64, _VP, c_u64, c_u64,
+                                                         _VP]),
+    "elb_verify_dedupe_grain_batch_sized": (ctypes.c_int, [_VP, c_u32, ctypes.c_uint,
+                                                           ctypes.c_uint, ctypes.c_uint, c_u64, _VP,
+                                                           _VP, c_u64, c_u64, _VP]),
+    "elb_fill_dedupe_grain_staged": (ctypes.c_int, [_VP, c_u32, ctypes.c_uint, ctypes.c_uint,
+                                                    ctypes.c_uint, c_u64, ctypes.c_int64, _VP,
+                                                    c_u64, c_u64, _VP]),
+    "elb_verify_dedupe_grain_staged": (ctypes.c_int, [_VP, c_u32, ctypes.c_uint, ctypes.c_uint,
+                                                      ctypes.c_uint, c_u64, ctypes.c_int64, _VP,
+                                                      _VP, _VP, _VP, c_u64, c_u64, _VP]),
+    "elb_rand_grain_content_key": (c_u64, [c_u64, c_u64, c_u64, ctypes.c_uint, ctypes.c_uint]),
     "elb_rand_pos_counter": (c_u64, [c_u64, c_u64]),
     "elb_rand_dir_file_key": (c_u64, [c_u64, c_u64, c_u64]),
     "elb_stage_copy": (ctypes.c_int, [_VP, c_u32, ctypes.c_int, ctypes.c_int64, c_u64, c_u64,

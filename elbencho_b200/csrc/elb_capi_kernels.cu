@@ -4,7 +4,8 @@
  * in place of LocalWorker::preWriteIntegrityCheckFillBuf / postReadIntegrityCheckVerifyBuf /
  * preWriteBufRandRefillCuda (source/workers/LocalWorker.cpp:2091-2277).
  *
- * Each fill / verify entry point states its content (elb_content: pattern, random or random grain)
+ * Each fill / verify entry point states its content (elb_content: pattern, random, random grain or
+ * random grain with pool duplicates)
  * and forwards to one of two bodies: singleBlock() for the single-block forms, batch() for the
  * _batch_sized and _staged forms. Both check the content's arguments first, even when there is
  * nothing to do, and prefix their errors with the entry point's name.
@@ -32,6 +33,13 @@ static int checkContent(const elb_content& content, int randAlgo)
 	{
 		elb_set_last_error("Block variance percent must be in range 0..100. Given: " +
 			std::to_string(content.pct) );
+		return -1;
+	}
+
+	if(content.dedupePct > 100)
+	{
+		elb_set_last_error("Dedupe percent must be in range 0..100. Given: " +
+			std::to_string(content.dedupePct) );
 		return -1;
 	}
 
@@ -109,6 +117,10 @@ static elb_content randomContent(unsigned pct, uint64_t seed)
 
 static elb_content grainContent(unsigned grainShift, unsigned pct, uint64_t seed)
 	{ return elb_content{elb_content::RANDOM_GRAIN, seed, pct, grainShift}; }
+
+static elb_content dedupeContent(unsigned grainShift, unsigned pct, unsigned dedupePct,
+	uint64_t seed)
+	{ return elb_content{elb_content::RANDOM_GRAIN, seed, pct, grainShift, dedupePct}; }
 
 extern "C" {
 
@@ -292,6 +304,70 @@ int elb_verify_random_grain_staged(const elb_block_desc* descs, uint32_t numDesc
 	return batch("elb_verify_random_grain_staged", grainContent(grainShift, pct, seed),
 		ELB_RANDALGO_SPLITMIX64, true, descs, numDescs, devResults, devCounters, totalBytes,
 		maxBlockLen, stream, &stage);
+}
+
+int elb_fill_dedupe_grain(void* devPtr, uint64_t len, uint64_t fileOffset, unsigned grainShift,
+	unsigned pct, unsigned dedupePct, uint64_t seed, uint64_t fileKey, void* stream)
+{
+	return singleBlock("elb_fill_dedupe_grain", dedupeContent(grainShift, pct, dedupePct, seed),
+		ELB_RANDALGO_SPLITMIX64, false, devPtr, len, fileOffset, fileKey, NULL, stream);
+}
+
+int elb_verify_dedupe_grain(const void* devPtr, uint64_t len, uint64_t fileOffset,
+	unsigned grainShift, unsigned pct, unsigned dedupePct, uint64_t seed, uint64_t fileKey,
+	elb_verify_result* devOut, void* stream)
+{
+	return singleBlock("elb_verify_dedupe_grain", dedupeContent(grainShift, pct, dedupePct, seed),
+		ELB_RANDALGO_SPLITMIX64, true, devPtr, len, fileOffset, fileKey, devOut, stream);
+}
+
+int elb_fill_dedupe_grain_batch_sized(const elb_block_desc* descs, uint32_t numDescs,
+	unsigned grainShift, unsigned pct, unsigned dedupePct, uint64_t seed, uint64_t* devCounters,
+	uint64_t totalBytes, uint64_t maxBlockLen, void* stream)
+{
+	return batch("elb_fill_dedupe_grain_batch", dedupeContent(grainShift, pct, dedupePct, seed),
+		ELB_RANDALGO_SPLITMIX64, false, descs, numDescs, NULL, devCounters, totalBytes,
+		maxBlockLen, stream);
+}
+
+int elb_verify_dedupe_grain_batch_sized(const elb_block_desc* descs, uint32_t numDescs,
+	unsigned grainShift, unsigned pct, unsigned dedupePct, uint64_t seed,
+	elb_verify_result* devResults, uint64_t* devCounters, uint64_t totalBytes,
+	uint64_t maxBlockLen, void* stream)
+{
+	return batch("elb_verify_dedupe_grain_batch", dedupeContent(grainShift, pct, dedupePct, seed),
+		ELB_RANDALGO_SPLITMIX64, true, descs, numDescs, devResults, devCounters, totalBytes,
+		maxBlockLen, stream);
+}
+
+int elb_fill_dedupe_grain_staged(const elb_block_desc* descs, uint32_t numDescs,
+	unsigned grainShift, unsigned pct, unsigned dedupePct, uint64_t seed, int64_t hostDelta,
+	uint64_t* devCounters, uint64_t totalBytes, uint64_t maxBlockLen, void* stream)
+{
+	const elb_stage_args stage{hostDelta};
+
+	return batch("elb_fill_dedupe_grain_staged", dedupeContent(grainShift, pct, dedupePct, seed),
+		ELB_RANDALGO_SPLITMIX64, false, descs, numDescs, NULL, devCounters, totalBytes,
+		maxBlockLen, stream, &stage);
+}
+
+int elb_verify_dedupe_grain_staged(const elb_block_desc* descs, uint32_t numDescs,
+	unsigned grainShift, unsigned pct, unsigned dedupePct, uint64_t seed, int64_t hostDelta,
+	elb_verify_result* devResults, elb_verify_result* hostResults, unsigned* devDoneTicket,
+	uint64_t* devCounters, uint64_t totalBytes, uint64_t maxBlockLen, void* stream)
+{
+	const elb_stage_args stage{hostDelta, hostResults, devDoneTicket};
+
+	return batch("elb_verify_dedupe_grain_staged",
+		dedupeContent(grainShift, pct, dedupePct, seed), ELB_RANDALGO_SPLITMIX64, true, descs,
+		numDescs, devResults, devCounters, totalBytes, maxBlockLen, stream, &stage);
+}
+
+uint64_t elb_rand_grain_content_key(uint64_t seed, uint64_t fileKey, uint64_t grainOffset,
+	unsigned grainShift, unsigned dedupePct)
+{
+	return elb_rand_dedupe_grain_key(seed, elb_rand_file_base(fileKey), grainOffset, grainShift,
+		dedupePct);
 }
 
 int elb_stage_copy(const elb_block_desc* descs, uint32_t numDescs, int hostToDevice,

@@ -89,6 +89,11 @@ static const OptDef optDefs[] =
 		"position in grains of this size (a power of two from 4K to 1G) instead of by block, so that "
 		"reads of any block size and offset (also --rand --norandalign) can check it. Writes and "
 		"reads must use the same value, seed and --blockvarpct. (Default: 0 = per block) [b200]"},
+	{"dedupepct", 0, Opt_U64, "Percentage of duplicate grains (0..100) in --verifyrandgrain data: "
+		"about this share of the grains are copies of grains from one pool of 4096 grains that is "
+		"the same for all files, so that storage which deduplicates finds them. Checked on reads "
+		"like all grains. Reads must use the write's value. Requires --verifyrandgrain. "
+		"(Default: 0) [b200]"},
 	{"rwmixpct", 0, Opt_U64, "Percentage of blocks that should be read in a write phase."},
 	{"rwmixthr", 0, Opt_U64, "Number of threads that should do reads in a write phase."},
 	// GPU
@@ -587,6 +592,7 @@ ProgArgs::ProgArgs(int argc, char** argv)
 	num("blockvarseed", blockVarianceSeed);
 	num("verifyrand", randomVerifySeed);
 	num("verifyrandgrain", randomVerifyGrain);
+	num("dedupepct", dedupePercent);
 	hasUserSetRWMixPercent = num("rwmixpct", rwMixReadPercent);
 	hasUserSetRWMixReadThreads = num("rwmixthr", numRWMixReadThreads);
 	num("rwmixthrpct", rwMixThreadsReadPercent);
@@ -965,6 +971,12 @@ void ProgArgs::checkArgs()
 		(randomVerifyGrain < (4ULL << 10) ) || (randomVerifyGrain > (1ULL << 30) ) ) )
 		throw ProgError("Option \"--verifyrandgrain\" must be a power of two from 4K to 1G");
 
+	if(dedupePercent && !randomVerifyGrain)
+		throw ProgError("Option \"--dedupepct\" requires \"--verifyrandgrain\"");
+
+	if(dedupePercent > 100)
+		throw ProgError("Option \"--dedupepct\" must be in range 0..100");
+
 	if(doDirectVerify && ( (!integrityCheckSalt && !randomVerifySeed) || !runCreateFilesPhase) )
 		throw ProgError("Direct verification requires --verify and --write"); // :1426-1428
 
@@ -1040,6 +1052,7 @@ void ProgArgs::toABIConfig(ABIConfig& out) const
 	cfg.randomVerifyGrainShift = 0;
 	for(uint64_t grain = randomVerifyGrain; grain > 1; grain >>= 1) // (a power of two, checked)
 		cfg.randomVerifyGrainShift++;
+	cfg.dedupePercent = (uint32_t)dedupePercent;
 	cfg.doDirectVerify = doDirectVerify;
 	cfg.doReadInline = doReadInline;
 	cfg.blockVariancePercent = (uint32_t)blockVariancePercent;

@@ -181,6 +181,16 @@ Config Config::fromABI(const elb_cfg* cfg)
 		throw WorkerError("A random verify grain (--verifyrandgrain) requires random data "
 			"verification (--verifyrand).");
 
+	if(cfg->dedupePercent > 100)
+		throw WorkerError("Dedupe percent must be in range 0..100. Given: " +
+			std::to_string(cfg->dedupePercent) );
+
+	c.dedupePercent = cfg->dedupePercent;
+
+	if(c.dedupePercent && !c.useRandomVerifyGrain() )
+		throw WorkerError("A dedupe percentage (--dedupepct) requires a random verify grain "
+			"(--verifyrandgrain).");
+
 	if(c.integrityCheckSalt && c.rwMixReadPercent) // :1414
 		throw WorkerError("Integrity check cannot be used together with rwmixpct.");
 

@@ -1016,6 +1016,9 @@ struct Config
 	bool useRandomVerifyGrain() const
 		{ return useRandomVerify() && randomVerifyGrainShift; }
 
+	/* --dedupepct: percent of the grains that are duplicates of pool grains (elb_patterns.cuh) */
+	unsigned dedupePercent{0};
+
 	/* @throw WorkerError on invalid combinations */
 	static Config fromABI(const elb_cfg* cfg);
 };

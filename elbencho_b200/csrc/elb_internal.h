@@ -39,6 +39,7 @@ struct elb_content
 	uint64_t key{0};        // pattern salt or random seed
 	unsigned pct{0};        // random: percent of a block (grain) that is random, 0..100
 	unsigned grainShift{0}; // random grain: grains of 2^grainShift bytes, 12..30
+	unsigned dedupePct{0};  // random grain: percent of the grains that are pool duplicates, 0..100
 };
 
 /* the expected byte at block position pos of the block desc (NONE: 0) */
@@ -58,6 +59,12 @@ ELB_HD uint8_t elb_content_byte(const elb_content& content, const elb_block_desc
 	if(content.kind == elb_content::RANDOM_GRAIN)
 	{
 		const uint64_t grainSize = 1ULL << content.grainShift;
+
+		if(content.dedupePct)
+			return elb_rand_dedupe_byte(desc.fileOffset + pos, content.key,
+				elb_rand_file_base(desc.blockCounter), content.grainShift,
+				elb_rand_var_fill_len(grainSize, content.pct), content.dedupePct);
+
 		return elb_rand_grain_byte(desc.fileOffset + pos, content.key,
 			elb_rand_file_base(desc.blockCounter), grainSize - 1,
 			elb_rand_var_fill_len(grainSize, content.pct) );

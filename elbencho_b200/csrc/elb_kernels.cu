@@ -7,9 +7,11 @@
  *   K4 verify_random  (no reference counterpart: --verifyrand checks K3's content on reads)
  *   K5 fill_random_grain, K6 verify_random_grain (no reference counterpart: --verifyrandgrain,
  *      K3's content per grain of the file, keyed by the grain's file position)
+ *   K7 fill_dedupe_grain, K8 verify_dedupe_grain (no reference counterpart: --dedupepct, K5 / K6
+ *      with a set share of the grains keyed as duplicates from a pool, elb_patterns.cuh)
  *
- * All six are HBM-bound byte/integer kernels (K1/K3/K5: 1 byte written per payload byte, K2/K4/K6:
- * 1 byte read per payload byte), so the design follows the streaming rules: 16-byte (128-bit) vector
+ * All eight are HBM-bound byte/integer kernels (K1/K3/K5/K7: 1 byte written per payload byte,
+ * K2/K4/K6/K8: 1 byte read per payload byte), so the design follows the streaming rules: 16-byte (128-bit) vector
  * accesses per thread (LDG/STG.E.128, the widest global access of sm_90), fully coalesced (a warp
  * covers 512 contiguous bytes per access), L1 no-allocate hints, several independent accesses in
  * flight per thread, and a grid sized to a multiple of the SM count that walks "tiles" of the whole
@@ -62,10 +64,12 @@
    for verify_pattern, 16 / 24 B for verify_random), and 3 x 256 threads with 128 B in flight each
    are still far more than the H100's HBM latency needs. verify_random_grain is a verify mode too.
    fill_random_grain would take all 64 registers of 4 CTAs per SM; 5 (48 registers, no spills)
-   keep it at least in fill_random's occupancy (48 / 50 registers: 5 / 4 CTAs per SM). */
+   keep it at least in fill_random's occupancy (48 / 50 registers: 5 / 4 CTAs per SM). The dedupe
+   modes take the bounds of their grain counterparts. */
 #define ELB_MIN_CTAS_PER_SM(mode) \
 	( ( (mode) == 1 /* MODE_VERIFY_PATTERN */ || (mode) == 5 /* MODE_VERIFY_RANDOM */ || \
-	(mode) == 7 /* MODE_VERIFY_RANDOM_GRAIN */) ? 3 : (mode) == 6 /* MODE_FILL_RANDOM_GRAIN */ ? 5 : 4)
+	(mode) == 7 /* MODE_VERIFY_RANDOM_GRAIN */ || (mode) == 9 /* MODE_VERIFY_DEDUPE_GRAIN */) ? 3 : \
+	( (mode) == 6 /* MODE_FILL_RANDOM_GRAIN */ || (mode) == 8 /* MODE_FILL_DEDUPE_GRAIN */) ? 5 : 4)
 
 struct __align__(16) u64x2
 {
@@ -256,6 +260,58 @@ struct GrainGen
 
 	__device__ __forceinline__ uint8_t byte(uint64_t pos) const
 		{ return elb_rand_grain_byte(fileOffset + pos, seed, fileBase, grainMask, varFillLen); }
+
+	/* key of the grain at file position grainOffset (walk_grain_span) */
+	__device__ __forceinline__ uint64_t grainKey(uint64_t grainOffset) const
+		{ return elb_rand_grain_key(seed, fileBase, grainOffset); }
+};
+
+/* --dedupepct content: GrainGen with the grain key of elb_rand_dedupe_grain_key, which makes
+   dedupePct percent of the grains duplicates of pool grains. Only the key differs from GrainGen. */
+struct DedupeGen
+{
+	uint64_t seed;
+	uint64_t fileBase;   // elb_rand_file_base(fileKey)
+	uint64_t fileOffset; // file position of block byte 0
+	uint64_t grainMask;  // grain size - 1
+	uint64_t varFillLen; // random part of a grain
+	unsigned grainShift; // grain size = 2^grainShift
+	unsigned dedupePct;  // 1..100
+
+	/* fast path is valid when every 16-byte vector starts on a word boundary of the file */
+	__device__ __forceinline__ bool canUseFast(uint64_t headLen) const
+		{ return ( (fileOffset + headLen) & 7) == 0; }
+
+	template<bool FAST>
+	__device__ __forceinline__ u64x2 vec16(uint64_t pos) const
+	{
+		uint64_t base = fileBase; // (of this vector only, as in GrainGen)
+		asm volatile("" : "+l"(base) );
+
+		const uint64_t filePos = fileOffset + pos;
+		const uint64_t q = filePos & grainMask;
+
+		if(FAST && ( (q + ELB_VEC_BYTES) <= varFillLen) )
+		{ // two whole random words of one grain
+			const uint64_t grainKey = elb_rand_dedupe_grain_key(seed, base, filePos - q,
+				grainShift, dedupePct);
+			return u64x2{elb_rand_word(grainKey, q >> 3), elb_rand_word(grainKey, (q >> 3) + 1)};
+		}
+
+		return u64x2{
+			elb_rand_dedupe_bytes8(filePos, seed, base, grainShift, varFillLen, dedupePct),
+			elb_rand_dedupe_bytes8(filePos + 8, seed, base, grainShift, varFillLen, dedupePct)};
+	}
+
+	__device__ __forceinline__ uint8_t byte(uint64_t pos) const
+	{
+		return elb_rand_dedupe_byte(fileOffset + pos, seed, fileBase, grainShift, varFillLen,
+			dedupePct);
+	}
+
+	/* key of the grain at file position grainOffset (walk_grain_span) */
+	__device__ __forceinline__ uint64_t grainKey(uint64_t grainOffset) const
+		{ return elb_rand_dedupe_grain_key(seed, fileBase, grainOffset, grainShift, dedupePct); }
 };
 
 struct NoGen {}; // the stage copies generate nothing
@@ -280,18 +336,25 @@ enum { STAGE_NONE = 0, STAGE_PUBLISH = 1, STAGE_FULL = 2 };
 enum { MODE_FILL_PATTERN = 0, MODE_VERIFY_PATTERN = 1, MODE_FILL_RANDOM = 2,
 	MODE_COPY_IN = 3 /* host slot -> device slot */, MODE_COPY_OUT = 4 /* device -> host */,
 	MODE_VERIFY_RANDOM = 5, MODE_FILL_RANDOM_GRAIN = 6, MODE_VERIFY_RANDOM_GRAIN = 7,
-	NUM_MODES = 8 };
+	MODE_FILL_DEDUPE_GRAIN = 8, MODE_VERIFY_DEDUPE_GRAIN = 9, NUM_MODES = 10 };
 
 /* the modes that compare the block with a generator and record per-block results */
 __host__ __device__ constexpr bool is_verify_mode(int mode)
 {
 	return (mode == MODE_VERIFY_PATTERN) || (mode == MODE_VERIFY_RANDOM) ||
-		(mode == MODE_VERIFY_RANDOM_GRAIN);
+		(mode == MODE_VERIFY_RANDOM_GRAIN) || (mode == MODE_VERIFY_DEDUPE_GRAIN);
 }
 
 /* the modes whose content is keyed by file position grains (descriptor blockCounter: fileKey) */
 __host__ __device__ constexpr bool is_grain_mode(int mode)
-	{ return (mode == MODE_FILL_RANDOM_GRAIN) || (mode == MODE_VERIFY_RANDOM_GRAIN); }
+{
+	return (mode == MODE_FILL_RANDOM_GRAIN) || (mode == MODE_VERIFY_RANDOM_GRAIN) ||
+		(mode == MODE_FILL_DEDUPE_GRAIN) || (mode == MODE_VERIFY_DEDUPE_GRAIN);
+}
+
+/* the grain modes of --dedupepct */
+__host__ __device__ constexpr bool is_dedupe_mode(int mode)
+	{ return (mode == MODE_FILL_DEDUPE_GRAIN) || (mode == MODE_VERIFY_DEDUPE_GRAIN); }
 
 struct KernelArgs
 {
@@ -301,6 +364,7 @@ struct KernelArgs
 	uint64_t salt;         // pattern
 	uint64_t seed;         // random (fill and verify)
 	unsigned pct;          // random (fill and verify)
+	unsigned dedupePct;    // dedupe modes: percent of pool duplicate grains (in pct's padding)
 	uint64_t grainMask;    // random grain: grain size - 1
 	uint64_t grainVarFillLen; // random grain: elb_rand_var_fill_len(grain size, pct)
 	elb_verify_result* results; // verify
@@ -568,16 +632,17 @@ __device__ __forceinline__ void walk_random_verify_span(const BlockGeom& g, cons
 }
 
 /**
- * A whole span of the grain modes. A span that lies wholly in one grain's random part is
- * RandomVarGen of the grain key, with the key advanced so that its word index of block position
- * pos is (file position mod grain size) / 8; one wholly in a grain's remainder is
+ * A whole span of the grain modes (Gen: GrainGen, or DedupeGen, which differs in the grain key
+ * only). A span that lies wholly in one grain's random part is RandomVarGen of the grain key,
+ * with the key advanced so that its word index of block position pos is (file position mod grain
+ * size) / 8; one wholly in a grain's remainder is
  * RandomRemainderGen of the grain. Both take the loads-first walk without a branch per vector, as
  * verify_random does. Spans that cross a grain or part boundary (also every span of a grain
  * smaller than the span), and spans whose file positions are not word aligned (!FAST), take the
- * bounds-checked walk with GrainGen.
+ * bounds-checked walk with the per-vector generator.
  */
-template<int MODE, bool STAGED, int GROUP, bool FAST>
-__device__ __forceinline__ void walk_grain_span(const BlockGeom& g, const GrainGen& gen,
+template<int MODE, bool STAGED, int GROUP, bool FAST, class Gen>
+__device__ __forceinline__ void walk_grain_span(const BlockGeom& g, const Gen& gen,
 	int64_t hostDelta, uint64_t spanStart, unsigned rank, VerifyAcc& acc)
 {
 	constexpr uint64_t SPAN_BYTES = (uint64_t)GROUP * ELB_VEC_BYTES * ELB_UNROLL;
@@ -587,7 +652,7 @@ __device__ __forceinline__ void walk_grain_span(const BlockGeom& g, const GrainG
 
 	if(FAST && ( (q + SPAN_BYTES - 1) <= gen.grainMask) )
 	{
-		const uint64_t grainKey = elb_rand_grain_key(gen.seed, gen.fileBase, filePos - q);
+		const uint64_t grainKey = gen.grainKey(filePos - q); // (once per span)
 
 		if( (q + SPAN_BYTES) <= gen.varFillLen)
 		{ // (vectors are 16 bytes apart: pos >> 3 advances with (q + pos - posBegin) >> 3)
@@ -658,6 +723,11 @@ __device__ __forceinline__ auto make_gen(const KernelArgs& args, const elb_block
 			elb_rand_remainder_val(blockKey)};
 	}
 	else
+	if constexpr(is_dedupe_mode(MODE) )
+		return DedupeGen{args.seed, elb_rand_file_base(desc.blockCounter /* fileKey */),
+			desc.fileOffset, args.grainMask, args.grainVarFillLen,
+			(unsigned)__popcll(args.grainMask) /* grainShift */, args.dedupePct};
+	else
 	if constexpr(is_grain_mode(MODE) )
 		return GrainGen{args.seed, elb_rand_file_base(desc.blockCounter /* fileKey */),
 			desc.fileOffset, args.grainMask, args.grainVarFillLen};
@@ -691,7 +761,8 @@ __device__ __forceinline__ int counter_slot_of()
 {
 	return is_verify_mode(MODE) ? ELB_DEVCTR_VERIFIED_BYTES :
 		( (MODE == MODE_FILL_PATTERN) || (MODE == MODE_FILL_RANDOM) ||
-		(MODE == MODE_FILL_RANDOM_GRAIN) ) ? ELB_DEVCTR_FILLED_BYTES : -1;
+		(MODE == MODE_FILL_RANDOM_GRAIN) || (MODE == MODE_FILL_DEDUPE_GRAIN) ) ?
+		ELB_DEVCTR_FILLED_BYTES : -1;
 }
 
 /**
@@ -947,8 +1018,10 @@ elb_blocks_tiled_kernel(const KernelArgs args, const uint32_t ctasPerBlock,
 
 #define ELB_WARPS (ELB_THREADS / 32)
 /* fill_random_grain would take all 80 registers that 3 CTAs per SM allow (the other modes need
-   no bound below that); 5 keep it in fill_random's occupancy, which uses 41 / 43 */
-#define ELB_WARP_MIN_CTAS_PER_SM(mode) ( (mode) == 6 /* MODE_FILL_RANDOM_GRAIN */ ? 5 : 3)
+   no bound below that); 5 keep it in fill_random's occupancy, which uses 41 / 43. So does
+   fill_dedupe_grain. */
+#define ELB_WARP_MIN_CTAS_PER_SM(mode) \
+	( ( (mode) == 6 /* MODE_FILL_RANDOM_GRAIN */ || (mode) == 8 /* MODE_FILL_DEDUPE_GRAIN */) ? 5 : 3)
 
 template<int MODE, int STAGE>
 __global__ void __launch_bounds__(ELB_THREADS, ELB_WARP_MIN_CTAS_PER_SM(MODE) )
@@ -1023,8 +1096,8 @@ struct DeviceLaunchInfo
 
 /* 32 KiB tiles per CTA of the hardware-scheduled kernel, per mode. H100: 1/1/4, 2/4/8, 4/4/16 for
    fill/verify/random were within 0.6 % of 1/2/8 (DESIGN.md). verify_random takes verify's 2; the
-   grain modes take those of their per-block counterparts, 8 and 2. */
-static const uint32_t gTilesPerCTA[NUM_MODES] = {1, 2, 8, 2, 2, 2, 8, 2};
+   grain and dedupe modes take those of their per-block counterparts, 8 and 2. */
+static const uint32_t gTilesPerCTA[NUM_MODES] = {1, 2, 8, 2, 2, 2, 8, 2, 8, 2};
 
 static DeviceLaunchInfo gDevInfo[ELB_MAX_DEVICES];
 static std::once_flag gDevInfoOnce[ELB_MAX_DEVICES];
@@ -1062,6 +1135,9 @@ static const DeviceLaunchInfo* getDeviceLaunchInfo()
 		gDevInfo[dev].ctasPerSM[MODE_FILL_RANDOM_GRAIN] = queryOccupancy<MODE_FILL_RANDOM_GRAIN>();
 		gDevInfo[dev].ctasPerSM[MODE_VERIFY_RANDOM_GRAIN] =
 			queryOccupancy<MODE_VERIFY_RANDOM_GRAIN>();
+		gDevInfo[dev].ctasPerSM[MODE_FILL_DEDUPE_GRAIN] = queryOccupancy<MODE_FILL_DEDUPE_GRAIN>();
+		gDevInfo[dev].ctasPerSM[MODE_VERIFY_DEDUPE_GRAIN] =
+			queryOccupancy<MODE_VERIFY_DEDUPE_GRAIN>();
 	});
 
 	if(gDevInfo[dev].numSMs <= 0)
@@ -1079,7 +1155,8 @@ static const char* modeName(int mode)
 {
 	static const char* names[NUM_MODES] =
 		{"fill_pattern", "verify_pattern", "fill_random", "stage_copy_in", "stage_copy_out",
-		"verify_random", "fill_random_grain", "verify_random_grain"};
+		"verify_random", "fill_random_grain", "verify_random_grain", "fill_dedupe_grain",
+		"verify_dedupe_grain"};
 	return names[mode];
 }
 
@@ -1210,6 +1287,7 @@ static void applyContent(KernelArgs& args, const elb_content& content)
 	{
 		args.grainMask = (1ULL << content.grainShift) - 1;
 		args.grainVarFillLen = elb_rand_var_fill_len(1ULL << content.grainShift, content.pct);
+		args.dedupePct = content.dedupePct;
 	}
 }
 
@@ -1227,6 +1305,10 @@ static int withContentMode(const elb_content& content, Launch launch)
 			return launch(std::integral_constant<int,
 				VERIFY ? MODE_VERIFY_RANDOM : MODE_FILL_RANDOM>() );
 		case elb_content::RANDOM_GRAIN:
+			if(content.dedupePct)
+				return launch(std::integral_constant<int,
+					VERIFY ? MODE_VERIFY_DEDUPE_GRAIN : MODE_FILL_DEDUPE_GRAIN>() );
+
 			return launch(std::integral_constant<int,
 				VERIFY ? MODE_VERIFY_RANDOM_GRAIN : MODE_FILL_RANDOM_GRAIN>() );
 		default:

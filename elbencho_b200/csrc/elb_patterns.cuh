@@ -26,6 +26,16 @@
  * elb_rand_pos_counter_hd(fileKey, g*G). A file written with --verifyrand -b G in sequential full
  * blocks is therefore the same file. A grain key costs two SplitMix64 mixes once the per-file base
  * elb_rand_file_base(fileKey) is known.
+ *
+ * --dedupepct P (with --verifyrandgrain) makes about P percent of the grains duplicates drawn from
+ * one pool of ELB_DEDUPE_POOL_GRAINS grains that is the same for every file, rank and host. For the
+ * grain at grainOffset, with ctr = splitmix64_mix(fileBase ^ grainOffset) (today's counter):
+ *   s      = splitmix64_mix(ctr + ELB_DEDUPE_TAG)
+ *   shared = ( ( (s >> 32) * 100) >> 32) < P      (a 0..99 draw without a 64-bit modulo)
+ *   key    = shared ? elb_rand_grain_key(seed, poolBase, (s & (POOL - 1)) << grainShift)
+ *                   : elb_rand_block_key(seed, ctr)              (today's grain key)
+ * with poolBase = elb_rand_file_base(ELB_DEDUPE_TAG): a shared grain holds the grain-mode content of
+ * pool slot s & (POOL - 1). --blockvarpct applies inside every grain. P = 0 is today's content.
  */
 #ifndef ELB_PATTERNS_CUH_
 #define ELB_PATTERNS_CUH_
@@ -194,6 +204,85 @@ ELB_HD uint64_t elb_rand_grain_bytes8(uint64_t filePos, uint64_t seed, uint64_t 
 	for(unsigned i = 0; i < 8; i++)
 		val |= (uint64_t)elb_rand_grain_byte(filePos + i, seed, fileBase, grainMask,
 			grainVarFillLen) << (i * 8);
+
+	return val;
+}
+
+/* --dedupepct: an odd tag that separates the share draw from the grain's other mixes and keys the
+   pool (header comment) */
+#define ELB_DEDUPE_TAG 0x5DEECE66D1B54A33ULL
+/* duplicate grains are drawn from this many pool grains (a power of two) */
+#define ELB_DEDUPE_POOL_GRAINS 4096
+
+/* the share draw of the grain at grainOffset: shared when ( ( (s >> 32) * 100) >> 32) < dedupePct,
+   and then pool slot s & (ELB_DEDUPE_POOL_GRAINS - 1) */
+ELB_HD uint64_t elb_rand_dedupe_draw(uint64_t fileBase, uint64_t grainOffset)
+{
+	return elb_splitmix64_mix(elb_splitmix64_mix(fileBase ^ grainOffset) + ELB_DEDUPE_TAG);
+}
+
+ELB_HD bool elb_rand_dedupe_is_shared(uint64_t draw, unsigned dedupePct)
+{
+	return ( ( (draw >> 32) * 100) >> 32) < dedupePct;
+}
+
+/* key of the grain at grainOffset of the file whose elb_rand_file_base() is fileBase, when
+   dedupePct percent of the grains are pool duplicates (dedupePct 0: elb_rand_grain_key) */
+ELB_HD uint64_t elb_rand_dedupe_grain_key(uint64_t seed, uint64_t fileBase, uint64_t grainOffset,
+	unsigned grainShift, unsigned dedupePct)
+{
+	const uint64_t ctr = elb_splitmix64_mix(fileBase ^ grainOffset);
+	const uint64_t draw = elb_splitmix64_mix(ctr + ELB_DEDUPE_TAG);
+
+	if(elb_rand_dedupe_is_shared(draw, dedupePct) )
+		return elb_rand_grain_key(seed, elb_rand_file_base(ELB_DEDUPE_TAG),
+			(draw & (ELB_DEDUPE_POOL_GRAINS - 1) ) << grainShift);
+
+	return elb_rand_block_key(seed, ctr);
+}
+
+/* single --dedupepct byte at file position filePos (elb_rand_grain_byte with the dedupe key) */
+ELB_HD uint8_t elb_rand_dedupe_byte(uint64_t filePos, uint64_t seed, uint64_t fileBase,
+	unsigned grainShift, uint64_t grainVarFillLen, unsigned dedupePct)
+{
+	const uint64_t grainMask = (1ULL << grainShift) - 1;
+	const uint64_t q = filePos & grainMask;
+	const uint64_t grainKey = elb_rand_dedupe_grain_key(seed, fileBase, filePos - q, grainShift,
+		dedupePct);
+
+	if(q < grainVarFillLen)
+		return elb_rand_byte(q, grainKey, grainVarFillLen, 0);
+
+	return elb_rand_byte(q, grainKey, grainVarFillLen, elb_rand_remainder_val(grainKey) );
+}
+
+/* 8 --dedupepct bytes starting at (arbitrary) file position filePos, as a little-endian u64 */
+ELB_HD uint64_t elb_rand_dedupe_bytes8(uint64_t filePos, uint64_t seed, uint64_t fileBase,
+	unsigned grainShift, uint64_t grainVarFillLen, unsigned dedupePct)
+{
+	const uint64_t grainMask = (1ULL << grainShift) - 1;
+	const uint64_t q = filePos & grainMask;
+
+	if(q <= (grainMask - 7) )
+	{ // inside one grain
+		const uint64_t grainKey = elb_rand_dedupe_grain_key(seed, fileBase, filePos - q,
+			grainShift, dedupePct);
+
+		if( !(q & 7) && ( (q + 8) <= grainVarFillLen) )
+			return elb_rand_word(grainKey, q >> 3);
+
+		return elb_rand_bytes8(q, grainKey, grainVarFillLen, elb_rand_remainder_val(grainKey) );
+	}
+
+	// crosses a grain boundary (rare path: keep its code small)
+	uint64_t val = 0;
+
+#if defined(__CUDA_ARCH__)
+	#pragma unroll 1
+#endif
+	for(unsigned i = 0; i < 8; i++)
+		val |= (uint64_t)elb_rand_dedupe_byte(filePos + i, seed, fileBase, grainShift,
+			grainVarFillLen, dedupePct) << (i * 8);
 
 	return val;
 }

@@ -1197,6 +1197,7 @@ HttpResponse Service::handlePreparePhase(const HttpRequest& request)
 		args.blockVarianceSeed = recvTree.getU64("b200_blockvarseed", 0);
 		args.randomVerifySeed = recvTree.getU64("b200_verifyrand", 0);
 		args.randomVerifyGrain = recvTree.getU64("b200_verifyrandgrain", 0);
+		args.dedupePercent = recvTree.getU64("b200_dedupepct", 0);
 		args.pipelineBatchBlocks = recvTree.getU64("b200_batchblocks", 0);
 		args.pipelineNumBatches = recvTree.getU64("b200_numbatches", 0);
 		args.serializeBufferedWrites = recvTree.getBool("b200_writegate", false);
@@ -1909,6 +1910,7 @@ static JsonTree progArgsToServiceTree(const ProgArgs& args, size_t serviceRank, 
 	tree.put("b200_blockvarseed", args.blockVarianceSeed);
 	tree.put("b200_verifyrand", args.randomVerifySeed);
 	tree.put("b200_verifyrandgrain", args.randomVerifyGrain);
+	tree.put("b200_dedupepct", args.dedupePercent);
 	tree.put("b200_batchblocks", args.pipelineBatchBlocks);
 	tree.put("b200_numbatches", args.pipelineNumBatches);
 	tree.putBool("b200_writegate", args.serializeBufferedWrites);

@@ -827,12 +827,14 @@ void Worker::allocRings()
 	/* write: pattern fill if salt != 0, else random refill if blockvarpct, else nothing
 	   (initPhaseFunctionPointers, LocalWorker.cpp:1249-1265); read: verify if salt != 0 (:1311).
 	   --verifyrand: random refill and its verify, keyed by the seed and the block positions;
-	   --verifyrandgrain: those of the grain mode, keyed by the seed and the file positions */
+	   --verifyrandgrain: those of the grain mode, keyed by the seed and the file positions, with
+	   --dedupepct percent of the grains keyed as pool duplicates */
 	const uint64_t salt = cfg.integrityCheckSalt;
 	const unsigned pct = cfg.blockVariancePercent;
 	const elb_content writeContent =
 		cfg.useRandomVerifyGrain() ?
-			elb_content{elb_content::RANDOM_GRAIN, salt, pct, cfg.randomVerifyGrainShift} :
+			elb_content{elb_content::RANDOM_GRAIN, salt, pct, cfg.randomVerifyGrainShift,
+				cfg.dedupePercent} :
 		cfg.useRandomVerify() ? elb_content{elb_content::RANDOM, salt, pct} :
 		salt ? elb_content{elb_content::PATTERN, salt} :
 		pct ? elb_content{elb_content::RANDOM, blockVarianceSeed, pct} : elb_content{};

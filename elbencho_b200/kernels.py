@@ -206,6 +206,76 @@ def verify_random_grain_staged(descs_ptr, num_descs, grain_shift, pct, seed, hos
            "elb_verify_random_grain_staged")
 
 
+# ---- --dedupepct: the grain-mode content with dedupe_pct percent of the grains keyed as
+# duplicates of the grains of one pool shared by all files. Arguments as for the grain forms.
+
+def fill_dedupe_grain(dev_ptr, length, file_offset, grain_shift, pct, dedupe_pct, seed, file_key,
+                      stream=0):
+    """K7: the --dedupepct content of file bytes [file_offset, file_offset + length)"""
+    _check(_native.load().elb_fill_dedupe_grain(dev_ptr, length, file_offset, grain_shift, pct,
+                                                dedupe_pct, seed, file_key, stream),
+           "elb_fill_dedupe_grain")
+
+
+def verify_dedupe_grain(dev_ptr, length, file_offset, grain_shift, pct, dedupe_pct, seed,
+                        file_key, dev_result_ptr, stream=0):
+    """K8: compare with the K7 content; dev_result_ptr as for verify_random"""
+    _check(_native.load().elb_verify_dedupe_grain(dev_ptr, length, file_offset, grain_shift, pct,
+                                                  dedupe_pct, seed, file_key, dev_result_ptr,
+                                                  stream),
+           "elb_verify_dedupe_grain")
+
+
+def fill_dedupe_grain_batch(dev_descs_ptr, num_descs, grain_shift, pct, dedupe_pct, seed,
+                            dev_counters_ptr=0, stream=0, total_bytes=0, max_block_len=0):
+    _check(_native.load().elb_fill_dedupe_grain_batch_sized(dev_descs_ptr, num_descs, grain_shift,
+                                                            pct, dedupe_pct, seed,
+                                                            dev_counters_ptr or None,
+                                                            total_bytes, max_block_len, stream),
+           "elb_fill_dedupe_grain_batch")
+
+
+def verify_dedupe_grain_batch(dev_descs_ptr, num_descs, grain_shift, pct, dedupe_pct, seed,
+                              dev_results_ptr, dev_counters_ptr=0, stream=0, total_bytes=0,
+                              max_block_len=0):
+    _check(_native.load().elb_verify_dedupe_grain_batch_sized(dev_descs_ptr, num_descs,
+                                                              grain_shift, pct, dedupe_pct, seed,
+                                                              dev_results_ptr,
+                                                              dev_counters_ptr or None,
+                                                              total_bytes, max_block_len, stream),
+           "elb_verify_dedupe_grain_batch")
+
+
+def fill_dedupe_grain_staged(descs_ptr, num_descs, grain_shift, pct, dedupe_pct, seed, host_delta,
+                             dev_counters_ptr=0, stream=0, total_bytes=0, max_block_len=0):
+    """K7 + stage-out, with the conventions of fill_pattern_staged"""
+    _check(_native.load().elb_fill_dedupe_grain_staged(descs_ptr, num_descs, grain_shift, pct,
+                                                       dedupe_pct, seed, host_delta,
+                                                       dev_counters_ptr or None, total_bytes,
+                                                       max_block_len, stream),
+           "elb_fill_dedupe_grain_staged")
+
+
+def verify_dedupe_grain_staged(descs_ptr, num_descs, grain_shift, pct, dedupe_pct, seed,
+                               host_delta, dev_results_ptr, host_results_ptr=0, dev_ticket_ptr=0,
+                               dev_counters_ptr=0, stream=0, total_bytes=0, max_block_len=0):
+    """stage-in + K8, with the conventions of verify_pattern_staged"""
+    _check(_native.load().elb_verify_dedupe_grain_staged(descs_ptr, num_descs, grain_shift, pct,
+                                                         dedupe_pct, seed, host_delta,
+                                                         dev_results_ptr,
+                                                         host_results_ptr or None,
+                                                         dev_ticket_ptr or None,
+                                                         dev_counters_ptr or None, total_bytes,
+                                                         max_block_len, stream),
+           "elb_verify_dedupe_grain_staged")
+
+
+def rand_grain_content_key(seed, file_key, grain_offset, grain_shift, dedupe_pct):
+    """the key of a grain's random fill (elb_rand_grain_content_key)"""
+    return int(_native.load().elb_rand_grain_content_key(seed, file_key, grain_offset, grain_shift,
+                                                         dedupe_pct))
+
+
 def stage_copy(descs_ptr, num_descs, host_to_device, host_delta, stream=0, total_bytes=0,
                max_block_len=0):
     _check(_native.load().elb_stage_copy(descs_ptr, num_descs, int(bool(host_to_device)),

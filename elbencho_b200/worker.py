@@ -97,6 +97,7 @@ class WorkerConfig:
     integrity_check_salt: int = 0     # --verify salt, or --verifyrand seed with VERIFY_RANDOM
     integrity_check_kind: int = 0     # elb_verify_kind: 0 pattern (--verify), 1 random (--verifyrand)
     verify_random_grain: int = 0      # --verifyrandgrain bytes (a power of two; 0 = per block)
+    dedupe_percent: int = 0           # --dedupepct (0..100, with verify_random_grain)
     do_direct_verify: bool = False    # --verifydirect
     do_read_inline: bool = False      # --readinline
     block_variance_percent: int = 0   # --blockvarpct
@@ -154,6 +155,7 @@ class WorkerConfig:
         # (not a power of two: a shift that the library rejects)
         cfg.randomVerifyGrainShift = (0 if not grain else grain.bit_length() - 1
                                       if not grain & (grain - 1) else -1)
+        cfg.dedupePercent = self.dedupe_percent
         cfg.doDirectVerify = int(self.do_direct_verify)
         cfg.doReadInline = int(self.do_read_inline)
         cfg.blockVariancePercent = self.block_variance_percent

@@ -234,6 +234,34 @@ int elb_verify_random_grain_staged(const elb_block_desc* descs, uint32_t numDesc
 	elb_verify_result* devResults, elb_verify_result* hostResults, unsigned* devDoneTicket,
 	uint64_t* devCounters, uint64_t totalBytes, uint64_t maxBlockLen, void* stream);
 
+/* K7 / K8, --dedupepct: the grain-mode content of K5 / K6 in which dedupePct percent (0..100) of
+ * the grains are duplicates of the grains of one pool of ELB_DEDUPE_POOL_GRAINS (4096) grains that
+ * is the same for every file (elb_patterns.cuh). dedupePct 0 is K5 / K6's content. The forms and
+ * their arguments mirror those of K5 / K6. */
+int elb_fill_dedupe_grain(void* devPtr, uint64_t len, uint64_t fileOffset, unsigned grainShift,
+	unsigned pct, unsigned dedupePct, uint64_t seed, uint64_t fileKey, void* stream);
+int elb_verify_dedupe_grain(const void* devPtr, uint64_t len, uint64_t fileOffset,
+	unsigned grainShift, unsigned pct, unsigned dedupePct, uint64_t seed, uint64_t fileKey,
+	elb_verify_result* devOut, void* stream);
+int elb_fill_dedupe_grain_batch_sized(const elb_block_desc* descs, uint32_t numDescs,
+	unsigned grainShift, unsigned pct, unsigned dedupePct, uint64_t seed, uint64_t* devCounters,
+	uint64_t totalBytes, uint64_t maxBlockLen, void* stream);
+int elb_verify_dedupe_grain_batch_sized(const elb_block_desc* descs, uint32_t numDescs,
+	unsigned grainShift, unsigned pct, unsigned dedupePct, uint64_t seed,
+	elb_verify_result* devResults, uint64_t* devCounters, uint64_t totalBytes,
+	uint64_t maxBlockLen, void* stream);
+int elb_fill_dedupe_grain_staged(const elb_block_desc* descs, uint32_t numDescs,
+	unsigned grainShift, unsigned pct, unsigned dedupePct, uint64_t seed, int64_t hostDelta,
+	uint64_t* devCounters, uint64_t totalBytes, uint64_t maxBlockLen, void* stream);
+int elb_verify_dedupe_grain_staged(const elb_block_desc* descs, uint32_t numDescs,
+	unsigned grainShift, unsigned pct, unsigned dedupePct, uint64_t seed, int64_t hostDelta,
+	elb_verify_result* devResults, elb_verify_result* hostResults, unsigned* devDoneTicket,
+	uint64_t* devCounters, uint64_t totalBytes, uint64_t maxBlockLen, void* stream);
+/* key of the grain at grainOffset (a multiple of 2^grainShift) of the file with fileKey: the
+ * blockKey whose random fill the grain holds. dedupePct 0 gives the --verifyrandgrain key. */
+uint64_t elb_rand_grain_content_key(uint64_t seed, uint64_t fileKey, uint64_t grainOffset,
+	unsigned grainShift, unsigned dedupePct);
+
 int elb_stage_copy(const elb_block_desc* descs, uint32_t numDescs, int hostToDevice,
 	int64_t hostDelta, uint64_t totalBytes, uint64_t maxBlockLen, void* stream);
 /* devResults[0..numDescs) <- {0, ~0} */
@@ -309,6 +337,10 @@ typedef struct elb_cfg
 
 	/* --rwmixpct */
 	uint32_t rwMixReadPercent;
+	/* --dedupepct (with randomVerifyGrainShift): percent of the grains, 0..100, that are
+	 * duplicates of the grains of one pool shared by all files (elb_rand_grain_content_key). It
+	 * takes the 4 bytes of padding in front of gpuIDs: no other field moves. */
+	uint32_t dedupePercent;
 
 	/* --gpuids / --cufile / --gds / --gdsbufreg / --cuhostbufreg */
 	const int32_t* gpuIDs;
