@@ -26,6 +26,17 @@ class BlockDesc(ctypes.Structure):
                 ("blockCounter", c_u64)]
 
 
+class SectorDamage(ctypes.Structure):
+    _fields_ = [("numDiffBytes", c_u32), ("firstDiff", c_u32), ("lastDiff", c_u32),
+                ("reserved", c_u32)]
+
+
+# elb_content_kind
+CONTENT_PATTERN = 1
+CONTENT_RANDOM = 2
+CONTENT_RANDOM_GRAIN = 3
+
+
 class Cfg(ctypes.Structure):
     _fields_ = [
         ("structSize", c_u32),
@@ -73,6 +84,7 @@ class Cfg(ctypes.Structure):
         ("serializeBufferedWrites", c_i32),
         ("numRWMixReadThreads", c_u32),
         ("randOffsetAlgo", ctypes.c_int32),
+        ("verifyDamageReport", ctypes.c_int32),
         ("limitReadBps", c_u64),
         ("limitWriteBps", c_u64),
         ("doInfiniteIOLoop", ctypes.c_int32),
@@ -230,6 +242,8 @@ SIGNATURES = {
     "elb_rand_grain_content_key": (c_u64, [c_u64, c_u64, c_u64, ctypes.c_uint, ctypes.c_uint]),
     "elb_rand_pos_counter": (c_u64, [c_u64, c_u64]),
     "elb_rand_dir_file_key": (c_u64, [c_u64, c_u64, c_u64]),
+    "elb_damage_map": (ctypes.c_int, [_VP, c_u32, ctypes.c_int, c_u64, ctypes.c_uint,
+                                      ctypes.c_uint, ctypes.c_uint, _VP, c_u64, _VP]),
     "elb_stage_copy": (ctypes.c_int, [_VP, c_u32, ctypes.c_int, ctypes.c_int64, c_u64, c_u64,
                                       _VP]),
     "elb_verify_results_init": (ctypes.c_int, [_VP, c_u32, _VP]),
@@ -292,6 +306,7 @@ SIGNATURES = {
     "elb_mgr_expected_totals": (ctypes.c_int, [_VP, ctypes.c_int, ctypes.POINTER(c_u64),
                                                 ctypes.POINTER(c_u64)]),
     "elb_mgr_interrupt": (ctypes.c_int, [_VP]),
+    "elb_mgr_verify_report": (ctypes.c_int64, [_VP, ctypes.c_char_p, c_u64]),
     "elb_mgr_num_workers": (c_u32, [_VP]),
     "elb_mgr_worker": (_VP, [_VP, c_u32]),
     "elb_mgr_last_error": (ctypes.c_char_p, [_VP]),

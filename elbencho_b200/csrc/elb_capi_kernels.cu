@@ -368,6 +368,41 @@ uint64_t elb_rand_grain_content_key(uint64_t seed, uint64_t fileKey, uint64_t gr
 		dedupePct);
 }
 
+int elb_damage_map(const elb_block_desc* descs, uint32_t numDescs, int contentKind, uint64_t key,
+	unsigned pct, unsigned grainShift, unsigned dedupePct, elb_sector_damage* devSectors,
+	uint64_t sectorsPerDesc, void* stream)
+{
+	static_assert( ( (int)ELB_CONTENT_PATTERN == (int)elb_content::PATTERN) &&
+		( (int)ELB_CONTENT_RANDOM == (int)elb_content::RANDOM) &&
+		( (int)ELB_CONTENT_RANDOM_GRAIN == (int)elb_content::RANDOM_GRAIN), "content kinds differ");
+
+	if( (contentKind < ELB_CONTENT_PATTERN) || (contentKind > ELB_CONTENT_RANDOM_GRAIN) )
+	{
+		elb_set_last_error("elb_damage_map: unknown content kind: " + std::to_string(contentKind) );
+		return -1;
+	}
+
+	const elb_content content{(elb_content::Kind)contentKind, key, pct, grainShift, dedupePct};
+
+	if(checkContent(content, ELB_RANDALGO_SPLITMIX64) )
+		return -1;
+
+	if(numDescs && (!descs || !devSectors) )
+	{
+		elb_set_last_error("elb_damage_map: NULL descriptor or sector array");
+		return -1;
+	}
+
+	if(elb_launch_damage_map(content, descs, numDescs, devSectors, sectorsPerDesc,
+		(cudaStream_t)stream) )
+	{
+		elb_set_last_error(std::string("elb_") + elb_last_error() );
+		return -1;
+	}
+
+	return 0;
+}
+
 int elb_stage_copy(const elb_block_desc* descs, uint32_t numDescs, int hostToDevice,
 	int64_t hostDelta, uint64_t totalBytes, uint64_t maxBlockLen, void* stream)
 {

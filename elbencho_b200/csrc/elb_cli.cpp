@@ -94,6 +94,12 @@ static const OptDef optDefs[] =
 		"the same for all files, so that storage which deduplicates finds them. Checked on reads "
 		"like all grains. Reads must use the write's value. Requires --verifyrandgrain. "
 		"(Default: 0) [b200]"},
+	{"verifyreport", 0, Opt_STR, "Path of a verify report file: a verifying phase does not stop at "
+		"the first bad block but reads on, maps the damaged 512-byte sectors of every bad block on "
+		"the GPU and appends one section to this file (truncated at start): \"# phase READ|WRITE\", "
+		"then one tab-separated line \"path offset length differing_bytes\" per damaged extent. "
+		"The phase still fails at its end with the error of the first bad block. Requires --verify "
+		"or --verifyrand. [b200]"},
 	{"rwmixpct", 0, Opt_U64, "Percentage of blocks that should be read in a write phase."},
 	{"rwmixthr", 0, Opt_U64, "Number of threads that should do reads in a write phase."},
 	// GPU
@@ -593,6 +599,7 @@ ProgArgs::ProgArgs(int argc, char** argv)
 	num("verifyrand", randomVerifySeed);
 	num("verifyrandgrain", randomVerifyGrain);
 	num("dedupepct", dedupePercent);
+	str("verifyreport", verifyReportPath);
 	hasUserSetRWMixPercent = num("rwmixpct", rwMixReadPercent);
 	hasUserSetRWMixReadThreads = num("rwmixthr", numRWMixReadThreads);
 	num("rwmixthrpct", rwMixThreadsReadPercent);
@@ -977,6 +984,12 @@ void ProgArgs::checkArgs()
 	if(dedupePercent > 100)
 		throw ProgError("Option \"--dedupepct\" must be in range 0..100");
 
+	if(!verifyReportPath.empty() && !integrityCheckSalt && !randomVerifySeed)
+		throw ProgError("Option \"--verifyreport\" requires \"--verify\" or \"--verifyrand\"");
+
+	if(!verifyReportPath.empty() && !hosts.empty() )
+		throw ProgError("Option \"--verifyreport\" cannot be used together with \"--hosts\"");
+
 	if(doDirectVerify && ( (!integrityCheckSalt && !randomVerifySeed) || !runCreateFilesPhase) )
 		throw ProgError("Direct verification requires --verify and --write"); // :1426-1428
 
@@ -1068,6 +1081,7 @@ void ProgArgs::toABIConfig(ABIConfig& out) const
 	cfg.ignoreDelErrors = ignoreDelErrors;
 	cfg.runAsService = runAsService;
 	cfg.verifyCollectAll = 0;
+	cfg.verifyDamageReport = !verifyReportPath.empty();
 	cfg.serializeBufferedWrites = neverSerializeBufferedWrites ? ELB_WRITEGATE_OFF :
 		(serializeBufferedWrites ? ELB_WRITEGATE_ON : ELB_WRITEGATE_AUTO);
 	cfg.noGPUNumaBinding = noGPUNumaBinding;

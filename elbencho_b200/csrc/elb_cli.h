@@ -85,6 +85,7 @@ class ProgArgs
 		uint64_t randomVerifySeed{0}; // --verifyrand
 		uint64_t randomVerifyGrain{0}; // --verifyrandgrain (bytes, 0 = per block)
 		uint64_t dedupePercent{0}; // --dedupepct
+		std::string verifyReportPath; // --verifyreport
 		uint64_t rwMixReadPercent{0};
 		bool hasUserSetRWMixPercent{false};
 		uint64_t numRWMixReadThreads{0};

@@ -101,6 +101,7 @@ Config Config::fromABI(const elb_cfg* cfg)
 	c.ignoreDelErrors = cfg->ignoreDelErrors;
 	c.runAsService = cfg->runAsService;
 	c.verifyCollectAll = cfg->verifyCollectAll;
+	c.verifyDamageReport = (cfg->verifyDamageReport != 0);
 	c.serializeBufferedWrites = cfg->serializeBufferedWrites;
 	c.numRWMixReadThreads = std::min(cfg->numRWMixReadThreads, cfg->numThreads); // :1088
 	c.treeFilePath = cfg->treeFilePath ? cfg->treeFilePath : "";
@@ -190,6 +191,10 @@ Config Config::fromABI(const elb_cfg* cfg)
 	if(c.dedupePercent && !c.useRandomVerifyGrain() )
 		throw WorkerError("A dedupe percentage (--dedupepct) requires a random verify grain "
 			"(--verifyrandgrain).");
+
+	if(c.verifyDamageReport && !c.integrityCheckSalt)
+		throw WorkerError("A verify report (--verifyreport) requires data verification (--verify "
+			"or --verifyrand).");
 
 	if(c.integrityCheckSalt && c.rwMixReadPercent) // :1414
 		throw WorkerError("Integrity check cannot be used together with rwmixpct.");

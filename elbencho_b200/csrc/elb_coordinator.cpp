@@ -99,6 +99,7 @@ class Coordinator
 			const elb_liveops oldLiveOps[2], uint64_t intervalUSec, size_t numWorkersDone,
 			uint64_t elapsedSec);
 		void printPhaseResultsEverywhere(int benchPhase, const std::string& isoStartDate);
+		void writeVerifyReportSection(int benchPhase);
 		void printDryRunInfo();
 };
 
@@ -405,6 +406,29 @@ void Coordinator::printPhaseResultsEverywhere(int benchPhase, const std::string&
 	}
 }
 
+/* --verifyreport: after each phase that verified data (a read, or a write with --verifydirect),
+ * its section of the report file and one console line */
+void Coordinator::writeVerifyReportSection(int benchPhase)
+{
+	if(progArgs.verifyReportPath.empty() ||
+		!( (benchPhase == ELB_PHASE_READFILES) ||
+		( (benchPhase == ELB_PHASE_CREATEFILES) && progArgs.doDirectVerify) ) )
+		return;
+
+	const Manager::VerifyReport report = manager->getVerifyReport();
+	std::ofstream fileStream(progArgs.verifyReportPath, std::ofstream::app);
+
+	fileStream << "# phase " << ( (benchPhase == ELB_PHASE_READFILES) ? "READ" : "WRITE") << "\n" <<
+		report.lines << std::flush;
+
+	if(!fileStream)
+		throw ProgError("Writing verify report file failed: " + progArgs.verifyReportPath);
+
+	std::cout << "Verify report: " << report.numExtents << " damaged extents, " <<
+		report.numBytes << " differing bytes in " << report.numFiles << " files: " <<
+		progArgs.verifyReportPath << std::endl;
+}
+
 /* Coordinator::runBenchmarkPhase (:248-272) + Statistics live loop (:1284-1345) */
 void Coordinator::runBenchmarkPhase(int benchPhase)
 {
@@ -518,6 +542,8 @@ void Coordinator::runBenchmarkPhase(int benchPhase)
 
 	if(waitRes < 0)
 	{
+		writeVerifyReportSection(benchPhase);
+
 		std::string errMsg;
 		{
 			std::unique_lock<std::mutex> lock(manager->shared.mutex);
@@ -531,7 +557,10 @@ void Coordinator::runBenchmarkPhase(int benchPhase)
 	}
 
 	if( (benchPhase != ELB_PHASE_SYNC) && (benchPhase != ELB_PHASE_DROPCACHES) )
+	{
 		printPhaseResultsEverywhere(benchPhase, isoStartDate);
+		writeVerifyReportSection(benchPhase);
+	}
 	else
 	{ // (sync and dropcache phases print only their elapsed time)
 		elb_phase_results res;
@@ -672,6 +701,10 @@ int Coordinator::main() // Coordinator.cpp:31-142
 		sigAction.sa_handler = interruptSignalHandler;
 		sigaction(SIGINT, &sigAction, NULL);
 		sigaction(SIGTERM, &sigAction, NULL);
+
+		if(!progArgs.verifyReportPath.empty() &&
+			!std::ofstream(progArgs.verifyReportPath, std::ofstream::trunc) )
+			throw ProgError("Unable to create verify report file: " + progArgs.verifyReportPath);
 
 		waitForUserDefinedStartTime(progArgs);
 

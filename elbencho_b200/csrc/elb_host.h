@@ -1000,6 +1000,7 @@ struct Config
 	bool ignoreDelErrors{false};
 	bool runAsService{false};
 	bool verifyCollectAll{false};
+	bool verifyDamageReport{false}; // --verifyreport
 	int serializeBufferedWrites{ELB_WRITEGATE_AUTO};
 	int stagingEngine{ELB_STAGING_AUTO};
 	bool noGPUNumaBinding{false};

@@ -86,6 +86,11 @@ int elb_launch_verify_init(elb_verify_result* devResults, uint32_t numDescs,
 	cudaStream_t stream);
 int elb_launch_stage_copy(const elb_block_desc* descs, uint32_t numDescs, bool hostToDevice,
 	int64_t hostDelta, uint64_t totalBytesHint, uint64_t maxBlockLenHint, cudaStream_t stream);
+/* the damage map of blocks known to be bad (elb_damage_map; descs must be host- and
+   device-readable: the host checks that each fits sectorsPerDesc records first) */
+int elb_launch_damage_map(const elb_content& content, const elb_block_desc* descs,
+	uint32_t numDescs, elb_sector_damage* devSectors, uint64_t sectorsPerDesc,
+	cudaStream_t stream);
 int elb_kernels_warmup();
 uint64_t elb_get_num_kernel_launches();
 

@@ -9,6 +9,8 @@
  *      K3's content per grain of the file, keyed by the grain's file position)
  *   K7 fill_dedupe_grain, K8 verify_dedupe_grain (no reference counterpart: --dedupepct, K5 / K6
  *      with the dedupe grain key, elb_patterns.cuh)
+ *   damage_map (no reference counterpart: --verifyreport, where the bytes of blocks known to be
+ *      bad differ, per 512-byte file sector; off the clean path, see its section below)
  *
  * All eight are HBM-bound byte/integer kernels (K1/K3/K5/K7: 1 byte written per payload byte,
  * K2/K4/K6/K8: 1 byte read per payload byte), so the design follows the streaming rules: 16-byte (128-bit) vector
@@ -42,6 +44,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
 #include <atomic>
 #include <mutex>
 #include <string>
@@ -1044,6 +1047,98 @@ __global__ void elb_verify_init_kernel(elb_verify_result* results, uint32_t numD
 	}
 }
 
+/* ---- damage map (--verifyreport) ------------------------------------------------------------
+ *
+ * Runs only on blocks whose verify result showed a mismatch, so it is off the clean path. Every
+ * 512-byte file sector that a block touches is owned by one warp: it compares the sector's bytes
+ * of the device slot with the verify mode's generator (make_gen), reduces count, first and last
+ * differing byte with redux.sync, and lane 0 stores the sector's record. One writer per record:
+ * no atomics and no init launch. Where the slot lies sector-aligned (device address == file
+ * offset mod 512, 16-byte aligned), a sector wholly inside the block is one 16-byte vector per
+ * lane, the same warp access as the verify kernels; the sectors at a block's head and tail and
+ * all sectors of other slots (unaligned file offsets of --norandalign) go byte by byte, each lane
+ * taking every 32nd byte. */
+
+#define ELB_SECTOR_BYTES 512
+#define ELB_MAP_SECTORS_PER_WARP 4 /* sectors a warp takes per CTA of the grid */
+
+/* index of the last differing byte (0..7) of two unequal u64 */
+__device__ __forceinline__ unsigned last_diff_byte64(uint64_t x, uint64_t y)
+{
+	return (unsigned)(63 - __clzll( (long long)(x ^ y) ) ) >> 3;
+}
+
+template<int MODE>
+__global__ void __launch_bounds__(ELB_THREADS)
+elb_damage_map_kernel(const KernelArgs args, elb_sector_damage* sectors, uint64_t sectorsPerDesc,
+	uint32_t ctasPerDesc)
+{
+	const uint32_t descIdx = blockIdx.x / ctasPerDesc;
+	const uint32_t ctaInDesc = blockIdx.x - descIdx * ctasPerDesc;
+	const elb_block_desc desc = args.descs[descIdx];
+
+	if(!desc.len)
+		return;
+
+	const uint64_t firstSector = desc.fileOffset / ELB_SECTOR_BYTES;
+	const uint64_t numSectors = (desc.fileOffset + desc.len - 1) / ELB_SECTOR_BYTES - firstSector + 1;
+	const uint8_t* ptr = (const uint8_t*)desc.devPtr;
+	const bool sectorAligned = !( ( (uint64_t)(uintptr_t)ptr - desc.fileOffset) %
+		ELB_SECTOR_BYTES) && !( (uintptr_t)ptr % ELB_VEC_BYTES);
+	const auto gen = make_gen<MODE>(args, desc);
+	const unsigned lane = threadIdx.x & 31;
+	elb_sector_damage* records = sectors + (uint64_t)descIdx * sectorsPerDesc;
+
+	for(uint64_t s = (uint64_t)ctaInDesc * ELB_WARPS + (threadIdx.x >> 5); s < numSectors;
+		s += (uint64_t)ctasPerDesc * ELB_WARPS)
+	{ // (uniform per warp) block positions [begin, end) of sector s
+		const uint64_t sectorFilePos = (firstSector + s) * ELB_SECTOR_BYTES;
+		const uint64_t begin = s ? (sectorFilePos - desc.fileOffset) : 0;
+		const uint64_t end = (s + 1 < numSectors) ?
+			(sectorFilePos + ELB_SECTOR_BYTES - desc.fileOffset) : desc.len;
+		unsigned numBad = 0, first = ~0u, last = 0; // first / last: positions in the sector
+
+		if(sectorAligned && (end - begin == ELB_SECTOR_BYTES) )
+		{
+			const uint64_t pos = begin + lane * ELB_VEC_BYTES;
+			const u64x2 got = ld_nc_na_128(ptr + pos);
+			const u64x2 exp = gen.template vec16<true>(pos);
+			const unsigned inSector = lane * ELB_VEC_BYTES;
+
+			numBad = diff_bytes64(got.a, exp.a) + diff_bytes64(got.b, exp.b);
+
+			if(got.a != exp.a)
+				first = inSector + first_diff_byte64(got.a, exp.a);
+			else
+			if(got.b != exp.b)
+				first = inSector + 8 + first_diff_byte64(got.b, exp.b);
+
+			if(got.b != exp.b)
+				last = inSector + 8 + last_diff_byte64(got.b, exp.b);
+			else
+			if(got.a != exp.a)
+				last = inSector + last_diff_byte64(got.a, exp.a);
+		}
+		else
+			for(uint64_t pos = begin + lane; pos < end; pos += 32)
+				if(ptr[pos] != gen.byte(pos) )
+				{
+					const unsigned inSector = (unsigned)( (desc.fileOffset + pos) % ELB_SECTOR_BYTES);
+
+					numBad++;
+					first = min(first, inSector);
+					last = max(last, inSector);
+				}
+
+		numBad = __reduce_add_sync(0xffffffffu, numBad);
+		first = __reduce_min_sync(0xffffffffu, first);
+		last = __reduce_max_sync(0xffffffffu, last);
+
+		if(!lane)
+			records[s] = elb_sector_damage{numBad, numBad ? first : 0, last, 0};
+	}
+}
+
 /* ---- host side launchers ------------------------------------------------------------------ */
 
 static std::atomic<uint64_t> gNumKernelLaunches{0};
@@ -1386,6 +1481,56 @@ int elb_launch_stage_copy(const elb_block_desc* descs, uint32_t numDescs, bool h
 	return hostToDevice ?
 		launchBlocksKernel<MODE_COPY_IN>(args, totalBytesHint, maxBlockLenHint, stream) :
 		launchBlocksKernel<MODE_COPY_OUT>(args, totalBytesHint, maxBlockLenHint, stream);
+}
+
+int elb_launch_damage_map(const elb_content& content, const elb_block_desc* descs,
+	uint32_t numDescs, elb_sector_damage* devSectors, uint64_t sectorsPerDesc,
+	cudaStream_t stream)
+{
+	uint64_t maxSectors = 0;
+
+	for(uint32_t i = 0; i < numDescs; i++)
+	{ // (descs are host-readable)
+		const uint64_t numSectors = !descs[i].len ? 0 : ( (descs[i].fileOffset + descs[i].len - 1) /
+			ELB_SECTOR_BYTES - descs[i].fileOffset / ELB_SECTOR_BYTES + 1);
+
+		if(numSectors > sectorsPerDesc)
+		{
+			elb_set_last_error("damage_map: descriptor " + std::to_string(i) + " touches " +
+				std::to_string(numSectors) + " sectors, more than sectorsPerDesc (" +
+				std::to_string(sectorsPerDesc) + ")");
+			return -1;
+		}
+
+		maxSectors = std::max(maxSectors, numSectors);
+	}
+
+	if(!maxSectors)
+		return 0;
+
+	const uint64_t ctasPerDesc = (maxSectors + ELB_WARPS * ELB_MAP_SECTORS_PER_WARP - 1) /
+		(ELB_WARPS * ELB_MAP_SECTORS_PER_WARP);
+
+	if(ctasPerDesc * numDescs > 0x7fffffffULL)
+	{
+		elb_set_last_error("damage_map: too many sectors for one launch");
+		return -1;
+	}
+
+	KernelArgs args{};
+	args.descs = descs;
+	args.numDescs = numDescs;
+	applyContent(args, content);
+
+	return withContentMode<true>(content, [&](auto mode)
+	{
+		elb_damage_map_kernel<decltype(mode)::value>
+			<<<(unsigned)(ctasPerDesc * numDescs), ELB_THREADS, 0, stream>>>(args, devSectors,
+			sectorsPerDesc, (uint32_t)ctasPerDesc);
+		gNumKernelLaunches.fetch_add(1, std::memory_order_relaxed);
+
+		return checkLaunch("damage_map");
+	});
 }
 
 /* query launch geometry of the current device now (so that no attribute/occupancy query happens

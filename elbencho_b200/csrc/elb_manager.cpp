@@ -4,6 +4,7 @@
  */
 #include <errno.h>
 #include <algorithm>
+#include <map>
 #include <fcntl.h>
 #include <string.h>
 #include <sys/stat.h>
@@ -414,6 +415,103 @@ void Manager::interruptAndNotifyWorkers() // WorkerManager.cpp:75-90
 	shared.currentBenchPhase = ELB_PHASE_TERMINATE;
 	shared.currentBenchSeq++;
 	shared.condition.notify_all();
+}
+
+/**
+ * --verifyreport: the runs of all workers, merged into extents. Sorted by path and first sector, a
+ * run that starts inside or right after the extent so far extends it. A sector's count is kept per
+ * part, a part being where the block that read it starts in the sector (0 when it starts before):
+ * reads of the same part (a sector read more than once) count once with the largest count, parts
+ * of different blocks (a sector split between two blocks) add up. The extent's bounds are the
+ * first and the last differing byte of all runs.
+ */
+Manager::VerifyReport Manager::getVerifyReport()
+{
+	std::vector<const DamageRun*> runs;
+	uint64_t numRunsDropped = 0, numBytesDropped = 0;
+
+	for(const std::unique_ptr<Worker>& worker : workers)
+	{
+		for(const DamageRun& run : worker->getDamageRuns() )
+			runs.push_back(&run);
+
+		numRunsDropped += worker->getNumDamageRunsDropped();
+		numBytesDropped += worker->getNumDamageBytesDropped();
+	}
+
+	std::sort(runs.begin(), runs.end(), [](const DamageRun* a, const DamageRun* b)
+		{ return (a->path != b->path) ? (a->path < b->path) : (a->firstSector < b->firstSector); });
+
+	VerifyReport report;
+	std::string lastExtentPath;
+	DamageRun extent; // sectorBytes: the parts that start at 0
+	std::map<uint64_t, std::map<uint16_t, uint16_t> > midParts; // sector -> part start -> count
+
+	auto addExtent = [&]()
+	{
+		uint64_t numBytes = 0;
+
+		for(uint16_t sectorBytes : extent.sectorBytes)
+			numBytes += sectorBytes;
+
+		for(const auto& sectorParts : midParts)
+			for(const auto& part : sectorParts.second)
+				numBytes += part.second;
+
+		report.lines += extent.path + "\t" + std::to_string(extent.firstByte) + "\t" +
+			std::to_string(extent.lastByte - extent.firstByte + 1) + "\t" +
+			std::to_string(numBytes) + "\n";
+
+		if(!report.numExtents || (extent.path != lastExtentPath) )
+			report.numFiles++;
+
+		report.numExtents++;
+		report.numBytes += numBytes;
+		lastExtentPath = extent.path;
+	};
+
+	for(size_t i = 0; i < runs.size(); i++)
+	{
+		const DamageRun& run = *runs[i];
+		const bool extends = i && (run.path == extent.path) &&
+			(run.firstSector <= extent.firstSector + extent.sectorBytes.size() );
+
+		if(!extends)
+		{
+			if(i)
+				addExtent();
+
+			extent = run;
+			extent.sectorBytes.assign(run.sectorBytes.size(), 0);
+			extent.firstSectorLo = 0;
+			midParts.clear();
+		}
+
+		const uint64_t shift = run.firstSector - extent.firstSector;
+
+		if(extent.sectorBytes.size() < shift + run.sectorBytes.size() )
+			extent.sectorBytes.resize(shift + run.sectorBytes.size(), 0);
+
+		for(size_t k = 0; k < run.sectorBytes.size(); k++)
+		{
+			uint16_t& count = (!k && run.firstSectorLo) ?
+				midParts[run.firstSector][run.firstSectorLo] : extent.sectorBytes[shift + k];
+
+			count = std::max(count, run.sectorBytes[k] );
+		}
+
+		extent.firstByte = std::min(extent.firstByte, run.firstByte);
+		extent.lastByte = std::max(extent.lastByte, run.lastByte);
+	}
+
+	if(!runs.empty() )
+		addExtent();
+
+	if(numRunsDropped)
+		report.lines += "# truncated: " + std::to_string(numRunsDropped) + " more extents, " +
+			std::to_string(numBytesDropped) + " differing bytes not listed\n";
+
+	return report;
 }
 
 /* Statistics::generatePhaseResults (Statistics.cpp:1641-1764) */
@@ -1136,6 +1234,26 @@ int elb_mgr_interrupt(elb_mgr* m)
 	m->impl->shared.condition.notify_all();
 
 	return 0;
+}
+
+int64_t elb_mgr_verify_report(elb_mgr* m, char* outBuf, uint64_t outBufLen)
+{
+	if(!m)
+	{
+		elb_set_last_error("elb_mgr_verify_report: NULL manager");
+		return -1;
+	}
+
+	const std::string text = m->impl->getVerifyReport().lines;
+
+	if(outBuf && outBufLen)
+	{
+		const size_t copyLen = std::min( (size_t)(outBufLen - 1), text.size() );
+		memcpy(outBuf, text.data(), copyLen);
+		outBuf[copyLen] = 0;
+	}
+
+	return (int64_t)text.size();
 }
 
 uint32_t elb_mgr_num_workers(elb_mgr* m)

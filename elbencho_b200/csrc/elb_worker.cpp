@@ -337,6 +337,10 @@ void Worker::resetStats() // Worker.h:92-110
 	numD2HBytes = 0;
 	numKernelLaunches = 0;
 	devKernelUSec = 0;
+	damageRuns.clear();
+	numDamageRunsDropped = 0;
+	numDamageBytesDropped = 0;
+	deferredVerifyError.clear();
 
 	std::unique_lock<std::mutex> lock(errorMutex);
 	lastError.clear();
@@ -399,6 +403,26 @@ void Worker::waitForNextPhase(uint64_t oldBenchSeq)
 		shared->condition.wait(lock);
 }
 
+/* --verifyreport: when the last worker of a phase is done, the workers that found damage count as
+ * done with error, and the error text is that of the lowest-ranked of them (unless an error of
+ * another kind came first). Called under Shared::mutex. */
+static void raiseDeferredVerifyErrors(Shared& shared)
+{
+	if(shared.numWorkersDone != shared.workers.size() )
+		return;
+
+	for(Worker* worker : shared.workers) // (in rank order)
+	{
+		if(worker->getDeferredVerifyError().empty() )
+			continue;
+
+		if(shared.firstErrorMsg.empty() )
+			shared.firstErrorMsg = worker->getDeferredVerifyError();
+
+		shared.numWorkersDoneWithError++;
+	}
+}
+
 void Worker::incNumWorkersDone() // Worker.cpp:33-55
 {
 	std::unique_lock<std::mutex> lock(shared->mutex);
@@ -426,6 +450,8 @@ void Worker::incNumWorkersDone() // Worker.cpp:33-55
 		shared->cpuUtilLastDonePercent = shared->cpuUtilLastDone.getCPUUtilPercent();
 	}
 
+	raiseDeferredVerifyErrors(*shared);
+
 	shared->condition.notify_all();
 }
 
@@ -444,6 +470,8 @@ void Worker::incNumWorkersDoneWithError() // WorkersSharedData.cpp:36-44
 
 	if(shared->firstErrorMsg.empty() )
 		shared->firstErrorMsg = getLastError();
+
+	raiseDeferredVerifyErrors(*shared);
 
 	shared->condition.notify_all();
 }
@@ -945,6 +973,19 @@ void Worker::allocRings()
 		ELB_CUDA_CHECK(cudaStreamSynchronize(batch.stream), "GPU batch setup");
 	}
 
+	if(cfg.verifyDamageReport)
+	{ // (a block at any file offset touches at most blockSize / 512 + 2 sectors)
+		sectorsPerSlot = (cfg.blockSize + 2 * 512 - 2) / 512;
+
+		ELB_CUDA_CHECK(cudaHostAlloc( (void**)&damageDescs, sizeof(elb_block_desc) * batchBlocks,
+			cudaHostAllocDefault), "Pinned damage map desc allocation");
+		ELB_CUDA_CHECK(cudaMalloc( (void**)&devSectorMap,
+			sizeof(elb_sector_damage) * batchBlocks * sectorsPerSlot), "GPU damage map allocation");
+		ELB_CUDA_CHECK(cudaHostAlloc( (void**)&hostSectorMap,
+			sizeof(elb_sector_damage) * batchBlocks * sectorsPerSlot, cudaHostAllocDefault),
+			"Pinned damage map allocation");
+	}
+
 	if(cfg.useCuFile && cfg.useGDSBufReg)
 	{ // register the whole device ring for DMA once (reference: per buffer, :1495-1509)
 		CUfileError_t registerRes = CuFileApi::get().BufRegister(devRing, ringBytes, 0);
@@ -1027,6 +1068,13 @@ void Worker::freeRings() // LocalWorker::cleanup (:1570-1641)
 	}
 
 	batches.clear();
+
+	if(damageDescs)
+		cudaFreeHost(damageDescs);
+	if(devSectorMap)
+		cudaFree(devSectorMap);
+	if(hostSectorMap)
+		cudaFreeHost(hostSectorMap);
 
 	if(hostRing)
 		cudaFreeHost(hostRing);
@@ -2340,8 +2388,8 @@ void Worker::gpuWait(Batch& batch)
 	}
 }
 
-/* the exception of postReadIntegrityCheckVerifyBuf (LocalWorker.cpp:2162-2177) */
-void Worker::throwVerifyError(Batch& batch, size_t blockIdx)
+/* the text of postReadIntegrityCheckVerifyBuf's exception (LocalWorker.cpp:2162-2177) */
+std::string Worker::verifyErrorText(Batch& batch, size_t blockIdx)
 {
 	const BlockRef& block = batch.blocks[blockIdx];
 	const uint64_t firstIdx = batch.hostResults[blockIdx].firstMismatchIdx;
@@ -2363,10 +2411,106 @@ void Worker::throwVerifyError(Batch& batch, size_t blockIdx)
 		actualVal = actualByte;
 	}
 
-	throw WorkerError("Data verification failed. "
+	return "Data verification failed. "
 		"Offset: " + std::to_string(badOffset) + "; "
 		"Expected value: " + std::to_string(expectedVal) + "; "
-		"Actual value: " + std::to_string(actualVal) );
+		"Actual value: " + std::to_string(actualVal);
+}
+
+void Worker::throwVerifyError(Batch& batch, size_t blockIdx)
+{
+	throw WorkerError(verifyErrorText(batch, blockIdx) );
+}
+
+/* at most this many runs per worker and phase are listed (--verifyreport) */
+#define ELB_MAX_DAMAGE_RUNS (1ULL << 20)
+
+/**
+ * --verifyreport: the damage map of the batch's bad blocks, launched on the batch's stream while
+ * their slots still hold what was read, and the runs of damaged sectors it found. The first bad
+ * block's error text is kept for the end of the phase instead of thrown. The map's time is not
+ * part of the blocks' latency (accountBatch uses the stage's events).
+ */
+void Worker::mapBatchDamage(Batch& batch)
+{
+	uint32_t numBad = 0;
+
+	for(size_t i = 0; i < batch.blocks.size(); i++)
+	{
+		if(!batch.hostResults[i].numMismatchBytes)
+			continue;
+
+		if(deferredVerifyError.empty() && !cfg.verifyCollectAll)
+			deferredVerifyError = verifyErrorText(batch, i);
+
+		damageDescs[numBad++] = batch.hostDescs[i]; // (the stage's descriptor of block i)
+	}
+
+	if(!numBad)
+		return;
+
+	if(elb_launch_damage_map(readStage.content, damageDescs, numBad, devSectorMap, sectorsPerSlot,
+		batch.stream) )
+		throw WorkerError(std::string("GPU damage map failed. ") + elb_last_error() );
+
+	numKernelLaunches++;
+
+	ELB_CUDA_CHECK(cudaMemcpyAsync(hostSectorMap, devSectorMap,
+		sizeof(elb_sector_damage) * numBad * sectorsPerSlot, cudaMemcpyDeviceToHost, batch.stream),
+		"Copy of damage map from GPU");
+	ELB_CUDA_CHECK(cudaStreamSynchronize(batch.stream), "Copy of damage map from GPU");
+
+	for(size_t i = 0, badIdx = 0; i < batch.blocks.size(); i++)
+		if(batch.hostResults[i].numMismatchBytes)
+			addDamageRuns(batch.blocks[i], &hostSectorMap[sectorsPerSlot * badIdx++] );
+}
+
+/* the runs of consecutive damaged sectors in the damage map records of one block */
+void Worker::addDamageRuns(const BlockRef& block, const elb_sector_damage* records)
+{
+	const uint64_t firstSector = block.offset / 512;
+	const uint64_t numSectors = !block.len ? 0 :
+		( (block.offset + block.len - 1) / 512 - firstSector + 1);
+	const std::string path = blockFilePath(block);
+	bool inRun = false;
+	bool listRun = false;
+
+	for(uint64_t i = 0; i < numSectors; i++)
+	{
+		const elb_sector_damage& record = records[i];
+		const uint64_t sectorPos = (firstSector + i) * 512;
+
+		if(!record.numDiffBytes)
+		{
+			inRun = false;
+			continue;
+		}
+
+		if(!inRun)
+		{ // a new run
+			inRun = true;
+			listRun = (damageRuns.size() < ELB_MAX_DAMAGE_RUNS);
+
+			if(listRun)
+			{
+				damageRuns.emplace_back();
+				damageRuns.back().path = path;
+				damageRuns.back().firstSector = firstSector + i;
+				damageRuns.back().firstSectorLo = i ? 0 : (uint16_t)(block.offset % 512);
+				damageRuns.back().firstByte = sectorPos + record.firstDiff;
+			}
+			else
+				numDamageRunsDropped++;
+		}
+
+		if(listRun)
+		{
+			damageRuns.back().lastByte = sectorPos + record.lastDiff;
+			damageRuns.back().sectorBytes.push_back( (uint16_t)record.numDiffBytes);
+		}
+		else
+			numDamageBytesDropped += record.numDiffBytes;
+	}
 }
 
 /* integrity results of a batch whose verify launch has completed, in submission order */
@@ -2374,6 +2518,12 @@ void Worker::checkVerifyResults(Batch& batch)
 {
 	if(!cfg.integrityCheckSalt)
 		return;
+
+	if(cfg.verifyDamageReport)
+	{
+		mapBatchDamage(batch);
+		return;
+	}
 
 	for(size_t i = 0; i < batch.blocks.size(); i++)
 		if(batch.hostResults[i].numMismatchBytes && !cfg.verifyCollectAll)
@@ -2444,6 +2594,33 @@ void Worker::accountBatch(Batch& batch, uint64_t gpuUSecTotal)
 		ioAccountBlock(batch.blocks[i], batch.blocks[i].ioUSec + gpuShareUSec);
 }
 
+/* dir mode: the path of the block's file relative to bench path outPathIndex */
+std::string Worker::dirModeRelativePath(const BlockRef& block, size_t& outPathIndex) const
+{
+	if(block.isTreeElem)
+	{ // custom tree: the path comes from the tree file
+		outPathIndex = 0;
+		return customTreeFiles.slices[block.fileIndex].path;
+	}
+
+	const DirNamespace names(cfg, rank, shared->pathFDs.size() );
+
+	outPathIndex = names.basePathIndex(block.dirIndex);
+	return names.filePath(cfg.numDirs > 0, block.dirIndex, block.fileIndex);
+}
+
+/* the path of the block's file as the worker opens it */
+std::string Worker::blockFilePath(const BlockRef& block) const
+{
+	if(cfg.pathType != ELB_PATH_DIR)
+		return cfg.paths[block.fileIdx];
+
+	size_t pathIndex;
+	const std::string relativePath = dirModeRelativePath(block, pathIndex);
+
+	return cfg.paths[pathIndex] + "/" + relativePath;
+}
+
 std::string Worker::blockPathForLog(const BlockRef& block) const
 {
 	if(cfg.pathType == ELB_PATH_DIR)
@@ -2476,27 +2653,20 @@ void Worker::throwIOError(const BlockRef& block, bool isRead, ssize_t ioRes, int
 /* dirModeOpenAndPrepFile (LocalWorker.cpp:7097-7161) with getDirModeOpenFlags (:7062-7082) */
 void Worker::dirModeOpenFile(const BlockRef& block, bool isRead)
 {
-	const DirNamespace names(cfg, rank, shared->pathFDs.size() );
-	std::string relativePath;
-	size_t pathFDsIndex = 0;
+	size_t pathFDsIndex;
+	const std::string relativePath = dirModeRelativePath(block, pathFDsIndex);
 	uint64_t fileSize = cfg.fileSize; // for --trunctosize / --preallocfile
 
 	dirModeCountsEntry = true;
 
 	if(block.isTreeElem)
-	{ // custom tree: the path comes from the tree file, the size is the entry's
+	{ // custom tree: the size is the entry's
 		const TreeSlice& elem = customTreeFiles.slices[block.fileIndex];
 
-		relativePath = elem.path;
 		fileSize = elem.totalLen;
 
 		// entry latency and count are only meaningful for fully processed entries (:3434-3447)
 		dirModeCountsEntry = elem.coversWholeFile();
-	}
-	else
-	{
-		relativePath = names.filePath(cfg.numDirs > 0, block.dirIndex, block.fileIndex);
-		pathFDsIndex = names.basePathIndex(block.dirIndex);
 	}
 
 	dirModeCurrentPath = cfg.paths[pathFDsIndex] + "/" + relativePath;

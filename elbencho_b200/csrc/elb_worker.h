@@ -106,6 +106,18 @@ struct BlockRef
 	                           // (the reference then leaves it out of the histogram, :1843-1845)
 };
 
+/* --verifyreport: a run of consecutive damaged 512-byte file sectors of one file, as the damage map
+ * of one block (or several merged) saw it */
+struct DamageRun
+{
+	std::string path;                  // as the worker opened the file
+	uint64_t firstSector{0};           // file offset / 512
+	uint64_t firstByte{0};             // file offset of the first differing byte
+	uint64_t lastByte{0};              // file offset of the last differing byte
+	std::vector<uint16_t> sectorBytes; // differing bytes of each sector, from firstSector on
+	uint16_t firstSectorLo{0}; // where the block starts in the first sector (0: before it)
+};
+
 /* produces the worker's blocks of a phase in submission order */
 class BlockSource
 {
@@ -206,6 +218,11 @@ class Worker
 		uint64_t getNumD2HBytes() const { return numD2HBytes; }
 		uint64_t getNumKernelLaunches() const { return numKernelLaunches; }
 		uint64_t getDevKernelUSec() const { return devKernelUSec; }
+		// --verifyreport results of the phase (read when all workers are done)
+		const std::vector<DamageRun>& getDamageRuns() const { return damageRuns; }
+		uint64_t getNumDamageRunsDropped() const { return numDamageRunsDropped; }
+		uint64_t getNumDamageBytesDropped() const { return numDamageBytesDropped; }
+		const std::string& getDeferredVerifyError() const { return deferredVerifyError; }
 
 		void interruptExecution() { isInterruptionRequested = true; }
 		void createStoneWallStats(); // called by the first finisher under Shared::mutex
@@ -302,6 +319,18 @@ class Worker
 		CuFileHandle dirModeCuFileHandle; // dir mode: handle of the currently open file
 		bool devRingCuFileRegistered{false};
 
+		/* --verifyreport: the damage map of a batch's bad blocks (one batch at a time), the runs it
+		   found in this phase and the error text of the phase's first bad block, which the worker
+		   keeps instead of throwing it (the last finisher raises it, incNumWorkersDone) */
+		elb_block_desc* damageDescs{NULL};      // pinned, batchBlocks
+		elb_sector_damage* devSectorMap{NULL};  // batchBlocks x sectorsPerSlot
+		elb_sector_damage* hostSectorMap{NULL}; // pinned copy
+		uint64_t sectorsPerSlot{0};
+		std::vector<DamageRun> damageRuns;
+		uint64_t numDamageRunsDropped{0};
+		uint64_t numDamageBytesDropped{0};
+		std::string deferredVerifyError;
+
 		// accounting
 		std::atomic<uint64_t> numH2DBytes{0};
 		std::atomic<uint64_t> numD2HBytes{0};
@@ -360,7 +389,12 @@ class Worker
 		void ioRunCuFileBatch(Batch& batch, bool isRead);
 		CUfileHandle_t resolveCuFileHandle(const BlockRef& block, bool isRead);
 		void ioAccountBlock(BlockRef& block, uint64_t latencyUSec);
+		std::string verifyErrorText(Batch& batch, size_t blockIdx);
 		void throwVerifyError(Batch& batch, size_t blockIdx);
+		void mapBatchDamage(Batch& batch);
+		void addDamageRuns(const BlockRef& block, const elb_sector_damage* records);
+		std::string blockFilePath(const BlockRef& block) const;
+		std::string dirModeRelativePath(const BlockRef& block, size_t& outPathIndex) const;
 		int resolveFD(const BlockRef& block, bool isRead);
 		void dirModeOpenFile(const BlockRef& block, bool isRead);
 		void dirModeCloseFile();
@@ -393,6 +427,16 @@ class Manager
 		void interruptAndNotifyWorkers();
 		void getPhaseResults(elb_phase_results& out);
 		void getExpectedTotals(int benchPhase, uint64_t& outEntries, uint64_t& outBytes);
+
+		/* --verifyreport: the damaged extents of the last phase, merged over all workers */
+		struct VerifyReport
+		{
+			std::string lines; // "<path>\t<offset>\t<length>\t<differing bytes>\n" + truncation line
+			uint64_t numExtents{0};
+			uint64_t numBytes{0};
+			uint64_t numFiles{0};
+		};
+		VerifyReport getVerifyReport();
 
 		Shared shared;
 		std::vector<std::unique_ptr<Worker> > workers;

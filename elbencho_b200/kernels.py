@@ -7,7 +7,8 @@ These replace the reference's CPU block modifiers (source/workers/LocalWorker.cp
 import ctypes
 
 from . import _native
-from ._native import BlockDesc, VerifyResult, DEVCTR_NUM  # noqa: F401
+from ._native import BlockDesc, VerifyResult, SectorDamage, DEVCTR_NUM  # noqa: F401
+from ._native import CONTENT_PATTERN, CONTENT_RANDOM, CONTENT_RANDOM_GRAIN  # noqa: F401
 
 RANDALGO_SPLITMIX64 = 0
 
@@ -20,6 +21,7 @@ DEVCTR_FILLED_BYTES = 2
 
 BLOCK_DESC_BYTES = ctypes.sizeof(BlockDesc)        # 32
 VERIFY_RESULT_BYTES = ctypes.sizeof(VerifyResult)  # 16
+SECTOR_DAMAGE_BYTES = ctypes.sizeof(SectorDamage)  # 16
 
 
 class KernelError(RuntimeError):
@@ -274,6 +276,17 @@ def rand_grain_content_key(seed, file_key, grain_offset, grain_shift, dedupe_pct
     """the key of a grain's random fill (elb_rand_grain_content_key)"""
     return int(_native.load().elb_rand_grain_content_key(seed, file_key, grain_offset, grain_shift,
                                                          dedupe_pct))
+
+
+def damage_map(pinned_descs_ptr, num_descs, content_kind, key, pct, grain_shift, dedupe_pct,
+               dev_sectors_ptr, sectors_per_desc, stream=0):
+    """Damage map of bad blocks (--verifyreport): record i * sectors_per_desc + k of
+    dev_sectors_ptr receives the elb_sector_damage of the k-th 512-byte file sector that
+    descriptor i touches. The descriptors must be in pinned host memory."""
+    _check(_native.load().elb_damage_map(pinned_descs_ptr, num_descs, content_kind, key, pct,
+                                         grain_shift, dedupe_pct, dev_sectors_ptr,
+                                         sectors_per_desc, stream),
+           "elb_damage_map")
 
 
 def stage_copy(descs_ptr, num_descs, host_to_device, host_delta, stream=0, total_bytes=0,

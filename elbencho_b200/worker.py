@@ -112,6 +112,7 @@ class WorkerConfig:
     ignore_del_errors: bool = False
     run_as_service: bool = False
     verify_collect_all: bool = False
+    verify_report: bool = False       # --verifyreport: map bad blocks' damage, fail at phase end
     serialize_buffered_writes: int = 0  # 0 auto, 1 on, 2 off (--writegate)
     staging_engine: int = 0           # 0 auto, 1 kernels move the data, 2 cudaMemcpyAsync
     no_gpu_numa_binding: bool = False  # --nogpunuma
@@ -171,6 +172,7 @@ class WorkerConfig:
         cfg.ignoreDelErrors = int(self.ignore_del_errors)
         cfg.runAsService = int(self.run_as_service)
         cfg.verifyCollectAll = int(self.verify_collect_all)
+        cfg.verifyDamageReport = int(self.verify_report)
         cfg.serializeBufferedWrites = int(self.serialize_buffered_writes)
         cfg.numRWMixReadThreads = self.num_rwmix_read_threads
         cfg.randOffsetAlgo = int(self.rand_offset_algo)
@@ -379,6 +381,26 @@ class WorkerManager:
         self._lib.elb_mgr_expected_totals(self._h, int(phase), ctypes.byref(entries),
                                           ctypes.byref(num_bytes))
         return entries.value, num_bytes.value
+
+    def verify_report_text(self) -> str:
+        """The last phase's damaged extents as the library formats them (verify_report)."""
+        size = self._lib.elb_mgr_verify_report(self._h, None, 0)
+        if size < 0:
+            raise WorkerError(_native.last_error())
+        buf = ctypes.create_string_buffer(size + 1)
+        self._lib.elb_mgr_verify_report(self._h, buf, size + 1)
+        return buf.value.decode("utf-8", "replace")
+
+    def verify_report(self):
+        """The last phase's damaged extents, merged over all workers and sorted:
+        [(path, offset, length, differing_bytes)] (the truncation line is left out)."""
+        extents = []
+        for line in self.verify_report_text().splitlines():
+            if line.startswith("#"):
+                continue
+            path, offset, length, num_bytes = line.rsplit("\t", 3)
+            extents.append((path, int(offset), int(length), int(num_bytes)))
+        return extents
 
     def interrupt(self):
         self._lib.elb_mgr_interrupt(self._h)

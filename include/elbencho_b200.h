@@ -262,6 +262,36 @@ int elb_verify_dedupe_grain_staged(const elb_block_desc* descs, uint32_t numDesc
 uint64_t elb_rand_grain_content_key(uint64_t seed, uint64_t fileKey, uint64_t grainOffset,
 	unsigned grainShift, unsigned dedupePct);
 
+/* What a block holds, for elb_damage_map (the values of the library's internal content kinds) */
+enum elb_content_kind
+{
+	ELB_CONTENT_PATTERN = 1,      /* --verify: key = salt */
+	ELB_CONTENT_RANDOM = 2,       /* --verifyrand per block: key = seed, desc blockCounter = the
+	                                 block counter (elb_rand_pos_counter) */
+	ELB_CONTENT_RANDOM_GRAIN = 3, /* --verifyrandgrain / --dedupepct: key = seed, desc blockCounter
+	                                 = fileKey */
+};
+
+/* Damage of one 512-byte file sector (file bytes [s * 512, s * 512 + 512)) within one block */
+typedef struct elb_sector_damage
+{
+	uint32_t numDiffBytes; /* bytes of the sector in this block that differ (0: none) */
+	uint32_t firstDiff;    /* file position mod 512 of the first differing byte (0 if none) */
+	uint32_t lastDiff;     /* file position mod 512 of the last differing byte (0 if none) */
+	uint32_t reserved;     /* 0 */
+} elb_sector_damage;
+
+/* Damage map of the blocks of descs (--verifyreport; meant for blocks whose verify result showed a
+ * mismatch). Descriptor i touches the file sectors s0 = fileOffset >> 9 .. (fileOffset + len - 1)
+ * >> 9; record devSectors[i * sectorsPerDesc + (s - s0)] (device memory) receives the damage of
+ * sector s, every one of them is written. The content arguments are those of the fill / verify
+ * forms of contentKind (grainShift and dedupePct: RANDOM_GRAIN only). `descs` must be pinned host
+ * memory: the host checks that every descriptor fits sectorsPerDesc before the launch, the device
+ * reads them. */
+int elb_damage_map(const elb_block_desc* descs, uint32_t numDescs, int contentKind, uint64_t key,
+	unsigned pct, unsigned grainShift, unsigned dedupePct, elb_sector_damage* devSectors,
+	uint64_t sectorsPerDesc, void* stream);
+
 int elb_stage_copy(const elb_block_desc* descs, uint32_t numDescs, int hostToDevice,
 	int64_t hostDelta, uint64_t totalBytes, uint64_t maxBlockLen, void* stream);
 /* devResults[0..numDescs) <- {0, ~0} */
@@ -367,6 +397,12 @@ typedef struct elb_cfg
 	 * phase; their stats go to the ReadMix counters (LocalWorker.cpp:1028-1041) */
 	uint32_t numRWMixReadThreads;
 	int32_t randOffsetAlgo; /* enum elb_offset_rand_algo (--randalgo) */
+	/* --verifyreport (needs integrityCheckSalt): a verifying phase reads on past bad blocks, maps
+	 * the damaged file sectors of each on the GPU (elb_damage_map) and fails only when all workers
+	 * are done (unless verifyCollectAll), with the error text of the lowest-ranked worker that
+	 * found damage; elb_mgr_verify_report lists the damaged extents. It takes the 4 bytes of
+	 * padding in front of limitReadBps: no other field moves. */
+	int32_t verifyDamageReport;
 
 	/* --limitread / --limitwrite: per-thread bytes per second, 0 = unlimited (RateLimiter.h:13-66,
 	 * LocalWorker.cpp:1293-1299, 1331-1337); applied per block before its storage call */
@@ -681,6 +717,16 @@ int elb_mgr_expected_totals(elb_mgr* m, int benchPhase, uint64_t* outEntries,
 
 /* Request friendly interruption of all workers (Worker::interruptExecution). */
 int elb_mgr_interrupt(elb_mgr* m);
+
+/* --verifyreport (elb_cfg::verifyDamageReport): the damaged extents of the last phase, merged over
+ * all workers, as text lines "<path>\t<offset>\t<length>\t<differing bytes>\n" sorted by path and
+ * offset. An extent is a maximal run of consecutive damaged 512-byte file sectors; offset and
+ * length span its first to its last differing byte; a sector read more than once counts once,
+ * with the largest count seen. Each worker lists at most 2^20 extents per phase (counted before
+ * the merge); if any were left out, the text ends with "# truncated: <n> more extents, <b>
+ * differing bytes not listed\n". Returns the length of the full text (truncated to outBufLen - 1
+ * bytes in outBuf), -1 on error. */
+int64_t elb_mgr_verify_report(elb_mgr* m, char* outBuf, uint64_t outBufLen);
 
 uint32_t elb_mgr_num_workers(elb_mgr* m);
 elb_worker* elb_mgr_worker(elb_mgr* m, uint32_t localIdx);
