@@ -16,221 +16,301 @@
 namespace elb
 {
 
-enum OptKind { Opt_FLAG, Opt_U64, Opt_BYTES, Opt_STR };
-
-struct OptDef
-{
-	const char* longName;
-	char shortName; // 0 = none
-	OptKind kind;
-	const char* help;
-};
-
 /* (order = order of the help text) */
 static const OptDef optDefs[] =
 {
-	{"help", 'h', Opt_FLAG, "Print this help message."},
-	{"help-all", 0, Opt_FLAG, "Print this help message (the categories of the reference's help are "
-		"one list here; also: --help-bdev, --help-dist, --help-large, --help-multi)."},
-	{"help-bdev", 0, Opt_FLAG, "Same as --help."},
-	{"help-dist", 0, Opt_FLAG, "Same as --help."},
-	{"help-large", 0, Opt_FLAG, "Same as --help."},
-	{"help-multi", 0, Opt_FLAG, "Same as --help."},
-	{"version", 0, Opt_FLAG, "Show version and included optional build features."},
+	{"help", 'h', Opt_FLAG, {}, Wire_NONE, "Print this help message."},
+	{"help-all", 0, Opt_FLAG, {}, Wire_NONE, "Print this help message (the categories of the "
+		"reference's help are one list here; also: --help-bdev, --help-dist, --help-large, "
+		"--help-multi)."},
+	{"help-bdev", 0, Opt_FLAG, {}, Wire_NONE, "Same as --help."},
+	{"help-dist", 0, Opt_FLAG, {}, Wire_NONE, "Same as --help."},
+	{"help-large", 0, Opt_FLAG, {}, Wire_NONE, "Same as --help."},
+	{"help-multi", 0, Opt_FLAG, {}, Wire_NONE, "Same as --help."},
+	{"version", 0, Opt_FLAG, &ProgArgs::printVersion, Wire_NONE, "Show version and included "
+		"optional build features."},
 	// phases
-	{"mkdirs", 'd', Opt_FLAG, "Create directories. (Already existing dirs are not treated as error.)"},
-	{"write", 'w', Opt_FLAG, "Write files. Create them if they don't exist."},
-	{"read", 'r', Opt_FLAG, "Read files."},
-	{"stat", 0, Opt_FLAG, "Read file status attributes (file size, owner etc)."},
-	{"delfiles", 'F', Opt_FLAG, "Delete files."},
-	{"deldirs", 'D', Opt_FLAG, "Delete directories."},
-	{"sync", 0, Opt_FLAG, "Sync Linux kernel page cache to stable storage before/after each phase."},
-	{"dropcache", 0, Opt_FLAG, "Drop Linux file system page cache, dentry cache and inode cache "
-		"before/after each phase. Requires root privileges."},
+	{"mkdirs", 'd', Opt_FLAG, &ProgArgs::runCreateDirsPhase, Wire_REF, "Create directories. "
+		"(Already existing dirs are not treated as error.)"},
+	{"write", 'w', Opt_FLAG, &ProgArgs::runCreateFilesPhase, Wire_REF, "Write files. Create them "
+		"if they don't exist."},
+	{"read", 'r', Opt_FLAG, &ProgArgs::runReadPhase, Wire_REF, "Read files."},
+	{"stat", 0, Opt_FLAG, &ProgArgs::runStatFilesPhase, Wire_REF, "Read file status attributes "
+		"(file size, owner etc)."},
+	{"delfiles", 'F', Opt_FLAG, &ProgArgs::runDeleteFilesPhase, Wire_REF, "Delete files."},
+	{"deldirs", 'D', Opt_FLAG, &ProgArgs::runDeleteDirsPhase, Wire_REF, "Delete directories."},
+	{"sync", 0, Opt_FLAG, &ProgArgs::runSyncPhase, Wire_REF, "Sync Linux kernel page cache to "
+		"stable storage before/after each phase."},
+	{"dropcache", 0, Opt_FLAG, &ProgArgs::runDropCachesPhase, Wire_REF, "Drop Linux file system "
+		"page cache, dentry cache and inode cache before/after each phase. Requires root "
+		"privileges."},
 	// basic
-	{"threads", 't', Opt_U64, "Number of I/O worker threads. (Default: 1)"},
-	{"dirs", 'n', Opt_U64, "Number of directories per I/O worker thread. (Default: 1)"},
-	{"files", 'N', Opt_U64, "Number of files per thread per directory. (Default: 1)"},
-	{"size", 's', Opt_BYTES, "File size. (Default: 0)"},
-	{"block", 'b', Opt_BYTES, "Number of bytes to read/write in a single operation. (Default: 1M)"},
-	{"iodepth", 0, Opt_U64, "Depth of I/O queue per thread for asynchronous I/O. (Default: 1)"},
-	{"direct", 0, Opt_FLAG, "Use direct IO (O_DIRECT) to avoid file system buffering/caching."},
-	{"dirsharing", 0, Opt_FLAG, "All threads share the same dirs of rank 0."},
-	{"trunc", 0, Opt_FLAG, "Truncate files to 0 size when opening for writing."},
-	{"trunctosize", 0, Opt_FLAG, "Truncate files to given --size via ftruncate() before writing."},
-	{"preallocfile", 0, Opt_FLAG, "Preallocate file disk space on creation via posix_fallocate()."},
-	{"nodelerr", 0, Opt_FLAG, "Ignore not existing files/dirs in deletion phase."},
+	{"threads", 't', Opt_U64, &ProgArgs::numThreads, Wire_REF, "Number of I/O worker threads. "
+		"(Default: 1)"},
+	{"dirs", 'n', Opt_U64, &ProgArgs::numDirs, Wire_REF, "Number of directories per I/O worker "
+		"thread. (Default: 1)"},
+	{"files", 'N', Opt_U64, &ProgArgs::numFiles, Wire_REF, "Number of files per thread per "
+		"directory. (Default: 1)"},
+	{"size", 's', Opt_BYTES, &ProgArgs::fileSize, Wire_REF, "File size. (Default: 0)"},
+	{"block", 'b', Opt_BYTES, &ProgArgs::blockSize, Wire_REF, "Number of bytes to read/write in a "
+		"single operation. (Default: 1M)"},
+	{"iodepth", 0, Opt_U64, &ProgArgs::ioDepth, Wire_REF, "Depth of I/O queue per thread for "
+		"asynchronous I/O. (Default: 1)"},
+	{"direct", 0, Opt_FLAG, &ProgArgs::useDirectIO, Wire_REF, "Use direct IO (O_DIRECT) to avoid "
+		"file system buffering/caching."},
+	{"dirsharing", 0, Opt_FLAG, &ProgArgs::doDirSharing, Wire_REF, "All threads share the same "
+		"dirs of rank 0."},
+	{"trunc", 0, Opt_FLAG, &ProgArgs::doTruncate, Wire_REF, "Truncate files to 0 size when opening "
+		"for writing."},
+	{"trunctosize", 0, Opt_FLAG, &ProgArgs::doTruncToSize, Wire_REF, "Truncate files to given "
+		"--size via ftruncate() before writing."},
+	{"preallocfile", 0, Opt_FLAG, &ProgArgs::doPreallocFile, Wire_REF, "Preallocate file disk "
+		"space on creation via posix_fallocate()."},
+	{"nodelerr", 0, Opt_FLAG, &ProgArgs::ignoreDelErrors, Wire_REF, "Ignore not existing "
+		"files/dirs in deletion phase."},
 	// offsets
-	{"rand", 0, Opt_FLAG, "Read/write at random offsets."},
-	{"randamount", 0, Opt_BYTES, "Number of bytes to write/read when using random offsets. "
-		"(Default: file size times number of files)"},
-	{"norandalign", 0, Opt_FLAG, "Do not align random offsets to block size."},
-	{"randalgo", 0, Opt_STR, "Random number algorithm for --rand. Giving one disables the full "
-		"coverage generator for random writes. Values: fast, balanced, balanced_single (default), "
-		"strong"},
-	{"randseed", 0, Opt_U64, "Seed for reproducible random offsets (0 = self-seed). [b200]"},
-	{"backward", 0, Opt_FLAG, "Do backwards sequential reads/writes."},
-	{"strided", 0, Opt_FLAG, "Use strided access pattern for files/blockdevs."},
+	{"rand", 0, Opt_FLAG, &ProgArgs::useRandomOffsets, Wire_REF, "Read/write at random offsets."},
+	{"randamount", 0, Opt_BYTES, &ProgArgs::randomAmount, Wire_REF, "Number of bytes to write/read "
+		"when using random offsets. (Default: file size times number of files)"},
+	{"norandalign", 0, Opt_FLAG, &ProgArgs::useRandomUnaligned, Wire_REF, "Do not align random "
+		"offsets to block size."},
+	{"randalgo", 0, Opt_STR, &ProgArgs::randOffsetAlgo, Wire_REF, "Random number algorithm for "
+		"--rand. Giving one disables the full coverage generator for random writes. Values: fast, "
+		"balanced, balanced_single (default), strong"},
+	{"randseed", 0, Opt_U64, &ProgArgs::randOffsetSeed, Wire_B200, "Seed for reproducible random "
+		"offsets (0 = self-seed). [b200]"},
+	{"backward", 0, Opt_FLAG, &ProgArgs::doReverseSeqOffsets, Wire_REF, "Do backwards sequential "
+		"reads/writes."},
+	{"strided", 0, Opt_FLAG, &ProgArgs::useStridedAccess, Wire_REF, "Use strided access pattern "
+		"for files/blockdevs."},
 	// integrity / content
-	{"verify", 0, Opt_U64, "Enable data integrity check with the given salt (non-zero). Written "
-		"on the GPU in the write phase, checked on the GPU in the read phase."},
-	{"verifydirect", 0, Opt_FLAG, "Verify data integrity by reading each block directly after writing."},
-	{"readinline", 0, Opt_FLAG, "Read each block directly after writing it."},
-	{"blockvarpct", 0, Opt_U64, "Block variance percentage: how much of each written block is "
-		"refilled with random data on the GPU. (Default: 100; forced 0 with --verify)"},
-	{"blockvaralgo", 0, Opt_STR, "Random number algorithm for --blockvarpct. Values: fast, balanced, "
-		"balanced_single, strong (all map to the counter based GPU generator)"},
-	{"blockvarseed", 0, Opt_U64, "Seed for reproducible block variance data (0 = self-seed). [b200]"},
-	{"verifyrand", 0, Opt_U64, "Enable data integrity check of random data with the given seed "
-		"(non-zero): writes --blockvarpct random data keyed by seed and block position, checks it on "
-		"the GPU in the read phase. Unlike --verify not block size independent: reads must use the "
-		"block size, file size and --blockvarpct of the write. [b200]"},
-	{"verifyrandgrain", 0, Opt_BYTES, "Grain mode of --verifyrand: the random data is keyed by file "
-		"position in grains of this size (a power of two from 4K to 1G) instead of by block, so that "
-		"reads of any block size and offset (also --rand --norandalign) can check it. Writes and "
-		"reads must use the same value, seed and --blockvarpct. (Default: 0 = per block) [b200]"},
-	{"dedupepct", 0, Opt_U64, "Percentage of duplicate grains (0..100) in --verifyrandgrain data: "
-		"about this share of the grains are copies of grains from one pool of 4096 grains that is "
-		"the same for all files, so that storage which deduplicates finds them. Checked on reads "
-		"like all grains. Reads must use the write's value. Requires --verifyrandgrain. "
-		"(Default: 0) [b200]"},
-	{"verifyreport", 0, Opt_STR, "Path of a verify report file: a verifying phase does not stop at "
-		"the first bad block but reads on, maps the damaged 512-byte sectors of every bad block on "
-		"the GPU and appends one section to this file (truncated at start): \"# phase READ|WRITE\", "
-		"then one tab-separated line \"path offset length differing_bytes\" per damaged extent. "
-		"The phase still fails at its end with the error of the first bad block. Requires --verify "
-		"or --verifyrand. [b200]"},
-	{"rwmixpct", 0, Opt_U64, "Percentage of blocks that should be read in a write phase."},
-	{"rwmixthr", 0, Opt_U64, "Number of threads that should do reads in a write phase."},
+	{"verify", 0, Opt_U64, &ProgArgs::integrityCheckSalt, Wire_REF, "Enable data integrity check "
+		"with the given salt (non-zero). Written on the GPU in the write phase, checked on the GPU "
+		"in the read phase."},
+	{"verifydirect", 0, Opt_FLAG, &ProgArgs::doDirectVerify, Wire_REF, "Verify data integrity by "
+		"reading each block directly after writing."},
+	{"readinline", 0, Opt_FLAG, &ProgArgs::doReadInline, Wire_REF, "Read each block directly after "
+		"writing it."},
+	{"blockvarpct", 0, Opt_U64, &ProgArgs::blockVariancePercent, Wire_REF, "Block variance "
+		"percentage: how much of each written block is refilled with random data on the GPU. "
+		"(Default: 100; forced 0 with --verify)"},
+	{"blockvaralgo", 0, Opt_STR, &ProgArgs::blockVarianceAlgo, Wire_NONE, "Random number algorithm "
+		"for --blockvarpct. Values: fast, balanced, balanced_single, strong (all map to the "
+		"counter based GPU generator)"},
+	{"blockvarseed", 0, Opt_U64, &ProgArgs::blockVarianceSeed, Wire_B200, "Seed for reproducible "
+		"block variance data (0 = self-seed). [b200]"},
+	{"verifyrand", 0, Opt_U64, &ProgArgs::randomVerifySeed, Wire_B200, "Enable data integrity "
+		"check of random data with the given seed (non-zero): writes --blockvarpct random data "
+		"keyed by seed and block position, checks it on the GPU in the read phase. Unlike --verify "
+		"not block size independent: reads must use the block size, file size and --blockvarpct of "
+		"the write. [b200]"},
+	{"verifyrandgrain", 0, Opt_BYTES, &ProgArgs::randomVerifyGrain, Wire_B200, "Grain mode of "
+		"--verifyrand: the random data is keyed by file position in grains of this size (a power "
+		"of two from 4K to 1G) instead of by block, so that reads of any block size and offset "
+		"(also --rand --norandalign) can check it. Writes and reads must use the same value, seed "
+		"and --blockvarpct. (Default: 0 = per block) [b200]"},
+	{"dedupepct", 0, Opt_U64, &ProgArgs::dedupePercent, Wire_B200, "Percentage of duplicate grains "
+		"(0..100) in --verifyrandgrain data: about this share of the grains are copies of grains "
+		"from one pool of 4096 grains that is the same for all files, so that storage which "
+		"deduplicates finds them. Checked on reads like all grains. Reads must use the write's "
+		"value. Requires --verifyrandgrain. (Default: 0) [b200]"},
+	{"verifyreport", 0, Opt_STR, &ProgArgs::verifyReportPath, Wire_NONE, "Path of a verify report "
+		"file: a verifying phase does not stop at the first bad block but reads on, maps the "
+		"damaged 512-byte sectors of every bad block on the GPU and appends one section to this "
+		"file (truncated at start): \"# phase READ|WRITE\", then one tab-separated line \"path "
+		"offset length differing_bytes\" per damaged extent. The phase still fails at its end with "
+		"the error of the first bad block. Requires --verify or --verifyrand. [b200]"},
+	{"rwmixpct", 0, Opt_U64, &ProgArgs::rwMixReadPercent, Wire_REF, "Percentage of blocks that "
+		"should be read in a write phase."},
+	{"rwmixthr", 0, Opt_U64, &ProgArgs::numRWMixReadThreads, Wire_REF, "Number of threads that "
+		"should do reads in a write phase."},
 	// GPU
-	{"rwmixthrpct", 0, Opt_U64, "Percentage of bytes that the --rwmixthr reader threads should "
-		"read out of all bytes of a write phase (rate balancing between readers and writers; "
-		"typically used with --infloop and --timelimit). (Default: 0 = no balancing)"},
-	{"gpuids", 0, Opt_STR, "Comma-separated list of CUDA GPU IDs (also \"all\", \"[0-7]\", "
-		"\"0-7\") to use for the on-GPU block fill/verify. Mandatory."},
-	{"cufiledriveropen", 0, Opt_FLAG, "Explicitly initialize the cuFile library and open the "
-		"nvidia-fs driver. (Always on with --cufile.)"},
-	{"cuhostbufreg", 0, Opt_FLAG, "Pin host memory buffers and register with CUDA for faster "
-		"transfer to/from GPU memory. (Always on: the host rings are cudaHostAlloc memory.)"},
-	{"nodiocheck", 0, Opt_FLAG, "Don't check direct IO alignment and sanity."},
-	{"nopathexp", 0, Opt_FLAG, "Disable expansion of number lists and ranges in square brackets "
-		"for given paths. (Always on: paths are taken literally.)"},
-	{"cufile", 0, Opt_FLAG, "Use cuFile API for reads/writes to/from GPU memory."},
-	{"gdsbufreg", 0, Opt_FLAG, "Register GPU buffers for GPUDirect Storage (GDS)."},
-	{"gds", 0, Opt_FLAG, "Use GPUDirect Storage: shortcut for --direct --cufile --gdsbufreg."},
-	{"batchblocks", 0, Opt_U64, "Blocks per pipeline batch (one kernel launch / staged copy). [b200]"},
-	{"numbatches", 0, Opt_U64, "Pipeline batches in flight per thread. [b200]"},
-	{"writegate", 0, Opt_FLAG, "Always queue buffered writers of one file in a FIFO gate in user "
-		"space (default: when several threads write one file). [b200]"},
-	{"nowritegate", 0, Opt_FLAG, "Never queue buffered writers of one file in user space. [b200]"},
-	{"staging", 0, Opt_STR, "Who moves blocks between the pinned host ring and GPU memory: "
-		"\"kernel\" (fill/verify kernels over PCIe, one launch per batch) or "
-		"\"copyengine\" (cudaMemcpyAsync + kernel; default). [b200]"},
-	{"nogpunuma", 0, Opt_FLAG, "Do not bind worker threads to the NUMA node of their GPU "
-		"(default: bound unless --zones or --cores are given). [b200]"},
-	{"nofdsharing", 0, Opt_FLAG, "If benchmark path is a file or block device, let each worker "
-		"thread open the given file/bdev separately instead of sharing the same file descriptor "
-		"among all threads."},
+	{"rwmixthrpct", 0, Opt_U64, &ProgArgs::rwMixThreadsReadPercent, Wire_REF, "Percentage of bytes "
+		"that the --rwmixthr reader threads should read out of all bytes of a write phase (rate "
+		"balancing between readers and writers; typically used with --infloop and --timelimit). "
+		"(Default: 0 = no balancing)"},
+	{"gpuids", 0, Opt_STR, &ProgArgs::gpuIDsStr, Wire_REF, "Comma-separated list of CUDA GPU IDs "
+		"(also \"all\", \"[0-7]\", \"0-7\") to use for the on-GPU block fill/verify. Mandatory."},
+	{"cufiledriveropen", 0, Opt_FLAG, {}, Wire_NONE, "Explicitly initialize the cuFile library and "
+		"open the nvidia-fs driver. (Always on with --cufile.)"},
+	{"cuhostbufreg", 0, Opt_FLAG, {}, Wire_NONE, "Pin host memory buffers and register with CUDA "
+		"for faster transfer to/from GPU memory. (Always on: the host rings are cudaHostAlloc "
+		"memory.)"},
+	{"nodiocheck", 0, Opt_FLAG, &ProgArgs::noDirectIOCheck, Wire_REF, "Don't check direct IO "
+		"alignment and sanity."},
+	{"nopathexp", 0, Opt_FLAG, {}, Wire_NONE, "Disable expansion of number lists and ranges in "
+		"square brackets for given paths. (Always on: paths are taken literally.)"},
+	{"cufile", 0, Opt_FLAG, &ProgArgs::useCuFile, Wire_REF, "Use cuFile API for reads/writes "
+		"to/from GPU memory."},
+	{"gdsbufreg", 0, Opt_FLAG, &ProgArgs::useGDSBufReg, Wire_REF, "Register GPU buffers for "
+		"GPUDirect Storage (GDS)."},
+	{"gds", 0, Opt_FLAG, &ProgArgs::useGPUDirectStorage, Wire_NONE, "Use GPUDirect Storage: "
+		"shortcut for --direct --cufile --gdsbufreg."},
+	{"batchblocks", 0, Opt_U64, &ProgArgs::pipelineBatchBlocks, Wire_B200, "Blocks per pipeline "
+		"batch (one kernel launch / staged copy). [b200]"},
+	{"numbatches", 0, Opt_U64, &ProgArgs::pipelineNumBatches, Wire_B200, "Pipeline batches in "
+		"flight per thread. [b200]"},
+	{"writegate", 0, Opt_FLAG, &ProgArgs::serializeBufferedWrites, Wire_B200, "Always queue "
+		"buffered writers of one file in a FIFO gate in user space (default: when several threads "
+		"write one file). [b200]"},
+	{"nowritegate", 0, Opt_FLAG, &ProgArgs::neverSerializeBufferedWrites, Wire_B200, "Never queue "
+		"buffered writers of one file in user space. [b200]"},
+	{"staging", 0, Opt_STR, &ProgArgs::stagingEngineStr, Wire_B200, "Who moves blocks between the "
+		"pinned host ring and GPU memory: \"kernel\" (fill/verify kernels over PCIe, one launch "
+		"per batch) or \"copyengine\" (cudaMemcpyAsync + kernel; default). [b200]"},
+	{"nogpunuma", 0, Opt_FLAG, &ProgArgs::noGPUNumaBinding, Wire_B200, "Do not bind worker threads "
+		"to the NUMA node of their GPU (default: bound unless --zones or --cores are given). "
+		"[b200]"},
+	{"nofdsharing", 0, Opt_FLAG, &ProgArgs::useNoFDSharing, Wire_REF, "If benchmark path is a file "
+		"or block device, let each worker thread open the given file/bdev separately instead of "
+		"sharing the same file descriptor among all threads."},
 	// results
-	{"lat", 0, Opt_FLAG, "Show minimum, average and maximum latency for I/Os and entries."},
-	{"latpercent", 0, Opt_FLAG, "Show latency percentiles."},
-	{"latpercent9s", 0, Opt_U64, "Number of decimal nines to show in latency percentiles."},
-	{"lathisto", 0, Opt_FLAG, "Show latency histogram."},
-	{"allelapsed", 0, Opt_FLAG, "Show elapsed time to completion of each I/O worker thread."},
-	{"cpu", 0, Opt_FLAG, "Show CPU utilization in phase stats results."},
-	{"dirstats", 0, Opt_FLAG, "Show directory completion statistics in file write/read phase."},
-	{"nolive", 0, Opt_FLAG, "Disable live statistics."},
-	{"live1", 0, Opt_FLAG, "Use brief live statistics format, i.e. a single line instead of full "
-		"screen stats. (Always on: this implementation has no full screen live stats.)"},
-	{"live1n", 0, Opt_FLAG, "Brief live statistics where every update is a new line."},
-	{"livecsvex", 0, Opt_FLAG, "Use extended live results CSV file. By default, only aggregate "
-		"results of all worker threads will be added. This option also adds results of "
-		"individual threads in standalone mode."},
-	{"livecsv", 0, Opt_STR, "Path to file for live statistics in CSV format ('stdout' for console). "
-		"One line per --liveint interval with the aggregate of all local workers."},
-	{"liveint", 0, Opt_U64, "Update interval for live statistics in milliseconds. (Default: 2000)"},
-	{"no0usecerr", 0, Opt_FLAG, "Do not warn if worker thread completion time is less than 1 usec."},
-	{"label", 0, Opt_STR, "Custom label to identify the benchmark run in result files."},
-	{"csvfile", 0, Opt_STR, "Path to file for end results in csv format (appended)."},
-	{"nocsvlabels", 0, Opt_FLAG, "Do not print headline with labels to csv file."},
-	{"jsonfile", 0, Opt_STR, "Path to file for end results in json format (appended)."},
-	{"resfile", 0, Opt_STR, "Path to file for human-readable end results (appended)."},
-	{"dryrun", 0, Opt_FLAG, "Don't run any benchmark phase, just print the number of expected "
-		"entries and dataset size per phase."},
-	{"iterations", 'i', Opt_U64, "Number of iterations to run the benchmark. (Default: 1)"},
-	{"flock", 0, Opt_STR, "Use POSIX file locks around each read/write. Possible values: "
-		"\"range\" to lock the specific range of each I/O operation, \"full\" to lock the "
-		"entire file for each I/O operation."},
-	{"fadv", 0, Opt_STR, "Provide file access hints via posix_fadvise(). Comma-separated list of "
-		"these flags: seq, rand, willneed, dontneed, noreuse."},
-	{"statinline", 0, Opt_FLAG, "When benchmark path is a directory, stat files immediately "
-		"after open in a write or read phase."},
-	{"cores", 0, Opt_STR, "Comma-separated list of CPU cores to bind this process to. If "
-		"multiple cores are given, then worker threads are bound round-robin to the cores. "
-		"(Hint: See 'lscpu' for available cores. Lists and ranges like \"0-3,8\" are supported.)"},
-	{"zones", 0, Opt_STR, "Comma-separated list of NUMA zones to bind this process to. If "
-		"multiple zones are given, then worker threads are bound round-robin to the zones. "
-		"(Hint: See 'lscpu' for available NUMA zones.)"},
-	{"treefile", 0, Opt_STR, "The path to a treefile containing a list of dirs and filenames to "
-		"use. This is called \"custom tree mode\" and enables testing with files of different "
-		"size. The benchmark path must be a directory. Lines: \"d <relative_path>\" and "
-		"\"f <size_in_bytes> <relative_path>\"."},
-	{"treescan", 0, Opt_STR, "Path to a directory to scan: its dirs and files are written to the "
-		"file given by --treefile (default: elbencho-treescan.txt) for use in custom tree mode."},
-	{"treerand", 0, Opt_FLAG, "In custom tree mode: randomize file order. (Default: order by "
-		"file size.)"},
-	{"treeroundup", 0, Opt_BYTES, "When loading a treefile, round up all contained file sizes to "
-		"a multiple of the given size. (Default: 0 = no rounding)"},
-	{"sharesize", 0, Opt_BYTES, "In custom tree mode, this defines the file size as of which "
-		"files are no longer exclusively assigned to a thread. (Default: 0 = 32 x blocksize)"},
-	{"infloop", 0, Opt_FLAG, "Let I/O threads run in an infinite repeat loop, i.e. each thread "
-		"individually restarts its work from the beginning when it reaches the end of its "
-		"workload. Terminate this via ctrl+c or by using \"--timelimit\"."},
-	{"limitread", 0, Opt_BYTES, "Per-thread read limit in bytes per second. (Default: 0 = off)"},
-	{"limitwrite", 0, Opt_BYTES, "Per-thread write limit in bytes per second. (Default: 0 = off)"},
-	{"start", 0, Opt_U64, "Start time of first benchmark in UTC seconds since the epoch, to "
-		"synchronize the start of benchmarks on different hosts."},
-	{"configfile", 'c', Opt_STR, "Path to benchmark configuration file. All command line options "
-		"starting with double dashes can be used as \"OPTIONNAME=VALUE\" in the config file."},
-	{"phasedelay", 0, Opt_U64, "Delay between different phases in seconds. (Default: 0)"},
-	{"timelimit", 0, Opt_U64, "Time limit in seconds for each phase. (Default: 0 = off)"},
-	{"log", 0, Opt_U64, "Log level. (Default: 0; Verbose: 1; Debug: 2)"},
+	{"lat", 0, Opt_FLAG, &ProgArgs::showLatency, Wire_NONE, "Show minimum, average and maximum "
+		"latency for I/Os and entries."},
+	{"latpercent", 0, Opt_FLAG, &ProgArgs::showLatencyPercentiles, Wire_NONE, "Show latency "
+		"percentiles."},
+	{"latpercent9s", 0, Opt_U64, &ProgArgs::numLatencyPercentile9s, Wire_NONE, "Number of decimal "
+		"nines to show in latency percentiles."},
+	{"lathisto", 0, Opt_FLAG, &ProgArgs::showLatencyHistogram, Wire_NONE, "Show latency "
+		"histogram."},
+	{"allelapsed", 0, Opt_FLAG, &ProgArgs::showAllElapsed, Wire_NONE, "Show elapsed time to "
+		"completion of each I/O worker thread."},
+	{"cpu", 0, Opt_FLAG, &ProgArgs::showCPUUtilization, Wire_NONE, "Show CPU utilization in phase "
+		"stats results."},
+	{"dirstats", 0, Opt_FLAG, &ProgArgs::showDirStats, Wire_NONE, "Show directory completion "
+		"statistics in file write/read phase."},
+	{"nolive", 0, Opt_FLAG, &ProgArgs::disableLiveStats, Wire_NONE, "Disable live statistics."},
+	{"live1", 0, Opt_FLAG, {}, Wire_NONE, "Use brief live statistics format, i.e. a single line "
+		"instead of full screen stats. (Always on: this implementation has no full screen live "
+		"stats.)"},
+	{"live1n", 0, Opt_FLAG, &ProgArgs::useBriefLiveStatsNewLine, Wire_NONE, "Brief live statistics "
+		"where every update is a new line."},
+	{"livecsvex", 0, Opt_FLAG, &ProgArgs::useExtendedLiveCSV, Wire_NONE, "Use extended live "
+		"results CSV file. By default, only aggregate results of all worker threads will be added. "
+		"This option also adds results of individual threads in standalone mode."},
+	{"livecsv", 0, Opt_STR, &ProgArgs::liveCSVFilePath, Wire_NONE, "Path to file for live "
+		"statistics in CSV format ('stdout' for console). One line per --liveint interval with the "
+		"aggregate of all local workers."},
+	{"liveint", 0, Opt_U64, &ProgArgs::liveStatsSleepMS, Wire_NONE, "Update interval for live "
+		"statistics in milliseconds. (Default: 2000)"},
+	{"no0usecerr", 0, Opt_FLAG, &ProgArgs::ignore0USecErrors, Wire_NONE, "Do not warn if worker "
+		"thread completion time is less than 1 usec."},
+	{"label", 0, Opt_STR, &ProgArgs::benchLabel, Wire_REF, "Custom label to identify the benchmark "
+		"run in result files."},
+	{"csvfile", 0, Opt_STR, &ProgArgs::csvFilePath, Wire_NONE, "Path to file for end results in "
+		"csv format (appended)."},
+	{"nocsvlabels", 0, Opt_FLAG, &ProgArgs::noCSVLabels, Wire_NONE, "Do not print headline with "
+		"labels to csv file."},
+	{"jsonfile", 0, Opt_STR, &ProgArgs::jsonFilePath, Wire_NONE, "Path to file for end results in "
+		"json format (appended)."},
+	{"resfile", 0, Opt_STR, &ProgArgs::resFilePath, Wire_NONE, "Path to file for human-readable "
+		"end results (appended)."},
+	{"dryrun", 0, Opt_FLAG, &ProgArgs::doDryRun, Wire_NONE, "Don't run any benchmark phase, just "
+		"print the number of expected entries and dataset size per phase."},
+	{"iterations", 'i', Opt_U64, &ProgArgs::iterations, Wire_NONE, "Number of iterations to run "
+		"the benchmark. (Default: 1)"},
+	{"flock", 0, Opt_STR, &ProgArgs::flockTypeStr, Wire_NONE, "Use POSIX file locks around each "
+		"read/write. Possible values: \"range\" to lock the specific range of each I/O operation, "
+		"\"full\" to lock the entire file for each I/O operation."},
+	{"fadv", 0, Opt_STR, &ProgArgs::fadviseFlagsStr, Wire_NONE, "Provide file access hints via "
+		"posix_fadvise(). Comma-separated list of these flags: seq, rand, willneed, dontneed, "
+		"noreuse."},
+	{"statinline", 0, Opt_FLAG, &ProgArgs::doStatInline, Wire_REF, "When benchmark path is a "
+		"directory, stat files immediately after open in a write or read phase."},
+	{"cores", 0, Opt_STR, &ProgArgs::cpuCoresStr, Wire_NONE, "Comma-separated list of CPU cores to "
+		"bind this process to. If multiple cores are given, then worker threads are bound "
+		"round-robin to the cores. (Hint: See 'lscpu' for available cores. Lists and ranges like "
+		"\"0-3,8\" are supported.)"},
+	{"zones", 0, Opt_STR, &ProgArgs::numaZonesStr, Wire_NONE, "Comma-separated list of NUMA zones "
+		"to bind this process to. If multiple zones are given, then worker threads are bound "
+		"round-robin to the zones. (Hint: See 'lscpu' for available NUMA zones.)"},
+	{"treefile", 0, Opt_STR, &ProgArgs::treeFilePath, Wire_REF, "The path to a treefile containing "
+		"a list of dirs and filenames to use. This is called \"custom tree mode\" and enables "
+		"testing with files of different size. The benchmark path must be a directory. Lines: \"d "
+		"<relative_path>\" and \"f <size_in_bytes> <relative_path>\"."},
+	{"treescan", 0, Opt_STR, &ProgArgs::treeScanPath, Wire_NONE, "Path to a directory to scan: its "
+		"dirs and files are written to the file given by --treefile (default: "
+		"elbencho-treescan.txt) for use in custom tree mode."},
+	{"treerand", 0, Opt_FLAG, &ProgArgs::useCustomTreeRandomize, Wire_REF, "In custom tree mode: "
+		"randomize file order. (Default: order by file size.)"},
+	{"treeroundup", 0, Opt_BYTES, &ProgArgs::treeRoundUpSize, Wire_REF, "When loading a treefile, "
+		"round up all contained file sizes to a multiple of the given size. (Default: 0 = no "
+		"rounding)"},
+	{"sharesize", 0, Opt_BYTES, &ProgArgs::fileShareSize, Wire_REF, "In custom tree mode, this "
+		"defines the file size as of which files are no longer exclusively assigned to a thread. "
+		"(Default: 0 = 32 x blocksize)"},
+	{"infloop", 0, Opt_FLAG, &ProgArgs::doInfiniteIOLoop, Wire_REF, "Let I/O threads run in an "
+		"infinite repeat loop, i.e. each thread individually restarts its work from the beginning "
+		"when it reaches the end of its workload. Terminate this via ctrl+c or by using "
+		"\"--timelimit\"."},
+	{"limitread", 0, Opt_BYTES, &ProgArgs::limitReadBps, Wire_REF, "Per-thread read limit in bytes "
+		"per second. (Default: 0 = off)"},
+	{"limitwrite", 0, Opt_BYTES, &ProgArgs::limitWriteBps, Wire_REF, "Per-thread write limit in "
+		"bytes per second. (Default: 0 = off)"},
+	{"start", 0, Opt_U64, &ProgArgs::startTime, Wire_NONE, "Start time of first benchmark in UTC "
+		"seconds since the epoch, to synchronize the start of benchmarks on different hosts."},
+	{"configfile", 'c', Opt_STR, &ProgArgs::configFilePath, Wire_NONE, "Path to benchmark "
+		"configuration file. All command line options starting with double dashes can be used as "
+		"\"OPTIONNAME=VALUE\" in the config file."},
+	{"phasedelay", 0, Opt_U64, &ProgArgs::nextPhaseDelaySecs, Wire_NONE, "Delay between different "
+		"phases in seconds. (Default: 0)"},
+	{"timelimit", 0, Opt_U64, &ProgArgs::timeLimitSecs, Wire_B200, "Time limit in seconds for each "
+		"phase. (Default: 0 = off)"},
+	{"log", 0, Opt_U64, &ProgArgs::logLevel, Wire_NONE, "Log level. (Default: 0; Verbose: 1; "
+		"Debug: 2)"},
 	// distributed
-	{"hosts", 0, Opt_STR, "Comma-separated list of hosts in service mode for coordinated benchmark."},
-	{"hostsfile", 0, Opt_STR, "Path to file containing line-separated service hosts to use for "
-		"benchmark. Lines starting with \"#\" will be ignored. (Format: hostname[:port])"},
-	{"numhosts", 0, Opt_STR, "Number of hosts to use from given hosts list or hosts file. "
-		"(Default: use all given hosts)"},
-	{"gpuperservice", 0, Opt_FLAG, "Assign GPUs round robin to service instances (one GPU of the "
-		"--gpuids list per service) instead of round robin to the threads of each service."},
-	{"svcelapsed", 0, Opt_FLAG, "Show elapsed time to completion of each service instance ordered "
-		"by slowest thread."},
-	{"svcupint", 0, Opt_U64, "Update retrieval interval for service hosts in milliseconds. "
-		"(Default: 500)"},
-	{"nosvcshare", 0, Opt_FLAG, "Benchmark paths are not shared between service instances. Thus, "
-		"each service instance will work on its own full dataset instead of a fraction of the "
-		"data set."},
-	{"rotatehosts", 0, Opt_U64, "Number by which to rotate hosts between phases to avoid caching "
-		"effects. (Default: 0)"},
-	{"nodetach", 0, Opt_FLAG, "When running as service, do not detach from the terminal."},
-	{"svcping", 0, Opt_FLAG, "Show response time of service instances in fullscreen live stats. "
-		"(Accepted: there is no fullscreen view here.)"},
-	{"althttpsvc", 0, Opt_FLAG, "Use alternative HTTP service implementation. (Accepted: this build "
-		"has one dependency-free HTTP server.)"},
-	{"svcpwfile", 0, Opt_STR, "Path to a text file containing a single line of text as shared "
-		"secret between service instances and master. This is to prevent unauthorized requests "
-		"to service instances."},
-	{"svcwait", 0, Opt_U64, "Number of seconds to wait for the services to become reachable. "
-		"(Default: 5)"},
-	{"datasetthreads", 0, Opt_U64, "Total number of threads that share the data set when several "
-		"independent instances each work on their --rankoffset share. (Default: --threads)"},
-	{"service", 0, Opt_FLAG, "Run as service for distributed mode, waiting for requests from master."},
-	{"foreground", 0, Opt_FLAG, "When running as service, stay in foreground and don't detach."},
-	{"port", 0, Opt_U64, "TCP port of background service. (Default: 1611)"},
-	{"rankoffset", 0, Opt_U64, "Rank offset for worker threads. (Default: 0)"},
-	{"interrupt", 0, Opt_FLAG, "Interrupt current benchmark phase on given service mode hosts."},
-	{"quit", 0, Opt_FLAG, "Quit services on given service mode hosts."},
+	{"hosts", 0, Opt_STR, &ProgArgs::hostsStr, Wire_NONE, "Comma-separated list of hosts in "
+		"service mode for coordinated benchmark."},
+	{"hostsfile", 0, Opt_STR, &ProgArgs::hostsFilePath, Wire_NONE, "Path to file containing "
+		"line-separated service hosts to use for benchmark. Lines starting with \"#\" will be "
+		"ignored. (Format: hostname[:port])"},
+	{"numhosts", 0, Opt_STR, {}, Wire_NONE, "Number of hosts to use from given hosts list or hosts "
+		"file. (Default: use all given hosts)"},
+	{"gpuperservice", 0, Opt_FLAG, &ProgArgs::assignGPUPerService, Wire_NONE, "Assign GPUs round "
+		"robin to service instances (one GPU of the --gpuids list per service) instead of round "
+		"robin to the threads of each service."},
+	{"svcelapsed", 0, Opt_FLAG, &ProgArgs::showServicesElapsed, Wire_NONE, "Show elapsed time to "
+		"completion of each service instance ordered by slowest thread."},
+	{"svcupint", 0, Opt_U64, &ProgArgs::svcUpdateIntervalMS, Wire_NONE, "Update retrieval interval "
+		"for service hosts in milliseconds. (Default: 500)"},
+	{"nosvcshare", 0, Opt_FLAG, &ProgArgs::noSharedServicePath, Wire_NONE, "Benchmark paths are "
+		"not shared between service instances. Thus, each service instance will work on its own "
+		"full dataset instead of a fraction of the data set."},
+	{"rotatehosts", 0, Opt_U64, &ProgArgs::rotateHostsNum, Wire_NONE, "Number by which to rotate "
+		"hosts between phases to avoid caching effects. (Default: 0)"},
+	{"nodetach", 0, Opt_FLAG, {}, Wire_NONE, "When running as service, do not detach from the "
+		"terminal."},
+	{"svcping", 0, Opt_FLAG, {}, Wire_NONE, "Show response time of service instances in fullscreen "
+		"live stats. (Accepted: there is no fullscreen view here.)"},
+	{"althttpsvc", 0, Opt_FLAG, {}, Wire_NONE, "Use alternative HTTP service implementation. "
+		"(Accepted: this build has one dependency-free HTTP server.)"},
+	{"svcpwfile", 0, Opt_STR, &ProgArgs::svcPasswordFile, Wire_NONE, "Path to a text file "
+		"containing a single line of text as shared secret between service instances and master. "
+		"This is to prevent unauthorized requests to service instances."},
+	{"svcwait", 0, Opt_U64, &ProgArgs::svcReadyWaitSec, Wire_NONE, "Number of seconds to wait for "
+		"the services to become reachable. (Default: 5)"},
+	{"datasetthreads", 0, Opt_U64, &ProgArgs::numDataSetThreads, Wire_NONE, "Total number of "
+		"threads that share the data set when several independent instances each work on their "
+		"--rankoffset share. (Default: --threads)"},
+	{"service", 0, Opt_FLAG, &ProgArgs::runAsService, Wire_NONE, "Run as service for distributed "
+		"mode, waiting for requests from master."},
+	{"foreground", 0, Opt_FLAG, {}, Wire_NONE, "When running as service, stay in foreground and "
+		"don't detach."},
+	{"port", 0, Opt_U64, &ProgArgs::servicePort, Wire_NONE, "TCP port of background service. "
+		"(Default: 1611)"},
+	{"rankoffset", 0, Opt_U64, &ProgArgs::rankOffset, Wire_REF, "Rank offset for worker threads. "
+		"(Default: 0)"},
+	{"interrupt", 0, Opt_FLAG, &ProgArgs::interruptServices, Wire_NONE, "Interrupt current "
+		"benchmark phase on given service mode hosts."},
+	{"quit", 0, Opt_FLAG, &ProgArgs::quitServices, Wire_NONE, "Quit services on given service mode "
+		"hosts."},
 };
+
+const OptDef* optionTable(size_t& outNumDefs)
+{
+	outNumDefs = sizeof(optDefs) / sizeof(optDefs[0] );
+	return optDefs;
+}
 
 static const OptDef* findLongOpt(const std::string& name)
 {
@@ -528,140 +608,46 @@ ProgArgs::ProgArgs(int argc, char** argv)
 			benchPaths = configPaths;
 	}
 
-	auto flag = [&](const char* name) { return values.count(name) != 0; };
-	auto num = [&](const char* name, uint64_t& target)
+	// options with a member: flags are set or cleared, numbers and strings are set when given
+	for(const OptDef& def : optDefs)
 	{
-		if(!values.count(name) )
-			return false;
+		const auto value = values.find(def.longName);
 
-		const std::string& raw = values[name];
-		const OptDef* def = findLongOpt(name);
+		if(def.member.flag)
+			this->*def.member.flag = (value != values.end() );
 
-		if(def->kind == Opt_BYTES)
-			target = numHumanToBytesBinary(raw);
+		if(value == values.end() )
+			continue;
+
+		const std::string& raw = value->second;
+
+		if(def.member.str)
+			this->*def.member.str = raw;
 		else
+		if(def.member.num && (def.kind == Opt_BYTES) )
+			this->*def.member.num = numHumanToBytesBinary(raw);
+		else
+		if(def.member.num)
 		{
 			char* endPtr = NULL;
-			target = strtoull(raw.c_str(), &endPtr, 10);
+			this->*def.member.num = strtoull(raw.c_str(), &endPtr, 10);
 
 			if(raw.empty() || (endPtr && *endPtr) )
 				throw ProgError(std::string("the argument ('") + raw + "') for option '--" +
-					name + "' is invalid");
+					def.longName + "' is invalid");
 		}
+	}
 
-		return true;
-	};
-	auto str = [&](const char* name, std::string& target)
-	{
-		if(values.count(name) )
-			target = values[name];
-	};
+	auto given = [&](const char* name) { return values.count(name) != 0; };
 
-	printHelp = flag("help") || flag("help-all") || flag("help-bdev") || flag("help-dist") ||
-		flag("help-large") || flag("help-multi");
-	printVersion = flag("version");
-	runCreateDirsPhase = flag("mkdirs");
-	runCreateFilesPhase = flag("write");
-	runReadPhase = flag("read");
-	runStatFilesPhase = flag("stat");
-	runDeleteFilesPhase = flag("delfiles");
-	runDeleteDirsPhase = flag("deldirs");
-	runSyncPhase = flag("sync");
-	runDropCachesPhase = flag("dropcache");
+	printHelp = given("help") || given("help-all") || given("help-bdev") || given("help-dist") ||
+		given("help-large") || given("help-multi");
+	runServiceInForeground = given("foreground") || given("nodetach");
+	hasUserSetBlockVariance = given("blockvarpct");
+	hasUserSetRWMixPercent = given("rwmixpct");
+	hasUserSetRWMixReadThreads = given("rwmixthr");
 
-	num("threads", numThreads);
-	num("dirs", numDirs);
-	num("files", numFiles);
-	num("size", fileSize);
-	num("block", blockSize);
-	num("iodepth", ioDepth);
-	useDirectIO = flag("direct");
-	doDirSharing = flag("dirsharing");
-	doTruncate = flag("trunc");
-	doTruncToSize = flag("trunctosize");
-	doPreallocFile = flag("preallocfile");
-	ignoreDelErrors = flag("nodelerr");
-
-	useRandomOffsets = flag("rand");
-	num("randamount", randomAmount);
-	useRandomUnaligned = flag("norandalign");
-	str("randalgo", randOffsetAlgo);
-	num("randseed", randOffsetSeed);
-	doReverseSeqOffsets = flag("backward");
-	useStridedAccess = flag("strided");
-
-	num("verify", integrityCheckSalt);
-	doDirectVerify = flag("verifydirect");
-	doReadInline = flag("readinline");
-	hasUserSetBlockVariance = num("blockvarpct", blockVariancePercent);
-	str("blockvaralgo", blockVarianceAlgo);
-	num("blockvarseed", blockVarianceSeed);
-	num("verifyrand", randomVerifySeed);
-	num("verifyrandgrain", randomVerifyGrain);
-	num("dedupepct", dedupePercent);
-	str("verifyreport", verifyReportPath);
-	hasUserSetRWMixPercent = num("rwmixpct", rwMixReadPercent);
-	hasUserSetRWMixReadThreads = num("rwmixthr", numRWMixReadThreads);
-	num("rwmixthrpct", rwMixThreadsReadPercent);
-
-	str("gpuids", gpuIDsStr);
-	useCuFile = flag("cufile");
-	useGDSBufReg = flag("gdsbufreg");
-	useGPUDirectStorage = flag("gds");
-	num("batchblocks", pipelineBatchBlocks);
-	num("numbatches", pipelineNumBatches);
-	serializeBufferedWrites = flag("writegate");
-	neverSerializeBufferedWrites = flag("nowritegate");
-	str("staging", stagingEngineStr);
-	noGPUNumaBinding = flag("nogpunuma");
-	useNoFDSharing = flag("nofdsharing");
-
-	showLatency = flag("lat");
-	showLatencyPercentiles = flag("latpercent");
-	num("latpercent9s", numLatencyPercentile9s);
-	showLatencyHistogram = flag("lathisto");
-	showAllElapsed = flag("allelapsed");
-	showServicesElapsed = flag("svcelapsed");
-	showCPUUtilization = flag("cpu");
-	showDirStats = flag("dirstats");
-	disableLiveStats = flag("nolive");
-	num("liveint", liveStatsSleepMS);
-	ignore0USecErrors = flag("no0usecerr");
-	str("label", benchLabel);
-	str("csvfile", csvFilePath);
-	noCSVLabels = flag("nocsvlabels");
-	str("jsonfile", jsonFilePath);
-	str("resfile", resFilePath);
-	doDryRun = flag("dryrun");
-	num("iterations", iterations);
-	num("phasedelay", nextPhaseDelaySecs);
-	num("timelimit", timeLimitSecs);
-	num("log", logLevel);
-
-	str("flock", flockTypeStr);
-	str("fadv", fadviseFlagsStr);
-	doStatInline = flag("statinline");
-	noDirectIOCheck = flag("nodiocheck");
-	str("cores", cpuCoresStr);
-	str("zones", numaZonesStr);
-	str("treefile", treeFilePath);
-	str("treescan", treeScanPath);
-	useCustomTreeRandomize = flag("treerand");
-	num("treeroundup", treeRoundUpSize);
-	num("sharesize", fileShareSize);
-	doInfiniteIOLoop = flag("infloop");
-	num("limitread", limitReadBps);
-	num("limitwrite", limitWriteBps);
-	num("start", startTime);
-	num("datasetthreads", numDataSetThreads);
-	useBriefLiveStatsNewLine = flag("live1n");
-	str("livecsv", liveCSVFilePath);
-	useExtendedLiveCSV = flag("livecsvex");
-	str("configfile", configFilePath);
-
-	str("hosts", hostsStr);
-	str("hostsfile", hostsFilePath);
-	if(values.count("numhosts") )
+	if(given("numhosts") )
 	{
 		char* endPtr = NULL;
 		numHosts = strtoll(values["numhosts"].c_str(), &endPtr, 10);
@@ -670,18 +656,6 @@ ProgArgs::ProgArgs(int argc, char** argv)
 			throw ProgError("the argument ('" + values["numhosts"] + "') for option "
 				"'--numhosts' is invalid");
 	}
-	assignGPUPerService = flag("gpuperservice");
-	str("svcpwfile", svcPasswordFile);
-	num("svcwait", svcReadyWaitSec);
-	num("svcupint", svcUpdateIntervalMS);
-	noSharedServicePath = flag("nosvcshare");
-	num("rotatehosts", rotateHostsNum);
-	runAsService = flag("service");
-	runServiceInForeground = flag("foreground") || flag("nodetach");
-	num("port", servicePort);
-	num("rankoffset", rankOffset);
-	interruptServices = flag("interrupt");
-	quitServices = flag("quit");
 
 	if(printHelp || printVersion)
 		return;

@@ -198,6 +198,46 @@ class ProgArgs
 		void parseHosts();          // ProgArgs.cpp:2221-2340
 };
 
+enum OptKind { Opt_FLAG, Opt_U64, Opt_BYTES, Opt_STR };
+
+/* how an option travels from the master to its services in the /preparephase tree */
+enum OptWire
+{
+	Wire_NONE, // not at all, or by hand (progArgsToServiceTree)
+	Wire_REF,  // under its own name: a key of the reference
+	Wire_B200, // as "b200_<name>": an extension of this build, which reference services ignore
+};
+
+/* the ProgArgs member an option sets: a bool for FLAG, a uint64_t for U64 and BYTES, a string for
+ * STR; none for the accepted no-ops and the options that the parser handles by hand */
+struct OptMember
+{
+	bool ProgArgs::* flag{nullptr};
+	uint64_t ProgArgs::* num{nullptr};
+	std::string ProgArgs::* str{nullptr};
+
+	constexpr OptMember() {}
+	constexpr OptMember(bool ProgArgs::* flag) : flag(flag) {}
+	constexpr OptMember(uint64_t ProgArgs::* num) : num(num) {}
+	constexpr OptMember(std::string ProgArgs::* str) : str(str) {}
+};
+
+/* one row of the option table (elb_cli.cpp) */
+struct OptDef
+{
+	const char* longName;
+	char shortName; // 0 = none
+	OptKind kind;
+	OptMember member;
+	OptWire wire;
+	const char* help;
+
+	std::string wireKey() const { return (wire == Wire_B200 ? "b200_" : "") + std::string(longName); }
+};
+
+/* the option table in the order of the help text */
+const OptDef* optionTable(size_t& outNumDefs);
+
 /* Statistics output (reference source/Statistics.cpp) */
 namespace stats
 {

@@ -1143,68 +1143,39 @@ HttpResponse Service::handlePreparePhase(const HttpRequest& request)
 
 		ProgArgs& args = progArgs;
 
-		args.benchLabel = recvTree.getStr("label", "");
+		/* every option that travels, so that no value of an earlier prepare survives: block and
+		   size are required, threads, dirs, files and iodepth default to 1, all others to 0, false or
+		   "" (also blockvarpct, whose command line default is 100) */
+		size_t numDefs;
+		const OptDef* defs = optionTable(numDefs);
+
+		for(size_t i = 0; i < numDefs; i++)
+		{
+			const OptDef& def = defs[i];
+
+			if(def.wire == Wire_NONE)
+				continue;
+
+			const std::string key = def.wireKey();
+
+			if(def.member.flag)
+				args.*def.member.flag = recvTree.getBool(key, false);
+			else
+			if(def.member.str)
+				args.*def.member.str = recvTree.getStr(key, "");
+			else
+			if( (key == "block") || (key == "size") )
+				args.*def.member.num = recvTree.getU64(key);
+			else
+				args.*def.member.num = recvTree.getU64(key, ( (key == "threads") || (key == "dirs") ||
+					(key == "files") || (key == "iodepth") ) ? 1 : 0);
+		}
+
 		benchPathStr = recvTree.getStr("path");
-		args.blockSize = recvTree.getU64("block");
-		args.blockVariancePercent = recvTree.getU64("blockvarpct", 0);
-		args.doDirectVerify = recvTree.getBool("verifydirect", false);
-		args.doDirSharing = recvTree.getBool("dirsharing", false);
-		args.doPreallocFile = recvTree.getBool("preallocfile", false);
-		args.doReadInline = recvTree.getBool("readinline", false);
-		args.doReverseSeqOffsets = recvTree.getBool("backward", false);
-		args.doTruncate = recvTree.getBool("trunc", false);
-		args.doTruncToSize = recvTree.getBool("trunctosize", false);
-		args.fileSize = recvTree.getU64("size");
-		args.gpuIDsStr = recvTree.getStr("gpuids", "");
-		args.ignoreDelErrors = recvTree.getBool("nodelerr", false);
-		args.integrityCheckSalt = recvTree.getU64("verify", 0);
+		args.hasUserSetRWMixReadThreads = (args.numRWMixReadThreads != 0);
+		args.hasUserSetRWMixPercent = (args.rwMixReadPercent != 0);
 		args.fadviseFlags = recvTree.getU64("fadv", 0);
 		args.flockType = recvTree.getU64("flock", 0);
-		args.doStatInline = recvTree.getBool("statinline", false);
-		args.noDirectIOCheck = recvTree.getBool("nodiocheck", false);
-		args.doInfiniteIOLoop = recvTree.getBool("infloop", false);
-		args.timeLimitSecs = recvTree.getU64("b200_timelimit", 0);
-		args.limitReadBps = recvTree.getU64("limitread", 0);
-		args.limitWriteBps = recvTree.getU64("limitwrite", 0);
-		args.ioDepth = recvTree.getU64("iodepth", 1);
-		args.numDirs = recvTree.getU64("dirs", 1);
-		args.numFiles = recvTree.getU64("files", 1);
-		args.numRWMixReadThreads = recvTree.getU64("rwmixthr", 0);
-		args.hasUserSetRWMixReadThreads = (args.numRWMixReadThreads != 0);
-		args.rwMixThreadsReadPercent = recvTree.getU64("rwmixthrpct", 0);
-		args.numThreads = recvTree.getU64("threads", 1);
-		args.randOffsetAlgo = recvTree.getStr("randalgo", "");
-		args.randomAmount = recvTree.getU64("randamount", 0);
-		args.rankOffset = recvTree.getU64("rankoffset", 0);
-		args.runCreateDirsPhase = recvTree.getBool("mkdirs", false);
-		args.runCreateFilesPhase = recvTree.getBool("write", false);
-		args.runDeleteDirsPhase = recvTree.getBool("deldirs", false);
-		args.runDeleteFilesPhase = recvTree.getBool("delfiles", false);
-		args.runDropCachesPhase = recvTree.getBool("dropcache", false);
-		args.runReadPhase = recvTree.getBool("read", false);
-		args.runStatFilesPhase = recvTree.getBool("stat", false);
-		args.runSyncPhase = recvTree.getBool("sync", false);
-		args.rwMixReadPercent = recvTree.getU64("rwmixpct", 0);
-		args.hasUserSetRWMixPercent = (args.rwMixReadPercent != 0);
-		args.useCuFile = recvTree.getBool("cufile", false);
-		args.useDirectIO = recvTree.getBool("direct", false);
-		args.useGDSBufReg = recvTree.getBool("gdsbufreg", false);
-		args.useRandomOffsets = recvTree.getBool("rand", false);
-		args.useRandomUnaligned = recvTree.getBool("norandalign", false);
-		args.useStridedAccess = recvTree.getBool("strided", false);
-		// extensions of this build (ignored by a reference service)
-		args.randOffsetSeed = recvTree.getU64("b200_randseed", 0);
-		args.blockVarianceSeed = recvTree.getU64("b200_blockvarseed", 0);
-		args.randomVerifySeed = recvTree.getU64("b200_verifyrand", 0);
-		args.randomVerifyGrain = recvTree.getU64("b200_verifyrandgrain", 0);
-		args.dedupePercent = recvTree.getU64("b200_dedupepct", 0);
-		args.pipelineBatchBlocks = recvTree.getU64("b200_batchblocks", 0);
-		args.pipelineNumBatches = recvTree.getU64("b200_numbatches", 0);
-		args.serializeBufferedWrites = recvTree.getBool("b200_writegate", false);
-		args.neverSerializeBufferedWrites = recvTree.getBool("b200_nowritegate", false);
-		args.stagingEngineStr = recvTree.getStr("b200_staging", "");
-		args.noGPUNumaBinding = recvTree.getBool("b200_nogpunuma", false);
-		args.useNoFDSharing = recvTree.getBool("nofdsharing", false);
 
 		const uint64_t numDataSetThreads = recvTree.getU64("datasetthreads", args.numThreads);
 
@@ -1217,8 +1188,6 @@ HttpResponse Service::handlePreparePhase(const HttpRequest& request)
 
 		/* custom tree mode: the file was uploaded to our tmp dir under the given name before
 		   (ProgArgs.cpp:3685-3698) */
-		args.treeFilePath = recvTree.getStr("treefile", "");
-
 		if(!args.treeFilePath.empty() )
 		{
 			const size_t slashPos = args.treeFilePath.find_last_of('/');
@@ -1228,10 +1197,6 @@ HttpResponse Service::handlePreparePhase(const HttpRequest& request)
 
 			args.treeFilePath = uploadBasePath() + "/" + args.treeFilePath;
 		}
-
-		args.useCustomTreeRandomize = recvTree.getBool("treerand", false);
-		args.treeRoundUpSize = recvTree.getU64("treeroundup", 0);
-		args.fileShareSize = recvTree.getU64("sharesize", 0);
 
 		if(args.gpuIDsStr.empty() )
 			throw ProgError("This service is the GPU worker build: the master has to give "
@@ -1803,66 +1768,62 @@ static JsonTree progArgsToServiceTree(const ProgArgs& args, size_t serviceRank, 
 		benchPathStr += absPath + ",";
 	}
 
-	tree.put("block", args.blockSize);
-	tree.put("blockvarpct", args.blockVariancePercent);
-	tree.put("blockvaralgo", args.blockVarianceAlgo.empty() ? "fast" : args.blockVarianceAlgo);
-	tree.put("label", args.benchLabel);
-	tree.put("benchmode", (uint64_t)1); // BenchMode_POSIX (Common.h:130-137)
+	size_t numDefs;
+	const OptDef* defs = optionTable(numDefs);
+
+	for(size_t i = 0; i < numDefs; i++)
+	{
+		const OptDef& def = defs[i];
+
+		if(def.wire == Wire_NONE)
+			continue;
+
+		if(def.member.flag)
+			tree.putBool(def.wireKey(), args.*def.member.flag);
+		else
+		if(def.member.num)
+			tree.put(def.wireKey(), args.*def.member.num);
+		else
+			tree.put(def.wireKey(), args.*def.member.str);
+	}
+
 	tree.put("path", benchPathStr);
-	tree.putBool("mkdirs", args.runCreateDirsPhase);
-	tree.putBool("write", args.runCreateFilesPhase);
-	tree.putBool("cufile", args.useCuFile);
+	tree.put("flock", args.flockType);
+	tree.put("fadv", args.fadviseFlags);
+	// for reference services only: this build's GPU block variance generator ignores the name
+	tree.put("blockvaralgo", args.blockVarianceAlgo.empty() ? "fast" : args.blockVarianceAlgo);
+	// for reference services only: here the master prints the results and their 0 usec warning
+	tree.putBool("no0usecerr", args.ignore0USecErrors);
+
+	// dynamically calculated values for service hosts (:3845-3861), replacing the loop's values
+	// (services that do not share their paths each work on a full data set, ProgArgs.cpp:1288)
+	tree.put("datasetthreads", args.noSharedServicePath ?
+		args.numThreads : (args.numThreads * numHosts) );
+	tree.put("rankoffset", args.noSharedServicePath ?
+		args.rankOffset : (args.rankOffset + (serviceRank * args.numThreads) ) );
+	tree.put("treefile", args.treeFilePath.empty() ? "" : "treefile.txt"); // ProgArgs.cpp:3850
+	if(args.assignGPUPerService && !args.gpuIDs.empty() )
+	{ // --gpuperservice: one GPU of the list per service instance (ProgArgs.cpp:3852-3859)
+		const size_t gpuIndex = serviceRank % args.gpuIDs.size();
+		tree.put("gpuids", std::to_string(args.gpuIDs[gpuIndex] ) );
+	}
+
+	// keys of reference modes that this build does not have: neutral values
+	tree.put("benchmode", (uint64_t)1); // BenchMode_POSIX (Common.h:130-137)
 	tree.putBool("cufiledriveropen", false);
 	tree.putBool("cuhostbufreg", false);
-	tree.putBool("deldirs", args.runDeleteDirsPhase);
-	tree.putBool("delfiles", args.runDeleteFilesPhase);
-	tree.putBool("dirsharing", args.doDirSharing);
-	tree.putBool("direct", args.useDirectIO);
-	tree.putBool("dropcache", args.runDropCachesPhase);
-	tree.put("fadv", args.fadviseFlags);
-	tree.put("sharesize", args.fileShareSize);
-	tree.put("size", args.fileSize);
-	tree.put("flock", args.flockType);
-	tree.putBool("gdsbufreg", args.useGDSBufReg);
 	tree.putBool("hdfs", false);
-	tree.putBool("no0usecerr", args.ignore0USecErrors);
-	tree.putBool("nodelerr", args.ignoreDelErrors);
-	tree.putBool("infloop", args.doInfiniteIOLoop);
-	tree.put("b200_timelimit", args.timeLimitSecs); // (applied by the service at /status time)
-	tree.put("verify", args.integrityCheckSalt);
-	tree.put("iodepth", args.ioDepth);
-	tree.put("limitread", args.limitReadBps);
-	tree.put("limitwrite", args.limitWriteBps);
 	tree.put("madv", (uint64_t)0);
 	tree.putBool("mmap", false);
 	tree.putBool("netbench", false);
 	tree.put("netbenchservers", "");
-	// (services that do not share their paths each work on a full data set, ProgArgs.cpp:1288)
-	tree.put("datasetthreads", args.noSharedServicePath ?
-		args.numThreads : (args.numThreads * numHosts) );
-	tree.put("dirs", args.numDirs);
-	tree.put("files", args.numFiles);
 	tree.put("numservers", (uint64_t)0);
-	tree.put("threads", args.numThreads);
-	tree.putBool("nofdsharing", args.useNoFDSharing);
-	tree.putBool("nodiocheck", args.noDirectIOCheck);
 	tree.putBool("opsloglock", false);
 	tree.put("opslog", "");
-	tree.putBool("preallocfile", args.doPreallocFile);
-	tree.putBool("norandalign", args.useRandomUnaligned);
-	tree.put("randamount", args.randomAmount);
-	tree.putBool("rand", args.useRandomOffsets);
-	tree.put("randalgo", args.randOffsetAlgo);
-	tree.putBool("read", args.runReadPhase);
-	tree.putBool("readinline", args.doReadInline);
 	tree.put("recvbuf", (uint64_t)0);
 	tree.put("respsize", (uint64_t)1);
-	tree.putBool("backward", args.doReverseSeqOffsets);
-	tree.put("rwmixpct", args.rwMixReadPercent);
-	tree.put("rwmixthr", args.numRWMixReadThreads);
-	tree.put("rwmixthrpct", args.rwMixThreadsReadPercent);
+	tree.put("sendbuf", (uint64_t)0);
 
-	// S3 keys: neutral values
 	const char* s3EmptyStrings[] = {"s3key", "s3secret", "s3aclgrantee", "s3aclgtype",
 		"s3aclgrants", "s3chksumalgo", "s3credfile", "s3credlist", "s3endpoints", "s3objprefix",
 		"s3region", "s3sessiontoken", "s3sseckey", "s3ssekmskey"};
@@ -1881,42 +1842,6 @@ static JsonTree progArgsToServiceTree(const ProgArgs& args, size_t serviceRank, 
 		"s3multidel", "s3sign", "s3targetgbps"};
 	for(const char* key : s3Zeros)
 		tree.put(key, (uint64_t)0);
-
-	tree.put("sendbuf", (uint64_t)0);
-	tree.putBool("stat", args.runStatFilesPhase);
-	tree.putBool("statinline", args.doStatInline);
-	tree.putBool("strided", args.useStridedAccess);
-	tree.putBool("sync", args.runSyncPhase);
-	tree.putBool("trunc", args.doTruncate);
-	tree.putBool("trunctosize", args.doTruncToSize);
-	tree.putBool("treerand", args.useCustomTreeRandomize);
-	tree.put("treeroundup", args.treeRoundUpSize);
-	tree.putBool("verifydirect", args.doDirectVerify);
-
-	// dynamically calculated values for service hosts (:3845-3861)
-	tree.put("rankoffset", args.noSharedServicePath ?
-		args.rankOffset : (args.rankOffset + (serviceRank * args.numThreads) ) );
-	tree.put("treefile", args.treeFilePath.empty() ? "" : "treefile.txt"); // ProgArgs.cpp:3850
-	if(!args.assignGPUPerService || args.gpuIDs.empty() )
-		tree.put("gpuids", args.gpuIDsStr);
-	else
-	{ // --gpuperservice: one GPU of the list per service instance (ProgArgs.cpp:3852-3859)
-		const size_t gpuIndex = serviceRank % args.gpuIDs.size();
-		tree.put("gpuids", std::to_string(args.gpuIDs[gpuIndex] ) );
-	}
-
-	// extensions of this build
-	tree.put("b200_randseed", args.randOffsetSeed);
-	tree.put("b200_blockvarseed", args.blockVarianceSeed);
-	tree.put("b200_verifyrand", args.randomVerifySeed);
-	tree.put("b200_verifyrandgrain", args.randomVerifyGrain);
-	tree.put("b200_dedupepct", args.dedupePercent);
-	tree.put("b200_batchblocks", args.pipelineBatchBlocks);
-	tree.put("b200_numbatches", args.pipelineNumBatches);
-	tree.putBool("b200_writegate", args.serializeBufferedWrites);
-	tree.putBool("b200_nowritegate", args.neverSerializeBufferedWrites);
-	tree.put("b200_staging", args.stagingEngineStr);
-	tree.putBool("b200_nogpunuma", args.noGPUNumaBinding);
 
 	return tree;
 }

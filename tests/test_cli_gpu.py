@@ -181,6 +181,45 @@ def test_distributed_mode_two_services_on_localhost(workdir):
                 svc.kill()
 
 
+def test_travelling_options_through_a_service_match_a_local_run(workdir):
+    """options that travel to a service, off their defaults: a run through one local service
+    writes the bytes of a local run, counts the same entries and bytes and verifies cleanly"""
+    common = ["-t", "2", "-b", "64k", "-s", "8m", "--gpuids", "0", "--nolive"]
+    verify = ["--verifyrand", "7", "--verifyrandgrain", "64k", "--dedupepct", "20",
+              "--blockvarpct", "37"]
+    runs = [  # (command, file name, bytes); the read reads the file of the verified write
+        (["-w", "--blockvarpct", "37", "--blockvarseed", "5", "--iodepth", "4", "--trunc",
+          "--staging", "kernel", "--batchblocks", "3", "--numbatches", "2", "--nogpunuma"],
+         "plain", 8 * MiB),
+        (["-w"] + verify, "verified", 8 * MiB),
+        (["-r", "--rand", "--norandalign", "--randseed", "9", "--randamount", "3m"] + verify,
+         "verified", 3 * MiB)]
+    port = free_port()
+    service = subprocess.Popen([CLI_PATH, "--service", "--foreground", "--port", str(port)],
+                               stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+    try:
+        wait_for_port(port)
+        for idx, (command, name, num_bytes) in enumerate(runs):
+            totals = []
+            for where, hosts in (("local", []), ("svc", ["--hosts", "127.0.0.1:%d" % port])):
+                json_path = os.path.join(workdir, "%s_%d.json" % (where, idx))
+                res = run_cli(*hosts, *common, *command, "--jsonfile", json_path,
+                              os.path.join(workdir, where + "_" + name))
+                assert res.returncode == 0, res.stdout + res.stderr
+                with open(json_path) as f:
+                    totals.append(json.loads(f.read())["last_done"])
+            assert totals[0]["bytes"] == totals[1]["bytes"] == str(num_bytes)
+            assert totals[0].get("entries") == totals[1].get("entries")
+            with open(os.path.join(workdir, "local_" + name), "rb") as local, \
+                    open(os.path.join(workdir, "svc_" + name), "rb") as remote:
+                assert local.read() == remote.read()
+        assert run_cli("--hosts", "127.0.0.1:%d" % port, "--quit").returncode == 0
+        service.wait(timeout=30)
+    finally:
+        if service.poll() is None:
+            service.kill()
+
+
 def test_rate_limit_infloop_livecsv_and_start_time(workdir):
     """run control options of the reference: --limitwrite (RateLimiter.h), --infloop +
     --timelimit (LocalWorker.cpp:196-364), --livecsv (Statistics.cpp:2944-3113), --start"""
