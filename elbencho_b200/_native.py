@@ -51,6 +51,7 @@ class Cfg(ctypes.Structure):
         ("ioDepth", c_u32),
         ("useDirectIO", c_i32),
         ("ioEngine", c_i32),
+        ("checksumReport", c_i32),
         ("numDirs", c_u64),
         ("numFiles", c_u64),
         ("doDirSharing", c_i32),
@@ -242,6 +243,9 @@ SIGNATURES = {
     "elb_rand_grain_content_key": (c_u64, [c_u64, c_u64, c_u64, ctypes.c_uint, ctypes.c_uint]),
     "elb_rand_pos_counter": (c_u64, [c_u64, c_u64]),
     "elb_rand_dir_file_key": (c_u64, [c_u64, c_u64, c_u64]),
+    "elb_crc32_blocks": (ctypes.c_int, [_VP, _VP, c_u32, _VP, _VP, _VP, _VP]),
+    "elb_crc32_shift": (c_u32, [c_u32, c_u64]),
+    "elb_crc32_finish": (c_u32, [c_u32, c_u64]),
     "elb_damage_map": (ctypes.c_int, [_VP, c_u32, ctypes.c_int, c_u64, ctypes.c_uint,
                                       ctypes.c_uint, ctypes.c_uint, _VP, c_u64, _VP]),
     "elb_stage_copy": (ctypes.c_int, [_VP, c_u32, ctypes.c_int, ctypes.c_int64, c_u64, c_u64,
@@ -307,6 +311,7 @@ SIGNATURES = {
                                                 ctypes.POINTER(c_u64)]),
     "elb_mgr_interrupt": (ctypes.c_int, [_VP]),
     "elb_mgr_verify_report": (ctypes.c_int64, [_VP, ctypes.c_char_p, c_u64]),
+    "elb_mgr_checksums": (ctypes.c_int64, [_VP, ctypes.c_char_p, c_u64]),
     "elb_mgr_num_workers": (c_u32, [_VP]),
     "elb_mgr_worker": (_VP, [_VP, c_u32]),
     "elb_mgr_last_error": (ctypes.c_char_p, [_VP]),

@@ -403,6 +403,41 @@ int elb_damage_map(const elb_block_desc* descs, uint32_t numDescs, int contentKi
 	return 0;
 }
 
+int elb_crc32_blocks(const elb_block_desc* descs, const uint64_t* shifts, uint32_t numDescs,
+	uint32_t* devCrcs, uint32_t* hostCrcs, unsigned* devTicket, void* stream)
+{
+	if(numDescs && (!descs || !shifts || !devCrcs) )
+	{
+		elb_set_last_error("elb_crc32_blocks: NULL descriptor, shift or CRC array");
+		return -1;
+	}
+
+	if(!hostCrcs != !devTicket)
+	{
+		elb_set_last_error("elb_crc32_blocks: host CRCs and device ticket go together");
+		return -1;
+	}
+
+	if(elb_launch_crc32(descs, shifts, numDescs, devCrcs, hostCrcs, devTicket,
+		(cudaStream_t)stream) )
+	{
+		elb_set_last_error(std::string("elb_") + elb_last_error() );
+		return -1;
+	}
+
+	return 0;
+}
+
+uint32_t elb_crc32_shift(uint32_t crc, uint64_t n)
+{
+	return elb_crc32_shift_hd(crc, n);
+}
+
+uint32_t elb_crc32_finish(uint32_t rawCrc, uint64_t size)
+{
+	return elb_crc32_finish_hd(rawCrc, size);
+}
+
 int elb_stage_copy(const elb_block_desc* descs, uint32_t numDescs, int hostToDevice,
 	int64_t hostDelta, uint64_t totalBytes, uint64_t maxBlockLen, void* stream)
 {

@@ -120,6 +120,13 @@ static const OptDef optDefs[] =
 		"file (truncated at start): \"# phase READ|WRITE\", then one tab-separated line \"path "
 		"offset length differing_bytes\" per damaged extent. The phase still fails at its end with "
 		"the error of the first bad block. Requires --verify or --verifyrand. [b200]"},
+	{"checksums", 0, Opt_STR, &ProgArgs::checksumsPath, Wire_NONE, "Path of a checksum file: every "
+		"write and read phase computes the CRC-32 (zlib, gzip, zip) of each file on the GPU from "
+		"the bytes that pass through GPU memory and appends one section to this file (truncated at "
+		"start): \"# phase WRITE|READ\", then one line \"path size bytes_covered crc32\" per "
+		"file, sorted by path. The CRC is given when the phase covered the file's first size "
+		"bytes exactly once, else \"-\". With --verifydirect only the written bytes count. Cannot "
+		"be used with --rand, --infloop, --rwmixpct, --rwmixthr or --hosts. [b200]"},
 	{"rwmixpct", 0, Opt_U64, &ProgArgs::rwMixReadPercent, Wire_REF, "Percentage of blocks that "
 		"should be read in a write phase."},
 	{"rwmixthr", 0, Opt_U64, &ProgArgs::numRWMixReadThreads, Wire_REF, "Number of threads that "
@@ -964,6 +971,24 @@ void ProgArgs::checkArgs()
 	if(!verifyReportPath.empty() && !hosts.empty() )
 		throw ProgError("Option \"--verifyreport\" cannot be used together with \"--hosts\"");
 
+	if(!checksumsPath.empty() )
+	{ // (each file's blocks exactly once, in one direction, on this host)
+		if(useRandomOffsets)
+			throw ProgError("Option \"--checksums\" cannot be used together with \"--rand\"");
+
+		if(doInfiniteIOLoop)
+			throw ProgError("Option \"--checksums\" cannot be used together with \"--infloop\"");
+
+		if(rwMixReadPercent)
+			throw ProgError("Option \"--checksums\" cannot be used together with \"--rwmixpct\"");
+
+		if(numRWMixReadThreads)
+			throw ProgError("Option \"--checksums\" cannot be used together with \"--rwmixthr\"");
+
+		if(!hosts.empty() )
+			throw ProgError("Option \"--checksums\" cannot be used together with \"--hosts\"");
+	}
+
 	if(doDirectVerify && ( (!integrityCheckSalt && !randomVerifySeed) || !runCreateFilesPhase) )
 		throw ProgError("Direct verification requires --verify and --write"); // :1426-1428
 
@@ -1056,6 +1081,7 @@ void ProgArgs::toABIConfig(ABIConfig& out) const
 	cfg.runAsService = runAsService;
 	cfg.verifyCollectAll = 0;
 	cfg.verifyDamageReport = !verifyReportPath.empty();
+	cfg.checksumReport = !checksumsPath.empty();
 	cfg.serializeBufferedWrites = neverSerializeBufferedWrites ? ELB_WRITEGATE_OFF :
 		(serializeBufferedWrites ? ELB_WRITEGATE_ON : ELB_WRITEGATE_AUTO);
 	cfg.noGPUNumaBinding = noGPUNumaBinding;

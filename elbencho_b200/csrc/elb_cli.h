@@ -86,6 +86,7 @@ class ProgArgs
 		uint64_t randomVerifyGrain{0}; // --verifyrandgrain (bytes, 0 = per block)
 		uint64_t dedupePercent{0}; // --dedupepct
 		std::string verifyReportPath; // --verifyreport
+		std::string checksumsPath; // --checksums
 		uint64_t rwMixReadPercent{0};
 		bool hasUserSetRWMixPercent{false};
 		uint64_t numRWMixReadThreads{0};

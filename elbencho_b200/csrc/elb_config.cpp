@@ -102,6 +102,7 @@ Config Config::fromABI(const elb_cfg* cfg)
 	c.runAsService = cfg->runAsService;
 	c.verifyCollectAll = cfg->verifyCollectAll;
 	c.verifyDamageReport = (cfg->verifyDamageReport != 0);
+	c.checksums = (cfg->checksumReport != 0);
 	c.serializeBufferedWrites = cfg->serializeBufferedWrites;
 	c.numRWMixReadThreads = std::min(cfg->numRWMixReadThreads, cfg->numThreads); // :1088
 	c.treeFilePath = cfg->treeFilePath ? cfg->treeFilePath : "";
@@ -191,6 +192,18 @@ Config Config::fromABI(const elb_cfg* cfg)
 	if(c.dedupePercent && !c.useRandomVerifyGrain() )
 		throw WorkerError("A dedupe percentage (--dedupepct) requires a random verify grain "
 			"(--verifyrandgrain).");
+
+	if(c.checksums && c.useRandomOffsets)
+		throw WorkerError("Checksums (--checksums) cannot be used together with random offsets: "
+			"they need every block of a file exactly once.");
+
+	if(c.checksums && c.doInfiniteIOLoop)
+		throw WorkerError("Checksums (--checksums) cannot be used together with an infinite I/O "
+			"loop (--infloop).");
+
+	if(c.checksums && (c.rwMixReadPercent || c.numRWMixReadThreads) )
+		throw WorkerError("Checksums (--checksums) cannot be used together with rwmix (a phase in "
+			"both directions).");
 
 	if(c.verifyDamageReport && !c.integrityCheckSalt)
 		throw WorkerError("A verify report (--verifyreport) requires data verification (--verify "

@@ -100,6 +100,7 @@ class Coordinator
 			uint64_t elapsedSec);
 		void printPhaseResultsEverywhere(int benchPhase, const std::string& isoStartDate);
 		void writeVerifyReportSection(int benchPhase);
+		void writeChecksumSection(int benchPhase);
 		void printDryRunInfo();
 };
 
@@ -429,6 +430,27 @@ void Coordinator::writeVerifyReportSection(int benchPhase)
 		progArgs.verifyReportPath << std::endl;
 }
 
+/* --checksums: after each write and read phase that succeeded, its section of the checksum file
+ * and one console line */
+void Coordinator::writeChecksumSection(int benchPhase)
+{
+	if(progArgs.checksumsPath.empty() ||
+		( (benchPhase != ELB_PHASE_CREATEFILES) && (benchPhase != ELB_PHASE_READFILES) ) )
+		return;
+
+	const Manager::ChecksumReport report = manager->getChecksumReport();
+	std::ofstream fileStream(progArgs.checksumsPath, std::ofstream::app);
+
+	fileStream << "# phase " << ( (benchPhase == ELB_PHASE_READFILES) ? "READ" : "WRITE") << "\n" <<
+		report.lines << std::flush;
+
+	if(!fileStream)
+		throw ProgError("Writing checksum file failed: " + progArgs.checksumsPath);
+
+	std::cout << "Checksums: " << report.numFiles << " files, " << report.numComplete <<
+		" complete: " << progArgs.checksumsPath << std::endl;
+}
+
 /* Coordinator::runBenchmarkPhase (:248-272) + Statistics live loop (:1284-1345) */
 void Coordinator::runBenchmarkPhase(int benchPhase)
 {
@@ -545,10 +567,24 @@ void Coordinator::runBenchmarkPhase(int benchPhase)
 		writeVerifyReportSection(benchPhase);
 
 		std::string errMsg;
+		bool failedOnlyOnDamage;
 		{
 			std::unique_lock<std::mutex> lock(manager->shared.mutex);
 			errMsg = manager->shared.firstErrorMsg;
+
+			size_t numDamaged = 0;
+			for(const std::unique_ptr<Worker>& worker : manager->workers)
+				numDamaged += !worker->getDeferredVerifyError().empty();
+
+			failedOnlyOnDamage = numDamaged &&
+				(manager->shared.numWorkersDone == manager->workers.size() ) &&
+				(manager->shared.numWorkersDoneWithError == numDamaged);
 		}
+
+		/* --verifyreport reads on past bad blocks: if they are all that failed, every block was
+		   read and the checksums are those of the damaged bytes */
+		if(failedOnlyOnDamage)
+			writeChecksumSection(benchPhase);
 
 		if(!errMsg.empty() )
 			std::cerr << "ERROR: " << errMsg << std::endl;
@@ -560,6 +596,7 @@ void Coordinator::runBenchmarkPhase(int benchPhase)
 	{
 		printPhaseResultsEverywhere(benchPhase, isoStartDate);
 		writeVerifyReportSection(benchPhase);
+		writeChecksumSection(benchPhase);
 	}
 	else
 	{ // (sync and dropcache phases print only their elapsed time)
@@ -705,6 +742,10 @@ int Coordinator::main() // Coordinator.cpp:31-142
 		if(!progArgs.verifyReportPath.empty() &&
 			!std::ofstream(progArgs.verifyReportPath, std::ofstream::trunc) )
 			throw ProgError("Unable to create verify report file: " + progArgs.verifyReportPath);
+
+		if(!progArgs.checksumsPath.empty() &&
+			!std::ofstream(progArgs.checksumsPath, std::ofstream::trunc) )
+			throw ProgError("Unable to create checksum file: " + progArgs.checksumsPath);
 
 		waitForUserDefinedStartTime(progArgs);
 

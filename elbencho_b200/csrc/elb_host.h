@@ -1001,6 +1001,7 @@ struct Config
 	bool runAsService{false};
 	bool verifyCollectAll{false};
 	bool verifyDamageReport{false}; // --verifyreport
+	bool checksums{false}; // --checksums
 	int serializeBufferedWrites{ELB_WRITEGATE_AUTO};
 	int stagingEngine{ELB_STAGING_AUTO};
 	bool noGPUNumaBinding{false};

@@ -11,6 +11,8 @@
  *      with the dedupe grain key, elb_patterns.cuh)
  *   damage_map (no reference counterpart: --verifyreport, where the bytes of blocks known to be
  *      bad differ, per 512-byte file sector; off the clean path, see its section below)
+ *   crc32 (no reference counterpart: --checksums, each block's share of its file's CRC-32; off the
+ *      clean path, see its section below)
  *
  * All eight are HBM-bound byte/integer kernels (K1/K3/K5/K7: 1 byte written per payload byte,
  * K2/K4/K6/K8: 1 byte read per payload byte), so the design follows the streaming rules: 16-byte (128-bit) vector
@@ -1139,6 +1141,211 @@ elb_damage_map_kernel(const KernelArgs args, elb_sector_damage* sectors, uint64_
 	}
 }
 
+/* ---- CRC-32 contributions (--checksums) ------------------------------------------------------
+ *
+ * One 32-bit contribution per descriptor: X(R(block), shifts[i]) (elb_patterns.cuh), XORed into
+ * crcs[i]. A warp takes one 4 KiB chunk of one block at a time, walking the grid-stride sequence of
+ * all (descriptor, chunk) pairs, so that the warps of a CTA never wait for each other and small
+ * blocks keep every warp busy. Chunks are laid out from the 16-byte aligned address at or below
+ * the block's device address, so that every lane loads 16-byte vectors: lane l owns the 128
+ * contiguous bytes [l * 128, l * 128 + 128) of the chunk, issues its 8 loads first and then folds
+ * them with slicing-by-8 tables that the CTA builds in shared memory once. Bytes of the chunk
+ * outside the block (its unaligned head and tail, past its end) count as zeros: zeros in front of
+ * the data do not change a raw CRC, zeros behind it shift it, which the shift to the file end
+ * takes back. Each lane shifts its value to the chunk end by a per-lane constant and the warp XORs
+ * the 32 values. The chunk's shift to the file end is known before its bytes arrive: while the
+ * loads are in flight, the warp computes x^(8n) with one lane per bit of n and a 5-level shuffle
+ * product; lane 0 applies it and atomicXors the result into crcs[i]. With hostCrcs, the last CTA
+ * of the launch (ticket) copies crcs to pinned host memory and zeroes them for the next launch, as
+ * the verify launches do with their results. */
+
+#define ELB_CRC_PART_BYTES (ELB_VEC_BYTES * ELB_UNROLL) /* 128: a lane's bytes of a chunk */
+#define ELB_CRC_CHUNK_BYTES (32 * ELB_CRC_PART_BYTES)  /* 4 KiB: a warp's bytes */
+
+struct Crc32Consts
+{
+	uint32_t x8pow2[32];    // x^(8 * 2^k) mod P
+	uint32_t laneShift[32]; // x^(8 * 128 * (31 - l)) mod P: lane l's part to the chunk end
+
+	constexpr Crc32Consts() : x8pow2{}, laneShift{}
+	{
+		for(unsigned k = 0; k < 32; k++)
+			x8pow2[k] = elb_crc32_x8pow2(k);
+
+		for(unsigned l = 0; l < 32; l++)
+		{
+			const uint32_t n = (31 - l) * ELB_CRC_PART_BYTES;
+			uint32_t shift = ELB_CRC32_ONE;
+
+			for(unsigned k = 0; k < 32; k++)
+				if( (n >> k) & 1)
+					shift = elb_crc32_mulmod(shift, x8pow2[k]);
+
+			laneShift[l] = shift;
+		}
+	}
+};
+
+static __constant__ Crc32Consts gCrc32Consts = Crc32Consts();
+
+/* 16 bytes at a 16-byte aligned address, with L1 allocation: a warp instruction takes 16 bytes of
+   32 different lines, the lane's next loads take the rest of those lines */
+__device__ __forceinline__ u64x2 ld_nc_128(const void* ptr)
+{
+	u64x2 v;
+	asm volatile("ld.global.nc.v2.u64 {%0,%1}, [%2];" : "=l"(v.a), "=l"(v.b) : "l"(ptr) );
+	return v;
+}
+
+/* R(crc's message || the 8 little-endian bytes of w) */
+__device__ __forceinline__ uint32_t crc32_fold8(uint32_t crc, uint64_t w,
+	const uint32_t (*table)[256])
+{
+	const uint32_t lo = crc ^ (uint32_t)w;
+	const uint32_t hi = (uint32_t)(w >> 32);
+
+	return table[7][lo & 0xff] ^ table[6][(lo >> 8) & 0xff] ^ table[5][(lo >> 16) & 0xff] ^
+		table[4][lo >> 24] ^ table[3][hi & 0xff] ^ table[2][(hi >> 8) & 0xff] ^
+		table[1][(hi >> 16) & 0xff] ^ table[0][hi >> 24];
+}
+
+__global__ void __launch_bounds__(ELB_THREADS)
+elb_crc32_kernel(const elb_block_desc* descs, const uint64_t* shifts, uint32_t numDescs,
+	uint64_t chunksPerDesc, uint32_t* crcs, uint32_t* hostCrcs, unsigned* doneTicket)
+{
+	__shared__ uint32_t sTable[8][256]; // sTable[k][i] = R(byte i followed by k zero bytes)
+	__shared__ bool sIsLastCTA;
+
+	const unsigned lane = threadIdx.x & 31;
+
+	{
+		uint32_t entry = elb_crc32_byte_table(threadIdx.x);
+		sTable[0][threadIdx.x] = entry;
+
+		__syncthreads();
+
+		#pragma unroll
+		for(int k = 1; k < 8; k++)
+		{
+			entry = (entry >> 8) ^ sTable[0][entry & 0xff];
+			sTable[k][threadIdx.x] = entry;
+		}
+
+		__syncthreads();
+	}
+
+	const uint32_t laneShift = gCrc32Consts.laneShift[lane];
+	const uint32_t laneX8Pow2 = gCrc32Consts.x8pow2[lane];
+	const uint64_t numItems = (uint64_t)numDescs * chunksPerDesc;
+	const uint64_t numWarps = (uint64_t)gridDim.x * ELB_WARPS;
+
+	for(uint64_t item = (uint64_t)blockIdx.x * ELB_WARPS + (threadIdx.x >> 5); item < numItems;
+		item += numWarps)
+	{ // (uniform for the warp)
+		const uint32_t descIdx = (uint32_t)( (chunksPerDesc == 1) ? item : (item / chunksPerDesc) );
+		const uint64_t chunkBegin = (item - (uint64_t)descIdx * chunksPerDesc) * ELB_CRC_CHUNK_BYTES;
+		const elb_block_desc desc = descs[descIdx];
+		const uint64_t shift = shifts[descIdx];
+		const uint64_t headPad = (uint64_t)(uintptr_t)desc.devPtr & (ELB_VEC_BYTES - 1);
+		const uint64_t end = headPad + desc.len; // chunk positions of the block: [headPad, end)
+
+		if(chunkBegin >= end)
+			continue;
+
+		const uint8_t* base = (const uint8_t*)desc.devPtr - headPad;
+		const uint64_t partBegin = chunkBegin + lane * ELB_CRC_PART_BYTES;
+		const bool hasBytes = (partBegin < end) && (partBegin + ELB_CRC_PART_BYTES > headPad);
+		const bool isWholePart = (partBegin >= headPad) && (partBegin + ELB_CRC_PART_BYTES <= end);
+		u64x2 vecs[ELB_UNROLL];
+
+		if(isWholePart)
+		{
+			#pragma unroll
+			for(int u = 0; u < ELB_UNROLL; u++)
+				vecs[u] = ld_nc_128(base + partBegin + u * ELB_VEC_BYTES);
+		}
+
+		/* (while the loads are in flight) x^(8n), n = bytes from the chunk end (chunkBegin +
+		   4 KiB) to the file end (end + shift) mod 2^32 - 1: lane k contributes bit k of n */
+		const uint64_t n = elb_crc32_mod_order(elb_crc32_mod_order(shift) +
+			elb_crc32_mod_order(end) + ELB_CRC32_ORDER -
+			elb_crc32_mod_order(chunkBegin + ELB_CRC_CHUNK_BYTES) );
+		uint32_t factor = ( (n >> lane) & 1) ? laneX8Pow2 : ELB_CRC32_ONE;
+
+		for(int offset = 16; offset > 0; offset >>= 1)
+			factor = elb_crc32_mulmod(factor, __shfl_xor_sync(0xffffffffu, factor, offset) );
+
+		uint32_t crc = 0;
+
+		if(hasBytes)
+		{ // (else the part is all zeros)
+			if(!isWholePart)
+			{ // the block's head or tail: byte by byte, zeros outside the block
+				#pragma unroll
+				for(int u = 0; u < ELB_UNROLL; u++)
+				{
+					const uint64_t vecBegin = partBegin + u * ELB_VEC_BYTES;
+					uint64_t lo = 0, hi = 0;
+
+					#pragma unroll 1
+					for(int b = 0; b < 8; b++)
+					{
+						if( (vecBegin + b >= headPad) && (vecBegin + b < end) )
+							lo |= (uint64_t)base[vecBegin + b] << (b * 8);
+
+						if( (vecBegin + 8 + b >= headPad) && (vecBegin + 8 + b < end) )
+							hi |= (uint64_t)base[vecBegin + 8 + b] << (b * 8);
+					}
+
+					vecs[u] = u64x2{lo, hi};
+				}
+			}
+
+			#pragma unroll
+			for(int u = 0; u < ELB_UNROLL; u++)
+			{
+				crc = crc32_fold8(crc, vecs[u].a, sTable);
+				crc = crc32_fold8(crc, vecs[u].b, sTable);
+			}
+
+			crc = elb_crc32_mulmod(crc, laneShift);
+		}
+
+		for(int offset = 16; offset > 0; offset >>= 1)
+			crc ^= __shfl_xor_sync(0xffffffffu, crc, offset);
+
+		if(!lane && crc)
+			atomicXor(&crcs[descIdx], elb_crc32_mulmod(crc, factor) );
+	}
+
+	if(!hostCrcs)
+		return;
+
+	__threadfence(); // order this CTA's atomics before its ticket
+	__syncthreads();
+
+	if(!threadIdx.x)
+		sIsLastCTA = (atomicAdd(doneTicket, 1u) == (gridDim.x - 1) );
+
+	__syncthreads();
+
+	if(!sIsLastCTA)
+		return;
+
+	__threadfence();
+
+	for(uint32_t i = threadIdx.x; i < numDescs; i += blockDim.x)
+	{
+		volatile uint32_t* devCrc = &crcs[i];
+
+		hostCrcs[i] = *devCrc;
+		*devCrc = 0;
+	}
+
+	if(!threadIdx.x)
+		*doneTicket = 0;
+}
+
 /* ---- host side launchers ------------------------------------------------------------------ */
 
 static std::atomic<uint64_t> gNumKernelLaunches{0};
@@ -1154,6 +1361,7 @@ struct DeviceLaunchInfo
 {
 	int numSMs{0};
 	int ctasPerSM[NUM_MODES]{};
+	int crcCtasPerSM{0};
 };
 
 /* 32 KiB tiles per CTA of the hardware-scheduled kernel, per mode. H100: 1/1/4, 2/4/8, 4/4/16 for
@@ -1200,6 +1408,9 @@ static const DeviceLaunchInfo* getDeviceLaunchInfo()
 		gDevInfo[dev].ctasPerSM[MODE_FILL_DEDUPE_GRAIN] = queryOccupancy<MODE_FILL_DEDUPE_GRAIN>();
 		gDevInfo[dev].ctasPerSM[MODE_VERIFY_DEDUPE_GRAIN] =
 			queryOccupancy<MODE_VERIFY_DEDUPE_GRAIN>();
+		cudaOccupancyMaxActiveBlocksPerMultiprocessor(&gDevInfo[dev].crcCtasPerSM, elb_crc32_kernel,
+			ELB_THREADS, 0);
+		gDevInfo[dev].crcCtasPerSM = std::max(gDevInfo[dev].crcCtasPerSM, 1);
 	});
 
 	if(gDevInfo[dev].numSMs <= 0)
@@ -1531,6 +1742,38 @@ int elb_launch_damage_map(const elb_content& content, const elb_block_desc* desc
 
 		return checkLaunch("damage_map");
 	});
+}
+
+int elb_launch_crc32(const elb_block_desc* descs, const uint64_t* shifts, uint32_t numDescs,
+	uint32_t* devCrcs, uint32_t* hostCrcs, unsigned* doneTicket, cudaStream_t stream)
+{
+	if(!numDescs)
+		return 0;
+
+	const DeviceLaunchInfo* devInfo = getDeviceLaunchInfo();
+	if(!devInfo)
+		return -1;
+
+	uint64_t chunksPerDesc = 0;
+
+	for(uint32_t i = 0; i < numDescs; i++)
+	{ // (descs are host-readable)
+		const uint64_t headPad = (uint64_t)(uintptr_t)descs[i].devPtr & (ELB_VEC_BYTES - 1);
+		chunksPerDesc = std::max(chunksPerDesc,
+			(headPad + descs[i].len + ELB_CRC_CHUNK_BYTES - 1) / ELB_CRC_CHUNK_BYTES);
+	}
+
+	/* a grid that stays resident: each CTA builds its tables once and its warps walk many chunks
+	   (at least one CTA, whose ticket publishes the results also when no block has a byte) */
+	const uint64_t numItems = (uint64_t)numDescs * chunksPerDesc;
+	const uint64_t gridSize = std::max( (uint64_t)1, std::min( (numItems + ELB_WARPS - 1) /
+		ELB_WARPS, (uint64_t)devInfo->numSMs * devInfo->crcCtasPerSM) );
+
+	elb_crc32_kernel<<<(unsigned)gridSize, ELB_THREADS, 0, stream>>>(descs, shifts, numDescs,
+		chunksPerDesc ? chunksPerDesc : 1, devCrcs, hostCrcs, doneTicket);
+	gNumKernelLaunches.fetch_add(1, std::memory_order_relaxed);
+
+	return checkLaunch("crc32");
 }
 
 /* query launch geometry of the current device now (so that no attribute/occupancy query happens

@@ -514,6 +514,48 @@ Manager::VerifyReport Manager::getVerifyReport()
 	return report;
 }
 
+/**
+ * --checksums: the workers' accumulators merged by path (a file that several workers share has a
+ * part in each): XOR of the raw CRCs, sum of the bytes. A file's CRC is complete when the phase
+ * moved as many bytes of it as its size; the phase's block sources cover each byte once at most.
+ */
+Manager::ChecksumReport Manager::getChecksumReport()
+{
+	std::map<std::string, FileChecksum> files;
+
+	for(const std::unique_ptr<Worker>& worker : workers)
+		for(const FileChecksum& part : worker->getFileChecksums() )
+		{
+			FileChecksum& file = files[part.path];
+
+			file.size = part.size;
+			file.numBytes += part.numBytes;
+			file.rawCrc ^= part.rawCrc;
+		}
+
+	ChecksumReport report;
+
+	for(const auto& entry : files)
+	{
+		const FileChecksum& file = entry.second;
+		std::string crcStr = "-";
+
+		if(file.numBytes == file.size)
+		{
+			char hex[9];
+			snprintf(hex, sizeof(hex), "%08x", elb_crc32_finish_hd(file.rawCrc, file.size) );
+			crcStr = hex;
+			report.numComplete++;
+		}
+
+		report.lines += entry.first + " " + std::to_string(file.size) + " " +
+			std::to_string(file.numBytes) + " " + crcStr + "\n";
+		report.numFiles++;
+	}
+
+	return report;
+}
+
 /* Statistics::generatePhaseResults (Statistics.cpp:1641-1764) */
 void Manager::getPhaseResults(elb_phase_results& out)
 {
@@ -1245,6 +1287,26 @@ int64_t elb_mgr_verify_report(elb_mgr* m, char* outBuf, uint64_t outBufLen)
 	}
 
 	const std::string text = m->impl->getVerifyReport().lines;
+
+	if(outBuf && outBufLen)
+	{
+		const size_t copyLen = std::min( (size_t)(outBufLen - 1), text.size() );
+		memcpy(outBuf, text.data(), copyLen);
+		outBuf[copyLen] = 0;
+	}
+
+	return (int64_t)text.size();
+}
+
+int64_t elb_mgr_checksums(elb_mgr* m, char* outBuf, uint64_t outBufLen)
+{
+	if(!m)
+	{
+		elb_set_last_error("elb_mgr_checksums: NULL manager");
+		return -1;
+	}
+
+	const std::string text = m->impl->getChecksumReport().lines;
 
 	if(outBuf && outBufLen)
 	{

@@ -276,4 +276,91 @@ ELB_HD uint64_t elb_rand_grain_bytes8(uint64_t filePos, const Keys& keys, uint64
 	return val;
 }
 
+/* ---- CRC-32 of what passed through GPU memory (--checksums) ------------------------------------
+ *
+ * R(M) is the raw reflected CRC-32 of M: polynomial P = 0xEDB88320, register 0 at the start, no
+ * final XOR. Bit 31 of a value is the coefficient of x^0. R is linear:
+ *   R(A || B) = X(R(A), |B|) ^ R(B),   X(c, n) = c * x^(8n) mod P (c followed by n zero bytes)
+ * so a block at file offset o of length len in a file of size S contributes X(R(block), S - o - len),
+ * and a file's R is the XOR of its blocks' contributions in any order. zlib's CRC-32 (gzip, zip,
+ * Python's zlib.crc32) starts with 0xFFFFFFFF and inverts at the end:
+ *   crc32(M) = R(M) ^ X(0xFFFFFFFF, |M|) ^ 0xFFFFFFFF
+ * x^(2^32 - 1) = 1 mod P, so X(c, n) = X(c, n mod (2^32 - 1)): shifts may also be negative. */
+
+#define ELB_CRC32_POLY 0xEDB88320u
+#define ELB_CRC32_ONE 0x80000000u           /* x^0 */
+#define ELB_CRC32_X8 0x00800000u            /* x^8: one zero byte */
+#define ELB_CRC32_ORDER 0xFFFFFFFFULL       /* x^ELB_CRC32_ORDER = 1 mod P */
+
+/* n mod ELB_CRC32_ORDER without a 64-bit division (2^32 = 1 mod 2^32 - 1) */
+ELB_HD constexpr uint64_t elb_crc32_mod_order(uint64_t n)
+{
+	n = (n & 0xFFFFFFFFULL) + (n >> 32); // < 2^33
+	n = (n & 0xFFFFFFFFULL) + (n >> 32); // <= 2^32
+	return (n >= ELB_CRC32_ORDER) ? (n - ELB_CRC32_ORDER) : n;
+}
+
+/* a * b mod P */
+ELB_HD constexpr uint32_t elb_crc32_mulmod(uint32_t a, uint32_t b)
+{
+	uint32_t prod = 0;
+
+	for(int bit = 31; bit >= 0; bit--)
+	{
+		prod ^= b & (0u - ( (a >> bit) & 1u) );
+		b = (b >> 1) ^ (ELB_CRC32_POLY & (0u - (b & 1u) ) );
+	}
+
+	return prod;
+}
+
+/* x^(8 * 2^k) mod P */
+ELB_HD constexpr uint32_t elb_crc32_x8pow2(unsigned k)
+{
+	uint32_t pow = ELB_CRC32_X8;
+
+	for(unsigned i = 0; i < k; i++)
+		pow = elb_crc32_mulmod(pow, pow);
+
+	return pow;
+}
+
+/* x^(8n) mod P by square-and-multiply */
+ELB_HD constexpr uint32_t elb_crc32_x8n(uint64_t n)
+{
+	uint32_t result = ELB_CRC32_ONE;
+	uint32_t pow = ELB_CRC32_X8;
+
+	for(n = elb_crc32_mod_order(n); n; n >>= 1)
+	{
+		if(n & 1)
+			result = elb_crc32_mulmod(result, pow);
+
+		pow = elb_crc32_mulmod(pow, pow);
+	}
+
+	return result;
+}
+
+/* X(crc, n): crc followed by n zero bytes */
+ELB_HD constexpr uint32_t elb_crc32_shift_hd(uint32_t crc, uint64_t n)
+{
+	return elb_crc32_mulmod(crc, elb_crc32_x8n(n) );
+}
+
+/* zlib's CRC-32 of a message of size bytes from its raw CRC R */
+ELB_HD constexpr uint32_t elb_crc32_finish_hd(uint32_t rawCrc, uint64_t size)
+{
+	return rawCrc ^ elb_crc32_shift_hd(0xFFFFFFFFu, size) ^ 0xFFFFFFFFu;
+}
+
+/* R of the single byte i (the byte-wise table; R(M || b) = (R(M) >> 8) ^ T[(R(M) ^ b) & 0xff]) */
+ELB_HD constexpr uint32_t elb_crc32_byte_table(uint32_t i)
+{
+	for(int bit = 0; bit < 8; bit++)
+		i = (i >> 1) ^ (ELB_CRC32_POLY & (0u - (i & 1u) ) );
+
+	return i;
+}
+
 #endif /* ELB_PATTERNS_CUH_ */

@@ -341,6 +341,7 @@ void Worker::resetStats() // Worker.h:92-110
 	numDamageRunsDropped = 0;
 	numDamageBytesDropped = 0;
 	deferredVerifyError.clear();
+	checksumAccs.clear();
 
 	std::unique_lock<std::mutex> lock(errorMutex);
 	lastError.clear();
@@ -867,8 +868,14 @@ void Worker::allocRings()
 		salt ? elb_content{elb_content::PATTERN, salt} :
 		pct ? elb_content{elb_content::RANDOM, blockVarianceSeed, pct} : elb_content{};
 
-	writeStage = GpuStage{false, transfer, writeContent, useGraph};
-	readStage = GpuStage{true, transfer, salt ? writeContent : elb_content{}, useGraph};
+	writeStage = GpuStage{false, transfer, writeContent, useGraph, cfg.checksums};
+	readStage = GpuStage{true, transfer, salt ? writeContent : elb_content{}, useGraph,
+		cfg.checksums};
+	/* --verifydirect: a write phase's checksums are those of the written bytes, so the read-back
+	   takes none, and must not share the read phase's batch graphs then */
+	verifyBackStage = readStage;
+	verifyBackStage.checksum = false;
+	verifyBackStage.useGraph = useGraph && !cfg.checksums;
 
 	if(cfg.pipelineBatchBlocks)
 		batchBlocks = cfg.pipelineBatchBlocks;
@@ -946,6 +953,18 @@ void Worker::allocRings()
 			"GPU ticket counter init");
 
 		memset(batch.hostResults, 0, sizeof(elb_verify_result) * batchBlocks);
+
+		if(cfg.checksums)
+		{
+			ELB_CUDA_CHECK(cudaHostAlloc( (void**)&batch.hostShifts, sizeof(uint64_t) * batchBlocks,
+				cudaHostAllocDefault), "Pinned checksum shift allocation");
+			ELB_CUDA_CHECK(cudaMalloc( (void**)&batch.devCrcs, sizeof(uint32_t) * batchBlocks),
+				"GPU checksum allocation");
+			ELB_CUDA_CHECK(cudaHostAlloc( (void**)&batch.hostCrcs, sizeof(uint32_t) * batchBlocks,
+				cudaHostAllocDefault), "Pinned checksum allocation");
+			ELB_CUDA_CHECK(cudaMemsetAsync(batch.devCrcs, 0, sizeof(uint32_t) * batchBlocks,
+				batch.stream), "GPU checksum init");
+		}
 
 		// arm the device results once; verify launches re-arm what they report
 		if(elb_launch_verify_init(batch.devResults, batchBlocks, batch.stream) )
@@ -1065,6 +1084,12 @@ void Worker::freeRings() // LocalWorker::cleanup (:1570-1641)
 			cudaFreeHost(batch.hostResults);
 		if(batch.devDoneTicket)
 			cudaFree(batch.devDoneTicket);
+		if(batch.hostShifts)
+			cudaFreeHost(batch.hostShifts);
+		if(batch.devCrcs)
+			cudaFree(batch.devCrcs);
+		if(batch.hostCrcs)
+			cudaFreeHost(batch.hostCrcs);
 	}
 
 	batches.clear();
@@ -1150,6 +1175,8 @@ void Worker::abortInFlight()
 			// (a failed launch may have left the ticket or the armed results behind)
 			cudaMemsetAsync(batch.devDoneTicket, 0, sizeof(unsigned), batch.stream);
 			elb_launch_verify_init(batch.devResults, batchBlocks, batch.stream);
+			if(batch.devCrcs)
+				cudaMemsetAsync(batch.devCrcs, 0, sizeof(uint32_t) * batchBlocks, batch.stream);
 			cudaStreamSynchronize(batch.stream);
 
 			batch.numIOPending = 0;
@@ -2139,6 +2166,9 @@ uint32_t Worker::fillStageDescs(Batch& batch, const GpuStage& stage, uint64_t& o
 		if(!stage.isRead && block.ioIsRead)
 			continue;
 
+		if(stage.checksum)
+			batch.hostShifts[numDescs] = blockFileSize(block) - block.offset - block.len;
+
 		batch.hostDescs[numDescs++] = elb_block_desc{slotDevPtr(batch, i), block.len,
 			block.offset, descBlockCounter(stage.content, block)};
 		outNumBytes += block.len;
@@ -2330,6 +2360,11 @@ void Worker::enqueueStage(Batch& batch, const GpuStage& stage, uint32_t numBlock
 			"CUDA event record");
 	}
 
+	// (a write's checksum reads the device slot before its stage-out copy)
+	if(stage.checksum && elb_launch_crc32(batch.hostDescs, batch.hostShifts, numBlocks,
+		batch.devCrcs, batch.hostCrcs, batch.devDoneTicket, batch.stream) )
+		throw WorkerError(std::string("GPU checksum failed. ") + elb_last_error() );
+
 	if( (stage.transfer == GpuStage::TRANSFER_COPY) && !stage.isRead)
 		enqueueStageCopies(batch, false, true);
 }
@@ -2341,7 +2376,8 @@ void Worker::enqueueStage(Batch& batch, const GpuStage& stage, uint32_t numBlock
  */
 void Worker::gpuLaunchStage(Batch& batch, bool isRead)
 {
-	const GpuStage& stage = isRead ? readStage : writeStage;
+	const GpuStage& stage = !isRead ? writeStage :
+		(benchPhase == ELB_PHASE_READFILES) ? readStage : verifyBackStage;
 	uint64_t numBytes;
 	const uint32_t numBlocks = fillStageDescs(batch, stage, numBytes);
 
@@ -2363,6 +2399,8 @@ void Worker::gpuLaunchStage(Batch& batch, bool isRead)
 
 	// (the stage-copy kernel of kernel staging counts as a launch, but is not timed)
 	if(batch.hadKernel || (numBlocks && (stage.transfer == GpuStage::TRANSFER_KERNEL) ) )
+		numKernelLaunches++;
+	if(numBlocks && stage.checksum)
 		numKernelLaunches++;
 
 	if(stage.transfer != GpuStage::TRANSFER_NONE)
@@ -2592,6 +2630,47 @@ void Worker::accountBatch(Batch& batch, uint64_t gpuUSecTotal)
 
 	for(size_t i = 0; i < numBlocks; i++)
 		ioAccountBlock(batch.blocks[i], batch.blocks[i].ioUSec + gpuShareUSec);
+
+	addBatchChecksums(batch);
+}
+
+/* --checksums: the CRC contributions of a batch whose blocks are done (no rwmix: descriptor i is
+ * block i), into the accumulator of each block's file */
+void Worker::addBatchChecksums(const Batch& batch)
+{
+	if(!cfg.checksums)
+		return;
+
+	for(size_t i = 0; i < batch.blocks.size(); i++)
+	{
+		const BlockRef& block = batch.blocks[i];
+		typedef std::pair<uint64_t, uint64_t> FileID;
+		const FileID fileID = (cfg.pathType != ELB_PATH_DIR) ? FileID(block.fileIdx, 0) :
+			block.isTreeElem ? FileID(~0ULL, block.fileIndex) :
+			FileID(block.dirIndex, block.fileIndex);
+
+		ChecksumAcc& acc = checksumAccs.try_emplace(fileID, ChecksumAcc{block}).first->second;
+
+		acc.rawCrc ^= batch.hostCrcs[i];
+		acc.numBytes += block.len;
+	}
+}
+
+/* the data set size of the block's file: -s, or the tree file's (rounded up) size of the entry */
+uint64_t Worker::blockFileSize(const BlockRef& block) const
+{
+	return block.isTreeElem ? customTreeFiles.slices[block.fileIndex].totalLen : cfg.fileSize;
+}
+
+std::vector<FileChecksum> Worker::getFileChecksums() const
+{
+	std::vector<FileChecksum> checksums;
+
+	for(const auto& entry : checksumAccs)
+		checksums.push_back(FileChecksum{blockFilePath(entry.second.block),
+			blockFileSize(entry.second.block), entry.second.numBytes, entry.second.rawCrc});
+
+	return checksums;
 }
 
 /* dir mode: the path of the block's file relative to bench path outPathIndex */

@@ -30,6 +30,7 @@
 #include <condition_variable>
 #include <deque>
 #include <functional>
+#include <map>
 #include <memory>
 #include <mutex>
 #include <shared_mutex>
@@ -118,6 +119,15 @@ struct DamageRun
 	uint16_t firstSectorLo{0}; // where the block starts in the first sector (0: before it)
 };
 
+/* --checksums: what a worker moved of one file in a phase */
+struct FileChecksum
+{
+	std::string path; // as the worker opened the file
+	uint64_t size{0};     // the file's data set size
+	uint64_t numBytes{0}; // bytes of the blocks the phase moved
+	uint32_t rawCrc{0};   // XOR of the blocks' contributions (elb_crc32_blocks)
+};
+
 /* produces the worker's blocks of a phase in submission order */
 class BlockSource
 {
@@ -142,6 +152,7 @@ struct GpuStage
 	elb_content content; // what the write fills or the read verifies (NONE: the blocks only move)
 	bool useGraph;    // replay full batches from a CUDA graph (one launch per batch anyway under
 	                  // kernel staging)
+	bool checksum;    // --checksums: each block's CRC-32 contribution from its device slot
 };
 
 /* a batch: a contiguous slice of the rings plus everything its GPU stage needs */
@@ -165,6 +176,12 @@ struct Batch
 	elb_verify_result* devResults{NULL};  // armed {0, ~0} once, self re-arming
 	elb_verify_result* hostResults{NULL}; // pinned
 	unsigned* devDoneTicket{NULL};
+
+	/* --checksums: bytes from each block's end to its file's end (pinned, read by the CRC kernel)
+	   and the blocks' CRC contributions, published to pinned memory by the kernel's last CTA */
+	uint64_t* hostShifts{NULL};
+	uint32_t* devCrcs{NULL};  // zero, re-zeroed by the kernel
+	uint32_t* hostCrcs{NULL};
 
 	// aio state
 	std::vector<struct iocb> iocbs;
@@ -223,6 +240,8 @@ class Worker
 		uint64_t getNumDamageRunsDropped() const { return numDamageRunsDropped; }
 		uint64_t getNumDamageBytesDropped() const { return numDamageBytesDropped; }
 		const std::string& getDeferredVerifyError() const { return deferredVerifyError; }
+		// --checksums results of the phase (read when all workers are done)
+		std::vector<FileChecksum> getFileChecksums() const;
 
 		void interruptExecution() { isInterruptionRequested = true; }
 		void createStoneWallStats(); // called by the first finisher under Shared::mutex
@@ -267,6 +286,7 @@ class Worker
 		int64_t hostDelta{0}; // hostRing - devRing: host slot of a block = device slot + hostDelta
 		GpuStage readStage{};  // resolved elb_cfg::stagingEngine, --cufile, --verify(rand), --blockvarpct
 		GpuStage writeStage{};
+	GpuStage verifyBackStage{}; // --verifydirect read-back: readStage without the checksum
 		bool useWriteGate{false};    // resolved elb_cfg::serializeBufferedWrites
 		int boundNumaNode{-1};       // NUMA node this worker bound itself to (-1: none)
 		std::vector<Batch> batches;
@@ -331,6 +351,16 @@ class Worker
 		uint64_t numDamageBytesDropped{0};
 		std::string deferredVerifyError;
 
+		/* --checksums: the XOR of the CRC contributions and the bytes of each file this worker
+		   moved in the phase, by numeric file identity; paths are resolved at the phase end */
+		struct ChecksumAcc
+		{
+			BlockRef block; // (a block of the file, for its path)
+			uint64_t numBytes{0};
+			uint32_t rawCrc{0};
+		};
+		std::map<std::pair<uint64_t, uint64_t>, ChecksumAcc> checksumAccs;
+
 		// accounting
 		std::atomic<uint64_t> numH2DBytes{0};
 		std::atomic<uint64_t> numD2HBytes{0};
@@ -369,6 +399,8 @@ class Worker
 			bool oneFilePerBatch = false);
 		void verifyWrittenBatch(Batch& batch);
 		void accountBatch(Batch& batch, uint64_t gpuUSecTotal);
+		void addBatchChecksums(const Batch& batch);
+		uint64_t blockFileSize(const BlockRef& block) const;
 		void gpuLaunchStage(Batch& batch, bool isRead);
 		uint32_t fillStageDescs(Batch& batch, const GpuStage& stage, uint64_t& outNumBytes);
 		uint64_t descBlockCounter(const elb_content& content, const BlockRef& block) const;
@@ -437,6 +469,15 @@ class Manager
 			uint64_t numFiles{0};
 		};
 		VerifyReport getVerifyReport();
+
+		/* --checksums: each file of the last phase, merged over all workers */
+		struct ChecksumReport
+		{
+			std::string lines; // "<path> <size> <bytes covered> <crc32 or ->\n", sorted by path
+			uint64_t numFiles{0};
+			uint64_t numComplete{0}; // files with a CRC
+		};
+		ChecksumReport getChecksumReport();
 
 		Shared shared;
 		std::vector<std::unique_ptr<Worker> > workers;

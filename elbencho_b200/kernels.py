@@ -289,6 +289,28 @@ def damage_map(pinned_descs_ptr, num_descs, content_kind, key, pct, grain_shift,
            "elb_damage_map")
 
 
+def crc32_blocks(pinned_descs_ptr, pinned_shifts_ptr, num_descs, dev_crcs_ptr,
+                 pinned_crcs_ptr=0, dev_ticket_ptr=0, stream=0):
+    """CRC-32 contributions (--checksums): XORs crc32_shift(R(block i), shifts[i]) into the
+    uint32 dev_crcs_ptr[i], R being the raw CRC-32 (init 0, no final XOR). With pinned_crcs_ptr and
+    dev_ticket_ptr (a zeroed uint32 device counter) the launch's last CTA copies the values there
+    and zeroes dev_crcs_ptr. Descriptors and uint64 shifts must be in pinned host memory."""
+    _check(_native.load().elb_crc32_blocks(pinned_descs_ptr, pinned_shifts_ptr, num_descs,
+                                           dev_crcs_ptr, pinned_crcs_ptr or None,
+                                           dev_ticket_ptr or None, stream),
+           "elb_crc32_blocks")
+
+
+def crc32_shift(crc, num_zero_bytes):
+    """the raw CRC-32 of crc's message followed by num_zero_bytes zero bytes"""
+    return int(_native.load().elb_crc32_shift(crc, num_zero_bytes))
+
+
+def crc32_finish(raw_crc, size):
+    """zlib's CRC-32 of a message of size bytes from its raw CRC-32"""
+    return int(_native.load().elb_crc32_finish(raw_crc, size))
+
+
 def stage_copy(descs_ptr, num_descs, host_to_device, host_delta, stream=0, total_bytes=0,
                max_block_len=0):
     _check(_native.load().elb_stage_copy(descs_ptr, num_descs, int(bool(host_to_device)),

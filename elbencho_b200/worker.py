@@ -113,6 +113,7 @@ class WorkerConfig:
     run_as_service: bool = False
     verify_collect_all: bool = False
     verify_report: bool = False       # --verifyreport: map bad blocks' damage, fail at phase end
+    checksums: bool = False           # --checksums: each file's CRC-32 per phase (checksums())
     serialize_buffered_writes: int = 0  # 0 auto, 1 on, 2 off (--writegate)
     staging_engine: int = 0           # 0 auto, 1 kernels move the data, 2 cudaMemcpyAsync
     no_gpu_numa_binding: bool = False  # --nogpunuma
@@ -137,6 +138,7 @@ class WorkerConfig:
         cfg.ioDepth = self.io_depth
         cfg.useDirectIO = int(self.use_direct_io)
         cfg.ioEngine = int(self.io_engine)
+        cfg.checksumReport = int(self.checksums)
         cfg.numDirs = self.num_dirs
         cfg.numFiles = self.num_files
         cfg.doDirSharing = int(self.do_dir_sharing)
@@ -401,6 +403,25 @@ class WorkerManager:
             path, offset, length, num_bytes = line.rsplit("\t", 3)
             extents.append((path, int(offset), int(length), int(num_bytes)))
         return extents
+
+    def checksums_text(self) -> str:
+        """The last phase's file checksums as the library formats them (checksums)."""
+        size = self._lib.elb_mgr_checksums(self._h, None, 0)
+        if size < 0:
+            raise WorkerError(_native.last_error())
+        buf = ctypes.create_string_buffer(size + 1)
+        self._lib.elb_mgr_checksums(self._h, buf, size + 1)
+        return buf.value.decode("utf-8", "replace")
+
+    def checksums(self):
+        """The last phase's files, merged over all workers and sorted by path:
+        [(path, size, bytes_covered, crc32)], crc32 an int (zlib.crc32 of the file's first size
+        bytes) or None if the phase did not cover them exactly once."""
+        files = []
+        for line in self.checksums_text().splitlines():
+            path, size, covered, crc = line.rsplit(" ", 3)
+            files.append((path, int(size), int(covered), None if crc == "-" else int(crc, 16)))
+        return files
 
     def interrupt(self):
         self._lib.elb_mgr_interrupt(self._h)

@@ -292,6 +292,23 @@ int elb_damage_map(const elb_block_desc* descs, uint32_t numDescs, int contentKi
 	unsigned pct, unsigned grainShift, unsigned dedupePct, elb_sector_damage* devSectors,
 	uint64_t sectorsPerDesc, void* stream);
 
+/* CRC-32 contributions (--checksums). For each descriptor i: X(R(block i), shifts[i]), with R the
+ * raw reflected CRC-32 of the block's device bytes (polynomial 0xEDB88320, init 0, no final XOR)
+ * and X(c, n) = c * x^(8n) mod P, the CRC of c followed by n zero bytes. With shifts[i] = the bytes
+ * from the block's end to its file's end, the XOR of all blocks' contributions of a file is the
+ * file's R, in any order (elb_crc32_finish makes zlib's CRC-32 of it). The result is XORed into
+ * devCrcs[i] (device memory, all 0 on the first launch). With hostCrcs (pinned host memory) and
+ * devTicket (a device counter, 0), the last CTA of the launch copies devCrcs[0..numDescs) to
+ * hostCrcs and zeroes them; the host reads them after the stream's work is done. descs and shifts
+ * must be pinned host memory: the host sizes the grid from the lengths, the device reads them.
+ * Blocks of any length (0 too) and any device address. */
+int elb_crc32_blocks(const elb_block_desc* descs, const uint64_t* shifts, uint32_t numDescs,
+	uint32_t* devCrcs, uint32_t* hostCrcs, unsigned* devTicket, void* stream);
+/* X(crc, n) of elb_crc32_blocks (n: any number of zero bytes) */
+uint32_t elb_crc32_shift(uint32_t crc, uint64_t n);
+/* zlib's CRC-32 of a message of size bytes from its raw CRC R (elb_crc32_blocks) */
+uint32_t elb_crc32_finish(uint32_t rawCrc, uint64_t size);
+
 int elb_stage_copy(const elb_block_desc* descs, uint32_t numDescs, int hostToDevice,
 	int64_t hostDelta, uint64_t totalBytes, uint64_t maxBlockLen, void* stream);
 /* devResults[0..numDescs) <- {0, ~0} */
@@ -334,6 +351,11 @@ typedef struct elb_cfg
 	uint32_t ioDepth;
 	int32_t useDirectIO;
 	int32_t ioEngine; /* enum elb_io_engine */
+	/* --checksums: every write and read phase computes each file's CRC-32 on the GPU from the
+	 * bytes in the device ring (elb_crc32_blocks); elb_mgr_checksums lists them. Rejects random
+	 * offsets, infinite loops and rwmix. It takes the 4 bytes of padding in front of numDirs: no
+	 * other field moves. */
+	int32_t checksumReport;
 
 	/* -n / -N / --dirsharing (dir mode) */
 	uint64_t numDirs;
@@ -727,6 +749,13 @@ int elb_mgr_interrupt(elb_mgr* m);
  * differing bytes not listed\n". Returns the length of the full text (truncated to outBufLen - 1
  * bytes in outBuf), -1 on error. */
 int64_t elb_mgr_verify_report(elb_mgr* m, char* outBuf, uint64_t outBufLen);
+
+/* --checksums (elb_cfg::checksumReport): the files of the last phase, merged over all workers, as
+ * text lines "<path> <size> <bytes covered> <crc>\n" sorted by path. size is the file's data set
+ * size, bytes covered the sum of the lengths of its blocks that the phase moved, crc zlib's CRC-32
+ * of the file's first size bytes as 8 lowercase hex digits if bytes covered == size, else "-".
+ * Returns the length of the full text (truncated to outBufLen - 1 bytes in outBuf), -1 on error. */
+int64_t elb_mgr_checksums(elb_mgr* m, char* outBuf, uint64_t outBufLen);
 
 uint32_t elb_mgr_num_workers(elb_mgr* m);
 elb_worker* elb_mgr_worker(elb_mgr* m, uint32_t localIdx);
