@@ -46,6 +46,7 @@ class Cfg(ctypes.Structure):
         ("numThreads", c_u32),
         ("rankOffset", c_u32),
         ("numDataSetThreads", c_u32),
+        ("checksumChunkShift", ctypes.c_int32),
         ("blockSize", c_u64),
         ("fileSize", c_u64),
         ("ioDepth", c_u32),
@@ -246,6 +247,8 @@ SIGNATURES = {
     "elb_crc32_blocks": (ctypes.c_int, [_VP, _VP, c_u32, _VP, _VP, _VP, _VP]),
     "elb_crc32_shift": (c_u32, [c_u32, c_u64]),
     "elb_crc32_finish": (c_u32, [c_u32, c_u64]),
+    "elb_crc32_chunks": (ctypes.c_int, [_VP, _VP, c_u32, ctypes.c_uint, c_u64, _VP, _VP, _VP,
+                                        _VP]),
     "elb_damage_map": (ctypes.c_int, [_VP, c_u32, ctypes.c_int, c_u64, ctypes.c_uint,
                                       ctypes.c_uint, ctypes.c_uint, _VP, c_u64, _VP]),
     "elb_stage_copy": (ctypes.c_int, [_VP, c_u32, ctypes.c_int, ctypes.c_int64, c_u64, c_u64,
@@ -312,6 +315,9 @@ SIGNATURES = {
     "elb_mgr_interrupt": (ctypes.c_int, [_VP]),
     "elb_mgr_verify_report": (ctypes.c_int64, [_VP, ctypes.c_char_p, c_u64]),
     "elb_mgr_checksums": (ctypes.c_int64, [_VP, ctypes.c_char_p, c_u64]),
+    "elb_mgr_set_checksum_list": (ctypes.c_int, [_VP, ctypes.c_char_p, c_u64]),
+    "elb_mgr_checksum_verify_counts": (ctypes.c_int, [_VP, ctypes.POINTER(c_u64),
+                                                      ctypes.POINTER(c_u64)]),
     "elb_mgr_num_workers": (c_u32, [_VP]),
     "elb_mgr_worker": (_VP, [_VP, c_u32]),
     "elb_mgr_last_error": (ctypes.c_char_p, [_VP]),

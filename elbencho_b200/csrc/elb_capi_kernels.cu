@@ -403,29 +403,62 @@ int elb_damage_map(const elb_block_desc* descs, uint32_t numDescs, int contentKi
 	return 0;
 }
 
-int elb_crc32_blocks(const elb_block_desc* descs, const uint64_t* shifts, uint32_t numDescs,
-	uint32_t* devCrcs, uint32_t* hostCrcs, unsigned* devTicket, void* stream)
+/* the argument checks of elb_crc32_blocks and elb_crc32_chunks, then the launch */
+static int crc32Launch(const char* what, const elb_block_desc* descs, const uint64_t* shifts,
+	uint32_t numDescs, unsigned chunkShift, uint64_t slotsPerDesc, uint32_t* devCrcs,
+	uint32_t* hostCrcs, unsigned* devTicket, void* stream)
 {
-	if(numDescs && (!descs || !shifts || !devCrcs) )
+	if(numDescs && (!descs || ( (chunkShift == 64) && !shifts) || !devCrcs) )
 	{
-		elb_set_last_error("elb_crc32_blocks: NULL descriptor, shift or CRC array");
+		elb_set_last_error(std::string(what) + ": NULL descriptor, shift or CRC array");
 		return -1;
 	}
 
 	if(!hostCrcs != !devTicket)
 	{
-		elb_set_last_error("elb_crc32_blocks: host CRCs and device ticket go together");
+		elb_set_last_error(std::string(what) + ": host CRCs and device ticket go together");
 		return -1;
 	}
 
-	if(elb_launch_crc32(descs, shifts, numDescs, devCrcs, hostCrcs, devTicket,
-		(cudaStream_t)stream) )
+	if(elb_launch_crc32(descs, shifts, numDescs, chunkShift, slotsPerDesc, devCrcs, hostCrcs,
+		devTicket, (cudaStream_t)stream) )
 	{
 		elb_set_last_error(std::string("elb_") + elb_last_error() );
 		return -1;
 	}
 
 	return 0;
+}
+
+int elb_crc32_blocks(const elb_block_desc* descs, const uint64_t* shifts, uint32_t numDescs,
+	uint32_t* devCrcs, uint32_t* hostCrcs, unsigned* devTicket, void* stream)
+{
+	return crc32Launch("elb_crc32_blocks", descs, shifts, numDescs, 64, 1, devCrcs, hostCrcs,
+		devTicket, stream);
+}
+
+int elb_crc32_chunks(const elb_block_desc* descs, const uint64_t* shifts, uint32_t numDescs,
+	unsigned chunkShift, uint64_t slotsPerDesc, uint32_t* devCrcs, uint32_t* hostCrcs,
+	unsigned* devTicket, void* stream)
+{
+	if( (chunkShift != 64) && ( (chunkShift < ELB_CRC32_MIN_CHUNK_SHIFT) ||
+		(chunkShift > ELB_CRC32_MAX_CHUNK_SHIFT) ) )
+	{
+		elb_set_last_error("elb_crc32_chunks: chunk shift " + std::to_string(chunkShift) +
+			" is neither 64 nor in [" + std::to_string(ELB_CRC32_MIN_CHUNK_SHIFT) + ", " +
+			std::to_string(ELB_CRC32_MAX_CHUNK_SHIFT) + "]");
+		return -1;
+	}
+
+	if(!slotsPerDesc || ( (chunkShift == 64) && (slotsPerDesc != 1) ) )
+	{
+		elb_set_last_error("elb_crc32_chunks: slots per descriptor must be at least 1, and 1 "
+			"without chunks");
+		return -1;
+	}
+
+	return crc32Launch("elb_crc32_chunks", descs, shifts, numDescs, chunkShift, slotsPerDesc,
+		devCrcs, hostCrcs, devTicket, stream);
 }
 
 uint32_t elb_crc32_shift(uint32_t crc, uint64_t n)

@@ -8,10 +8,12 @@
 #include <sys/stat.h>
 
 #include <algorithm>
+#include <fstream>
 #include <sstream>
 
 #include "elb_cli.h"
 #include "elb_host.h"
+#include "elb_worker.h"
 
 namespace elb
 {
@@ -127,6 +129,18 @@ static const OptDef optDefs[] =
 		"file, sorted by path. The CRC is given when the phase covered the file's first size "
 		"bytes exactly once, else \"-\". With --verifydirect only the written bytes count. Cannot "
 		"be used with --rand, --infloop, --rwmixpct, --rwmixthr or --hosts. [b200]"},
+	{"checksumchunk", 0, Opt_BYTES, &ProgArgs::checksumChunkSize, Wire_NONE, "Chunk size of "
+		"--checksums and --checksumverify: a power of two from 4K to 1G that the block size is a "
+		"multiple of. --checksums then lists the CRC-32 of every chunk the phase moved: each section "
+		"starts with \"# phase WRITE|READ chunk <K>\", then one line \"path offset length crc32\" "
+		"per chunk, sorted by path and offset. Cannot be used with --norandalign. [b200]"},
+	{"checksumverify", 0, Opt_STR, &ProgArgs::checksumVerifyPath, Wire_NONE, "Path of a checksum "
+		"list that --checksums with --checksumchunk wrote: every read phase checks the CRC-32 of "
+		"each chunk it reads, on the GPU, against the list's last section with a chunk size, and "
+		"fails at the first chunk that differs or has no line. Works with --rand, --randamount, "
+		"--infloop and custom tree mode. The block size must be a multiple of the list's chunk "
+		"size. Cannot be used with --norandalign, --rwmixpct, --rwmixthr, --hosts or "
+		"--verifyreport. [b200]"},
 	{"rwmixpct", 0, Opt_U64, &ProgArgs::rwMixReadPercent, Wire_REF, "Percentage of blocks that "
 		"should be read in a write phase."},
 	{"rwmixthr", 0, Opt_U64, &ProgArgs::numRWMixReadThreads, Wire_REF, "Number of threads that "
@@ -989,6 +1003,71 @@ void ProgArgs::checkArgs()
 			throw ProgError("Option \"--checksums\" cannot be used together with \"--hosts\"");
 	}
 
+	if(checksumChunkSize)
+	{
+		if(checksumsPath.empty() && checksumVerifyPath.empty() )
+			throw ProgError("Option \"--checksumchunk\" requires \"--checksums\" or "
+				"\"--checksumverify\"");
+
+		if( (checksumChunkSize < (1ULL << ELB_CHECKSUM_MIN_CHUNK_SHIFT) ) ||
+			(checksumChunkSize > (1ULL << ELB_CHECKSUM_MAX_CHUNK_SHIFT) ) ||
+			(checksumChunkSize & (checksumChunkSize - 1) ) )
+			throw ProgError("Option \"--checksumchunk\" must be a power of two from 4K to 1G");
+
+		if(blockSize % checksumChunkSize)
+			throw ProgError("The block size (" + std::to_string(blockSize) + ") must be a multiple "
+				"of \"--checksumchunk\" (" + std::to_string(checksumChunkSize) + ")");
+
+		if(useRandomUnaligned)
+			throw ProgError("Option \"--checksumchunk\" cannot be used together with "
+				"\"--norandalign\"");
+	}
+
+	if(!checksumVerifyPath.empty() )
+	{ // (the list's chunks are checked wherever and however often they are read, on this host)
+		const char* conflicts[][2] = { {"--norandalign", useRandomUnaligned ? "1" : NULL},
+			{"--rwmixpct", rwMixReadPercent ? "1" : NULL},
+			{"--rwmixthr", numRWMixReadThreads ? "1" : NULL},
+			{"--hosts", !hosts.empty() ? "1" : NULL},
+			{"--verifyreport", !verifyReportPath.empty() ? "1" : NULL} };
+
+		for(const auto& conflict : conflicts)
+			if(conflict[1])
+				throw ProgError(std::string("Option \"--checksumverify\" cannot be used together "
+					"with \"") + conflict[0] + "\"");
+
+		if(checksumVerifyPath == checksumsPath)
+			throw ProgError("Options \"--checksumverify\" and \"--checksums\" cannot name the "
+				"same file");
+
+		std::ifstream listStream(checksumVerifyPath);
+		std::stringstream listText;
+		listText << listStream.rdbuf();
+
+		if(!listStream)
+			throw ProgError("Unable to read checksum list: " + checksumVerifyPath);
+
+		try
+		{
+			checksumList = ChecksumList::parse(listText.str() );
+		}
+		catch(WorkerError& e)
+		{
+			throw ProgError(checksumVerifyPath + ": " + e.what() );
+		}
+
+		const uint64_t listChunkSize = 1ULL << checksumList->chunkShift;
+
+		if(checksumChunkSize && (checksumChunkSize != listChunkSize) )
+			throw ProgError("Option \"--checksumchunk\" (" + std::to_string(checksumChunkSize) +
+				") differs from the chunk size of the checksum list (" +
+				std::to_string(listChunkSize) + ")");
+
+		if(blockSize % listChunkSize)
+			throw ProgError("The block size (" + std::to_string(blockSize) + ") must be a multiple "
+				"of the chunk size of the checksum list (" + std::to_string(listChunkSize) + ")");
+	}
+
 	if(doDirectVerify && ( (!integrityCheckSalt && !randomVerifySeed) || !runCreateFilesPhase) )
 		throw ProgError("Direct verification requires --verify and --write"); // :1426-1428
 
@@ -1082,6 +1161,8 @@ void ProgArgs::toABIConfig(ABIConfig& out) const
 	cfg.verifyCollectAll = 0;
 	cfg.verifyDamageReport = !verifyReportPath.empty();
 	cfg.checksumReport = !checksumsPath.empty();
+	cfg.checksumChunkShift = checksumList ? (int32_t)checksumList->chunkShift :
+		checksumChunkSize ? __builtin_ctzll(checksumChunkSize) : 0;
 	cfg.serializeBufferedWrites = neverSerializeBufferedWrites ? ELB_WRITEGATE_OFF :
 		(serializeBufferedWrites ? ELB_WRITEGATE_ON : ELB_WRITEGATE_AUTO);
 	cfg.noGPUNumaBinding = noGPUNumaBinding;

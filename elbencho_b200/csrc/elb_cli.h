@@ -12,6 +12,7 @@
 #include <stdint.h>
 
 #include <map>
+#include <memory>
 #include <ostream>
 #include <stdexcept>
 #include <string>
@@ -21,6 +22,8 @@
 
 namespace elb
 {
+
+struct ChecksumList;
 
 /* reference: ProgException (source/ProgException.h) */
 class ProgError : public std::runtime_error
@@ -87,6 +90,9 @@ class ProgArgs
 		uint64_t dedupePercent{0}; // --dedupepct
 		std::string verifyReportPath; // --verifyreport
 		std::string checksumsPath; // --checksums
+		uint64_t checksumChunkSize{0}; // --checksumchunk
+		std::string checksumVerifyPath; // --checksumverify
+		std::shared_ptr<const ChecksumList> checksumList; // --checksumverify, parsed by checkArgs
 		uint64_t rwMixReadPercent{0};
 		bool hasUserSetRWMixPercent{false};
 		uint64_t numRWMixReadThreads{0};

@@ -30,6 +30,21 @@ void CPUUtil::update()
 		currentTotal += cpuTime;
 }
 
+/* --checksumchunk, --checksumverify: every chunk must lie inside one block, blocks start at
+   multiples of the block size */
+void checkChecksumChunks(const Config& c, unsigned chunkShift, const std::string& what)
+{
+	const uint64_t chunkSize = (uint64_t)1 << chunkShift;
+
+	if( (c.blockSize % chunkSize) && (c.blockSize != c.fileSize) ) // (one block per file: any size)
+		throw WorkerError("The block size (" + std::to_string(c.blockSize) + ") is not a multiple "
+			"of " + what + " (" + std::to_string(chunkSize) + ").");
+
+	if(c.useRandomOffsets && c.useRandomUnaligned)
+		throw WorkerError("Checksum chunks cannot be used together with unaligned random offsets "
+			"(--norandalign).");
+}
+
 Config Config::fromABI(const elb_cfg* cfg)
 {
 	if(!cfg)
@@ -103,6 +118,7 @@ Config Config::fromABI(const elb_cfg* cfg)
 	c.verifyCollectAll = cfg->verifyCollectAll;
 	c.verifyDamageReport = (cfg->verifyDamageReport != 0);
 	c.checksums = (cfg->checksumReport != 0);
+	c.checksumChunkShift = (cfg->checksumChunkShift > 0) ? (unsigned)cfg->checksumChunkShift : 0;
 	c.serializeBufferedWrites = cfg->serializeBufferedWrites;
 	c.numRWMixReadThreads = std::min(cfg->numRWMixReadThreads, cfg->numThreads); // :1088
 	c.treeFilePath = cfg->treeFilePath ? cfg->treeFilePath : "";
@@ -192,6 +208,15 @@ Config Config::fromABI(const elb_cfg* cfg)
 	if(c.dedupePercent && !c.useRandomVerifyGrain() )
 		throw WorkerError("A dedupe percentage (--dedupepct) requires a random verify grain "
 			"(--verifyrandgrain).");
+
+	if(cfg->checksumChunkShift && ( (cfg->checksumChunkShift < ELB_CHECKSUM_MIN_CHUNK_SHIFT) ||
+		(cfg->checksumChunkShift > ELB_CHECKSUM_MAX_CHUNK_SHIFT) ) )
+		throw WorkerError("The checksum chunk shift (" + std::to_string(cfg->checksumChunkShift) +
+			") is not in [" + std::to_string(ELB_CHECKSUM_MIN_CHUNK_SHIFT) + ", " +
+			std::to_string(ELB_CHECKSUM_MAX_CHUNK_SHIFT) + "].");
+
+	if(c.checksumChunkShift)
+		checkChecksumChunks(c, c.checksumChunkShift, "the checksum chunk size (--checksumchunk)");
 
 	if(c.checksums && c.useRandomOffsets)
 		throw WorkerError("Checksums (--checksums) cannot be used together with random offsets: "

@@ -101,6 +101,7 @@ class Coordinator
 		void printPhaseResultsEverywhere(int benchPhase, const std::string& isoStartDate);
 		void writeVerifyReportSection(int benchPhase);
 		void writeChecksumSection(int benchPhase);
+		void printChecksumVerifyLine(int benchPhase);
 		void printDryRunInfo();
 };
 
@@ -439,16 +440,38 @@ void Coordinator::writeChecksumSection(int benchPhase)
 		return;
 
 	const Manager::ChecksumReport report = manager->getChecksumReport();
+	const unsigned chunkShift = manager->shared.cfg.checksumChunkShift;
 	std::ofstream fileStream(progArgs.checksumsPath, std::ofstream::app);
 
-	fileStream << "# phase " << ( (benchPhase == ELB_PHASE_READFILES) ? "READ" : "WRITE") << "\n" <<
-		report.lines << std::flush;
+	fileStream << "# phase " << ( (benchPhase == ELB_PHASE_READFILES) ? "READ" : "WRITE");
+
+	if(chunkShift)
+		fileStream << " chunk " << (1ULL << chunkShift);
+
+	fileStream << "\n" << report.lines << std::flush;
 
 	if(!fileStream)
 		throw ProgError("Writing checksum file failed: " + progArgs.checksumsPath);
 
-	std::cout << "Checksums: " << report.numFiles << " files, " << report.numComplete <<
-		" complete: " << progArgs.checksumsPath << std::endl;
+	if(chunkShift)
+		std::cout << "Checksums: " << report.numChunks << " chunks in " << report.numFiles <<
+			" files: " << progArgs.checksumsPath << std::endl;
+	else
+		std::cout << "Checksums: " << report.numFiles << " files, " << report.numComplete <<
+			" complete: " << progArgs.checksumsPath << std::endl;
+}
+
+/* --checksumverify: after each read phase that succeeded, what it checked */
+void Coordinator::printChecksumVerifyLine(int benchPhase)
+{
+	if(progArgs.checksumVerifyPath.empty() || (benchPhase != ELB_PHASE_READFILES) )
+		return;
+
+	uint64_t numChunks, numFiles;
+	manager->getChecksumVerifyCounts(numChunks, numFiles);
+
+	std::cout << "Checksum verify: " << numChunks << " chunks checked in " << numFiles <<
+		" files: " << progArgs.checksumVerifyPath << std::endl;
 }
 
 /* Coordinator::runBenchmarkPhase (:248-272) + Statistics live loop (:1284-1345) */
@@ -597,6 +620,7 @@ void Coordinator::runBenchmarkPhase(int benchPhase)
 		printPhaseResultsEverywhere(benchPhase, isoStartDate);
 		writeVerifyReportSection(benchPhase);
 		writeChecksumSection(benchPhase);
+		printChecksumVerifyLine(benchPhase);
 	}
 	else
 	{ // (sync and dropcache phases print only their elapsed time)
@@ -723,6 +747,9 @@ int Coordinator::main() // Coordinator.cpp:31-142
 		progArgs.toABIConfig(abiConfig);
 
 		manager.reset(new Manager(&abiConfig.cfg) );
+
+		if(progArgs.checksumList)
+			manager->setChecksumList(progArgs.checksumList);
 
 		/* workers on several GPUs: create the NCCL communicators of the statistics reduce now,
 		   while the workers are idle (and before any result output) */

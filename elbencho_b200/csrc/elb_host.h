@@ -1002,6 +1002,8 @@ struct Config
 	bool verifyCollectAll{false};
 	bool verifyDamageReport{false}; // --verifyreport
 	bool checksums{false}; // --checksums
+	unsigned checksumChunkShift{0}; // --checksumchunk / the checksum list's (0: whole files),
+	                                // ELB_CHECKSUM_MIN/MAX_CHUNK_SHIFT
 	int serializeBufferedWrites{ELB_WRITEGATE_AUTO};
 	int stagingEngine{ELB_STAGING_AUTO};
 	bool noGPUNumaBinding{false};
@@ -1024,6 +1026,14 @@ struct Config
 	/* @throw WorkerError on invalid combinations */
 	static Config fromABI(const elb_cfg* cfg);
 };
+
+/* checksum chunks of 2^shift bytes (--checksumchunk, --checksumverify): 4 KiB .. 1 GiB */
+#define ELB_CHECKSUM_MIN_CHUNK_SHIFT 12
+#define ELB_CHECKSUM_MAX_CHUNK_SHIFT 30
+
+/* throws WorkerError unless every chunk of 2^chunkShift bytes lies inside one block of c; what
+   names the chunk size in the message */
+void checkChecksumChunks(const Config& c, unsigned chunkShift, const std::string& what);
 
 } // namespace elb
 

@@ -11,8 +11,8 @@
  *      with the dedupe grain key, elb_patterns.cuh)
  *   damage_map (no reference counterpart: --verifyreport, where the bytes of blocks known to be
  *      bad differ, per 512-byte file sector; off the clean path, see its section below)
- *   crc32 (no reference counterpart: --checksums, each block's share of its file's CRC-32; off the
- *      clean path, see its section below)
+ *   crc32 (no reference counterpart: --checksums / --checksumverify, each block's share of its
+ *      file's CRC-32 or its chunks' CRC-32s; off the clean path, see its section below)
  *
  * All eight are HBM-bound byte/integer kernels (K1/K3/K5/K7: 1 byte written per payload byte,
  * K2/K4/K6/K8: 1 byte read per payload byte), so the design follows the streaming rules: 16-byte (128-bit) vector
@@ -1141,33 +1141,48 @@ elb_damage_map_kernel(const KernelArgs args, elb_sector_damage* sectors, uint64_
 	}
 }
 
-/* ---- CRC-32 contributions (--checksums) ------------------------------------------------------
+/* ---- CRC-32 contributions (--checksums, --checksumchunk, --checksumverify) -------------------
  *
- * One 32-bit contribution per descriptor: X(R(block), shifts[i]) (elb_patterns.cuh), XORed into
- * crcs[i]. A warp takes one 4 KiB chunk of one block at a time, walking the grid-stride sequence of
- * all (descriptor, chunk) pairs, so that the warps of a CTA never wait for each other and small
- * blocks keep every warp busy. Chunks are laid out from the 16-byte aligned address at or below
- * the block's device address, so that every lane loads 16-byte vectors: lane l owns the 128
- * contiguous bytes [l * 128, l * 128 + 128) of the chunk, issues its 8 loads first and then folds
- * them with slicing-by-8 tables that the CTA builds in shared memory once. Bytes of the chunk
- * outside the block (its unaligned head and tail, past its end) count as zeros: zeros in front of
- * the data do not change a raw CRC, zeros behind it shift it, which the shift to the file end
- * takes back. Each lane shifts its value to the chunk end by a per-lane constant and the warp XORs
- * the 32 values. The chunk's shift to the file end is known before its bytes arrive: while the
- * loads are in flight, the warp computes x^(8n) with one lane per bit of n and a 5-level shuffle
- * product; lane 0 applies it and atomicXors the result into crcs[i]. With hostCrcs, the last CTA
- * of the launch (ticket) copies crcs to pinned host memory and zeroes them for the next launch, as
- * the verify launches do with their results. */
+ * Each descriptor's bytes are cut at the chunk boundaries of its file offsets (every 2^chunkShift
+ * bytes; chunkShift 64: none, the whole-file mode of --checksums). Slot j of descriptor i,
+ * crcs[i * slotsPerDesc + j], takes X(R(bytes of chunk c0 + j), chunkEnd) (elb_patterns.cuh), c0
+ * being the chunk of the block's first byte and chunkEnd the bytes from their end to the chunk's
+ * end (the next boundary, or the block end if that comes first) plus, in whole-file mode,
+ * shifts[i] (the bytes from the block end to the file end).
+ *
+ * A warp takes one 4 KiB piece of one block at a time, walking the grid-stride sequence of all
+ * (descriptor, piece) pairs, so that the warps of a CTA never wait for each other and small blocks
+ * keep every warp busy. Pieces are laid out from the 16-byte aligned address at or below the
+ * block's device address, so that every lane loads 16-byte vectors: lane l owns the 128
+ * contiguous bytes [l * 128, l * 128 + 128) of the piece, issues its 8 loads first and then folds
+ * them with slicing-by-8 tables that the CTA builds in shared memory once. Bytes of the piece
+ * outside the segment it is summing (the block's unaligned head and tail, past its end, the other
+ * side of a chunk boundary) count as zeros: zeros in front of the data do not change a raw CRC,
+ * zeros behind it shift it, which the shift to the chunk end takes back. Each lane shifts its
+ * value to the piece end by a per-lane constant and the warp XORs the 32 values; lane 0 applies
+ * the shift from the piece end to the chunk end and atomicXors the result into the slot.
+ *
+ * Chunks are at least 4 KiB, so a piece meets at most one boundary: then it is summed twice, once
+ * per side. Where the device address and the file offset agree mod 4 KiB (the worker's slots) no
+ * piece meets one, and the shift to the chunk end is a multiple of 4 KiB below 2^30: two lookups
+ * in tables of x^(8 * 4 KiB * j) and one product at most. Any other shift (whole-file mode, block
+ * tails, other layouts) is computed while the loads are in flight: x^(8n) with one lane per bit of
+ * n and a 5-level shuffle product. With hostCrcs, the last CTA of the launch (ticket) copies the
+ * slots to pinned host memory and zeroes them for the next launch, as the verify launches do with
+ * their results. */
 
-#define ELB_CRC_PART_BYTES (ELB_VEC_BYTES * ELB_UNROLL) /* 128: a lane's bytes of a chunk */
-#define ELB_CRC_CHUNK_BYTES (32 * ELB_CRC_PART_BYTES)  /* 4 KiB: a warp's bytes */
+#define ELB_CRC_PART_BYTES (ELB_VEC_BYTES * ELB_UNROLL) /* 128: a lane's bytes of a piece */
+#define ELB_CRC_PIECE_BYTES (32 * ELB_CRC_PART_BYTES)  /* 4 KiB: a warp's bytes */
+#define ELB_CRC_TABLE_SHIFT_LIMIT (1ULL << 30) /* shifts by table: multiples of 4 KiB below this */
 
 struct Crc32Consts
 {
 	uint32_t x8pow2[32];    // x^(8 * 2^k) mod P
-	uint32_t laneShift[32]; // x^(8 * 128 * (31 - l)) mod P: lane l's part to the chunk end
+	uint32_t laneShift[32]; // x^(8 * 128 * (31 - l)) mod P: lane l's part to the piece end
+	uint32_t x8pieces[256];      // x^(8 * 4 KiB * j) mod P
+	uint32_t x8pieces256[1024];  // x^(8 * 4 KiB * 256 * j) mod P
 
-	constexpr Crc32Consts() : x8pow2{}, laneShift{}
+	constexpr Crc32Consts() : x8pow2{}, laneShift{}, x8pieces{}, x8pieces256{}
 	{
 		for(unsigned k = 0; k < 32; k++)
 			x8pow2[k] = elb_crc32_x8pow2(k);
@@ -1183,6 +1198,14 @@ struct Crc32Consts
 
 			laneShift[l] = shift;
 		}
+
+		x8pieces[0] = ELB_CRC32_ONE;
+		for(unsigned j = 1; j < 256; j++)
+			x8pieces[j] = elb_crc32_mulmod(x8pieces[j - 1], x8pow2[12]);
+
+		x8pieces256[0] = ELB_CRC32_ONE;
+		for(unsigned j = 1; j < 1024; j++)
+			x8pieces256[j] = elb_crc32_mulmod(x8pieces256[j - 1], x8pow2[20]);
 	}
 };
 
@@ -1211,7 +1234,8 @@ __device__ __forceinline__ uint32_t crc32_fold8(uint32_t crc, uint64_t w,
 
 __global__ void __launch_bounds__(ELB_THREADS)
 elb_crc32_kernel(const elb_block_desc* descs, const uint64_t* shifts, uint32_t numDescs,
-	uint64_t chunksPerDesc, uint32_t* crcs, uint32_t* hostCrcs, unsigned* doneTicket)
+	uint64_t piecesPerDesc, unsigned chunkShift, uint64_t slotsPerDesc, uint32_t* crcs,
+	uint32_t* hostCrcs, unsigned* doneTicket)
 {
 	__shared__ uint32_t sTable[8][256]; // sTable[k][i] = R(byte i followed by k zero bytes)
 	__shared__ bool sIsLastCTA;
@@ -1236,86 +1260,135 @@ elb_crc32_kernel(const elb_block_desc* descs, const uint64_t* shifts, uint32_t n
 
 	const uint32_t laneShift = gCrc32Consts.laneShift[lane];
 	const uint32_t laneX8Pow2 = gCrc32Consts.x8pow2[lane];
-	const uint64_t numItems = (uint64_t)numDescs * chunksPerDesc;
+	const bool isChunked = (chunkShift < 64);
+	const uint64_t numItems = (uint64_t)numDescs * piecesPerDesc;
 	const uint64_t numWarps = (uint64_t)gridDim.x * ELB_WARPS;
 
 	for(uint64_t item = (uint64_t)blockIdx.x * ELB_WARPS + (threadIdx.x >> 5); item < numItems;
 		item += numWarps)
 	{ // (uniform for the warp)
-		const uint32_t descIdx = (uint32_t)( (chunksPerDesc == 1) ? item : (item / chunksPerDesc) );
-		const uint64_t chunkBegin = (item - (uint64_t)descIdx * chunksPerDesc) * ELB_CRC_CHUNK_BYTES;
+		const uint32_t descIdx = (uint32_t)( (piecesPerDesc == 1) ? item : (item / piecesPerDesc) );
+		const uint64_t pieceBegin = (item - (uint64_t)descIdx * piecesPerDesc) * ELB_CRC_PIECE_BYTES;
+		const uint64_t pieceEnd = pieceBegin + ELB_CRC_PIECE_BYTES;
 		const elb_block_desc desc = descs[descIdx];
-		const uint64_t shift = shifts[descIdx];
 		const uint64_t headPad = (uint64_t)(uintptr_t)desc.devPtr & (ELB_VEC_BYTES - 1);
-		const uint64_t end = headPad + desc.len; // chunk positions of the block: [headPad, end)
+		const uint64_t end = headPad + desc.len; // piece positions of the block: [headPad, end)
 
-		if(chunkBegin >= end)
+		if(pieceBegin >= end)
 			continue;
 
 		const uint8_t* base = (const uint8_t*)desc.devPtr - headPad;
-		const uint64_t partBegin = chunkBegin + lane * ELB_CRC_PART_BYTES;
-		const bool hasBytes = (partBegin < end) && (partBegin + ELB_CRC_PART_BYTES > headPad);
-		const bool isWholePart = (partBegin >= headPad) && (partBegin + ELB_CRC_PART_BYTES <= end);
-		u64x2 vecs[ELB_UNROLL];
 
-		if(isWholePart)
+		/* the piece's first segment [segBegin, segEnd): its bytes in the chunk of its first byte,
+		   whose end is segEnd (whole-file mode: all its bytes, and the file end is shift behind) */
+		uint64_t segBegin = headPad;
+		uint64_t segEnd = end;
+		uint64_t shift = 0;
+		uint64_t slot = descIdx;
+
+		if(isChunked)
 		{
-			#pragma unroll
-			for(int u = 0; u < ELB_UNROLL; u++)
-				vecs[u] = ld_nc_128(base + partBegin + u * ELB_VEC_BYTES);
+			const uint64_t fileBase = desc.fileOffset - headPad; // file offset of position 0
+			const uint64_t chunk = (fileBase + max(pieceBegin, headPad) ) >> chunkShift;
+
+			slot = descIdx * slotsPerDesc + chunk - (desc.fileOffset >> chunkShift);
+			segEnd = min( ( (chunk + 1) << chunkShift) - fileBase, end);
 		}
+		else
+			shift = shifts[descIdx];
 
-		/* (while the loads are in flight) x^(8n), n = bytes from the chunk end (chunkBegin +
-		   4 KiB) to the file end (end + shift) mod 2^32 - 1: lane k contributes bit k of n */
-		const uint64_t n = elb_crc32_mod_order(elb_crc32_mod_order(shift) +
-			elb_crc32_mod_order(end) + ELB_CRC32_ORDER -
-			elb_crc32_mod_order(chunkBegin + ELB_CRC_CHUNK_BYTES) );
-		uint32_t factor = ( (n >> lane) & 1) ? laneX8Pow2 : ELB_CRC32_ONE;
+		for( ; ; )
+		{
+			const uint64_t partBegin = pieceBegin + lane * ELB_CRC_PART_BYTES;
+			const bool hasBytes = (partBegin < segEnd) && (partBegin + ELB_CRC_PART_BYTES > segBegin);
+			const bool isWholePart = (partBegin >= segBegin) &&
+				(partBegin + ELB_CRC_PART_BYTES <= segEnd);
+			u64x2 vecs[ELB_UNROLL];
 
-		for(int offset = 16; offset > 0; offset >>= 1)
-			factor = elb_crc32_mulmod(factor, __shfl_xor_sync(0xffffffffu, factor, offset) );
+			if(isWholePart)
+			{
+				#pragma unroll
+				for(int u = 0; u < ELB_UNROLL; u++)
+					vecs[u] = ld_nc_128(base + partBegin + u * ELB_VEC_BYTES);
+			}
 
-		uint32_t crc = 0;
+			/* (while the loads are in flight) x^(8n), n = bytes from the piece end to the segment's
+			   chunk end (segEnd + shift) */
+			const uint64_t nPlain = segEnd - pieceEnd; // (chunked: shift is 0; wraps if negative)
+			uint32_t factor;
 
-		if(hasBytes)
-		{ // (else the part is all zeros)
-			if(!isWholePart)
-			{ // the block's head or tail: byte by byte, zeros outside the block
+			if(isChunked && (nPlain < ELB_CRC_TABLE_SHIFT_LIMIT) &&
+				!(nPlain & (ELB_CRC_PIECE_BYTES - 1) ) )
+			{
+				const uint64_t j = nPlain / ELB_CRC_PIECE_BYTES;
+
+				factor = gCrc32Consts.x8pieces[j & 255];
+
+				if(j >> 8)
+					factor = elb_crc32_mulmod(factor, gCrc32Consts.x8pieces256[j >> 8]);
+			}
+			else
+			{ // n mod 2^32 - 1: lane k contributes bit k of n
+				const uint64_t n = elb_crc32_mod_order(elb_crc32_mod_order(shift) +
+					elb_crc32_mod_order(segEnd) + ELB_CRC32_ORDER - elb_crc32_mod_order(pieceEnd) );
+
+				factor = ( (n >> lane) & 1) ? laneX8Pow2 : ELB_CRC32_ONE;
+
+				for(int offset = 16; offset > 0; offset >>= 1)
+					factor = elb_crc32_mulmod(factor, __shfl_xor_sync(0xffffffffu, factor, offset) );
+			}
+
+			uint32_t crc = 0;
+
+			if(hasBytes)
+			{ // (else the part is all zeros)
+				if(!isWholePart)
+				{ // the segment's head or tail: byte by byte, zeros outside it
+					#pragma unroll
+					for(int u = 0; u < ELB_UNROLL; u++)
+					{
+						const uint64_t vecBegin = partBegin + u * ELB_VEC_BYTES;
+						uint64_t lo = 0, hi = 0;
+
+						#pragma unroll 1
+						for(int b = 0; b < 8; b++)
+						{
+							if( (vecBegin + b >= segBegin) && (vecBegin + b < segEnd) )
+								lo |= (uint64_t)base[vecBegin + b] << (b * 8);
+
+							if( (vecBegin + 8 + b >= segBegin) && (vecBegin + 8 + b < segEnd) )
+								hi |= (uint64_t)base[vecBegin + 8 + b] << (b * 8);
+						}
+
+						vecs[u] = u64x2{lo, hi};
+					}
+				}
+
 				#pragma unroll
 				for(int u = 0; u < ELB_UNROLL; u++)
 				{
-					const uint64_t vecBegin = partBegin + u * ELB_VEC_BYTES;
-					uint64_t lo = 0, hi = 0;
-
-					#pragma unroll 1
-					for(int b = 0; b < 8; b++)
-					{
-						if( (vecBegin + b >= headPad) && (vecBegin + b < end) )
-							lo |= (uint64_t)base[vecBegin + b] << (b * 8);
-
-						if( (vecBegin + 8 + b >= headPad) && (vecBegin + 8 + b < end) )
-							hi |= (uint64_t)base[vecBegin + 8 + b] << (b * 8);
-					}
-
-					vecs[u] = u64x2{lo, hi};
+					crc = crc32_fold8(crc, vecs[u].a, sTable);
+					crc = crc32_fold8(crc, vecs[u].b, sTable);
 				}
+
+				crc = elb_crc32_mulmod(crc, laneShift);
 			}
 
-			#pragma unroll
-			for(int u = 0; u < ELB_UNROLL; u++)
-			{
-				crc = crc32_fold8(crc, vecs[u].a, sTable);
-				crc = crc32_fold8(crc, vecs[u].b, sTable);
-			}
+			for(int offset = 16; offset > 0; offset >>= 1)
+				crc ^= __shfl_xor_sync(0xffffffffu, crc, offset);
 
-			crc = elb_crc32_mulmod(crc, laneShift);
+			if(!lane && crc)
+				atomicXor(&crcs[slot], (factor == ELB_CRC32_ONE) ? crc :
+					elb_crc32_mulmod(crc, factor) );
+
+			if(segEnd >= min(pieceEnd, end) )
+				break;
+
+			// (chunked) the rest of the piece: the first bytes of the next chunk
+			segBegin = segEnd;
+			segEnd = min(segBegin + ( (uint64_t)1 << chunkShift), end);
+			slot++;
 		}
-
-		for(int offset = 16; offset > 0; offset >>= 1)
-			crc ^= __shfl_xor_sync(0xffffffffu, crc, offset);
-
-		if(!lane && crc)
-			atomicXor(&crcs[descIdx], elb_crc32_mulmod(crc, factor) );
 	}
 
 	if(!hostCrcs)
@@ -1334,7 +1407,9 @@ elb_crc32_kernel(const elb_block_desc* descs, const uint64_t* shifts, uint32_t n
 
 	__threadfence();
 
-	for(uint32_t i = threadIdx.x; i < numDescs; i += blockDim.x)
+	const uint64_t numSlots = (uint64_t)numDescs * slotsPerDesc;
+
+	for(uint64_t i = threadIdx.x; i < numSlots; i += blockDim.x)
 	{
 		volatile uint32_t* devCrc = &crcs[i];
 
@@ -1745,32 +1820,46 @@ int elb_launch_damage_map(const elb_content& content, const elb_block_desc* desc
 }
 
 int elb_launch_crc32(const elb_block_desc* descs, const uint64_t* shifts, uint32_t numDescs,
-	uint32_t* devCrcs, uint32_t* hostCrcs, unsigned* doneTicket, cudaStream_t stream)
+	unsigned chunkShift, uint64_t slotsPerDesc, uint32_t* devCrcs, uint32_t* hostCrcs,
+	unsigned* doneTicket, cudaStream_t stream)
 {
 	if(!numDescs)
 		return 0;
+
+	uint64_t piecesPerDesc = 0;
+
+	for(uint32_t i = 0; i < numDescs; i++)
+	{ // (descs are host-readable)
+		const uint64_t headPad = (uint64_t)(uintptr_t)descs[i].devPtr & (ELB_VEC_BYTES - 1);
+		piecesPerDesc = std::max(piecesPerDesc,
+			(headPad + descs[i].len + ELB_CRC_PIECE_BYTES - 1) / ELB_CRC_PIECE_BYTES);
+
+		const uint64_t numChunks = (chunkShift >= 64) ? 1 : !descs[i].len ? 0 :
+			( ( (descs[i].fileOffset + descs[i].len - 1) >> chunkShift) -
+			(descs[i].fileOffset >> chunkShift) + 1);
+
+		if(numChunks > slotsPerDesc)
+		{
+			elb_set_last_error("crc32_chunks: descriptor " + std::to_string(i) + " spans " +
+				std::to_string(numChunks) + " chunks, more than " + std::to_string(slotsPerDesc) +
+				" slots per descriptor");
+			return -1;
+		}
+	}
 
 	const DeviceLaunchInfo* devInfo = getDeviceLaunchInfo();
 	if(!devInfo)
 		return -1;
 
-	uint64_t chunksPerDesc = 0;
-
-	for(uint32_t i = 0; i < numDescs; i++)
-	{ // (descs are host-readable)
-		const uint64_t headPad = (uint64_t)(uintptr_t)descs[i].devPtr & (ELB_VEC_BYTES - 1);
-		chunksPerDesc = std::max(chunksPerDesc,
-			(headPad + descs[i].len + ELB_CRC_CHUNK_BYTES - 1) / ELB_CRC_CHUNK_BYTES);
-	}
-
-	/* a grid that stays resident: each CTA builds its tables once and its warps walk many chunks
+	/* a grid that stays resident: each CTA builds its tables once and its warps walk many pieces
 	   (at least one CTA, whose ticket publishes the results also when no block has a byte) */
-	const uint64_t numItems = (uint64_t)numDescs * chunksPerDesc;
+	const uint64_t numItems = (uint64_t)numDescs * piecesPerDesc;
 	const uint64_t gridSize = std::max( (uint64_t)1, std::min( (numItems + ELB_WARPS - 1) /
 		ELB_WARPS, (uint64_t)devInfo->numSMs * devInfo->crcCtasPerSM) );
 
 	elb_crc32_kernel<<<(unsigned)gridSize, ELB_THREADS, 0, stream>>>(descs, shifts, numDescs,
-		chunksPerDesc ? chunksPerDesc : 1, devCrcs, hostCrcs, doneTicket);
+		piecesPerDesc ? piecesPerDesc : 1, chunkShift, slotsPerDesc, devCrcs, hostCrcs,
+		doneTicket);
 	gNumKernelLaunches.fetch_add(1, std::memory_order_relaxed);
 
 	return checkLaunch("crc32");

@@ -5,6 +5,8 @@
 #include <errno.h>
 #include <algorithm>
 #include <map>
+#include <set>
+#include <sstream>
 #include <fcntl.h>
 #include <string.h>
 #include <sys/stat.h>
@@ -521,6 +523,9 @@ Manager::VerifyReport Manager::getVerifyReport()
  */
 Manager::ChecksumReport Manager::getChecksumReport()
 {
+	if(shared.cfg.checksumChunkShift)
+		return getChunkChecksumReport();
+
 	std::map<std::string, FileChecksum> files;
 
 	for(const std::unique_ptr<Worker>& worker : workers)
@@ -554,6 +559,209 @@ Manager::ChecksumReport Manager::getChecksumReport()
 	}
 
 	return report;
+}
+
+/* --checksumchunk: one line per chunk that the last phase moved, sorted by path and offset */
+Manager::ChecksumReport Manager::getChunkChecksumReport()
+{
+	std::map<std::string, std::vector<ChunkChecksum> > files;
+
+	for(const std::unique_ptr<Worker>& worker : workers)
+		for(const FileChecksum& part : worker->getFileChecksums() )
+		{
+			std::vector<ChunkChecksum>& chunks = files[part.path];
+			chunks.insert(chunks.end(), part.chunks.begin(), part.chunks.end() );
+		}
+
+	ChecksumReport report;
+
+	for(auto& entry : files)
+	{
+		std::vector<ChunkChecksum>& chunks = entry.second;
+
+		std::sort(chunks.begin(), chunks.end(),
+			[](const ChunkChecksum& a, const ChunkChecksum& b) { return a.offset < b.offset; } );
+
+		for(const ChunkChecksum& chunk : chunks)
+		{
+			char hex[9];
+			snprintf(hex, sizeof(hex), "%08x", elb_crc32_finish_hd(chunk.rawCrc, chunk.length) );
+			report.lines += entry.first + " " + std::to_string(chunk.offset) + " " +
+				std::to_string(chunk.length) + " " + hex + "\n";
+		}
+
+		report.numChunks += chunks.size();
+		report.numFiles++;
+	}
+
+	return report;
+}
+
+/* a decimal number of up to 19 digits (no sign, no blanks) */
+static bool parseChecksumListNum(const std::string& str, uint64_t& outVal)
+{
+	if(str.empty() || (str.size() > 19) ||
+		(str.find_first_not_of("0123456789") != std::string::npos) )
+		return false;
+
+	outVal = std::stoull(str);
+	return true;
+}
+
+/**
+ * --checksumverify: the last section with a chunk size of a checksum list (--checksums with
+ * --checksumchunk). Lines are split at their last three blanks, as paths may contain blanks.
+ * Blank lines and the lines of whole-file sections are skipped.
+ */
+std::shared_ptr<const ChecksumList> ChecksumList::parse(const std::string& text)
+{
+	std::shared_ptr<ChecksumList> list;   // the last chunked section so far
+	std::shared_ptr<ChecksumList> section; // the current chunked section (NULL: whole files)
+	bool inSection = false;
+	uint64_t lineNum = 0;
+
+	for(size_t lineBegin = 0; lineBegin < text.size(); )
+	{
+		size_t lineEnd = text.find('\n', lineBegin);
+		if(lineEnd == std::string::npos)
+			lineEnd = text.size();
+
+		const std::string line = text.substr(lineBegin, lineEnd - lineBegin);
+		lineBegin = lineEnd + 1;
+		lineNum++;
+
+		auto fail = [&](const std::string& reason)
+		{
+			throw WorkerError("Checksum list line " + std::to_string(lineNum) + ": " + reason +
+				": \"" + line + "\"");
+		};
+
+		if(line.empty() )
+			continue;
+
+		if(!line.compare(0, 8, "# phase ") )
+		{ // "# phase WRITE|READ" or "# phase WRITE|READ chunk <K>"
+			std::istringstream words(line.substr(8) );
+			std::string phase, chunkWord, chunkSizeStr, extra;
+			uint64_t chunkSize = 0;
+
+			words >> phase >> chunkWord >> chunkSizeStr >> extra;
+
+			if( ( (phase != "WRITE") && (phase != "READ") ) || !extra.empty() ||
+				( !chunkWord.empty() && ( (chunkWord != "chunk") ||
+				!parseChecksumListNum(chunkSizeStr, chunkSize) ) ) )
+				fail("not a phase header");
+
+			inSection = true;
+			section.reset();
+
+			if(chunkWord.empty() )
+				continue; // a whole-file section
+
+			if( (chunkSize < (1ULL << ELB_CHECKSUM_MIN_CHUNK_SHIFT) ) ||
+				(chunkSize > (1ULL << ELB_CHECKSUM_MAX_CHUNK_SHIFT) ) || (chunkSize & (chunkSize - 1) ) )
+				fail("the chunk size is not a power of two from 4K to 1G");
+
+			section = std::make_shared<ChecksumList>();
+			section->chunkShift = __builtin_ctzll(chunkSize);
+			list = section;
+			continue;
+		}
+
+		if(!inSection)
+			fail("a line before the first \"# phase\" header");
+
+		if(!section)
+			continue; // (a line of a whole-file section)
+
+		const size_t crcBlank = line.rfind(' ');
+		const size_t lenBlank = (crcBlank && (crcBlank != std::string::npos) ) ?
+			line.rfind(' ', crcBlank - 1) : std::string::npos;
+		const size_t offBlank = (lenBlank && (lenBlank != std::string::npos) ) ?
+			line.rfind(' ', lenBlank - 1) : std::string::npos;
+
+		if( (offBlank == std::string::npos) || !offBlank)
+			fail("not \"path offset length crc32\"");
+
+		const std::string crcStr = line.substr(crcBlank + 1);
+		const uint64_t chunkSize = 1ULL << section->chunkShift;
+		uint64_t offset, length;
+
+		if(!parseChecksumListNum(line.substr(offBlank + 1, lenBlank - offBlank - 1), offset) ||
+			!parseChecksumListNum(line.substr(lenBlank + 1, crcBlank - lenBlank - 1), length) ||
+			(crcStr.size() != 8) || (crcStr.find_first_not_of("0123456789abcdefABCDEF") !=
+			std::string::npos) )
+			fail("not \"path offset length crc32\"");
+
+		if( (offset % chunkSize) || !length || (length > chunkSize) )
+			fail("not a chunk of " + std::to_string(chunkSize) + " bytes");
+
+		ChecksumList::File& file = section->files[line.substr(0, offBlank)];
+		const uint64_t chunkIdx = offset >> section->chunkShift;
+
+		if(file.hasLine(chunkIdx) )
+			fail("a second line for this path and offset");
+
+		if(chunkIdx >= file.present.size() )
+		{
+			file.present.resize(chunkIdx + 1);
+			file.crcs.resize(chunkIdx + 1);
+		}
+
+		file.path = line.substr(0, offBlank);
+		file.present[chunkIdx] = true;
+		file.crcs[chunkIdx] = (uint32_t)std::stoul(crcStr, NULL, 16);
+		section->numChunks++;
+
+		if(length != chunkSize)
+			file.shortLengths[chunkIdx] = length;
+	}
+
+	if(!list)
+		throw WorkerError("Checksum list has no section with a chunk size (\"# phase WRITE|READ "
+			"chunk <K>\"); write it with --checksums and --checksumchunk.");
+
+	return list;
+}
+
+void Manager::setChecksumList(std::shared_ptr<const ChecksumList> list)
+{
+	Config& cfg = shared.cfg;
+
+	if(cfg.checksumChunkShift && (cfg.checksumChunkShift != list->chunkShift) )
+		throw WorkerError("The checksum chunk size (--checksumchunk " +
+			std::to_string(1ULL << cfg.checksumChunkShift) + ") differs from the checksum list's (" +
+			std::to_string(1ULL << list->chunkShift) + ").");
+
+	checkChecksumChunks(cfg, list->chunkShift, "the checksum list's chunk size");
+
+	if(cfg.rwMixReadPercent || cfg.numRWMixReadThreads)
+		throw WorkerError("Checksum verification (--checksumverify) cannot be used together with "
+			"rwmix (a phase in both directions).");
+
+	if(cfg.verifyDamageReport)
+		throw WorkerError("Checksum verification (--checksumverify) cannot be used together with a "
+			"verify report (--verifyreport).");
+
+	cfg.checksumChunkShift = list->chunkShift;
+	shared.checksumList = list;
+}
+
+void Manager::getChecksumVerifyCounts(uint64_t& outNumChunks, uint64_t& outNumFiles)
+{
+	std::set<std::string> paths;
+
+	outNumChunks = 0;
+
+	for(const std::unique_ptr<Worker>& worker : workers)
+	{
+		outNumChunks += worker->getNumChecksumChunksChecked();
+
+		for(const std::string& path : worker->getChecksumVerifiedFiles() )
+			paths.insert(path);
+	}
+
+	outNumFiles = paths.size();
 }
 
 /* Statistics::generatePhaseResults (Statistics.cpp:1641-1764) */
@@ -1316,6 +1524,39 @@ int64_t elb_mgr_checksums(elb_mgr* m, char* outBuf, uint64_t outBufLen)
 	}
 
 	return (int64_t)text.size();
+}
+
+int elb_mgr_set_checksum_list(elb_mgr* m, const char* text, uint64_t len)
+{
+	if(!m || (!text && len) )
+	{
+		elb_set_last_error("elb_mgr_set_checksum_list: NULL manager or text");
+		return -1;
+	}
+
+	try
+	{
+		m->impl->setChecksumList(elb::ChecksumList::parse(std::string(text ? text : "", len) ) );
+	}
+	catch(std::exception& e)
+	{
+		elb_set_last_error(e.what() );
+		return -1;
+	}
+
+	return 0;
+}
+
+int elb_mgr_checksum_verify_counts(elb_mgr* m, uint64_t* outNumChunks, uint64_t* outNumFiles)
+{
+	if(!m || !outNumChunks || !outNumFiles)
+	{
+		elb_set_last_error("elb_mgr_checksum_verify_counts: NULL argument");
+		return -1;
+	}
+
+	m->impl->getChecksumVerifyCounts(*outNumChunks, *outNumFiles);
+	return 0;
 }
 
 uint32_t elb_mgr_num_workers(elb_mgr* m)

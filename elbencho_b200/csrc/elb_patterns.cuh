@@ -291,6 +291,10 @@ ELB_HD uint64_t elb_rand_grain_bytes8(uint64_t filePos, const Keys& keys, uint64
 #define ELB_CRC32_ONE 0x80000000u           /* x^0 */
 #define ELB_CRC32_X8 0x00800000u            /* x^8: one zero byte */
 #define ELB_CRC32_ORDER 0xFFFFFFFFULL       /* x^ELB_CRC32_ORDER = 1 mod P */
+/* chunked CRCs (elb_crc32_chunks): chunks of 2^shift bytes; at least 4 KiB, so that a kernel
+   piece meets one chunk boundary at most */
+#define ELB_CRC32_MIN_CHUNK_SHIFT 12
+#define ELB_CRC32_MAX_CHUNK_SHIFT 40
 
 /* n mod ELB_CRC32_ORDER without a 64-bit division (2^32 = 1 mod 2^32 - 1) */
 ELB_HD constexpr uint64_t elb_crc32_mod_order(uint64_t n)

@@ -342,6 +342,8 @@ void Worker::resetStats() // Worker.h:92-110
 	numDamageBytesDropped = 0;
 	deferredVerifyError.clear();
 	checksumAccs.clear();
+	checksumListFiles.clear();
+	numChecksumChunksChecked = 0;
 
 	std::unique_lock<std::mutex> lock(errorMutex);
 	lastError.clear();
@@ -813,6 +815,69 @@ void Worker::preparePhase()
 	takeCustomTreeShare();
 
 	allocRings();
+	setupChecksums();
+}
+
+/**
+ * --checksums / --checksumverify: which stages take the CRC launch, in chunks of which size, and
+ * the batches' CRC slots. Runs after the rings are made and at the start of every write and read
+ * phase, since a checksum list (elb_mgr_set_checksum_list) may be set between phases; a change
+ * drops the batch graphs, which hold the launches of the old setup. Without either option it
+ * allocates and changes nothing.
+ */
+void Worker::setupChecksums()
+{
+	const bool readChecksum = cfg.checksums || shared->checksumList;
+	const unsigned chunkShift = cfg.checksumChunkShift ? cfg.checksumChunkShift : 64;
+	const uint64_t slotsPerDesc = (chunkShift == 64) ? 1 :
+		std::max( (cfg.blockSize + ( (uint64_t)1 << chunkShift) - 1) >> chunkShift, (uint64_t)1);
+
+	if(batches.empty() || ( (readChecksum == readStage.checksum) &&
+		(chunkShift == crcChunkShift) && (slotsPerDesc == crcSlotsPerDesc) ) )
+		return;
+
+	std::shared_lock<std::shared_timed_mutex> allocLock(shared->gpuAllocMutex);
+
+	writeStage.checksum = cfg.checksums;
+	readStage.checksum = readChecksum;
+	/* --verifydirect: a write phase's checksums are those of the written bytes, so the read-back
+	   takes none, and must not share the read phase's batch graphs then */
+	verifyBackStage.useGraph = readStage.useGraph && !readChecksum;
+	crcChunkShift = chunkShift;
+	crcSlotsPerDesc = slotsPerDesc;
+
+	for(Batch& batch : batches)
+	{
+		if(batch.readGraphExec)
+			cudaGraphExecDestroy(batch.readGraphExec);
+		if(batch.writeGraphExec)
+			cudaGraphExecDestroy(batch.writeGraphExec);
+		if(batch.devCrcs)
+			cudaFree(batch.devCrcs);
+		if(batch.hostCrcs)
+			cudaFreeHost(batch.hostCrcs);
+
+		batch.readGraphExec = NULL;
+		batch.writeGraphExec = NULL;
+		batch.devCrcs = NULL;
+		batch.hostCrcs = NULL;
+
+		if(!readChecksum)
+			continue;
+
+		const uint64_t numSlots = batchBlocks * slotsPerDesc;
+
+		if(!batch.hostShifts)
+			ELB_CUDA_CHECK(cudaHostAlloc( (void**)&batch.hostShifts, sizeof(uint64_t) * batchBlocks,
+				cudaHostAllocDefault), "Pinned checksum shift allocation");
+		ELB_CUDA_CHECK(cudaMalloc( (void**)&batch.devCrcs, sizeof(uint32_t) * numSlots),
+			"GPU checksum allocation");
+		ELB_CUDA_CHECK(cudaHostAlloc( (void**)&batch.hostCrcs, sizeof(uint32_t) * numSlots,
+			cudaHostAllocDefault), "Pinned checksum allocation");
+		ELB_CUDA_CHECK(cudaMemsetAsync(batch.devCrcs, 0, sizeof(uint32_t) * numSlots,
+			batch.stream), "GPU checksum init");
+		ELB_CUDA_CHECK(cudaStreamSynchronize(batch.stream), "GPU checksum init");
+	}
 }
 
 /**
@@ -868,14 +933,9 @@ void Worker::allocRings()
 		salt ? elb_content{elb_content::PATTERN, salt} :
 		pct ? elb_content{elb_content::RANDOM, blockVarianceSeed, pct} : elb_content{};
 
-	writeStage = GpuStage{false, transfer, writeContent, useGraph, cfg.checksums};
-	readStage = GpuStage{true, transfer, salt ? writeContent : elb_content{}, useGraph,
-		cfg.checksums};
-	/* --verifydirect: a write phase's checksums are those of the written bytes, so the read-back
-	   takes none, and must not share the read phase's batch graphs then */
+	writeStage = GpuStage{false, transfer, writeContent, useGraph, false};
+	readStage = GpuStage{true, transfer, salt ? writeContent : elb_content{}, useGraph, false};
 	verifyBackStage = readStage;
-	verifyBackStage.checksum = false;
-	verifyBackStage.useGraph = useGraph && !cfg.checksums;
 
 	if(cfg.pipelineBatchBlocks)
 		batchBlocks = cfg.pipelineBatchBlocks;
@@ -953,18 +1013,6 @@ void Worker::allocRings()
 			"GPU ticket counter init");
 
 		memset(batch.hostResults, 0, sizeof(elb_verify_result) * batchBlocks);
-
-		if(cfg.checksums)
-		{
-			ELB_CUDA_CHECK(cudaHostAlloc( (void**)&batch.hostShifts, sizeof(uint64_t) * batchBlocks,
-				cudaHostAllocDefault), "Pinned checksum shift allocation");
-			ELB_CUDA_CHECK(cudaMalloc( (void**)&batch.devCrcs, sizeof(uint32_t) * batchBlocks),
-				"GPU checksum allocation");
-			ELB_CUDA_CHECK(cudaHostAlloc( (void**)&batch.hostCrcs, sizeof(uint32_t) * batchBlocks,
-				cudaHostAllocDefault), "Pinned checksum allocation");
-			ELB_CUDA_CHECK(cudaMemsetAsync(batch.devCrcs, 0, sizeof(uint32_t) * batchBlocks,
-				batch.stream), "GPU checksum init");
-		}
 
 		// arm the device results once; verify launches re-arm what they report
 		if(elb_launch_verify_init(batch.devResults, batchBlocks, batch.stream) )
@@ -1176,7 +1224,8 @@ void Worker::abortInFlight()
 			cudaMemsetAsync(batch.devDoneTicket, 0, sizeof(unsigned), batch.stream);
 			elb_launch_verify_init(batch.devResults, batchBlocks, batch.stream);
 			if(batch.devCrcs)
-				cudaMemsetAsync(batch.devCrcs, 0, sizeof(uint32_t) * batchBlocks, batch.stream);
+				cudaMemsetAsync(batch.devCrcs, 0, sizeof(uint32_t) * batchBlocks * crcSlotsPerDesc,
+					batch.stream);
 			cudaStreamSynchronize(batch.stream);
 
 			batch.numIOPending = 0;
@@ -1775,6 +1824,8 @@ void Worker::rwPhase()
 		ELB_CUDA_CHECK(cudaStreamSynchronize(batches[0].stream), "GPU counter block reset");
 	}
 
+	setupChecksums();
+
 	initPhaseOffsetPlan();
 
 	openThreadFDs(benchPhase == ELB_PHASE_CREATEFILES);
@@ -2166,8 +2217,12 @@ uint32_t Worker::fillStageDescs(Batch& batch, const GpuStage& stage, uint64_t& o
 		if(!stage.isRead && block.ioIsRead)
 			continue;
 
-		if(stage.checksum)
+		if(stage.checksum && (crcChunkShift == 64) )
 			batch.hostShifts[numDescs] = blockFileSize(block) - block.offset - block.len;
+		else if(stage.checksum && (block.offset & ( ( (uint64_t)1 << crcChunkShift) - 1) ) )
+			throw WorkerError("Checksum chunks need blocks at multiples of the chunk size. "
+				"File: " + blockFilePath(block) + "; Offset: " + std::to_string(block.offset) +
+				"; Chunk size: " + std::to_string( (uint64_t)1 << crcChunkShift) );
 
 		batch.hostDescs[numDescs++] = elb_block_desc{slotDevPtr(batch, i), block.len,
 			block.offset, descBlockCounter(stage.content, block)};
@@ -2362,7 +2417,8 @@ void Worker::enqueueStage(Batch& batch, const GpuStage& stage, uint32_t numBlock
 
 	// (a write's checksum reads the device slot before its stage-out copy)
 	if(stage.checksum && elb_launch_crc32(batch.hostDescs, batch.hostShifts, numBlocks,
-		batch.devCrcs, batch.hostCrcs, batch.devDoneTicket, batch.stream) )
+		crcChunkShift, crcSlotsPerDesc, batch.devCrcs, batch.hostCrcs, batch.devDoneTicket,
+		batch.stream) )
 		throw WorkerError(std::string("GPU checksum failed. ") + elb_last_error() );
 
 	if( (stage.transfer == GpuStage::TRANSFER_COPY) && !stage.isRead)
@@ -2575,6 +2631,7 @@ void Worker::retireReadBatch(Batch& batch)
 {
 	gpuWait(batch);
 	checkVerifyResults(batch);
+	checkBatchChecksums(batch);
 	accountBatch(batch, (uint64_t)(batch.gpuMilliSecs * 1000) );
 }
 
@@ -2634,8 +2691,16 @@ void Worker::accountBatch(Batch& batch, uint64_t gpuUSecTotal)
 	addBatchChecksums(batch);
 }
 
+/* the numeric identity of a block's file: its bench path index (file mode), its dir and file
+ * index (dir mode) or its tree file entry */
+Worker::FileID Worker::blockFileID(const BlockRef& block) const
+{
+	return (cfg.pathType != ELB_PATH_DIR) ? FileID(block.fileIdx, 0) :
+		block.isTreeElem ? FileID(~0ULL, block.fileIndex) : FileID(block.dirIndex, block.fileIndex);
+}
+
 /* --checksums: the CRC contributions of a batch whose blocks are done (no rwmix: descriptor i is
- * block i), into the accumulator of each block's file */
+ * block i), into the accumulator of each block's file: XORed per file, or one entry per chunk */
 void Worker::addBatchChecksums(const Batch& batch)
 {
 	if(!cfg.checksums)
@@ -2644,16 +2709,95 @@ void Worker::addBatchChecksums(const Batch& batch)
 	for(size_t i = 0; i < batch.blocks.size(); i++)
 	{
 		const BlockRef& block = batch.blocks[i];
-		typedef std::pair<uint64_t, uint64_t> FileID;
-		const FileID fileID = (cfg.pathType != ELB_PATH_DIR) ? FileID(block.fileIdx, 0) :
-			block.isTreeElem ? FileID(~0ULL, block.fileIndex) :
-			FileID(block.dirIndex, block.fileIndex);
+		ChecksumAcc& acc = checksumAccs.try_emplace(blockFileID(block), ChecksumAcc{block}).first->
+			second;
 
-		ChecksumAcc& acc = checksumAccs.try_emplace(fileID, ChecksumAcc{block}).first->second;
-
-		acc.rawCrc ^= batch.hostCrcs[i];
 		acc.numBytes += block.len;
+
+		if(crcChunkShift == 64)
+		{
+			acc.rawCrc ^= batch.hostCrcs[i];
+			continue;
+		}
+
+		const uint64_t chunkSize = (uint64_t)1 << crcChunkShift;
+		const uint64_t blockEnd = block.offset + block.len;
+
+		for(uint64_t pos = block.offset, slot = i * crcSlotsPerDesc; pos < blockEnd;
+			pos += chunkSize, slot++)
+			acc.chunks.push_back(ChunkChecksum{pos, std::min(chunkSize, blockEnd - pos),
+				batch.hostCrcs[slot]});
 	}
+}
+
+/**
+ * --checksumverify: compare the CRC of each chunk of a read batch with the list line of its file
+ * and offset (blocks start at chunk boundaries, fillStageDescs). The file's list entry is looked up
+ * once per file and phase. The first chunk without a matching line fails the worker.
+ */
+void Worker::checkBatchChecksums(const Batch& batch)
+{
+	const ChecksumList* list = shared->checksumList.get();
+
+	if(!list || !readStage.checksum || (benchPhase != ELB_PHASE_READFILES) )
+		return;
+
+	const uint64_t chunkSize = (uint64_t)1 << crcChunkShift;
+	const uint32_t fullChunkXor = elb_crc32_finish_hd(0, chunkSize);
+
+	for(size_t i = 0; i < batch.blocks.size(); i++)
+	{
+		const BlockRef& block = batch.blocks[i];
+		const uint64_t blockEnd = block.offset + block.len;
+		auto fileIter = checksumListFiles.find(blockFileID(block) );
+
+		if(fileIter == checksumListFiles.end() )
+			fileIter = checksumListFiles.emplace(blockFileID(block),
+				list->findFile(blockFilePath(block) ) ).first;
+
+		const ChecksumList::File* file = fileIter->second;
+
+		for(uint64_t pos = block.offset, slot = i * crcSlotsPerDesc; pos < blockEnd;
+			pos += chunkSize, slot++)
+		{
+			const uint64_t len = std::min(chunkSize, blockEnd - pos);
+			const uint32_t rawCrc = batch.hostCrcs[slot];
+			const uint32_t crc = (len == chunkSize) ? (rawCrc ^ fullChunkXor) :
+				elb_crc32_finish_hd(rawCrc, len);
+			const uint64_t chunkIdx = pos >> crcChunkShift;
+			const bool hasLine = file && file->hasLine(chunkIdx);
+
+			if(hasLine && (file->chunkLength(chunkIdx, chunkSize) == len) &&
+				(file->crcs[chunkIdx] == crc) )
+			{
+				numChecksumChunksChecked++;
+				continue;
+			}
+
+			char expected[9] = "-";
+			char actual[9];
+
+			if(hasLine)
+				snprintf(expected, sizeof(expected), "%08x", file->crcs[chunkIdx]);
+			snprintf(actual, sizeof(actual), "%08x", crc);
+
+			throw WorkerError("Checksum verification failed. File: " + blockFilePath(block) + "; "
+				"Offset: " + std::to_string(pos) + "; Length: " + std::to_string(len) + "; "
+				"Expected CRC-32: " + expected + "; Actual CRC-32: " + actual);
+		}
+	}
+}
+
+/* --checksumverify: the paths of the files this worker checked in the phase */
+std::vector<std::string> Worker::getChecksumVerifiedFiles() const
+{
+	std::vector<std::string> paths;
+
+	for(const auto& entry : checksumListFiles)
+		if(entry.second)
+			paths.push_back(entry.second->path);
+
+	return paths;
 }
 
 /* the data set size of the block's file: -s, or the tree file's (rounded up) size of the entry */
@@ -2668,7 +2812,8 @@ std::vector<FileChecksum> Worker::getFileChecksums() const
 
 	for(const auto& entry : checksumAccs)
 		checksums.push_back(FileChecksum{blockFilePath(entry.second.block),
-			blockFileSize(entry.second.block), entry.second.numBytes, entry.second.rawCrc});
+			blockFileSize(entry.second.block), entry.second.numBytes, entry.second.rawCrc,
+			entry.second.chunks});
 
 	return checksums;
 }

@@ -50,6 +50,8 @@ typedef std::chrono::steady_clock Clock;
 
 class Worker;
 
+struct ChecksumList;
+
 /* WorkersSharedData (reference source/workers/WorkersSharedData.h:33-107): phase barrier and
  * done counters. The reference's boost uuid bench ID becomes a sequence number. */
 struct Shared
@@ -72,6 +74,7 @@ struct Shared
 	RWMixThreadsBalancer rwMixThreadsBalancer; // --rwmixthrpct (reset by the manager per phase)
 
 	TreeManifest customTree; // --treefile, parsed once by the manager (ProgArgs::loadCustomTreeFile)
+	std::shared_ptr<const ChecksumList> checksumList; // --checksumverify (set between phases)
 
 	/* workers hold this shared while they allocate / free device memory or instantiate graphs;
 	   the live stats reducer holds it exclusively while its collective is in flight, because a
@@ -119,6 +122,14 @@ struct DamageRun
 	uint16_t firstSectorLo{0}; // where the block starts in the first sector (0: before it)
 };
 
+/* --checksumchunk: the CRC of one chunk of a file that a phase moved */
+struct ChunkChecksum
+{
+	uint64_t offset;
+	uint64_t length;
+	uint32_t rawCrc; // (elb_crc32_chunks)
+};
+
 /* --checksums: what a worker moved of one file in a phase */
 struct FileChecksum
 {
@@ -126,6 +137,44 @@ struct FileChecksum
 	uint64_t size{0};     // the file's data set size
 	uint64_t numBytes{0}; // bytes of the blocks the phase moved
 	uint32_t rawCrc{0};   // XOR of the blocks' contributions (elb_crc32_blocks)
+	std::vector<ChunkChecksum> chunks; // --checksumchunk: the chunks instead, in the order moved
+};
+
+/**
+ * --checksumverify: the last section with a chunk size of a checksum list that --checksums
+ * --checksumchunk wrote: "# phase WRITE|READ chunk <K>", then lines "path offset length crc32".
+ * One CRC and one bit per chunk of each listed file; lines shorter than K (a file's last chunk)
+ * keep their length aside.
+ */
+struct ChecksumList
+{
+	struct File
+	{
+		std::string path;
+		std::vector<uint32_t> crcs;  // zlib CRC-32 by chunk index
+		std::vector<bool> present;   // whether the chunk has a line
+		std::map<uint64_t, uint64_t> shortLengths; // chunk index -> length of lines shorter than K
+
+		bool hasLine(uint64_t chunkIdx) const
+			{ return (chunkIdx < present.size() ) && present[chunkIdx]; }
+		uint64_t chunkLength(uint64_t chunkIdx, uint64_t chunkSize) const
+		{
+			const auto iter = shortLengths.find(chunkIdx);
+			return (iter == shortLengths.end() ) ? chunkSize : iter->second;
+		}
+	};
+
+	unsigned chunkShift{0};
+	uint64_t numChunks{0};
+	std::map<std::string, File> files;
+
+	// throws WorkerError naming the line number of a malformed line
+	static std::shared_ptr<const ChecksumList> parse(const std::string& text);
+	const File* findFile(const std::string& path) const
+	{
+		const auto iter = files.find(path);
+		return (iter == files.end() ) ? NULL : &iter->second;
+	}
 };
 
 /* produces the worker's blocks of a phase in submission order */
@@ -242,6 +291,9 @@ class Worker
 		const std::string& getDeferredVerifyError() const { return deferredVerifyError; }
 		// --checksums results of the phase (read when all workers are done)
 		std::vector<FileChecksum> getFileChecksums() const;
+		// --checksumverify results of the phase (read when all workers are done)
+		uint64_t getNumChecksumChunksChecked() const { return numChecksumChunksChecked; }
+		std::vector<std::string> getChecksumVerifiedFiles() const;
 
 		void interruptExecution() { isInterruptionRequested = true; }
 		void createStoneWallStats(); // called by the first finisher under Shared::mutex
@@ -353,13 +405,21 @@ class Worker
 
 		/* --checksums: the XOR of the CRC contributions and the bytes of each file this worker
 		   moved in the phase, by numeric file identity; paths are resolved at the phase end */
+		typedef std::pair<uint64_t, uint64_t> FileID; // (blockFileID)
 		struct ChecksumAcc
 		{
 			BlockRef block; // (a block of the file, for its path)
 			uint64_t numBytes{0};
 			uint32_t rawCrc{0};
+			std::vector<ChunkChecksum> chunks; // --checksumchunk
 		};
-		std::map<std::pair<uint64_t, uint64_t>, ChecksumAcc> checksumAccs;
+		std::map<FileID, ChecksumAcc> checksumAccs;
+		unsigned crcChunkShift{64};    // the CRC launch's chunks (64: whole files), setupChecksums
+		uint64_t crcSlotsPerDesc{1};   // CRC slots per block
+		/* --checksumverify: the list entry of each file the phase read (NULL: not listed) and the
+		   chunks that matched */
+		std::map<FileID, const ChecksumList::File*> checksumListFiles;
+		uint64_t numChecksumChunksChecked{0};
 
 		// accounting
 		std::atomic<uint64_t> numH2DBytes{0};
@@ -400,6 +460,9 @@ class Worker
 		void verifyWrittenBatch(Batch& batch);
 		void accountBatch(Batch& batch, uint64_t gpuUSecTotal);
 		void addBatchChecksums(const Batch& batch);
+		void checkBatchChecksums(const Batch& batch);
+		void setupChecksums();
+		FileID blockFileID(const BlockRef& block) const;
 		uint64_t blockFileSize(const BlockRef& block) const;
 		void gpuLaunchStage(Batch& batch, bool isRead);
 		uint32_t fillStageDescs(Batch& batch, const GpuStage& stage, uint64_t& outNumBytes);
@@ -473,11 +536,19 @@ class Manager
 		/* --checksums: each file of the last phase, merged over all workers */
 		struct ChecksumReport
 		{
-			std::string lines; // "<path> <size> <bytes covered> <crc32 or ->\n", sorted by path
+			std::string lines; // "<path> <size> <bytes covered> <crc32 or ->\n", sorted by path;
+			                   // --checksumchunk: "<path> <offset> <length> <crc32>\n" per chunk
 			uint64_t numFiles{0};
 			uint64_t numComplete{0}; // files with a CRC
+			uint64_t numChunks{0};   // --checksumchunk
 		};
 		ChecksumReport getChecksumReport();
+		ChecksumReport getChunkChecksumReport();
+
+		/* --checksumverify: parse a checksum list and check the following read phases against
+		   it (throws WorkerError); the chunks and files the last phase checked */
+		void setChecksumList(std::shared_ptr<const ChecksumList> list);
+		void getChecksumVerifyCounts(uint64_t& outNumChunks, uint64_t& outNumFiles);
 
 		Shared shared;
 		std::vector<std::unique_ptr<Worker> > workers;

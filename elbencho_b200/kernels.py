@@ -301,6 +301,21 @@ def crc32_blocks(pinned_descs_ptr, pinned_shifts_ptr, num_descs, dev_crcs_ptr,
            "elb_crc32_blocks")
 
 
+def crc32_chunks(pinned_descs_ptr, pinned_shifts_ptr, num_descs, chunk_shift, slots_per_desc,
+                 dev_crcs_ptr, pinned_crcs_ptr=0, dev_ticket_ptr=0, stream=0):
+    """Chunked CRC-32s (--checksumchunk, --checksumverify): crc32_blocks with each block cut at
+    the multiples of 2**chunk_shift of its file offset (chunk_shift 12..40, or 64 for no cuts,
+    which is crc32_blocks with slots_per_desc 1). The uint32 dev_crcs_ptr[i * slots_per_desc + j]
+    takes the raw CRC-32 of block i's bytes in its (j+1)-th chunk, shifted to that chunk's end
+    (the next multiple, or the block end if that comes first); crc32_finish(value, length) of a
+    chunk that lies inside the block is its zlib.crc32. pinned_shifts_ptr may be 0 with chunks."""
+    _check(_native.load().elb_crc32_chunks(pinned_descs_ptr, pinned_shifts_ptr or None, num_descs,
+                                           chunk_shift, slots_per_desc, dev_crcs_ptr,
+                                           pinned_crcs_ptr or None, dev_ticket_ptr or None,
+                                           stream),
+           "elb_crc32_chunks")
+
+
 def crc32_shift(crc, num_zero_bytes):
     """the raw CRC-32 of crc's message followed by num_zero_bytes zero bytes"""
     return int(_native.load().elb_crc32_shift(crc, num_zero_bytes))

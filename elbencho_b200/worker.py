@@ -114,6 +114,7 @@ class WorkerConfig:
     verify_collect_all: bool = False
     verify_report: bool = False       # --verifyreport: map bad blocks' damage, fail at phase end
     checksums: bool = False           # --checksums: each file's CRC-32 per phase (checksums())
+    checksum_chunk_shift: int = 0     # --checksumchunk: CRC-32s of 2**shift byte chunks (0: files)
     serialize_buffered_writes: int = 0  # 0 auto, 1 on, 2 off (--writegate)
     staging_engine: int = 0           # 0 auto, 1 kernels move the data, 2 cudaMemcpyAsync
     no_gpu_numa_binding: bool = False  # --nogpunuma
@@ -133,6 +134,7 @@ class WorkerConfig:
         cfg.numThreads = self.num_threads
         cfg.rankOffset = self.rank_offset
         cfg.numDataSetThreads = self.num_dataset_threads
+        cfg.checksumChunkShift = self.checksum_chunk_shift
         cfg.blockSize = self.block_size
         cfg.fileSize = self.file_size
         cfg.ioDepth = self.io_depth
@@ -413,10 +415,27 @@ class WorkerManager:
         self._lib.elb_mgr_checksums(self._h, buf, size + 1)
         return buf.value.decode("utf-8", "replace")
 
+    def set_checksum_list(self, text):
+        """--checksumverify: check every chunk the following read phases read against the last
+        section with a chunk size of this checksum list (str or bytes, as checksums_text() of a
+        chunked phase, under a "# phase WRITE|READ chunk <K>" header, gives it)."""
+        data = text.encode("utf-8") if isinstance(text, str) else bytes(text)
+        if self._lib.elb_mgr_set_checksum_list(self._h, data, len(data)) != 0:
+            raise WorkerError(_native.last_error())
+
+    def checksum_verify_counts(self):
+        """--checksumverify: (chunks checked, files) of the last phase."""
+        chunks, files = ctypes.c_uint64(0), ctypes.c_uint64(0)
+        if self._lib.elb_mgr_checksum_verify_counts(self._h, ctypes.byref(chunks),
+                                                    ctypes.byref(files)) != 0:
+            raise WorkerError(_native.last_error())
+        return chunks.value, files.value
+
     def checksums(self):
         """The last phase's files, merged over all workers and sorted by path:
         [(path, size, bytes_covered, crc32)], crc32 an int (zlib.crc32 of the file's first size
-        bytes) or None if the phase did not cover them exactly once."""
+        bytes) or None if the phase did not cover them exactly once. With checksum_chunk_shift:
+        [(path, offset, length, crc32)] per chunk, sorted by path and offset."""
         files = []
         for line in self.checksums_text().splitlines():
             path, size, covered, crc = line.rsplit(" ", 3)

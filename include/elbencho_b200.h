@@ -304,6 +304,19 @@ int elb_damage_map(const elb_block_desc* descs, uint32_t numDescs, int contentKi
  * Blocks of any length (0 too) and any device address. */
 int elb_crc32_blocks(const elb_block_desc* descs, const uint64_t* shifts, uint32_t numDescs,
 	uint32_t* devCrcs, uint32_t* hostCrcs, unsigned* devTicket, void* stream);
+/* Chunked CRC-32s (--checksumchunk, --checksumverify): elb_crc32_blocks with each block cut at
+ * the chunk boundaries of its file offsets (descs[i].fileOffset), every 2^chunkShift bytes
+ * (chunkShift 12..40; 64 = no boundaries: exactly elb_crc32_blocks, slotsPerDesc must be 1). Slot
+ * j of descriptor i, devCrcs[i * slotsPerDesc + j], takes X(R(the block's bytes in chunk c0 + j),
+ * n), c0 being the chunk of the block's first byte and n the bytes from the block's last byte in
+ * that chunk to the chunk's end (the next boundary, or the block end if that comes first), plus
+ * shifts[i] with chunkShift 64. So a slot whose chunk lies inside the block is the chunk's raw CRC,
+ * and elb_crc32_finish(slot, chunk length) is its zlib CRC-32. shifts may be NULL with chunks.
+ * Fails without launching if a descriptor spans more than slotsPerDesc chunks. hostCrcs and
+ * devTicket publish all numDescs * slotsPerDesc slots as with elb_crc32_blocks. */
+int elb_crc32_chunks(const elb_block_desc* descs, const uint64_t* shifts, uint32_t numDescs,
+	unsigned chunkShift, uint64_t slotsPerDesc, uint32_t* devCrcs, uint32_t* hostCrcs,
+	unsigned* devTicket, void* stream);
 /* X(crc, n) of elb_crc32_blocks (n: any number of zero bytes) */
 uint32_t elb_crc32_shift(uint32_t crc, uint64_t n);
 /* zlib's CRC-32 of a message of size bytes from its raw CRC R (elb_crc32_blocks) */
@@ -344,6 +357,10 @@ typedef struct elb_cfg
 	uint32_t numThreads;
 	uint32_t rankOffset;
 	uint32_t numDataSetThreads; /* 0 = numThreads */
+	/* --checksumchunk (with --checksums or a checksum list, elb_mgr_set_checksum_list): CRC-32s
+	 * of chunks of 2^shift file bytes (12..30) instead of whole files, 0 = whole files. It takes
+	 * the 4 bytes of padding in front of blockSize: no other field moves. */
+	int32_t checksumChunkShift;
 
 	/* -b / -s / --iodepth / --direct */
 	uint64_t blockSize;
@@ -754,8 +771,20 @@ int64_t elb_mgr_verify_report(elb_mgr* m, char* outBuf, uint64_t outBufLen);
  * text lines "<path> <size> <bytes covered> <crc>\n" sorted by path. size is the file's data set
  * size, bytes covered the sum of the lengths of its blocks that the phase moved, crc zlib's CRC-32
  * of the file's first size bytes as 8 lowercase hex digits if bytes covered == size, else "-".
- * Returns the length of the full text (truncated to outBufLen - 1 bytes in outBuf), -1 on error. */
+ * Returns the length of the full text (truncated to outBufLen - 1 bytes in outBuf), -1 on error.
+ * With elb_cfg::checksumChunkShift, the text is instead one line "<path> <offset> <length> <crc>\n"
+ * per chunk the last phase moved, sorted by path and offset. */
 int64_t elb_mgr_checksums(elb_mgr* m, char* outBuf, uint64_t outBufLen);
+
+/* --checksumverify: parse a checksum list (text of len bytes, as --checksums with a chunk size
+ * writes it) and check every chunk that the following read phases move against the last section
+ * of it that has a chunk size. Its chunk size becomes elb_cfg::checksumChunkShift. A read phase
+ * then fails at the first chunk whose CRC-32 differs from its line, that has no line, or whose
+ * line has another length. Call it between phases. Returns -1 (elb_last_error names the line of a
+ * malformed line, or the option the list conflicts with), else 0. */
+int elb_mgr_set_checksum_list(elb_mgr* m, const char* text, uint64_t len);
+/* --checksumverify: the chunks the last phase checked and the files they belong to */
+int elb_mgr_checksum_verify_counts(elb_mgr* m, uint64_t* outNumChunks, uint64_t* outNumFiles);
 
 uint32_t elb_mgr_num_workers(elb_mgr* m);
 elb_worker* elb_mgr_worker(elb_mgr* m, uint32_t localIdx);
