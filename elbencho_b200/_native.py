@@ -64,6 +64,7 @@ class Cfg(ctypes.Structure):
         ("useExplicitRandOffsetAlgo", c_i32),
         ("doReverseSeqOffsets", c_i32),
         ("useStridedAccess", c_i32),
+        ("checksumAlgo", c_i32),
         ("randomAmount", c_u64),
         ("randOffsetSeed", c_u64),
         ("integrityCheckSalt", c_u64),
@@ -247,6 +248,10 @@ SIGNATURES = {
     "elb_crc32_blocks": (ctypes.c_int, [_VP, _VP, c_u32, _VP, _VP, _VP, _VP]),
     "elb_crc32_shift": (c_u32, [c_u32, c_u64]),
     "elb_crc32_finish": (c_u32, [c_u32, c_u64]),
+    "elb_crc_chunks": (ctypes.c_int, [ctypes.c_int32, _VP, _VP, c_u32, ctypes.c_uint, c_u64, _VP,
+                                      _VP, _VP, _VP]),
+    "elb_crc_shift": (c_u64, [ctypes.c_int32, c_u64, c_u64]),
+    "elb_crc_finish": (c_u64, [ctypes.c_int32, c_u64, c_u64]),
     "elb_crc32_chunks": (ctypes.c_int, [_VP, _VP, c_u32, ctypes.c_uint, c_u64, _VP, _VP, _VP,
                                         _VP]),
     "elb_damage_map": (ctypes.c_int, [_VP, c_u32, ctypes.c_int, c_u64, ctypes.c_uint,

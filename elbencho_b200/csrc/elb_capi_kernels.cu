@@ -403,10 +403,14 @@ int elb_damage_map(const elb_block_desc* descs, uint32_t numDescs, int contentKi
 	return 0;
 }
 
-/* the argument checks of elb_crc32_blocks and elb_crc32_chunks, then the launch */
-static int crc32Launch(const char* what, const elb_block_desc* descs, const uint64_t* shifts,
-	uint32_t numDescs, unsigned chunkShift, uint64_t slotsPerDesc, uint32_t* devCrcs,
-	uint32_t* hostCrcs, unsigned* devTicket, void* stream)
+static_assert( (elb_crc32_algo::ID == ELB_CHECKSUM_CRC32) &&
+	(elb_crc32c_algo::ID == ELB_CHECKSUM_CRC32C) &&
+	(elb_crc64nvme_algo::ID == ELB_CHECKSUM_CRC64NVME), "elb_crc_algo IDs");
+
+/* the argument checks of elb_crc32_blocks, elb_crc32_chunks and elb_crc_chunks, then the launch */
+static int crcLaunch(const char* what, int algo, const elb_block_desc* descs,
+	const uint64_t* shifts, uint32_t numDescs, unsigned chunkShift, uint64_t slotsPerDesc,
+	void* devCrcs, void* hostCrcs, unsigned* devTicket, void* stream)
 {
 	if(numDescs && (!descs || ( (chunkShift == 64) && !shifts) || !devCrcs) )
 	{
@@ -420,7 +424,7 @@ static int crc32Launch(const char* what, const elb_block_desc* descs, const uint
 		return -1;
 	}
 
-	if(elb_launch_crc32(descs, shifts, numDescs, chunkShift, slotsPerDesc, devCrcs, hostCrcs,
+	if(elb_launch_crc(algo, descs, shifts, numDescs, chunkShift, slotsPerDesc, devCrcs, hostCrcs,
 		devTicket, (cudaStream_t)stream) )
 	{
 		elb_set_last_error(std::string("elb_") + elb_last_error() );
@@ -430,45 +434,90 @@ static int crc32Launch(const char* what, const elb_block_desc* descs, const uint
 	return 0;
 }
 
+/* the chunk checks of elb_crc32_chunks and elb_crc_chunks, then crcLaunch */
+static int crcChunksLaunch(const char* what, int algo, const elb_block_desc* descs,
+	const uint64_t* shifts, uint32_t numDescs, unsigned chunkShift, uint64_t slotsPerDesc,
+	void* devCrcs, void* hostCrcs, unsigned* devTicket, void* stream)
+{
+	if( (chunkShift != 64) && ( (chunkShift < ELB_CRC_MIN_CHUNK_SHIFT) ||
+		(chunkShift > ELB_CRC_MAX_CHUNK_SHIFT) ) )
+	{
+		elb_set_last_error(std::string(what) + ": chunk shift " + std::to_string(chunkShift) +
+			" is neither 64 nor in [" + std::to_string(ELB_CRC_MIN_CHUNK_SHIFT) + ", " +
+			std::to_string(ELB_CRC_MAX_CHUNK_SHIFT) + "]");
+		return -1;
+	}
+
+	if(!slotsPerDesc || ( (chunkShift == 64) && (slotsPerDesc != 1) ) )
+	{
+		elb_set_last_error(std::string(what) + ": slots per descriptor must be at least 1, and 1 "
+			"without chunks");
+		return -1;
+	}
+
+	return crcLaunch(what, algo, descs, shifts, numDescs, chunkShift, slotsPerDesc, devCrcs,
+		hostCrcs, devTicket, stream);
+}
+
 int elb_crc32_blocks(const elb_block_desc* descs, const uint64_t* shifts, uint32_t numDescs,
 	uint32_t* devCrcs, uint32_t* hostCrcs, unsigned* devTicket, void* stream)
 {
-	return crc32Launch("elb_crc32_blocks", descs, shifts, numDescs, 64, 1, devCrcs, hostCrcs,
-		devTicket, stream);
+	return crcLaunch("elb_crc32_blocks", ELB_CHECKSUM_CRC32, descs, shifts, numDescs, 64, 1,
+		devCrcs, hostCrcs, devTicket, stream);
 }
 
 int elb_crc32_chunks(const elb_block_desc* descs, const uint64_t* shifts, uint32_t numDescs,
 	unsigned chunkShift, uint64_t slotsPerDesc, uint32_t* devCrcs, uint32_t* hostCrcs,
 	unsigned* devTicket, void* stream)
 {
-	if( (chunkShift != 64) && ( (chunkShift < ELB_CRC32_MIN_CHUNK_SHIFT) ||
-		(chunkShift > ELB_CRC32_MAX_CHUNK_SHIFT) ) )
+	return crcChunksLaunch("elb_crc32_chunks", ELB_CHECKSUM_CRC32, descs, shifts, numDescs,
+		chunkShift, slotsPerDesc, devCrcs, hostCrcs, devTicket, stream);
+}
+
+int elb_crc_chunks(int32_t algo, const elb_block_desc* descs, const uint64_t* shifts,
+	uint32_t numDescs, unsigned chunkShift, uint64_t slotsPerDesc, void* devCrcs, void* hostCrcs,
+	unsigned* devTicket, void* stream)
+{
+	if( (algo < 0) || (algo >= ELB_CRC_NUM_ALGOS) )
 	{
-		elb_set_last_error("elb_crc32_chunks: chunk shift " + std::to_string(chunkShift) +
-			" is neither 64 nor in [" + std::to_string(ELB_CRC32_MIN_CHUNK_SHIFT) + ", " +
-			std::to_string(ELB_CRC32_MAX_CHUNK_SHIFT) + "]");
+		elb_set_last_error("elb_crc_chunks: unknown checksum algorithm " + std::to_string(algo) );
 		return -1;
 	}
 
-	if(!slotsPerDesc || ( (chunkShift == 64) && (slotsPerDesc != 1) ) )
-	{
-		elb_set_last_error("elb_crc32_chunks: slots per descriptor must be at least 1, and 1 "
-			"without chunks");
-		return -1;
-	}
-
-	return crc32Launch("elb_crc32_chunks", descs, shifts, numDescs, chunkShift, slotsPerDesc,
-		devCrcs, hostCrcs, devTicket, stream);
+	return crcChunksLaunch("elb_crc_chunks", algo, descs, shifts, numDescs, chunkShift,
+		slotsPerDesc, devCrcs, hostCrcs, devTicket, stream);
 }
 
 uint32_t elb_crc32_shift(uint32_t crc, uint64_t n)
 {
-	return elb_crc32_shift_hd(crc, n);
+	return (uint32_t)elb_crc_shift(ELB_CHECKSUM_CRC32, crc, n);
 }
 
 uint32_t elb_crc32_finish(uint32_t rawCrc, uint64_t size)
 {
-	return elb_crc32_finish_hd(rawCrc, size);
+	return (uint32_t)elb_crc_finish(ELB_CHECKSUM_CRC32, rawCrc, size);
+}
+
+uint64_t elb_crc_shift(int32_t algo, uint64_t crc, uint64_t n)
+{
+	uint64_t result = 0;
+
+	if(!elb_with_crc_algo(algo, [&](auto crcAlgo)
+		{ result = crcAlgo.shift( (typename decltype(crcAlgo)::word)crc, n); } ) )
+		elb_set_last_error("elb_crc_shift: unknown checksum algorithm " + std::to_string(algo) );
+
+	return result;
+}
+
+uint64_t elb_crc_finish(int32_t algo, uint64_t rawCrc, uint64_t size)
+{
+	uint64_t result = 0;
+
+	if(!elb_with_crc_algo(algo, [&](auto crcAlgo)
+		{ result = crcAlgo.finish( (typename decltype(crcAlgo)::word)rawCrc, size); } ) )
+		elb_set_last_error("elb_crc_finish: unknown checksum algorithm " + std::to_string(algo) );
+
+	return result;
 }
 
 int elb_stage_copy(const elb_block_desc* descs, uint32_t numDescs, int hostToDevice,

@@ -123,24 +123,30 @@ static const OptDef optDefs[] =
 		"offset length differing_bytes\" per damaged extent. The phase still fails at its end with "
 		"the error of the first bad block. Requires --verify or --verifyrand. [b200]"},
 	{"checksums", 0, Opt_STR, &ProgArgs::checksumsPath, Wire_NONE, "Path of a checksum file: every "
-		"write and read phase computes the CRC-32 (zlib, gzip, zip) of each file on the GPU from "
+		"write and read phase computes the CRC (--checksumalgo) of each file on the GPU from "
 		"the bytes that pass through GPU memory and appends one section to this file (truncated at "
-		"start): \"# phase WRITE|READ\", then one line \"path size bytes_covered crc32\" per "
+		"start): \"# phase WRITE|READ\", then one line \"path size bytes_covered crc\" per "
 		"file, sorted by path. The CRC is given when the phase covered the file's first size "
 		"bytes exactly once, else \"-\". With --verifydirect only the written bytes count. Cannot "
 		"be used with --rand, --infloop, --rwmixpct, --rwmixthr or --hosts. [b200]"},
 	{"checksumchunk", 0, Opt_BYTES, &ProgArgs::checksumChunkSize, Wire_NONE, "Chunk size of "
 		"--checksums and --checksumverify: a power of two from 4K to 1G that the block size is a "
-		"multiple of. --checksums then lists the CRC-32 of every chunk the phase moved: each section "
-		"starts with \"# phase WRITE|READ chunk <K>\", then one line \"path offset length crc32\" "
+		"multiple of. --checksums then lists the CRC of every chunk the phase moved: each section "
+		"starts with \"# phase WRITE|READ chunk <K>\", then one line \"path offset length crc\" "
 		"per chunk, sorted by path and offset. Cannot be used with --norandalign. [b200]"},
 	{"checksumverify", 0, Opt_STR, &ProgArgs::checksumVerifyPath, Wire_NONE, "Path of a checksum "
-		"list that --checksums with --checksumchunk wrote: every read phase checks the CRC-32 of "
+		"list that --checksums with --checksumchunk wrote: every read phase checks the CRC of "
 		"each chunk it reads, on the GPU, against the list's last section with a chunk size, and "
 		"fails at the first chunk that differs or has no line. Works with --rand, --randamount, "
 		"--infloop and custom tree mode. The block size must be a multiple of the list's chunk "
 		"size. Cannot be used with --norandalign, --rwmixpct, --rwmixthr, --hosts or "
 		"--verifyreport. [b200]"},
+	{"checksumalgo", 0, Opt_STR, &ProgArgs::checksumAlgoName, Wire_NONE, "CRC of --checksums and "
+		"--checksumverify: crc32 (zlib, gzip, zip), crc32c (Castagnoli: iSCSI, GCS, btrfs) or "
+		"crc64nvme (NVMe protection information, S3). Other than crc32, each section header ends "
+		"with the name, and crc64nvme CRCs have 16 hex digits instead of 8. A list's own "
+		"algorithm is used for --checksumverify. Requires --checksums or --checksumverify. "
+		"(Default: crc32) [b200]"},
 	{"rwmixpct", 0, Opt_U64, &ProgArgs::rwMixReadPercent, Wire_REF, "Percentage of blocks that "
 		"should be read in a write phase."},
 	{"rwmixthr", 0, Opt_U64, &ProgArgs::numRWMixReadThreads, Wire_REF, "Number of threads that "
@@ -1023,6 +1029,16 @@ void ProgArgs::checkArgs()
 				"\"--norandalign\"");
 	}
 
+	if(!checksumAlgoName.empty() )
+	{
+		if(checksumsPath.empty() && checksumVerifyPath.empty() )
+			throw ProgError("Option \"--checksumalgo\" requires \"--checksums\" or "
+				"\"--checksumverify\"");
+
+		if(elb_crc_algo_by_name(checksumAlgoName.c_str() ) < 0)
+			throw ProgError("Option \"--checksumalgo\" must be crc32, crc32c or crc64nvme");
+	}
+
 	if(!checksumVerifyPath.empty() )
 	{ // (the list's chunks are checked wherever and however often they are read, on this host)
 		const char* conflicts[][2] = { {"--norandalign", useRandomUnaligned ? "1" : NULL},
@@ -1066,6 +1082,11 @@ void ProgArgs::checkArgs()
 		if(blockSize % listChunkSize)
 			throw ProgError("The block size (" + std::to_string(blockSize) + ") must be a multiple "
 				"of the chunk size of the checksum list (" + std::to_string(listChunkSize) + ")");
+
+		if(!checksumAlgoName.empty() &&
+			(elb_crc_algo_by_name(checksumAlgoName.c_str() ) != checksumList->algo) )
+			throw ProgError("Option \"--checksumalgo\" (" + checksumAlgoName + ") differs from "
+				"the algorithm of the checksum list (" + elb_crc_algo_name(checksumList->algo) + ")");
 	}
 
 	if(doDirectVerify && ( (!integrityCheckSalt && !randomVerifySeed) || !runCreateFilesPhase) )
@@ -1163,6 +1184,8 @@ void ProgArgs::toABIConfig(ABIConfig& out) const
 	cfg.checksumReport = !checksumsPath.empty();
 	cfg.checksumChunkShift = checksumList ? (int32_t)checksumList->chunkShift :
 		checksumChunkSize ? __builtin_ctzll(checksumChunkSize) : 0;
+	cfg.checksumAlgo = checksumList ? checksumList->algo : checksumAlgoName.empty() ?
+		ELB_CHECKSUM_CRC32 : elb_crc_algo_by_name(checksumAlgoName.c_str() );
 	cfg.serializeBufferedWrites = neverSerializeBufferedWrites ? ELB_WRITEGATE_OFF :
 		(serializeBufferedWrites ? ELB_WRITEGATE_ON : ELB_WRITEGATE_AUTO);
 	cfg.noGPUNumaBinding = noGPUNumaBinding;

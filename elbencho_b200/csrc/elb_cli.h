@@ -92,6 +92,7 @@ class ProgArgs
 		std::string checksumsPath; // --checksums
 		uint64_t checksumChunkSize{0}; // --checksumchunk
 		std::string checksumVerifyPath; // --checksumverify
+		std::string checksumAlgoName; // --checksumalgo
 		std::shared_ptr<const ChecksumList> checksumList; // --checksumverify, parsed by checkArgs
 		uint64_t rwMixReadPercent{0};
 		bool hasUserSetRWMixPercent{false};

@@ -119,6 +119,7 @@ Config Config::fromABI(const elb_cfg* cfg)
 	c.verifyDamageReport = (cfg->verifyDamageReport != 0);
 	c.checksums = (cfg->checksumReport != 0);
 	c.checksumChunkShift = (cfg->checksumChunkShift > 0) ? (unsigned)cfg->checksumChunkShift : 0;
+	c.checksumAlgo = cfg->checksumAlgo;
 	c.serializeBufferedWrites = cfg->serializeBufferedWrites;
 	c.numRWMixReadThreads = std::min(cfg->numRWMixReadThreads, cfg->numThreads); // :1088
 	c.treeFilePath = cfg->treeFilePath ? cfg->treeFilePath : "";
@@ -214,6 +215,9 @@ Config Config::fromABI(const elb_cfg* cfg)
 		throw WorkerError("The checksum chunk shift (" + std::to_string(cfg->checksumChunkShift) +
 			") is not in [" + std::to_string(ELB_CHECKSUM_MIN_CHUNK_SHIFT) + ", " +
 			std::to_string(ELB_CHECKSUM_MAX_CHUNK_SHIFT) + "].");
+
+	if( (c.checksumAlgo < 0) || (c.checksumAlgo > ELB_CHECKSUM_CRC64NVME) )
+		throw WorkerError("Invalid checksum algorithm: " + std::to_string(c.checksumAlgo) );
 
 	if(c.checksumChunkShift)
 		checkChecksumChunks(c, c.checksumChunkShift, "the checksum chunk size (--checksumchunk)");

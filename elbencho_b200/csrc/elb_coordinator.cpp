@@ -448,6 +448,10 @@ void Coordinator::writeChecksumSection(int benchPhase)
 	if(chunkShift)
 		fileStream << " chunk " << (1ULL << chunkShift);
 
+	// (the default CRC-32 keeps the headers that have no algorithm name)
+	if(manager->shared.cfg.checksumAlgo != ELB_CHECKSUM_CRC32)
+		fileStream << " " << elb_crc_algo_name(manager->shared.cfg.checksumAlgo);
+
 	fileStream << "\n" << report.lines << std::flush;
 
 	if(!fileStream)

@@ -1004,6 +1004,7 @@ struct Config
 	bool checksums{false}; // --checksums
 	unsigned checksumChunkShift{0}; // --checksumchunk / the checksum list's (0: whole files),
 	                                // ELB_CHECKSUM_MIN/MAX_CHUNK_SHIFT
+	int checksumAlgo{ELB_CHECKSUM_CRC32}; // --checksumalgo / the checksum list's (elb_crc_algo::ID)
 	int serializeBufferedWrites{ELB_WRITEGATE_AUTO};
 	int stagingEngine{ELB_STAGING_AUTO};
 	bool noGPUNumaBinding{false};

@@ -91,11 +91,12 @@ int elb_launch_stage_copy(const elb_block_desc* descs, uint32_t numDescs, bool h
 int elb_launch_damage_map(const elb_content& content, const elb_block_desc* descs,
 	uint32_t numDescs, elb_sector_damage* devSectors, uint64_t sectorsPerDesc,
 	cudaStream_t stream);
-/* CRC-32 contributions (elb_crc32_chunks; chunkShift 64: elb_crc32_blocks). descs and shifts
-   must be host- and device-readable: the host sizes the grid from the descriptors' lengths and
-   checks their chunks against slotsPerDesc */
-int elb_launch_crc32(const elb_block_desc* descs, const uint64_t* shifts, uint32_t numDescs,
-	unsigned chunkShift, uint64_t slotsPerDesc, uint32_t* devCrcs, uint32_t* hostCrcs,
+/* CRC contributions of algo (enum elb_checksum_algo; elb_crc_chunks, chunkShift 64: whole files).
+   The slots are the algorithm's word (elb_crc_algo::word). descs and shifts must be host- and
+   device-readable: the host sizes the grid from the descriptors' lengths and checks their chunks
+   against slotsPerDesc */
+int elb_launch_crc(int algo, const elb_block_desc* descs, const uint64_t* shifts,
+	uint32_t numDescs, unsigned chunkShift, uint64_t slotsPerDesc, void* devCrcs, void* hostCrcs,
 	unsigned* doneTicket, cudaStream_t stream);
 int elb_kernels_warmup();
 uint64_t elb_get_num_kernel_launches();

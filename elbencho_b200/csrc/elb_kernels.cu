@@ -11,8 +11,8 @@
  *      with the dedupe grain key, elb_patterns.cuh)
  *   damage_map (no reference counterpart: --verifyreport, where the bytes of blocks known to be
  *      bad differ, per 512-byte file sector; off the clean path, see its section below)
- *   crc32 (no reference counterpart: --checksums / --checksumverify, each block's share of its
- *      file's CRC-32 or its chunks' CRC-32s; off the clean path, see its section below)
+ *   crc (no reference counterpart: --checksums / --checksumverify / --checksumalgo, each block's
+ *      share of its file's CRC or its chunks' CRCs; off the clean path, see its section below)
  *
  * All eight are HBM-bound byte/integer kernels (K1/K3/K5/K7: 1 byte written per payload byte,
  * K2/K4/K6/K8: 1 byte read per payload byte), so the design follows the streaming rules: 16-byte (128-bit) vector
@@ -1141,7 +1141,7 @@ elb_damage_map_kernel(const KernelArgs args, elb_sector_damage* sectors, uint64_
 	}
 }
 
-/* ---- CRC-32 contributions (--checksums, --checksumchunk, --checksumverify) -------------------
+/* ---- CRC contributions (--checksums, --checksumchunk, --checksumverify, --checksumalgo) ------
  *
  * Each descriptor's bytes are cut at the chunk boundaries of its file offsets (every 2^chunkShift
  * bytes; chunkShift 64: none, the whole-file mode of --checksums). Slot j of descriptor i,
@@ -1169,47 +1169,56 @@ elb_damage_map_kernel(const KernelArgs args, elb_sector_damage* sectors, uint64_
  * tails, other layouts) is computed while the loads are in flight: x^(8n) with one lane per bit of
  * n and a 5-level shuffle product. With hostCrcs, the last CTA of the launch (ticket) copies the
  * slots to pinned host memory and zeroes them for the next launch, as the verify launches do with
- * their results. */
+ * their results.
+ *
+ * One body serves every algorithm (elb_crc_algo): its word is the slot, table and product width.
+ * The order of x of CRC-64/NVME, 2^64 - 1, takes 64 bits of n: each lane of the shift chain then
+ * takes bits l and l + 32, one more product. The order of CRC-32C, 2^31 - 1, fits 31 lanes. */
 
 #define ELB_CRC_PART_BYTES (ELB_VEC_BYTES * ELB_UNROLL) /* 128: a lane's bytes of a piece */
 #define ELB_CRC_PIECE_BYTES (32 * ELB_CRC_PART_BYTES)  /* 4 KiB: a warp's bytes */
 #define ELB_CRC_TABLE_SHIFT_LIMIT (1ULL << 30) /* shifts by table: multiples of 4 KiB below this */
 
-struct Crc32Consts
+template<class A>
+struct CrcConsts
 {
-	uint32_t x8pow2[32];    // x^(8 * 2^k) mod P
-	uint32_t laneShift[32]; // x^(8 * 128 * (31 - l)) mod P: lane l's part to the piece end
-	uint32_t x8pieces[256];      // x^(8 * 4 KiB * j) mod P
-	uint32_t x8pieces256[1024];  // x^(8 * 4 KiB * 256 * j) mod P
+	typedef typename A::word word;
 
-	constexpr Crc32Consts() : x8pow2{}, laneShift{}, x8pieces{}, x8pieces256{}
+	word x8pow2[A::BITS];   // x^(8 * 2^k) mod P
+	word laneShift[32];     // x^(8 * 128 * (31 - l)) mod P: lane l's part to the piece end
+	word x8pieces[256];     // x^(8 * 4 KiB * j) mod P
+	word x8pieces256[1024]; // x^(8 * 4 KiB * 256 * j) mod P
+
+	constexpr CrcConsts() : x8pow2{}, laneShift{}, x8pieces{}, x8pieces256{}
 	{
-		for(unsigned k = 0; k < 32; k++)
-			x8pow2[k] = elb_crc32_x8pow2(k);
+		x8pow2[0] = A::X8;
+		for(unsigned k = 1; k < A::BITS; k++)
+			x8pow2[k] = A::mulmod(x8pow2[k - 1], x8pow2[k - 1]);
 
 		for(unsigned l = 0; l < 32; l++)
 		{
 			const uint32_t n = (31 - l) * ELB_CRC_PART_BYTES;
-			uint32_t shift = ELB_CRC32_ONE;
+			word shift = A::ONE;
 
 			for(unsigned k = 0; k < 32; k++)
 				if( (n >> k) & 1)
-					shift = elb_crc32_mulmod(shift, x8pow2[k]);
+					shift = A::mulmod(shift, x8pow2[k]);
 
 			laneShift[l] = shift;
 		}
 
-		x8pieces[0] = ELB_CRC32_ONE;
+		x8pieces[0] = A::ONE;
 		for(unsigned j = 1; j < 256; j++)
-			x8pieces[j] = elb_crc32_mulmod(x8pieces[j - 1], x8pow2[12]);
+			x8pieces[j] = A::mulmod(x8pieces[j - 1], x8pow2[12]);
 
-		x8pieces256[0] = ELB_CRC32_ONE;
+		x8pieces256[0] = A::ONE;
 		for(unsigned j = 1; j < 1024; j++)
-			x8pieces256[j] = elb_crc32_mulmod(x8pieces256[j - 1], x8pow2[20]);
+			x8pieces256[j] = A::mulmod(x8pieces256[j - 1], x8pow2[20]);
 	}
 };
 
-static __constant__ Crc32Consts gCrc32Consts = Crc32Consts();
+template<class A>
+static __constant__ CrcConsts<A> gCrcConsts = CrcConsts<A>();
 
 /* 16 bytes at a 16-byte aligned address, with L1 allocation: a warp instruction takes 16 bytes of
    32 different lines, the lane's next loads take the rest of those lines */
@@ -1221,29 +1230,37 @@ __device__ __forceinline__ u64x2 ld_nc_128(const void* ptr)
 }
 
 /* R(crc's message || the 8 little-endian bytes of w) */
-__device__ __forceinline__ uint32_t crc32_fold8(uint32_t crc, uint64_t w,
-	const uint32_t (*table)[256])
+template<class Word>
+__device__ __forceinline__ Word crc_fold8(Word crc, uint64_t w, const Word (*table)[256])
 {
-	const uint32_t lo = crc ^ (uint32_t)w;
-	const uint32_t hi = (uint32_t)(w >> 32);
+	const uint32_t lo = (uint32_t)crc ^ (uint32_t)w;
+	const uint32_t hi = (uint32_t)(w >> 32) ^ (uint32_t)( (uint64_t)crc >> 32);
 
 	return table[7][lo & 0xff] ^ table[6][(lo >> 8) & 0xff] ^ table[5][(lo >> 16) & 0xff] ^
 		table[4][lo >> 24] ^ table[3][hi & 0xff] ^ table[2][(hi >> 8) & 0xff] ^
 		table[1][(hi >> 16) & 0xff] ^ table[0][hi >> 24];
 }
 
+__device__ __forceinline__ void crc_atomic_xor(uint32_t* slot, uint32_t val)
+	{ atomicXor(slot, val); }
+__device__ __forceinline__ void crc_atomic_xor(uint64_t* slot, uint64_t val)
+	{ atomicXor( (unsigned long long*)slot, (unsigned long long)val); }
+
+template<class A>
 __global__ void __launch_bounds__(ELB_THREADS)
-elb_crc32_kernel(const elb_block_desc* descs, const uint64_t* shifts, uint32_t numDescs,
-	uint64_t piecesPerDesc, unsigned chunkShift, uint64_t slotsPerDesc, uint32_t* crcs,
-	uint32_t* hostCrcs, unsigned* doneTicket)
+elb_crc_kernel(const elb_block_desc* descs, const uint64_t* shifts, uint32_t numDescs,
+	uint64_t piecesPerDesc, unsigned chunkShift, uint64_t slotsPerDesc, typename A::word* crcs,
+	typename A::word* hostCrcs, unsigned* doneTicket)
 {
-	__shared__ uint32_t sTable[8][256]; // sTable[k][i] = R(byte i followed by k zero bytes)
+	typedef typename A::word word;
+
+	__shared__ word sTable[8][256]; // sTable[k][i] = R(byte i followed by k zero bytes)
 	__shared__ bool sIsLastCTA;
 
 	const unsigned lane = threadIdx.x & 31;
 
 	{
-		uint32_t entry = elb_crc32_byte_table(threadIdx.x);
+		word entry = A::byte_table(threadIdx.x);
 		sTable[0][threadIdx.x] = entry;
 
 		__syncthreads();
@@ -1258,8 +1275,12 @@ elb_crc32_kernel(const elb_block_desc* descs, const uint64_t* shifts, uint32_t n
 		__syncthreads();
 	}
 
-	const uint32_t laneShift = gCrc32Consts.laneShift[lane];
-	const uint32_t laneX8Pow2 = gCrc32Consts.x8pow2[lane];
+	const word laneShift = gCrcConsts<A>.laneShift[lane];
+	const word laneX8Pow2 = gCrcConsts<A>.x8pow2[lane];
+	word laneX8Pow2Hi = 0; // (orders above 2^32: the lane's second bit of n, l + 32)
+
+	if constexpr(A::ORDER_BITS > 32)
+		laneX8Pow2Hi = gCrcConsts<A>.x8pow2[lane + 32];
 	const bool isChunked = (chunkShift < 64);
 	const uint64_t numItems = (uint64_t)numDescs * piecesPerDesc;
 	const uint64_t numWarps = (uint64_t)gridDim.x * ELB_WARPS;
@@ -1315,30 +1336,33 @@ elb_crc32_kernel(const elb_block_desc* descs, const uint64_t* shifts, uint32_t n
 			/* (while the loads are in flight) x^(8n), n = bytes from the piece end to the segment's
 			   chunk end (segEnd + shift) */
 			const uint64_t nPlain = segEnd - pieceEnd; // (chunked: shift is 0; wraps if negative)
-			uint32_t factor;
+			word factor;
 
 			if(isChunked && (nPlain < ELB_CRC_TABLE_SHIFT_LIMIT) &&
 				!(nPlain & (ELB_CRC_PIECE_BYTES - 1) ) )
 			{
 				const uint64_t j = nPlain / ELB_CRC_PIECE_BYTES;
 
-				factor = gCrc32Consts.x8pieces[j & 255];
+				factor = gCrcConsts<A>.x8pieces[j & 255];
 
 				if(j >> 8)
-					factor = elb_crc32_mulmod(factor, gCrc32Consts.x8pieces256[j >> 8]);
+					factor = A::mulmod(factor, gCrcConsts<A>.x8pieces256[j >> 8]);
 			}
 			else
-			{ // n mod 2^32 - 1: lane k contributes bit k of n
-				const uint64_t n = elb_crc32_mod_order(elb_crc32_mod_order(shift) +
-					elb_crc32_mod_order(segEnd) + ELB_CRC32_ORDER - elb_crc32_mod_order(pieceEnd) );
+			{ // n mod the order of x: lane k contributes bit k of n (and bit k + 32)
+				const uint64_t n = A::mod_order_sum(shift, segEnd, pieceEnd);
 
-				factor = ( (n >> lane) & 1) ? laneX8Pow2 : ELB_CRC32_ONE;
+				factor = ( (n >> lane) & 1) ? laneX8Pow2 : A::ONE;
+
+				if constexpr(A::ORDER_BITS > 32)
+					if( (n >> (lane + 32) ) & 1)
+						factor = A::mulmod(factor, laneX8Pow2Hi);
 
 				for(int offset = 16; offset > 0; offset >>= 1)
-					factor = elb_crc32_mulmod(factor, __shfl_xor_sync(0xffffffffu, factor, offset) );
+					factor = A::mulmod(factor, __shfl_xor_sync(0xffffffffu, factor, offset) );
 			}
 
-			uint32_t crc = 0;
+			word crc = 0;
 
 			if(hasBytes)
 			{ // (else the part is all zeros)
@@ -1367,19 +1391,18 @@ elb_crc32_kernel(const elb_block_desc* descs, const uint64_t* shifts, uint32_t n
 				#pragma unroll
 				for(int u = 0; u < ELB_UNROLL; u++)
 				{
-					crc = crc32_fold8(crc, vecs[u].a, sTable);
-					crc = crc32_fold8(crc, vecs[u].b, sTable);
+					crc = crc_fold8<word>(crc, vecs[u].a, sTable);
+					crc = crc_fold8<word>(crc, vecs[u].b, sTable);
 				}
 
-				crc = elb_crc32_mulmod(crc, laneShift);
+				crc = A::mulmod(crc, laneShift);
 			}
 
 			for(int offset = 16; offset > 0; offset >>= 1)
 				crc ^= __shfl_xor_sync(0xffffffffu, crc, offset);
 
 			if(!lane && crc)
-				atomicXor(&crcs[slot], (factor == ELB_CRC32_ONE) ? crc :
-					elb_crc32_mulmod(crc, factor) );
+				crc_atomic_xor(&crcs[slot], (factor == A::ONE) ? crc : A::mulmod(crc, factor) );
 
 			if(segEnd >= min(pieceEnd, end) )
 				break;
@@ -1411,7 +1434,7 @@ elb_crc32_kernel(const elb_block_desc* descs, const uint64_t* shifts, uint32_t n
 
 	for(uint64_t i = threadIdx.x; i < numSlots; i += blockDim.x)
 	{
-		volatile uint32_t* devCrc = &crcs[i];
+		volatile word* devCrc = &crcs[i];
 
 		hostCrcs[i] = *devCrc;
 		*devCrc = 0;
@@ -1436,7 +1459,7 @@ struct DeviceLaunchInfo
 {
 	int numSMs{0};
 	int ctasPerSM[NUM_MODES]{};
-	int crcCtasPerSM{0};
+	int crcCtasPerSM[ELB_CRC_NUM_ALGOS]{};
 };
 
 /* 32 KiB tiles per CTA of the hardware-scheduled kernel, per mode. H100: 1/1/4, 2/4/8, 4/4/16 for
@@ -1483,9 +1506,14 @@ static const DeviceLaunchInfo* getDeviceLaunchInfo()
 		gDevInfo[dev].ctasPerSM[MODE_FILL_DEDUPE_GRAIN] = queryOccupancy<MODE_FILL_DEDUPE_GRAIN>();
 		gDevInfo[dev].ctasPerSM[MODE_VERIFY_DEDUPE_GRAIN] =
 			queryOccupancy<MODE_VERIFY_DEDUPE_GRAIN>();
-		cudaOccupancyMaxActiveBlocksPerMultiprocessor(&gDevInfo[dev].crcCtasPerSM, elb_crc32_kernel,
-			ELB_THREADS, 0);
-		gDevInfo[dev].crcCtasPerSM = std::max(gDevInfo[dev].crcCtasPerSM, 1);
+		for(int algo = 0; algo < ELB_CRC_NUM_ALGOS; algo++)
+			elb_with_crc_algo(algo, [&](auto crcAlgo)
+			{
+				int& numBlocks = gDevInfo[dev].crcCtasPerSM[algo];
+				cudaOccupancyMaxActiveBlocksPerMultiprocessor(&numBlocks,
+					elb_crc_kernel<decltype(crcAlgo)>, ELB_THREADS, 0);
+				numBlocks = std::max(numBlocks, 1);
+			});
 	});
 
 	if(gDevInfo[dev].numSMs <= 0)
@@ -1819,10 +1847,16 @@ int elb_launch_damage_map(const elb_content& content, const elb_block_desc* desc
 	});
 }
 
-int elb_launch_crc32(const elb_block_desc* descs, const uint64_t* shifts, uint32_t numDescs,
-	unsigned chunkShift, uint64_t slotsPerDesc, uint32_t* devCrcs, uint32_t* hostCrcs,
+int elb_launch_crc(int algo, const elb_block_desc* descs, const uint64_t* shifts,
+	uint32_t numDescs, unsigned chunkShift, uint64_t slotsPerDesc, void* devCrcs, void* hostCrcs,
 	unsigned* doneTicket, cudaStream_t stream)
 {
+	if( (algo < 0) || (algo >= ELB_CRC_NUM_ALGOS) )
+	{
+		elb_set_last_error("crc_chunks: unknown checksum algorithm " + std::to_string(algo) );
+		return -1;
+	}
+
 	if(!numDescs)
 		return 0;
 
@@ -1840,7 +1874,7 @@ int elb_launch_crc32(const elb_block_desc* descs, const uint64_t* shifts, uint32
 
 		if(numChunks > slotsPerDesc)
 		{
-			elb_set_last_error("crc32_chunks: descriptor " + std::to_string(i) + " spans " +
+			elb_set_last_error("crc_chunks: descriptor " + std::to_string(i) + " spans " +
 				std::to_string(numChunks) + " chunks, more than " + std::to_string(slotsPerDesc) +
 				" slots per descriptor");
 			return -1;
@@ -1855,14 +1889,19 @@ int elb_launch_crc32(const elb_block_desc* descs, const uint64_t* shifts, uint32
 	   (at least one CTA, whose ticket publishes the results also when no block has a byte) */
 	const uint64_t numItems = (uint64_t)numDescs * piecesPerDesc;
 	const uint64_t gridSize = std::max( (uint64_t)1, std::min( (numItems + ELB_WARPS - 1) /
-		ELB_WARPS, (uint64_t)devInfo->numSMs * devInfo->crcCtasPerSM) );
+		ELB_WARPS, (uint64_t)devInfo->numSMs * devInfo->crcCtasPerSM[algo]) );
 
-	elb_crc32_kernel<<<(unsigned)gridSize, ELB_THREADS, 0, stream>>>(descs, shifts, numDescs,
-		piecesPerDesc ? piecesPerDesc : 1, chunkShift, slotsPerDesc, devCrcs, hostCrcs,
-		doneTicket);
+	elb_with_crc_algo(algo, [&](auto crcAlgo)
+	{
+		typedef typename decltype(crcAlgo)::word word;
+
+		elb_crc_kernel<decltype(crcAlgo)><<<(unsigned)gridSize, ELB_THREADS, 0, stream>>>(descs,
+			shifts, numDescs, piecesPerDesc ? piecesPerDesc : 1, chunkShift, slotsPerDesc,
+			(word*)devCrcs, (word*)hostCrcs, doneTicket);
+	});
 	gNumKernelLaunches.fetch_add(1, std::memory_order_relaxed);
 
-	return checkLaunch("crc32");
+	return checkLaunch("crc");
 }
 
 /* query launch geometry of the current device now (so that no attribute/occupancy query happens

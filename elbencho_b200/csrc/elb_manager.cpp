@@ -65,6 +65,7 @@ Manager::Manager(const elb_cfg* abiCfg)
 	sizedCfg.fileSize = detectFileSize(abiCfg);
 
 	shared.cfg = Config::fromABI(&sizedCfg);
+	configChecksumAlgo = shared.cfg.checksumAlgo;
 
 	prepareBenchPathFDs();
 
@@ -516,6 +517,21 @@ Manager::VerifyReport Manager::getVerifyReport()
 	return report;
 }
 
+/* the published CRC of algo of size bytes from their raw CRC, as lowercase hex digits of the
+   algorithm's width (8 or 16) */
+static std::string finishedCrcHex(int algo, uint64_t rawCrc, uint64_t size)
+{
+	char hex[17] = "";
+
+	elb_with_crc_algo(algo, [&](auto crcAlgo)
+	{
+		const auto crc = crcAlgo.finish( (typename decltype(crcAlgo)::word)rawCrc, size);
+		snprintf(hex, sizeof(hex), "%0*llx", (int)sizeof(crc) * 2, (unsigned long long)crc);
+	});
+
+	return hex;
+}
+
 /**
  * --checksums: the workers' accumulators merged by path (a file that several workers share has a
  * part in each): XOR of the raw CRCs, sum of the bytes. A file's CRC is complete when the phase
@@ -547,9 +563,7 @@ Manager::ChecksumReport Manager::getChecksumReport()
 
 		if(file.numBytes == file.size)
 		{
-			char hex[9];
-			snprintf(hex, sizeof(hex), "%08x", elb_crc32_finish_hd(file.rawCrc, file.size) );
-			crcStr = hex;
+			crcStr = finishedCrcHex(shared.cfg.checksumAlgo, file.rawCrc, file.size);
 			report.numComplete++;
 		}
 
@@ -583,12 +597,9 @@ Manager::ChecksumReport Manager::getChunkChecksumReport()
 			[](const ChunkChecksum& a, const ChunkChecksum& b) { return a.offset < b.offset; } );
 
 		for(const ChunkChecksum& chunk : chunks)
-		{
-			char hex[9];
-			snprintf(hex, sizeof(hex), "%08x", elb_crc32_finish_hd(chunk.rawCrc, chunk.length) );
 			report.lines += entry.first + " " + std::to_string(chunk.offset) + " " +
-				std::to_string(chunk.length) + " " + hex + "\n";
-		}
+				std::to_string(chunk.length) + " " +
+				finishedCrcHex(shared.cfg.checksumAlgo, chunk.rawCrc, chunk.length) + "\n";
 
 		report.numChunks += chunks.size();
 		report.numFiles++;
@@ -640,16 +651,25 @@ std::shared_ptr<const ChecksumList> ChecksumList::parse(const std::string& text)
 			continue;
 
 		if(!line.compare(0, 8, "# phase ") )
-		{ // "# phase WRITE|READ" or "# phase WRITE|READ chunk <K>"
+		{ // "# phase WRITE|READ [algorithm]" or "# phase WRITE|READ chunk <K> [algorithm]"
 			std::istringstream words(line.substr(8) );
-			std::string phase, chunkWord, chunkSizeStr, extra;
+			std::string phase, chunkWord, chunkSizeStr, algoName, extra;
 			uint64_t chunkSize = 0;
 
-			words >> phase >> chunkWord >> chunkSizeStr >> extra;
+			words >> phase >> chunkWord;
 
-			if( ( (phase != "WRITE") && (phase != "READ") ) || !extra.empty() ||
-				( !chunkWord.empty() && ( (chunkWord != "chunk") ||
-				!parseChecksumListNum(chunkSizeStr, chunkSize) ) ) )
+			if(!chunkWord.empty() && (chunkWord != "chunk") )
+				algoName.swap(chunkWord); // a whole-file section's algorithm
+			else
+				words >> chunkSizeStr >> algoName;
+
+			words >> extra;
+
+			const int algo = algoName.empty() ? ELB_CHECKSUM_CRC32 :
+				elb_crc_algo_by_name(algoName.c_str() );
+
+			if( ( (phase != "WRITE") && (phase != "READ") ) || !extra.empty() || (algo < 0) ||
+				( !chunkWord.empty() && !parseChecksumListNum(chunkSizeStr, chunkSize) ) )
 				fail("not a phase header");
 
 			inSection = true;
@@ -664,6 +684,7 @@ std::shared_ptr<const ChecksumList> ChecksumList::parse(const std::string& text)
 
 			section = std::make_shared<ChecksumList>();
 			section->chunkShift = __builtin_ctzll(chunkSize);
+			section->algo = algo;
 			list = section;
 			continue;
 		}
@@ -680,8 +701,19 @@ std::shared_ptr<const ChecksumList> ChecksumList::parse(const std::string& text)
 		const size_t offBlank = (lenBlank && (lenBlank != std::string::npos) ) ?
 			line.rfind(' ', lenBlank - 1) : std::string::npos;
 
+		size_t numDigits = 0; // (the algorithm's width)
+		std::string lineFormat;
+
+		elb_with_crc_algo(section->algo, [&](auto algo)
+		{
+			numDigits = sizeof(typename decltype(algo)::word) * 2;
+			lineFormat = std::string("not \"path offset length ") + algo.NAME + "\"";
+		});
+
+		const bool is64 = (numDigits == 16);
+
 		if( (offBlank == std::string::npos) || !offBlank)
-			fail("not \"path offset length crc32\"");
+			fail(lineFormat);
 
 		const std::string crcStr = line.substr(crcBlank + 1);
 		const uint64_t chunkSize = 1ULL << section->chunkShift;
@@ -689,9 +721,9 @@ std::shared_ptr<const ChecksumList> ChecksumList::parse(const std::string& text)
 
 		if(!parseChecksumListNum(line.substr(offBlank + 1, lenBlank - offBlank - 1), offset) ||
 			!parseChecksumListNum(line.substr(lenBlank + 1, crcBlank - lenBlank - 1), length) ||
-			(crcStr.size() != 8) || (crcStr.find_first_not_of("0123456789abcdefABCDEF") !=
-			std::string::npos) )
-			fail("not \"path offset length crc32\"");
+			(crcStr.size() != numDigits) ||
+			(crcStr.find_first_not_of("0123456789abcdefABCDEF") != std::string::npos) )
+			fail(lineFormat);
 
 		if( (offset % chunkSize) || !length || (length > chunkSize) )
 			fail("not a chunk of " + std::to_string(chunkSize) + " bytes");
@@ -706,11 +738,19 @@ std::shared_ptr<const ChecksumList> ChecksumList::parse(const std::string& text)
 		{
 			file.present.resize(chunkIdx + 1);
 			file.crcs.resize(chunkIdx + 1);
+
+			if(is64)
+				file.crcsHi.resize(chunkIdx + 1);
 		}
+
+		const uint64_t crc = std::stoull(crcStr, NULL, 16);
 
 		file.path = line.substr(0, offBlank);
 		file.present[chunkIdx] = true;
-		file.crcs[chunkIdx] = (uint32_t)std::stoul(crcStr, NULL, 16);
+		file.crcs[chunkIdx] = (uint32_t)crc;
+
+		if(is64)
+			file.crcsHi[chunkIdx] = (uint32_t)(crc >> 32);
 		section->numChunks++;
 
 		if(length != chunkSize)
@@ -733,6 +773,11 @@ void Manager::setChecksumList(std::shared_ptr<const ChecksumList> list)
 			std::to_string(1ULL << cfg.checksumChunkShift) + ") differs from the checksum list's (" +
 			std::to_string(1ULL << list->chunkShift) + ").");
 
+	if( (configChecksumAlgo != ELB_CHECKSUM_CRC32) && (configChecksumAlgo != list->algo) )
+		throw WorkerError(std::string("The checksum algorithm (--checksumalgo ") +
+			elb_crc_algo_name(configChecksumAlgo) + ") differs from the checksum list's (" +
+			elb_crc_algo_name(list->algo) + ").");
+
 	checkChecksumChunks(cfg, list->chunkShift, "the checksum list's chunk size");
 
 	if(cfg.rwMixReadPercent || cfg.numRWMixReadThreads)
@@ -744,6 +789,7 @@ void Manager::setChecksumList(std::shared_ptr<const ChecksumList> list)
 			"verify report (--verifyreport).");
 
 	cfg.checksumChunkShift = list->chunkShift;
+	cfg.checksumAlgo = list->algo;
 	shared.checksumList = list;
 }
 

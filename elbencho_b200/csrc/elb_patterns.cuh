@@ -44,6 +44,7 @@
 #define ELB_PATTERNS_CUH_
 
 #include <stdint.h>
+#include <string.h>
 
 #if defined(__CUDACC__)
 #define ELB_HD __host__ __device__ __forceinline__
@@ -276,95 +277,185 @@ ELB_HD uint64_t elb_rand_grain_bytes8(uint64_t filePos, const Keys& keys, uint64
 	return val;
 }
 
-/* ---- CRC-32 of what passed through GPU memory (--checksums) ------------------------------------
+/* ---- CRCs of what passed through GPU memory (--checksums, --checksumalgo) ----------------------
  *
- * R(M) is the raw reflected CRC-32 of M: polynomial P = 0xEDB88320, register 0 at the start, no
- * final XOR. Bit 31 of a value is the coefficient of x^0. R is linear:
+ * R(M) is the raw reflected CRC of M: a W-bit register, reflected polynomial P, register 0 at the
+ * start, no final XOR. Bit W-1 of a value is the coefficient of x^0. R is linear:
  *   R(A || B) = X(R(A), |B|) ^ R(B),   X(c, n) = c * x^(8n) mod P (c followed by n zero bytes)
  * so a block at file offset o of length len in a file of size S contributes X(R(block), S - o - len),
- * and a file's R is the XOR of its blocks' contributions in any order. zlib's CRC-32 (gzip, zip,
- * Python's zlib.crc32) starts with 0xFFFFFFFF and inverts at the end:
- *   crc32(M) = R(M) ^ X(0xFFFFFFFF, |M|) ^ 0xFFFFFFFF
- * x^(2^32 - 1) = 1 mod P, so X(c, n) = X(c, n mod (2^32 - 1)): shifts may also be negative. */
+ * and a file's R is the XOR of its blocks' contributions in any order. The published CRC starts
+ * with all ones and inverts at the end:
+ *   crc(M) = R(M) ^ X(~0, |M|) ^ ~0
+ * x^ORDER = 1 mod P, so X(c, n) = X(c, n mod ORDER): shifts may also be negative. The order is not
+ * the same for all algorithms, and reducing by another one gives wrong CRCs:
+ *   crc32      P = 0xEDB88320 (zlib, gzip, zip)   ORDER = 2^32 - 1
+ *   crc32c     P = 0x82F63B78 (Castagnoli)        ORDER = 2^31 - 1 (P = (x+1) * Q, 2^31 - 1 prime)
+ *   crc64nvme  P = 0x9A6C9329AC4BC9B5 (NVMe)      ORDER = 2^64 - 1
+ * Each algorithm is one elb_crc_algo below; everything else takes its facts from there. */
 
-#define ELB_CRC32_POLY 0xEDB88320u
-#define ELB_CRC32_ONE 0x80000000u           /* x^0 */
-#define ELB_CRC32_X8 0x00800000u            /* x^8: one zero byte */
-#define ELB_CRC32_ORDER 0xFFFFFFFFULL       /* x^ELB_CRC32_ORDER = 1 mod P */
-/* chunked CRCs (elb_crc32_chunks): chunks of 2^shift bytes; at least 4 KiB, so that a kernel
-   piece meets one chunk boundary at most */
-#define ELB_CRC32_MIN_CHUNK_SHIFT 12
-#define ELB_CRC32_MAX_CHUNK_SHIFT 40
+/* chunked CRCs (elb_crc_chunks): chunks of 2^shift bytes; at least 4 KiB, so that a kernel piece
+   meets one chunk boundary at most */
+#define ELB_CRC_MIN_CHUNK_SHIFT 12
+#define ELB_CRC_MAX_CHUNK_SHIFT 40
 
-/* n mod ELB_CRC32_ORDER without a 64-bit division (2^32 = 1 mod 2^32 - 1) */
-ELB_HD constexpr uint64_t elb_crc32_mod_order(uint64_t n)
+/* a reflected CRC with register Word, reflected polynomial POLY_ and x^(2^ORDER_BITS_ - 1) = 1 */
+template<class Word, Word POLY_, unsigned ORDER_BITS_>
+struct elb_crc_algo
 {
-	n = (n & 0xFFFFFFFFULL) + (n >> 32); // < 2^33
-	n = (n & 0xFFFFFFFFULL) + (n >> 32); // <= 2^32
-	return (n >= ELB_CRC32_ORDER) ? (n - ELB_CRC32_ORDER) : n;
-}
+	typedef Word word;
 
-/* a * b mod P */
-ELB_HD constexpr uint32_t elb_crc32_mulmod(uint32_t a, uint32_t b)
-{
-	uint32_t prod = 0;
+	static constexpr unsigned BITS = sizeof(Word) * 8;
+	static constexpr Word POLY = POLY_;
+	static constexpr Word ONE = (Word)1 << (BITS - 1); /* x^0 */
+	static constexpr Word X8 = (Word)1 << (BITS - 9);  /* x^8: one zero byte */
+	static constexpr unsigned ORDER_BITS = ORDER_BITS_;
+	static constexpr uint64_t ORDER = ~0ULL >> (64 - ORDER_BITS); /* x^ORDER = 1 mod P */
 
-	for(int bit = 31; bit >= 0; bit--)
+	/* n mod ORDER without a 64-bit division (2^ORDER_BITS = 1 mod ORDER) */
+	static ELB_HD_MEMBER constexpr uint64_t mod_order(uint64_t n)
 	{
-		prod ^= b & (0u - ( (a >> bit) & 1u) );
-		b = (b >> 1) ^ (ELB_CRC32_POLY & (0u - (b & 1u) ) );
+		if constexpr(ORDER_BITS == 64)
+			return (n == ORDER) ? 0 : n;
+		else
+		{
+			n = (n & ORDER) + (n >> ORDER_BITS);
+			n = (n & ORDER) + (n >> ORDER_BITS);
+			return (n >= ORDER) ? (n - ORDER) : n;
+		}
 	}
 
-	return prod;
-}
-
-/* x^(8 * 2^k) mod P */
-ELB_HD constexpr uint32_t elb_crc32_x8pow2(unsigned k)
-{
-	uint32_t pow = ELB_CRC32_X8;
-
-	for(unsigned i = 0; i < k; i++)
-		pow = elb_crc32_mulmod(pow, pow);
-
-	return pow;
-}
-
-/* x^(8n) mod P by square-and-multiply */
-ELB_HD constexpr uint32_t elb_crc32_x8n(uint64_t n)
-{
-	uint32_t result = ELB_CRC32_ONE;
-	uint32_t pow = ELB_CRC32_X8;
-
-	for(n = elb_crc32_mod_order(n); n; n >>= 1)
+	/* (a + b - c) mod ORDER, for any 64-bit a, b, c */
+	static ELB_HD_MEMBER constexpr uint64_t mod_order_sum(uint64_t a, uint64_t b, uint64_t c)
 	{
-		if(n & 1)
-			result = elb_crc32_mulmod(result, pow);
-
-		pow = elb_crc32_mulmod(pow, pow);
+		if constexpr(ORDER_BITS == 64)
+		{ // 2^64 = 1 mod ORDER: an end-around carry and an end-around borrow
+			uint64_t sum = a + b;
+			sum += (sum < a);
+			return mod_order(sum - c - (sum < c) );
+		}
+		else
+			return mod_order(mod_order(a) + mod_order(b) + ORDER - mod_order(c) );
 	}
 
-	return result;
+	/* a * b mod P */
+	static ELB_HD_MEMBER constexpr Word mulmod(Word a, Word b)
+	{
+		Word prod = 0;
+
+		for(int bit = BITS - 1; bit >= 0; bit--)
+		{
+			prod ^= b & ( (Word)0 - ( (a >> bit) & 1) );
+			b = (b >> 1) ^ (POLY & ( (Word)0 - (b & 1) ) );
+		}
+
+		return prod;
+	}
+
+	/* x^(8 * 2^k) mod P */
+	static ELB_HD_MEMBER constexpr Word x8pow2(unsigned k)
+	{
+		Word pow = X8;
+
+		for(unsigned i = 0; i < k; i++)
+			pow = mulmod(pow, pow);
+
+		return pow;
+	}
+
+	/* x^(8n) mod P by square-and-multiply */
+	static ELB_HD_MEMBER constexpr Word x8n(uint64_t n)
+	{
+		Word result = ONE;
+		Word pow = X8;
+
+		for(n = mod_order(n); n; n >>= 1)
+		{
+			if(n & 1)
+				result = mulmod(result, pow);
+
+			pow = mulmod(pow, pow);
+		}
+
+		return result;
+	}
+
+	/* X(crc, n): crc followed by n zero bytes */
+	static ELB_HD_MEMBER constexpr Word shift(Word crc, uint64_t n)
+	{
+		return mulmod(crc, x8n(n) );
+	}
+
+	/* the published CRC of a message of size bytes from its raw CRC R */
+	static ELB_HD_MEMBER constexpr Word finish(Word rawCrc, uint64_t size)
+	{
+		return rawCrc ^ shift(~(Word)0, size) ^ ~(Word)0;
+	}
+
+	/* R of the single byte i (the byte-wise table; R(M || b) = (R(M) >> 8) ^ T[(R(M) ^ b) & 0xff]) */
+	static ELB_HD_MEMBER constexpr Word byte_table(Word i)
+	{
+		for(int bit = 0; bit < 8; bit++)
+			i = (i >> 1) ^ (POLY & ( (Word)0 - (i & 1) ) );
+
+		return i;
+	}
+};
+
+/* ID: enum elb_checksum_algo; NAME: --checksumalgo and the list headers; LABEL: messages */
+struct elb_crc32_algo : elb_crc_algo<uint32_t, 0xEDB88320u, 32>
+{
+	static constexpr int ID = 0;
+	static constexpr const char* NAME = "crc32";
+	static constexpr const char* LABEL = "CRC-32";
+};
+
+struct elb_crc32c_algo : elb_crc_algo<uint32_t, 0x82F63B78u, 31>
+{
+	static constexpr int ID = 1;
+	static constexpr const char* NAME = "crc32c";
+	static constexpr const char* LABEL = "CRC-32C";
+};
+
+struct elb_crc64nvme_algo : elb_crc_algo<uint64_t, 0x9A6C9329AC4BC9B5ULL, 64>
+{
+	static constexpr int ID = 2;
+	static constexpr const char* NAME = "crc64nvme";
+	static constexpr const char* LABEL = "CRC-64/NVME";
+};
+
+#define ELB_CRC_NUM_ALGOS 3
+
+/* f(the algorithm object of ID algo); false (f not called) for an unknown ID */
+template<class F>
+inline bool elb_with_crc_algo(int algo, F&& f)
+{
+	switch(algo)
+	{
+		case elb_crc32_algo::ID: f(elb_crc32_algo{}); return true;
+		case elb_crc32c_algo::ID: f(elb_crc32c_algo{}); return true;
+		case elb_crc64nvme_algo::ID: f(elb_crc64nvme_algo{}); return true;
+		default: return false;
+	}
 }
 
-/* X(crc, n): crc followed by n zero bytes */
-ELB_HD constexpr uint32_t elb_crc32_shift_hd(uint32_t crc, uint64_t n)
+/* the name of the algorithm with ID algo ("" for none) */
+inline const char* elb_crc_algo_name(int algo)
 {
-	return elb_crc32_mulmod(crc, elb_crc32_x8n(n) );
+	const char* name = "";
+	elb_with_crc_algo(algo, [&](auto crcAlgo) { name = crcAlgo.NAME; } );
+	return name;
 }
 
-/* zlib's CRC-32 of a message of size bytes from its raw CRC R */
-ELB_HD constexpr uint32_t elb_crc32_finish_hd(uint32_t rawCrc, uint64_t size)
+/* the ID of the algorithm called name (--checksumalgo, list headers), -1 if none is */
+inline int elb_crc_algo_by_name(const char* name)
 {
-	return rawCrc ^ elb_crc32_shift_hd(0xFFFFFFFFu, size) ^ 0xFFFFFFFFu;
-}
+	int found = -1;
 
-/* R of the single byte i (the byte-wise table; R(M || b) = (R(M) >> 8) ^ T[(R(M) ^ b) & 0xff]) */
-ELB_HD constexpr uint32_t elb_crc32_byte_table(uint32_t i)
-{
-	for(int bit = 0; bit < 8; bit++)
-		i = (i >> 1) ^ (ELB_CRC32_POLY & (0u - (i & 1u) ) );
+	for(int algo = 0; algo < ELB_CRC_NUM_ALGOS; algo++)
+		elb_with_crc_algo(algo, [&](auto crcAlgo)
+			{ if(!strcmp(crcAlgo.NAME, name) ) found = algo; } );
 
-	return i;
+	return found;
 }
 
 #endif /* ELB_PATTERNS_CUH_ */

@@ -819,8 +819,8 @@ void Worker::preparePhase()
 }
 
 /**
- * --checksums / --checksumverify: which stages take the CRC launch, in chunks of which size, and
- * the batches' CRC slots. Runs after the rings are made and at the start of every write and read
+ * --checksums / --checksumverify: which stages take the CRC launch, in chunks of which size and of
+ * which algorithm, and the batches' CRC slots. Runs after the rings are made and at the start of every write and read
  * phase, since a checksum list (elb_mgr_set_checksum_list) may be set between phases; a change
  * drops the batch graphs, which hold the launches of the old setup. Without either option it
  * allocates and changes nothing.
@@ -831,9 +831,14 @@ void Worker::setupChecksums()
 	const unsigned chunkShift = cfg.checksumChunkShift ? cfg.checksumChunkShift : 64;
 	const uint64_t slotsPerDesc = (chunkShift == 64) ? 1 :
 		std::max( (cfg.blockSize + ( (uint64_t)1 << chunkShift) - 1) >> chunkShift, (uint64_t)1);
+	size_t wordBytes = 0;
+
+	elb_with_crc_algo(cfg.checksumAlgo, [&](auto algo)
+		{ wordBytes = sizeof(typename decltype(algo)::word); } );
 
 	if(batches.empty() || ( (readChecksum == readStage.checksum) &&
-		(chunkShift == crcChunkShift) && (slotsPerDesc == crcSlotsPerDesc) ) )
+		(chunkShift == crcChunkShift) && (slotsPerDesc == crcSlotsPerDesc) &&
+		(cfg.checksumAlgo == crcAlgo) ) )
 		return;
 
 	std::shared_lock<std::shared_timed_mutex> allocLock(shared->gpuAllocMutex);
@@ -845,6 +850,8 @@ void Worker::setupChecksums()
 	verifyBackStage.useGraph = readStage.useGraph && !readChecksum;
 	crcChunkShift = chunkShift;
 	crcSlotsPerDesc = slotsPerDesc;
+	crcAlgo = cfg.checksumAlgo;
+	crcWordBytes = wordBytes;
 
 	for(Batch& batch : batches)
 	{
@@ -870,11 +877,11 @@ void Worker::setupChecksums()
 		if(!batch.hostShifts)
 			ELB_CUDA_CHECK(cudaHostAlloc( (void**)&batch.hostShifts, sizeof(uint64_t) * batchBlocks,
 				cudaHostAllocDefault), "Pinned checksum shift allocation");
-		ELB_CUDA_CHECK(cudaMalloc( (void**)&batch.devCrcs, sizeof(uint32_t) * numSlots),
+		ELB_CUDA_CHECK(cudaMalloc(&batch.devCrcs, crcWordBytes * numSlots),
 			"GPU checksum allocation");
-		ELB_CUDA_CHECK(cudaHostAlloc( (void**)&batch.hostCrcs, sizeof(uint32_t) * numSlots,
+		ELB_CUDA_CHECK(cudaHostAlloc(&batch.hostCrcs, crcWordBytes * numSlots,
 			cudaHostAllocDefault), "Pinned checksum allocation");
-		ELB_CUDA_CHECK(cudaMemsetAsync(batch.devCrcs, 0, sizeof(uint32_t) * numSlots,
+		ELB_CUDA_CHECK(cudaMemsetAsync(batch.devCrcs, 0, crcWordBytes * numSlots,
 			batch.stream), "GPU checksum init");
 		ELB_CUDA_CHECK(cudaStreamSynchronize(batch.stream), "GPU checksum init");
 	}
@@ -1224,7 +1231,7 @@ void Worker::abortInFlight()
 			cudaMemsetAsync(batch.devDoneTicket, 0, sizeof(unsigned), batch.stream);
 			elb_launch_verify_init(batch.devResults, batchBlocks, batch.stream);
 			if(batch.devCrcs)
-				cudaMemsetAsync(batch.devCrcs, 0, sizeof(uint32_t) * batchBlocks * crcSlotsPerDesc,
+				cudaMemsetAsync(batch.devCrcs, 0, crcWordBytes * batchBlocks * crcSlotsPerDesc,
 					batch.stream);
 			cudaStreamSynchronize(batch.stream);
 
@@ -2416,7 +2423,7 @@ void Worker::enqueueStage(Batch& batch, const GpuStage& stage, uint32_t numBlock
 	}
 
 	// (a write's checksum reads the device slot before its stage-out copy)
-	if(stage.checksum && elb_launch_crc32(batch.hostDescs, batch.hostShifts, numBlocks,
+	if(stage.checksum && elb_launch_crc(crcAlgo, batch.hostDescs, batch.hostShifts, numBlocks,
 		crcChunkShift, crcSlotsPerDesc, batch.devCrcs, batch.hostCrcs, batch.devDoneTicket,
 		batch.stream) )
 		throw WorkerError(std::string("GPU checksum failed. ") + elb_last_error() );
@@ -2699,6 +2706,13 @@ Worker::FileID Worker::blockFileID(const BlockRef& block) const
 		block.isTreeElem ? FileID(~0ULL, block.fileIndex) : FileID(block.dirIndex, block.fileIndex);
 }
 
+/* the raw CRC in host slot slot of a batch whose CRC launch is done */
+uint64_t Worker::batchCrc(const Batch& batch, uint64_t slot) const
+{
+	return (crcWordBytes == sizeof(uint64_t) ) ? ( (const uint64_t*)batch.hostCrcs)[slot] :
+		( (const uint32_t*)batch.hostCrcs)[slot];
+}
+
 /* --checksums: the CRC contributions of a batch whose blocks are done (no rwmix: descriptor i is
  * block i), into the accumulator of each block's file: XORed per file, or one entry per chunk */
 void Worker::addBatchChecksums(const Batch& batch)
@@ -2716,7 +2730,7 @@ void Worker::addBatchChecksums(const Batch& batch)
 
 		if(crcChunkShift == 64)
 		{
-			acc.rawCrc ^= batch.hostCrcs[i];
+			acc.rawCrc ^= batchCrc(batch, i);
 			continue;
 		}
 
@@ -2726,7 +2740,7 @@ void Worker::addBatchChecksums(const Batch& batch)
 		for(uint64_t pos = block.offset, slot = i * crcSlotsPerDesc; pos < blockEnd;
 			pos += chunkSize, slot++)
 			acc.chunks.push_back(ChunkChecksum{pos, std::min(chunkSize, blockEnd - pos),
-				batch.hostCrcs[slot]});
+				batchCrc(batch, slot)});
 	}
 }
 
@@ -2742,50 +2756,58 @@ void Worker::checkBatchChecksums(const Batch& batch)
 	if(!list || !readStage.checksum || (benchPhase != ELB_PHASE_READFILES) )
 		return;
 
-	const uint64_t chunkSize = (uint64_t)1 << crcChunkShift;
-	const uint32_t fullChunkXor = elb_crc32_finish_hd(0, chunkSize);
-
-	for(size_t i = 0; i < batch.blocks.size(); i++)
+	elb_with_crc_algo(crcAlgo, [&](auto algo)
 	{
-		const BlockRef& block = batch.blocks[i];
-		const uint64_t blockEnd = block.offset + block.len;
-		auto fileIter = checksumListFiles.find(blockFileID(block) );
+		typedef decltype(algo) Algo;
 
-		if(fileIter == checksumListFiles.end() )
-			fileIter = checksumListFiles.emplace(blockFileID(block),
-				list->findFile(blockFilePath(block) ) ).first;
+		const uint64_t chunkSize = (uint64_t)1 << crcChunkShift;
+		const typename Algo::word fullChunkXor = Algo::finish(0, chunkSize);
 
-		const ChecksumList::File* file = fileIter->second;
-
-		for(uint64_t pos = block.offset, slot = i * crcSlotsPerDesc; pos < blockEnd;
-			pos += chunkSize, slot++)
+		for(size_t i = 0; i < batch.blocks.size(); i++)
 		{
-			const uint64_t len = std::min(chunkSize, blockEnd - pos);
-			const uint32_t rawCrc = batch.hostCrcs[slot];
-			const uint32_t crc = (len == chunkSize) ? (rawCrc ^ fullChunkXor) :
-				elb_crc32_finish_hd(rawCrc, len);
-			const uint64_t chunkIdx = pos >> crcChunkShift;
-			const bool hasLine = file && file->hasLine(chunkIdx);
+			const BlockRef& block = batch.blocks[i];
+			const uint64_t blockEnd = block.offset + block.len;
+			auto fileIter = checksumListFiles.find(blockFileID(block) );
 
-			if(hasLine && (file->chunkLength(chunkIdx, chunkSize) == len) &&
-				(file->crcs[chunkIdx] == crc) )
+			if(fileIter == checksumListFiles.end() )
+				fileIter = checksumListFiles.emplace(blockFileID(block),
+					list->findFile(blockFilePath(block) ) ).first;
+
+			const ChecksumList::File* file = fileIter->second;
+
+			for(uint64_t pos = block.offset, slot = i * crcSlotsPerDesc; pos < blockEnd;
+				pos += chunkSize, slot++)
 			{
-				numChecksumChunksChecked++;
-				continue;
+				const uint64_t len = std::min(chunkSize, blockEnd - pos);
+				const typename Algo::word rawCrc = (typename Algo::word)batchCrc(batch, slot);
+				const typename Algo::word crc = (len == chunkSize) ? (rawCrc ^ fullChunkXor) :
+					Algo::finish(rawCrc, len);
+				const uint64_t chunkIdx = pos >> crcChunkShift;
+				const bool hasLine = file && file->hasLine(chunkIdx);
+
+				if(hasLine && (file->chunkLength(chunkIdx, chunkSize) == len) &&
+					(file->crc(chunkIdx) == crc) )
+				{
+					numChecksumChunksChecked++;
+					continue;
+				}
+
+				const int numDigits = (int)sizeof(crc) * 2;
+				char expected[17] = "-";
+				char actual[17];
+
+				if(hasLine)
+					snprintf(expected, sizeof(expected), "%0*llx", numDigits,
+						(unsigned long long)file->crc(chunkIdx) );
+				snprintf(actual, sizeof(actual), "%0*llx", numDigits, (unsigned long long)crc);
+
+				throw WorkerError("Checksum verification failed. File: " + blockFilePath(block) +
+					"; Offset: " + std::to_string(pos) + "; Length: " + std::to_string(len) + "; "
+					"Expected " + Algo::LABEL + ": " + expected + "; Actual " + Algo::LABEL + ": " +
+					actual);
 			}
-
-			char expected[9] = "-";
-			char actual[9];
-
-			if(hasLine)
-				snprintf(expected, sizeof(expected), "%08x", file->crcs[chunkIdx]);
-			snprintf(actual, sizeof(actual), "%08x", crc);
-
-			throw WorkerError("Checksum verification failed. File: " + blockFilePath(block) + "; "
-				"Offset: " + std::to_string(pos) + "; Length: " + std::to_string(len) + "; "
-				"Expected CRC-32: " + expected + "; Actual CRC-32: " + actual);
 		}
-	}
+	});
 }
 
 /* --checksumverify: the paths of the files this worker checked in the phase */

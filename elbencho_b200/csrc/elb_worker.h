@@ -127,7 +127,7 @@ struct ChunkChecksum
 {
 	uint64_t offset;
 	uint64_t length;
-	uint32_t rawCrc; // (elb_crc32_chunks)
+	uint64_t rawCrc; // (elb_crc_chunks)
 };
 
 /* --checksums: what a worker moved of one file in a phase */
@@ -136,23 +136,27 @@ struct FileChecksum
 	std::string path; // as the worker opened the file
 	uint64_t size{0};     // the file's data set size
 	uint64_t numBytes{0}; // bytes of the blocks the phase moved
-	uint32_t rawCrc{0};   // XOR of the blocks' contributions (elb_crc32_blocks)
+	uint64_t rawCrc{0};   // XOR of the blocks' contributions (elb_crc_chunks)
 	std::vector<ChunkChecksum> chunks; // --checksumchunk: the chunks instead, in the order moved
 };
 
 /**
  * --checksumverify: the last section with a chunk size of a checksum list that --checksums
- * --checksumchunk wrote: "# phase WRITE|READ chunk <K>", then lines "path offset length crc32".
- * One CRC and one bit per chunk of each listed file; lines shorter than K (a file's last chunk)
- * keep their length aside.
+ * --checksumchunk wrote: "# phase WRITE|READ chunk <K> [algorithm]", then lines "path offset
+ * length crc". One CRC (4 bytes, 8 for 64-bit algorithms) and one bit per chunk of each listed
+ * file; lines shorter than K (a file's last chunk) keep their length aside.
  */
 struct ChecksumList
 {
 	struct File
 	{
 		std::string path;
-		std::vector<uint32_t> crcs;  // zlib CRC-32 by chunk index
-		std::vector<bool> present;   // whether the chunk has a line
+		std::vector<uint32_t> crcs;   // the CRC by chunk index (64-bit algorithms: the low half)
+		std::vector<uint32_t> crcsHi; // 64-bit algorithms: the high half, else empty
+		std::vector<bool> present;    // whether the chunk has a line
+
+		uint64_t crc(uint64_t chunkIdx) const
+			{ return crcs[chunkIdx] | (crcsHi.empty() ? 0 : (uint64_t)crcsHi[chunkIdx] << 32); }
 		std::map<uint64_t, uint64_t> shortLengths; // chunk index -> length of lines shorter than K
 
 		bool hasLine(uint64_t chunkIdx) const
@@ -165,6 +169,7 @@ struct ChecksumList
 	};
 
 	unsigned chunkShift{0};
+	int algo{ELB_CHECKSUM_CRC32}; // elb_crc_algo::ID
 	uint64_t numChunks{0};
 	std::map<std::string, File> files;
 
@@ -201,7 +206,7 @@ struct GpuStage
 	elb_content content; // what the write fills or the read verifies (NONE: the blocks only move)
 	bool useGraph;    // replay full batches from a CUDA graph (one launch per batch anyway under
 	                  // kernel staging)
-	bool checksum;    // --checksums: each block's CRC-32 contribution from its device slot
+	bool checksum;    // --checksums: each block's CRC contribution from its device slot
 };
 
 /* a batch: a contiguous slice of the rings plus everything its GPU stage needs */
@@ -229,8 +234,8 @@ struct Batch
 	/* --checksums: bytes from each block's end to its file's end (pinned, read by the CRC kernel)
 	   and the blocks' CRC contributions, published to pinned memory by the kernel's last CTA */
 	uint64_t* hostShifts{NULL};
-	uint32_t* devCrcs{NULL};  // zero, re-zeroed by the kernel
-	uint32_t* hostCrcs{NULL};
+	void* devCrcs{NULL};  // zero, re-zeroed by the kernel (the algorithm's word per slot)
+	void* hostCrcs{NULL};
 
 	// aio state
 	std::vector<struct iocb> iocbs;
@@ -410,12 +415,14 @@ class Worker
 		{
 			BlockRef block; // (a block of the file, for its path)
 			uint64_t numBytes{0};
-			uint32_t rawCrc{0};
+			uint64_t rawCrc{0};
 			std::vector<ChunkChecksum> chunks; // --checksumchunk
 		};
 		std::map<FileID, ChecksumAcc> checksumAccs;
 		unsigned crcChunkShift{64};    // the CRC launch's chunks (64: whole files), setupChecksums
 		uint64_t crcSlotsPerDesc{1};   // CRC slots per block
+		int crcAlgo{ELB_CHECKSUM_CRC32}; // the CRC launch's algorithm (elb_crc_algo::ID)
+		size_t crcWordBytes{4};          // bytes of a CRC slot
 		/* --checksumverify: the list entry of each file the phase read (NULL: not listed) and the
 		   chunks that matched */
 		std::map<FileID, const ChecksumList::File*> checksumListFiles;
@@ -459,6 +466,7 @@ class Worker
 			bool oneFilePerBatch = false);
 		void verifyWrittenBatch(Batch& batch);
 		void accountBatch(Batch& batch, uint64_t gpuUSecTotal);
+		uint64_t batchCrc(const Batch& batch, uint64_t slot) const;
 		void addBatchChecksums(const Batch& batch);
 		void checkBatchChecksums(const Batch& batch);
 		void setupChecksums();
@@ -536,8 +544,8 @@ class Manager
 		/* --checksums: each file of the last phase, merged over all workers */
 		struct ChecksumReport
 		{
-			std::string lines; // "<path> <size> <bytes covered> <crc32 or ->\n", sorted by path;
-			                   // --checksumchunk: "<path> <offset> <length> <crc32>\n" per chunk
+			std::string lines; // "<path> <size> <bytes covered> <crc or ->\n", sorted by path;
+			                   // --checksumchunk: "<path> <offset> <length> <crc>\n" per chunk
 			uint64_t numFiles{0};
 			uint64_t numComplete{0}; // files with a CRC
 			uint64_t numChunks{0};   // --checksumchunk
@@ -562,6 +570,7 @@ class Manager
 		void closeBenchPathFDs();
 		bool pathFDsOpenedForWrite{false};
 		bool hadCreateFilesPhase{false}; // (size check of read-only runs, ProgArgs.cpp:2099)
+		int configChecksumAlgo{ELB_CHECKSUM_CRC32}; // elb_cfg::checksumAlgo (a list's may replace it)
 		std::unique_ptr<LiveStatsReducer> liveStatsReducer; // created on first use
 		std::mutex liveStatsReducerMutex;
 };

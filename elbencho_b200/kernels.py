@@ -12,6 +12,9 @@ from ._native import CONTENT_PATTERN, CONTENT_RANDOM, CONTENT_RANDOM_GRAIN  # no
 
 RANDALGO_SPLITMIX64 = 0
 
+# elb_checksum_algo by --checksumalgo name; crc64nvme slots are uint64, the others uint32
+CHECKSUM_ALGOS = {"crc32": 0, "crc32c": 1, "crc64nvme": 2}
+
 VERIFY_PATTERN = 0  # elb_verify_kind
 VERIFY_RANDOM = 1
 
@@ -324,6 +327,37 @@ def crc32_shift(crc, num_zero_bytes):
 def crc32_finish(raw_crc, size):
     """zlib's CRC-32 of a message of size bytes from its raw CRC-32"""
     return int(_native.load().elb_crc32_finish(raw_crc, size))
+
+
+def _checksum_algo_id(algo):
+    """an elb_checksum_algo from a --checksumalgo name or the number itself"""
+    if isinstance(algo, str):
+        if algo not in CHECKSUM_ALGOS:
+            raise KernelError("unknown checksum algorithm %r" % algo)
+        return CHECKSUM_ALGOS[algo]
+    return int(algo)
+
+
+def crc_chunks(pinned_descs_ptr, pinned_shifts_ptr, num_descs, chunk_shift, slots_per_desc,
+               dev_crcs_ptr, pinned_crcs_ptr=0, dev_ticket_ptr=0, stream=0, algo="crc32"):
+    """crc32_chunks for the CRC algo (a CHECKSUM_ALGOS name or number): the slots are uint64 for
+    crc64nvme, uint32 for the others; crc_finish(algo, value, length) of a chunk that lies inside
+    the block is its CRC."""
+    _check(_native.load().elb_crc_chunks(_checksum_algo_id(algo), pinned_descs_ptr,
+                                         pinned_shifts_ptr or None, num_descs, chunk_shift,
+                                         slots_per_desc, dev_crcs_ptr, pinned_crcs_ptr or None,
+                                         dev_ticket_ptr or None, stream),
+           "elb_crc_chunks")
+
+
+def crc_shift(crc, num_zero_bytes, algo="crc32"):
+    """the raw CRC of algo of crc's message followed by num_zero_bytes zero bytes"""
+    return int(_native.load().elb_crc_shift(_checksum_algo_id(algo), crc, num_zero_bytes))
+
+
+def crc_finish(raw_crc, size, algo="crc32"):
+    """the CRC of algo of a message of size bytes from its raw CRC"""
+    return int(_native.load().elb_crc_finish(_checksum_algo_id(algo), raw_crc, size))
 
 
 def stage_copy(descs_ptr, num_descs, host_to_device, host_delta, stream=0, total_bytes=0,

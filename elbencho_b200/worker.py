@@ -13,6 +13,7 @@ from typing import List, Optional, Sequence
 from . import _native
 from ._native import (Cfg, Histogram, LiveLat, LiveOps, LiveSnapshot, PhaseResults,
                       DEVCTR_NUM)
+from .kernels import CHECKSUM_ALGOS
 
 
 class BenchPhase(enum.IntEnum):
@@ -113,8 +114,9 @@ class WorkerConfig:
     run_as_service: bool = False
     verify_collect_all: bool = False
     verify_report: bool = False       # --verifyreport: map bad blocks' damage, fail at phase end
-    checksums: bool = False           # --checksums: each file's CRC-32 per phase (checksums())
-    checksum_chunk_shift: int = 0     # --checksumchunk: CRC-32s of 2**shift byte chunks (0: files)
+    checksums: bool = False           # --checksums: each file's CRC per phase (checksums())
+    checksum_chunk_shift: int = 0     # --checksumchunk: CRCs of 2**shift byte chunks (0: files)
+    checksum_algo: str = "crc32"      # --checksumalgo: "crc32", "crc32c" or "crc64nvme"
     serialize_buffered_writes: int = 0  # 0 auto, 1 on, 2 off (--writegate)
     staging_engine: int = 0           # 0 auto, 1 kernels move the data, 2 cudaMemcpyAsync
     no_gpu_numa_binding: bool = False  # --nogpunuma
@@ -152,6 +154,8 @@ class WorkerConfig:
         cfg.useExplicitRandOffsetAlgo = int(self.use_explicit_rand_offset_algo)
         cfg.doReverseSeqOffsets = int(self.do_reverse_seq_offsets)
         cfg.useStridedAccess = int(self.use_strided_access)
+        # (an unknown name: an algorithm that the library rejects)
+        cfg.checksumAlgo = CHECKSUM_ALGOS.get(self.checksum_algo, -1)
         cfg.randomAmount = self.random_amount
         cfg.randOffsetSeed = self.rand_offset_seed
         cfg.integrityCheckSalt = self.integrity_check_salt

@@ -321,6 +321,16 @@ int elb_crc32_chunks(const elb_block_desc* descs, const uint64_t* shifts, uint32
 uint32_t elb_crc32_shift(uint32_t crc, uint64_t n);
 /* zlib's CRC-32 of a message of size bytes from its raw CRC R (elb_crc32_blocks) */
 uint32_t elb_crc32_finish(uint32_t rawCrc, uint64_t size);
+/* elb_crc32_chunks for the CRC of algo (enum elb_checksum_algo): devCrcs and hostCrcs hold
+ * uint32_t slots for the 32-bit algorithms and uint64_t slots for ELB_CHECKSUM_CRC64NVME.
+ * elb_crc32_chunks is the ELB_CHECKSUM_CRC32 case. Fails for an unknown algo. */
+int elb_crc_chunks(int32_t algo, const elb_block_desc* descs, const uint64_t* shifts,
+	uint32_t numDescs, unsigned chunkShift, uint64_t slotsPerDesc, void* devCrcs, void* hostCrcs,
+	unsigned* devTicket, void* stream);
+/* X(crc, n) and the published CRC of a message of size bytes from its raw CRC, for algo (32-bit
+ * algorithms: the low 32 bits). An unknown algo returns 0 and sets the last error. */
+uint64_t elb_crc_shift(int32_t algo, uint64_t crc, uint64_t n);
+uint64_t elb_crc_finish(int32_t algo, uint64_t rawCrc, uint64_t size);
 
 int elb_stage_copy(const elb_block_desc* descs, uint32_t numDescs, int hostToDevice,
 	int64_t hostDelta, uint64_t totalBytes, uint64_t maxBlockLen, void* stream);
@@ -390,6 +400,10 @@ typedef struct elb_cfg
 	int32_t useExplicitRandOffsetAlgo; /* nonzero = user gave --randalgo => no full coverage */
 	int32_t doReverseSeqOffsets;
 	int32_t useStridedAccess;
+	/* --checksumalgo: enum elb_checksum_algo of --checksums and a checksum list
+	 * (elb_mgr_set_checksum_list; a list's own algorithm replaces the default CRC32). It takes the
+	 * 4 bytes of padding in front of randomAmount: no other field moves. */
+	int32_t checksumAlgo;
 	uint64_t randomAmount; /* 0 = default (ProgArgs.cpp:1558-1561) */
 	uint64_t randOffsetSeed; /* 0 = self-seed (std::random_device) like the reference */
 
@@ -517,6 +531,15 @@ enum elb_staging_engine
 	ELB_STAGING_AUTO = 0,
 	ELB_STAGING_KERNEL = 1, /* fused: fill + stage-out, stage-in + verify, stage copy */
 	ELB_STAGING_COPYENGINE = 2, /* cudaMemcpyAsync + kernel on the device slot */
+};
+
+/* elb_cfg::checksumAlgo values: reflected CRCs, published as R ^ X(all ones, size) ^ all ones
+ * (elb_crc_finish) */
+enum elb_checksum_algo
+{
+	ELB_CHECKSUM_CRC32 = 0,     /* zlib, gzip, zip: polynomial 0xEDB88320, 32 bits */
+	ELB_CHECKSUM_CRC32C = 1,    /* Castagnoli (iSCSI, GCS, btrfs): 0x82F63B78, 32 bits */
+	ELB_CHECKSUM_CRC64NVME = 2, /* NVMe protection information guard: 0x9A6C9329AC4BC9B5, 64 bits */
 };
 
 /* elb_cfg::serializeBufferedWrites values */
@@ -769,8 +792,9 @@ int64_t elb_mgr_verify_report(elb_mgr* m, char* outBuf, uint64_t outBufLen);
 
 /* --checksums (elb_cfg::checksumReport): the files of the last phase, merged over all workers, as
  * text lines "<path> <size> <bytes covered> <crc>\n" sorted by path. size is the file's data set
- * size, bytes covered the sum of the lengths of its blocks that the phase moved, crc zlib's CRC-32
- * of the file's first size bytes as 8 lowercase hex digits if bytes covered == size, else "-".
+ * size, bytes covered the sum of the lengths of its blocks that the phase moved, crc the CRC of
+ * elb_cfg::checksumAlgo (zlib's CRC-32 by default) of the file's first size bytes as lowercase hex
+ * digits (8, or 16 for ELB_CHECKSUM_CRC64NVME) if bytes covered == size, else "-".
  * Returns the length of the full text (truncated to outBufLen - 1 bytes in outBuf), -1 on error.
  * With elb_cfg::checksumChunkShift, the text is instead one line "<path> <offset> <length> <crc>\n"
  * per chunk the last phase moved, sorted by path and offset. */
@@ -778,8 +802,10 @@ int64_t elb_mgr_checksums(elb_mgr* m, char* outBuf, uint64_t outBufLen);
 
 /* --checksumverify: parse a checksum list (text of len bytes, as --checksums with a chunk size
  * writes it) and check every chunk that the following read phases move against the last section
- * of it that has a chunk size. Its chunk size becomes elb_cfg::checksumChunkShift. A read phase
- * then fails at the first chunk whose CRC-32 differs from its line, that has no line, or whose
+ * of it that has a chunk size. Its chunk size becomes elb_cfg::checksumChunkShift, and its
+ * algorithm (the header's last word: "crc32c", "crc64nvme"; none: "crc32") elb_cfg::checksumAlgo;
+ * a checksumAlgo other than ELB_CHECKSUM_CRC32 that differs from the list's is rejected. A read
+ * phase then fails at the first chunk whose CRC differs from its line, that has no line, or whose
  * line has another length. Call it between phases. Returns -1 (elb_last_error names the line of a
  * malformed line, or the option the list conflicts with), else 0. */
 int elb_mgr_set_checksum_list(elb_mgr* m, const char* text, uint64_t len);
