@@ -254,6 +254,10 @@ SIGNATURES = {
     "elb_crc_finish": (c_u64, [ctypes.c_int32, c_u64, c_u64]),
     "elb_crc32_chunks": (ctypes.c_int, [_VP, _VP, c_u32, ctypes.c_uint, c_u64, _VP, _VP, _VP,
                                         _VP]),
+    "elb_blake3_chunks": (ctypes.c_int, [_VP, _VP, c_u32, ctypes.c_uint, c_u64, _VP, _VP, _VP,
+                                         _VP]),
+    "elb_blake3_parent": (None, [_VP, _VP, ctypes.c_int, _VP]),
+    "elb_blake3_fold": (ctypes.c_int, [_VP, c_u64, c_u64, _VP]),
     "elb_damage_map": (ctypes.c_int, [_VP, c_u32, ctypes.c_int, c_u64, ctypes.c_uint,
                                       ctypes.c_uint, ctypes.c_uint, _VP, c_u64, _VP]),
     "elb_stage_copy": (ctypes.c_int, [_VP, c_u32, ctypes.c_int, ctypes.c_int64, c_u64, c_u64,

@@ -520,6 +520,78 @@ uint64_t elb_crc_finish(int32_t algo, uint64_t rawCrc, uint64_t size)
 	return result;
 }
 
+static_assert(elb_blake3_algo::ID == ELB_CHECKSUM_BLAKE3, "elb_blake3_algo ID");
+
+int elb_blake3_chunks(const elb_block_desc* descs, const uint64_t* shifts, uint32_t numDescs,
+	unsigned chunkShift, uint64_t slotsPerDesc, void* devDigests, void* hostDigests,
+	unsigned* devTicket, void* stream)
+{
+	const char* what = "elb_blake3_chunks";
+
+	if( (chunkShift != 64) && ( (chunkShift < ELB_CRC_MIN_CHUNK_SHIFT) ||
+		(chunkShift > ELB_CRC_MAX_CHUNK_SHIFT) ) )
+	{
+		elb_set_last_error(std::string(what) + ": chunk shift " + std::to_string(chunkShift) +
+			" is neither 64 nor in [" + std::to_string(ELB_CRC_MIN_CHUNK_SHIFT) + ", " +
+			std::to_string(ELB_CRC_MAX_CHUNK_SHIFT) + "]");
+		return -1;
+	}
+
+	if(!slotsPerDesc)
+	{
+		elb_set_last_error(std::string(what) + ": slots per descriptor must be at least 1");
+		return -1;
+	}
+
+	if(numDescs && (!descs || ( (chunkShift == 64) && !shifts) || !devDigests) )
+	{
+		elb_set_last_error(std::string(what) + ": NULL descriptor, shift or digest array");
+		return -1;
+	}
+
+	if(!hostDigests != !devTicket)
+	{
+		elb_set_last_error(std::string(what) + ": host digests and device ticket go together");
+		return -1;
+	}
+
+	if(elb_launch_blake3(descs, shifts, numDescs, chunkShift, slotsPerDesc, devDigests,
+		hostDigests, (cudaStream_t)stream) )
+	{
+		elb_set_last_error(std::string("elb_") + elb_last_error() );
+		return -1;
+	}
+
+	return 0;
+}
+
+void elb_blake3_parent(const uint8_t* left, const uint8_t* right, int root, uint8_t* out)
+{
+	uint32_t l[8], r[8], cv[8];
+
+	memcpy(l, left, 32);
+	memcpy(r, right, 32);
+	elb_blake3_parent_cv(l, r, root != 0, cv);
+	memcpy(out, cv, 32);
+}
+
+int elb_blake3_fold(const uint8_t* runs, uint64_t numRuns, uint64_t fileSize, uint8_t* out)
+{
+	const uint64_t numChunks = elb_blake3_num_chunks(fileSize);
+	uint32_t cv[8];
+
+	if(!runs || !out || !elb_blake3_fold_cvs( (const uint32_t (*)[8])runs, numRuns, numChunks, cv) )
+	{
+		elb_set_last_error("elb_blake3_fold: " + std::to_string(numRuns) + " runs do not make a "
+			"file of " + std::to_string(fileSize) + " bytes (" + std::to_string(numChunks) +
+			" chunks)");
+		return -1;
+	}
+
+	memcpy(out, cv, 32);
+	return 0;
+}
+
 int elb_stage_copy(const elb_block_desc* descs, uint32_t numDescs, int hostToDevice,
 	int64_t hostDelta, uint64_t totalBytes, uint64_t maxBlockLen, void* stream)
 {

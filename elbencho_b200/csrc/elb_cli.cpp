@@ -143,7 +143,8 @@ static const OptDef optDefs[] =
 		"--verifyreport. [b200]"},
 	{"checksumalgo", 0, Opt_STR, &ProgArgs::checksumAlgoName, Wire_NONE, "CRC of --checksums and "
 		"--checksumverify: crc32 (zlib, gzip, zip), crc32c (Castagnoli: iSCSI, GCS, btrfs) or "
-		"crc64nvme (NVMe protection information, S3). Other than crc32, each section header ends "
+		"crc64nvme (NVMe protection information, S3), or blake3 (BLAKE3-256 as b3sum prints it, "
+		"64 hex digits; block size a multiple of 1K). Other than crc32, each section header ends "
 		"with the name, and crc64nvme CRCs have 16 hex digits instead of 8. A list's own "
 		"algorithm is used for --checksumverify. Requires --checksums or --checksumverify. "
 		"(Default: crc32) [b200]"},
@@ -1035,8 +1036,9 @@ void ProgArgs::checkArgs()
 			throw ProgError("Option \"--checksumalgo\" requires \"--checksums\" or "
 				"\"--checksumverify\"");
 
-		if(elb_crc_algo_by_name(checksumAlgoName.c_str() ) < 0)
-			throw ProgError("Option \"--checksumalgo\" must be crc32, crc32c or crc64nvme");
+		if(elb_checksum_algo_by_name(checksumAlgoName.c_str() ) < 0)
+			throw ProgError("Option \"--checksumalgo\" must be crc32, crc32c or crc64nvme, or "
+				"blake3");
 	}
 
 	if(!checksumVerifyPath.empty() )
@@ -1084,9 +1086,10 @@ void ProgArgs::checkArgs()
 				"of the chunk size of the checksum list (" + std::to_string(listChunkSize) + ")");
 
 		if(!checksumAlgoName.empty() &&
-			(elb_crc_algo_by_name(checksumAlgoName.c_str() ) != checksumList->algo) )
+			(elb_checksum_algo_by_name(checksumAlgoName.c_str() ) != checksumList->algo) )
 			throw ProgError("Option \"--checksumalgo\" (" + checksumAlgoName + ") differs from "
-				"the algorithm of the checksum list (" + elb_crc_algo_name(checksumList->algo) + ")");
+				"the algorithm of the checksum list (" + elb_checksum_algo_name(checksumList->algo) +
+				")");
 	}
 
 	if(doDirectVerify && ( (!integrityCheckSalt && !randomVerifySeed) || !runCreateFilesPhase) )
@@ -1185,7 +1188,7 @@ void ProgArgs::toABIConfig(ABIConfig& out) const
 	cfg.checksumChunkShift = checksumList ? (int32_t)checksumList->chunkShift :
 		checksumChunkSize ? __builtin_ctzll(checksumChunkSize) : 0;
 	cfg.checksumAlgo = checksumList ? checksumList->algo : checksumAlgoName.empty() ?
-		ELB_CHECKSUM_CRC32 : elb_crc_algo_by_name(checksumAlgoName.c_str() );
+		ELB_CHECKSUM_CRC32 : elb_checksum_algo_by_name(checksumAlgoName.c_str() );
 	cfg.serializeBufferedWrites = neverSerializeBufferedWrites ? ELB_WRITEGATE_OFF :
 		(serializeBufferedWrites ? ELB_WRITEGATE_ON : ELB_WRITEGATE_AUTO);
 	cfg.noGPUNumaBinding = noGPUNumaBinding;

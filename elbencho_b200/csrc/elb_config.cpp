@@ -216,7 +216,7 @@ Config Config::fromABI(const elb_cfg* cfg)
 			") is not in [" + std::to_string(ELB_CHECKSUM_MIN_CHUNK_SHIFT) + ", " +
 			std::to_string(ELB_CHECKSUM_MAX_CHUNK_SHIFT) + "].");
 
-	if( (c.checksumAlgo < 0) || (c.checksumAlgo > ELB_CHECKSUM_CRC64NVME) )
+	if( (c.checksumAlgo < 0) || (c.checksumAlgo > ELB_CHECKSUM_BLAKE3) )
 		throw WorkerError("Invalid checksum algorithm: " + std::to_string(c.checksumAlgo) );
 
 	if(c.checksumChunkShift)
@@ -303,6 +303,17 @@ Config Config::fromABI(const elb_cfg* cfg)
 	if( (c.useDirectIO || c.useRandomOffsets || c.useStridedAccess) && c.fileSize &&
 		(c.fileSize % c.blockSize) ) // :1543-1555
 		c.fileSize -= (c.fileSize % c.blockSize);
+
+	/* BLAKE3 hashes 1 KiB chunks, so blocks must start on chunk boundaries; a block reduced to the
+	   file size is the whole file */
+	if( (c.checksumAlgo == ELB_CHECKSUM_BLAKE3) && (c.blockSize % 1024) &&
+		(c.blockSize != c.fileSize) )
+		throw WorkerError("Option \"--checksumalgo\" blake3 requires a block size that is a "
+			"multiple of 1K");
+
+	if( (c.checksumAlgo == ELB_CHECKSUM_BLAKE3) && c.useRandomUnaligned)
+		throw WorkerError("Option \"--checksumalgo\" blake3 cannot be used together with "
+			"\"--norandalign\"");
 
 	if(!c.randomAmount && (c.pathType != ELB_PATH_DIR) && c.useRandomOffsets) // :1558-1561
 		c.randomAmount = c.fileSize * c.paths.size();

@@ -450,7 +450,7 @@ void Coordinator::writeChecksumSection(int benchPhase)
 
 	// (the default CRC-32 keeps the headers that have no algorithm name)
 	if(manager->shared.cfg.checksumAlgo != ELB_CHECKSUM_CRC32)
-		fileStream << " " << elb_crc_algo_name(manager->shared.cfg.checksumAlgo);
+		fileStream << " " << elb_checksum_algo_name(manager->shared.cfg.checksumAlgo);
 
 	fileStream << "\n" << report.lines << std::flush;
 

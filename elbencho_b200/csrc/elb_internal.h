@@ -98,6 +98,13 @@ int elb_launch_damage_map(const elb_content& content, const elb_block_desc* desc
 int elb_launch_crc(int algo, const elb_block_desc* descs, const uint64_t* shifts,
 	uint32_t numDescs, unsigned chunkShift, uint64_t slotsPerDesc, void* devCrcs, void* hostCrcs,
 	unsigned* doneTicket, cudaStream_t stream);
+/* BLAKE3 digests (elb_blake3_chunks; chunkShift 64: the runs of whole-file mode). Slots are 32
+   bytes, written to devDigests and, if not NULL, to the pinned hostDigests. descs and shifts must
+   be host- and device-readable: the host checks them against slotsPerDesc and sizes the grid from
+   their lengths */
+int elb_launch_blake3(const elb_block_desc* descs, const uint64_t* shifts, uint32_t numDescs,
+	unsigned chunkShift, uint64_t slotsPerDesc, void* devDigests, void* hostDigests,
+	cudaStream_t stream);
 int elb_kernels_warmup();
 uint64_t elb_get_num_kernel_launches();
 

@@ -13,6 +13,8 @@
  *      bad differ, per 512-byte file sector; off the clean path, see its section below)
  *   crc (no reference counterpart: --checksums / --checksumverify / --checksumalgo, each block's
  *      share of its file's CRC or its chunks' CRCs; off the clean path, see its section below)
+ *   blake3 (no reference counterpart: --checksumalgo blake3, the BLAKE3 runs of each block or the
+ *      digests of its chunks; compute-bound on the integer pipes, see its section below)
  *
  * All eight are HBM-bound byte/integer kernels (K1/K3/K5/K7: 1 byte written per payload byte,
  * K2/K4/K6/K8: 1 byte read per payload byte), so the design follows the streaming rules: 16-byte (128-bit) vector
@@ -1444,6 +1446,375 @@ elb_crc_kernel(const elb_block_desc* descs, const uint64_t* shifts, uint32_t num
 		*doneTicket = 0;
 }
 
+/* ---- BLAKE3 digests (--checksumalgo blake3) -------------------------------------------------
+ *
+ * Each descriptor's chunks (1 KiB, elb_patterns.cuh) are numbered in a coordinate in which the
+ * tree's runs are aligned: whole-file mode (chunkShift 64), the file's chunk index; chunked mode,
+ * the chunk index in the block, since a block starts on a K-chunk boundary. A unit is what the
+ * kernel finishes: whole-file mode, the descriptor (its canonical cut, the maximal aligned runs,
+ * one slot each; or, when the descriptor is the whole file, the file's digest in slot 0); chunked
+ * mode, each K-chunk of 2^chunkShift bytes, a message of its own whose digest fills one slot.
+ *
+ * A CTA of ELB_B3_THREADS threads takes a window of that many consecutive chunks, one per thread.
+ * Each thread compresses its chunk's 16 blocks in registers, loading each 64-byte block as four
+ * 16-byte vectors where the address allows. The window's CVs then go to shared memory (word-major:
+ * no bank conflicts) and are joined level by level into the maximal aligned runs inside the window
+ * and the unit; a run that is the whole message takes ROOT. A unit inside the window is finished
+ * by the thread of its first chunk: it writes the runs, or folds them from the right into the
+ * digest. Small descriptors are packed 2^packShift chunks apart, so that one window holds many.
+ * Units larger than a window (whole-file descriptors and K-chunks above ELB_B3_THREADS KiB) belong
+ * to one CTA that walks their windows in order; its thread 0 keeps the runs on a stack in shared
+ * memory and joins aligned siblings as they arrive. With hostDigests, the thread that finishes
+ * a slot also writes it to pinned host memory, so that no copy is left for the host to wait on;
+ * BLAKE3 slots are final where they are made, so no last CTA has anything to join. */
+
+#define ELB_B3_THREADS 512
+#define ELB_B3_WINDOW_SHIFT 9
+#define ELB_B3_STACK 128 /* runs of a prefix of a unit: at most 2 * 64 */
+
+/* a chunk's unit, in chunk coordinates */
+struct B3Unit
+{
+	uint64_t begin;
+	uint64_t end;
+	uint64_t slot; // its first slot
+	bool isRoot;   // its message is the unit: the top run takes ROOT
+};
+
+/* the unit of chunk x of descriptor descIdx (cb: coordinate of the block's first chunk, n: its
+   number of chunks) */
+__device__ __forceinline__ B3Unit b3_unit(uint64_t x, uint64_t cb, uint64_t n, bool wholeFileRoot,
+	unsigned chunkShift, uint32_t descIdx, uint64_t slotsPerDesc)
+{
+	if(chunkShift == 64)
+		return B3Unit{cb, cb + n, (uint64_t)descIdx * slotsPerDesc, wholeFileRoot};
+
+	const unsigned kShift = chunkShift - ELB_BLAKE3_CHUNK_SHIFT;
+	const uint64_t begin = x & ~( (1ULL << kShift) - 1);
+
+	const uint64_t end = begin + ( (uint64_t)1 << kShift);
+
+	return B3Unit{begin, (end < n) ? end : n, (uint64_t)descIdx * slotsPerDesc + (begin >> kShift),
+		true};
+}
+
+/* slot <- cv, in device memory and, with hostDigests, in pinned host memory (posted writes from
+   every CTA: a last CTA copying all slots was the bottleneck at K = 4 KiB, 32 bytes per 4 KiB) */
+__device__ __forceinline__ void b3_store(uint32_t* digests, uint32_t* hostDigests, uint64_t slot,
+	const uint32_t cv[8])
+{
+	const uint4 lo = make_uint4(cv[0], cv[1], cv[2], cv[3]);
+	const uint4 hi = make_uint4(cv[4], cv[5], cv[6], cv[7]);
+	uint4* out = (uint4*)(digests + slot * 8);
+
+	out[0] = lo;
+	out[1] = hi;
+
+	if(hostDigests)
+	{
+		uint4* hostOut = (uint4*)(hostDigests + slot * 8);
+
+		hostOut[0] = lo;
+		hostOut[1] = hi;
+	}
+}
+
+/* the CV of the len <= 1024 bytes at p, counter t (root: the chunk is the whole message) */
+__device__ __forceinline__ void b3_chunk_cv(const uint8_t* p, uint32_t len, uint64_t t, bool root,
+	uint32_t cv[8])
+{
+	const uint32_t numBlocks = len ? (len + 63) >> 6 : 1;
+	const bool isAligned = !( (uintptr_t)p & 15);
+
+	elb_blake3_iv(cv);
+
+	#pragma unroll 1
+	for(uint32_t b = 0; b < numBlocks; b++)
+	{
+		const uint32_t blockLen = min(len - b * 64, 64u);
+		const uint8_t* block = p + b * 64;
+		uint32_t m[16];
+
+		if(isAligned && (blockLen == 64) )
+		{
+			#pragma unroll
+			for(int v = 0; v < 4; v++)
+			{
+				uint4 vec;
+				asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(vec.x), "=r"(vec.y),
+					"=r"(vec.z), "=r"(vec.w) : "l"(block + v * 16) );
+				m[4 * v] = vec.x;
+				m[4 * v + 1] = vec.y;
+				m[4 * v + 2] = vec.z;
+				m[4 * v + 3] = vec.w;
+			}
+		}
+		else
+		{ // unaligned or short: byte by byte, zeros past the end
+			#pragma unroll
+			for(int w = 0; w < 16; w++)
+			{
+				uint32_t word = 0;
+
+				#pragma unroll
+				for(int k = 0; k < 4; k++)
+					if(w * 4 + k < (int)blockLen)
+						word |= (uint32_t)block[w * 4 + k] << (8 * k);
+
+				m[w] = word;
+			}
+		}
+
+		uint32_t flags = b ? 0 : ELB_BLAKE3_CHUNK_START;
+
+		if(b + 1 == numBlocks)
+			flags |= ELB_BLAKE3_CHUNK_END | (root ? ELB_BLAKE3_ROOT : 0);
+
+		elb_blake3_compress(cv, m, t, blockLen, flags);
+	}
+}
+
+__device__ __forceinline__ void b3_load_cv(const uint32_t (*sCv)[ELB_B3_THREADS], unsigned j,
+	uint32_t cv[8])
+{
+	#pragma unroll
+	for(int k = 0; k < 8; k++)
+		cv[k] = sCv[k][j];
+}
+
+__global__ void __launch_bounds__(ELB_B3_THREADS)
+elb_blake3_kernel(const elb_block_desc* descs, const uint64_t* shifts, uint32_t numDescs,
+	unsigned chunkShift, uint64_t slotsPerDesc, unsigned packShift, uint64_t itemsPerDesc,
+	uint32_t* digests, uint32_t* hostDigests)
+{
+	__shared__ uint32_t sCv[8][ELB_B3_THREADS];
+	__shared__ int8_t sLevel[ELB_B3_THREADS]; // top level of the run at the chunk; -1: none
+	__shared__ uint64_t sStackPos[ELB_B3_STACK];
+	__shared__ uint8_t sStackShift[ELB_B3_STACK];
+	__shared__ uint32_t sStackCv[ELB_B3_STACK][8];
+
+	const unsigned j = threadIdx.x;
+	const bool isPacked = (packShift <= ELB_B3_WINDOW_SHIFT);
+	const bool isChunked = (chunkShift < 64);
+
+	/* this CTA's descriptor and chunk range [rangeBegin, rangeEnd) in window mode; in packed mode
+	   descriptor descIdx = first + j >> packShift, chunks cb + (j & (2^packShift - 1)) */
+	uint32_t descIdx;
+	uint64_t rangeBegin = 0, rangeEnd = 0;
+
+	if(isPacked)
+		descIdx = (uint32_t)( ( (uint64_t)blockIdx.x << (ELB_B3_WINDOW_SHIFT - packShift) ) +
+			(j >> packShift) );
+	else
+		descIdx = (uint32_t)(blockIdx.x / itemsPerDesc);
+
+	elb_block_desc desc{};
+	bool wholeFileRoot = false;
+
+	if(descIdx < numDescs)
+	{
+		desc = descs[descIdx];
+		wholeFileRoot = !isChunked && !desc.fileOffset && !shifts[descIdx];
+	}
+
+	const uint64_t cb = isChunked ? 0 : (desc.fileOffset >> ELB_BLAKE3_CHUNK_SHIFT);
+	const uint64_t n = wholeFileRoot ? elb_blake3_num_chunks(desc.len) :
+		( (desc.len + 1023) >> ELB_BLAKE3_CHUNK_SHIFT);
+
+	if(!isPacked && (descIdx < numDescs) )
+	{ // whole-file: the descriptor; chunked: a window, or a K-chunk larger than one
+		const uint64_t item = blockIdx.x - (uint64_t)descIdx * itemsPerDesc;
+		const unsigned itemShift = !isChunked ? 64 :
+			max(chunkShift - ELB_BLAKE3_CHUNK_SHIFT, (unsigned)ELB_B3_WINDOW_SHIFT);
+
+		rangeBegin = (itemShift == 64) ? cb : min(item << itemShift, n);
+		rangeEnd = (itemShift == 64) ? (cb + n) : min( (item + 1) << itemShift, n);
+	}
+
+	const uint64_t firstWindow = rangeBegin >> ELB_B3_WINDOW_SHIFT;
+	const uint64_t numWindows = isPacked ? 1 : (rangeEnd > rangeBegin) ?
+		( ( (rangeEnd - 1) >> ELB_B3_WINDOW_SHIFT) - firstWindow + 1) : 0;
+
+	/* window mode: the unit that spans windows, whose runs thread 0 stacks (none: begin == end) */
+	B3Unit bigUnit{0, 0, 0, false};
+
+	if(!isPacked && (rangeEnd > rangeBegin) )
+	{
+		bigUnit = b3_unit(rangeBegin, cb, n, wholeFileRoot, chunkShift, descIdx, slotsPerDesc);
+
+		if( (bigUnit.begin >> ELB_B3_WINDOW_SHIFT) == ( (bigUnit.end - 1) >> ELB_B3_WINDOW_SHIFT) )
+			bigUnit.end = bigUnit.begin;
+	}
+
+	unsigned stackTop = 0; // (thread 0)
+
+	for(uint64_t w = firstWindow; w < firstWindow + numWindows; w++)
+	{
+		const uint64_t winBegin = w << ELB_B3_WINDOW_SHIFT;
+		const uint64_t winEnd = winBegin + ELB_B3_THREADS;
+		uint64_t x;
+		bool hasChunk;
+
+		if(isPacked)
+		{
+			x = cb + (j & ( (1u << packShift) - 1) );
+			hasChunk = (descIdx < numDescs) && (x - cb < n);
+		}
+		else
+		{
+			x = winBegin + j;
+			hasChunk = (x >= rangeBegin) && (x < rangeEnd);
+		}
+
+		B3Unit unit{0, 0, 0, false};
+
+		if(hasChunk)
+		{
+			unit = b3_unit(x, cb, n, wholeFileRoot, chunkShift, descIdx, slotsPerDesc);
+
+			const uint64_t byteOffset = (x - cb) << ELB_BLAKE3_CHUNK_SHIFT;
+			const uint32_t len = (uint32_t)min(desc.len - byteOffset, (uint64_t)1024);
+			uint32_t cv[8];
+
+			b3_chunk_cv( (const uint8_t*)desc.devPtr + byteOffset, len, x - (isChunked ? unit.begin : 0),
+				unit.isRoot && (unit.end - unit.begin == 1), cv);
+
+			#pragma unroll
+			for(int k = 0; k < 8; k++)
+				sCv[k][j] = cv[k];
+		}
+
+		sLevel[j] = hasChunk ? 0 : -1;
+
+		// join aligned siblings inside the window and the unit, level by level
+		#pragma unroll 1
+		for(unsigned level = 1; level <= ELB_B3_WINDOW_SHIFT; level++)
+		{
+			__syncthreads();
+
+			const uint64_t size = 1ULL << level;
+
+			if(hasChunk && (sLevel[j] == (int)level - 1) && !(x & (size - 1) ) &&
+				(x + size <= unit.end) && (sLevel[j + (size >> 1)] == (int)level - 1) )
+			{
+				uint32_t left[8], right[8];
+
+				b3_load_cv(sCv, j, left);
+				b3_load_cv(sCv, j + (unsigned)(size >> 1), right);
+				elb_blake3_parent_cv(left, right,
+					unit.isRoot && (x == unit.begin) && (x + size == unit.end), left);
+
+				#pragma unroll
+				for(int k = 0; k < 8; k++)
+					sCv[k][j] = left[k];
+
+				sLevel[j] = (int8_t)level;
+				sLevel[j + (size >> 1)] = -2; // (now inside the run at j)
+			}
+		}
+
+		__syncthreads();
+
+		// units inside the window: the thread of the first chunk writes the runs or the digest
+		if(hasChunk && (x == unit.begin) && (isPacked || ( (unit.begin >= winBegin) &&
+			(unit.end <= winEnd) ) ) )
+		{
+			const uint64_t numChunks = unit.end - unit.begin;
+			uint32_t acc[8];
+
+			if(!unit.isRoot || !(numChunks & (numChunks - 1) ) )
+			{ // the canonical cut, left to right (a root message of 2^k chunks: its one run)
+				uint64_t slot = unit.slot;
+
+				for(uint64_t pos = unit.begin; pos < unit.end; slot++)
+				{
+					const unsigned t = j + (unsigned)(pos - x);
+
+					b3_load_cv(sCv, t, acc);
+					b3_store(digests, hostDigests, slot, acc);
+					pos += 1ULL << sLevel[t];
+				}
+			}
+			else
+			{ // the runs of the digits of numChunks, joined from the right
+				bool isFirst = true;
+
+				for(unsigned bit = 0; bit < 64; bit++)
+				{
+					if( !( (numChunks >> bit) & 1) )
+						continue;
+
+					const uint64_t start = numChunks & ~( (2ULL << bit) - 1);
+					uint32_t run[8];
+
+					b3_load_cv(sCv, j + (unsigned)start, run);
+
+					if(isFirst)
+						memcpy(acc, run, sizeof(acc) );
+					else
+						elb_blake3_parent_cv(run, acc, !start, acc);
+
+					isFirst = false;
+				}
+
+				b3_store(digests, hostDigests, unit.slot, acc);
+			}
+		}
+
+		// the unit that spans windows: its runs in this window onto the stack
+		if(!j && (bigUnit.end > bigUnit.begin) )
+		{
+			const uint64_t partEnd = min(bigUnit.end, winEnd);
+
+			for(uint64_t pos = max(bigUnit.begin, winBegin); pos < partEnd; )
+			{
+				const unsigned t = (unsigned)(pos - winBegin);
+				uint64_t runPos = pos;
+				unsigned runShift = (unsigned)sLevel[t];
+				uint32_t cv[8];
+
+				b3_load_cv(sCv, t, cv);
+				pos += 1ULL << runShift;
+
+				while(stackTop && (sStackShift[stackTop - 1] == runShift) &&
+					!(sStackPos[stackTop - 1] & ( (2ULL << runShift) - 1) ) )
+				{ // the left sibling is on top: join
+					stackTop--;
+					runPos = sStackPos[stackTop];
+					runShift++;
+					elb_blake3_parent_cv(sStackCv[stackTop], cv, bigUnit.isRoot &&
+						(runPos == bigUnit.begin) && (runPos + (1ULL << runShift) == bigUnit.end), cv);
+				}
+
+				sStackPos[stackTop] = runPos;
+				sStackShift[stackTop] = (uint8_t)runShift;
+				memcpy(sStackCv[stackTop], cv, sizeof(cv) );
+				stackTop++;
+			}
+
+			if(bigUnit.end <= winEnd)
+			{ // the unit is complete
+				if(!bigUnit.isRoot)
+					for(unsigned i = 0; i < stackTop; i++)
+						b3_store(digests, hostDigests, bigUnit.slot + i, sStackCv[i]);
+				else
+				{ // (one run: it took ROOT when it was joined)
+					uint32_t acc[8];
+
+					memcpy(acc, sStackCv[stackTop - 1], sizeof(acc) );
+
+					for(unsigned i = stackTop - 1; i-- > 0; )
+						elb_blake3_parent_cv(sStackCv[i], acc, !i, acc);
+
+					b3_store(digests, hostDigests, bigUnit.slot, acc);
+				}
+			}
+		}
+
+		__syncthreads(); // (the next window reuses the shared arrays)
+	}
+}
+
 /* ---- host side launchers ------------------------------------------------------------------ */
 
 static std::atomic<uint64_t> gNumKernelLaunches{0};
@@ -1902,6 +2273,91 @@ int elb_launch_crc(int algo, const elb_block_desc* descs, const uint64_t* shifts
 	gNumKernelLaunches.fetch_add(1, std::memory_order_relaxed);
 
 	return checkLaunch("crc");
+}
+
+int elb_launch_blake3(const elb_block_desc* descs, const uint64_t* shifts, uint32_t numDescs,
+	unsigned chunkShift, uint64_t slotsPerDesc, void* devDigests, void* hostDigests,
+	cudaStream_t stream)
+{
+	const bool isChunked = (chunkShift < 64);
+	const uint64_t chunkSize = isChunked ? (1ULL << chunkShift) : 0;
+	uint64_t maxChunks = 0;
+
+	for(uint32_t i = 0; i < numDescs; i++)
+	{ // (descs and shifts are host-readable)
+		const elb_block_desc& desc = descs[i];
+		const uint64_t end = desc.fileOffset + desc.len;
+		const bool isFileEnd = shifts && !shifts[i];
+		const uint64_t boundary = isChunked ? chunkSize : 1024;
+		auto where = [&]() { return "descriptor " + std::to_string(i) + " (offset " +
+			std::to_string(desc.fileOffset) + ", length " + std::to_string(desc.len) + ")"; };
+
+		if( (desc.fileOffset % boundary) || ( (end % boundary) && shifts && !isFileEnd) )
+		{
+			elb_set_last_error("blake3_chunks: " + where() + " is not on " +
+				(isChunked ? "chunk" : "1 KiB") + " boundaries");
+			return -1;
+		}
+
+		const bool isWholeFile = !isChunked && !desc.fileOffset && isFileEnd;
+		const uint64_t numChunks = isWholeFile ? elb_blake3_num_chunks(desc.len) :
+			( (desc.len + 1023) >> ELB_BLAKE3_CHUNK_SHIFT);
+		const uint64_t cb = desc.fileOffset >> ELB_BLAKE3_CHUNK_SHIFT;
+		const uint64_t numSlots = isChunked ? ( (desc.len + chunkSize - 1) >> chunkShift) :
+			isWholeFile ? 1 : elb_blake3_num_runs(cb, cb + numChunks);
+
+		if(numSlots > slotsPerDesc)
+		{
+			elb_set_last_error("blake3_chunks: " + where() + " needs " + std::to_string(numSlots) +
+				" slots, more than " + std::to_string(slotsPerDesc) + " slots per descriptor");
+			return -1;
+		}
+
+		maxChunks = std::max(maxChunks, numChunks);
+	}
+
+	if(!numDescs)
+		return 0;
+
+	/* packed: windows of 2^packShift chunks per descriptor; else one CTA per descriptor
+	   (whole-file), per window, or per K-chunk larger than a window */
+	unsigned packShift = ELB_B3_WINDOW_SHIFT + 1;
+	uint64_t itemsPerDesc = 1;
+	uint64_t gridSize;
+
+	if(maxChunks <= ELB_B3_THREADS)
+	{
+		packShift = 0;
+		while( (1ULL << packShift) < maxChunks)
+			packShift++;
+
+		const uint64_t descsPerCTA = 1ULL << (ELB_B3_WINDOW_SHIFT - packShift);
+		gridSize = (numDescs + descsPerCTA - 1) / descsPerCTA;
+	}
+	else
+	{
+		if(isChunked)
+		{
+			const unsigned itemShift = std::max(chunkShift - ELB_BLAKE3_CHUNK_SHIFT,
+				(unsigned)ELB_B3_WINDOW_SHIFT);
+			itemsPerDesc = (maxChunks + (1ULL << itemShift) - 1) >> itemShift;
+		}
+
+		gridSize = numDescs * itemsPerDesc;
+	}
+
+	if(gridSize > 0x7fffffffULL)
+	{
+		elb_set_last_error("blake3_chunks: " + std::to_string(gridSize) + " CTAs are too many");
+		return -1;
+	}
+
+	elb_blake3_kernel<<<(unsigned)gridSize, ELB_B3_THREADS, 0, stream>>>(descs, shifts, numDescs,
+		chunkShift, slotsPerDesc, packShift, itemsPerDesc, (uint32_t*)devDigests,
+		(uint32_t*)hostDigests);
+	gNumKernelLaunches.fetch_add(1, std::memory_order_relaxed);
+
+	return checkLaunch("blake3");
 }
 
 /* query launch geometry of the current device now (so that no attribute/occupancy query happens

@@ -542,6 +542,7 @@ Manager::ChecksumReport Manager::getChecksumReport()
 	if(shared.cfg.checksumChunkShift)
 		return getChunkChecksumReport();
 
+	const bool isBlake3 = (shared.cfg.checksumAlgo == ELB_CHECKSUM_BLAKE3);
 	std::map<std::string, FileChecksum> files;
 
 	for(const std::unique_ptr<Worker>& worker : workers)
@@ -552,6 +553,9 @@ Manager::ChecksumReport Manager::getChecksumReport()
 			file.size = part.size;
 			file.numBytes += part.numBytes;
 			file.rawCrc ^= part.rawCrc;
+
+			if(isBlake3) // (blake3: the runs joined by the rule of the workers' maps)
+				file.blake3.merge(part.blake3, elb_blake3_num_chunks(part.size) );
 		}
 
 	ChecksumReport report;
@@ -560,8 +564,17 @@ Manager::ChecksumReport Manager::getChecksumReport()
 	{
 		const FileChecksum& file = entry.second;
 		std::string crcStr = "-";
+		uint32_t digest[8];
 
-		if(file.numBytes == file.size)
+		if(isBlake3)
+		{
+			if( (file.numBytes == file.size) && file.blake3.finish(file.size, digest) )
+			{
+				crcStr = elb_blake3_hex(digest);
+				report.numComplete++;
+			}
+		}
+		else if(file.numBytes == file.size)
 		{
 			crcStr = finishedCrcHex(shared.cfg.checksumAlgo, file.rawCrc, file.size);
 			report.numComplete++;
@@ -578,6 +591,9 @@ Manager::ChecksumReport Manager::getChecksumReport()
 /* --checksumchunk: one line per chunk that the last phase moved, sorted by path and offset */
 Manager::ChecksumReport Manager::getChunkChecksumReport()
 {
+	if(shared.cfg.checksumAlgo == ELB_CHECKSUM_BLAKE3)
+		return getChunkDigestReport();
+
 	std::map<std::string, std::vector<ChunkChecksum> > files;
 
 	for(const std::unique_ptr<Worker>& worker : workers)
@@ -600,6 +616,38 @@ Manager::ChecksumReport Manager::getChunkChecksumReport()
 			report.lines += entry.first + " " + std::to_string(chunk.offset) + " " +
 				std::to_string(chunk.length) + " " +
 				finishedCrcHex(shared.cfg.checksumAlgo, chunk.rawCrc, chunk.length) + "\n";
+
+		report.numChunks += chunks.size();
+		report.numFiles++;
+	}
+
+	return report;
+}
+
+/* getChunkChecksumReport of --checksumalgo blake3: the chunks' digests */
+Manager::ChecksumReport Manager::getChunkDigestReport()
+{
+	std::map<std::string, std::vector<ChunkDigest> > files;
+
+	for(const std::unique_ptr<Worker>& worker : workers)
+		for(const FileChecksum& part : worker->getFileChecksums() )
+		{
+			std::vector<ChunkDigest>& chunks = files[part.path];
+			chunks.insert(chunks.end(), part.chunkDigests.begin(), part.chunkDigests.end() );
+		}
+
+	ChecksumReport report;
+
+	for(auto& entry : files)
+	{
+		std::vector<ChunkDigest>& chunks = entry.second;
+
+		std::sort(chunks.begin(), chunks.end(),
+			[](const ChunkDigest& a, const ChunkDigest& b) { return a.offset < b.offset; } );
+
+		for(const ChunkDigest& chunk : chunks)
+			report.lines += entry.first + " " + std::to_string(chunk.offset) + " " +
+				std::to_string(chunk.length) + " " + elb_blake3_hex(chunk.digest) + "\n";
 
 		report.numChunks += chunks.size();
 		report.numFiles++;
@@ -666,7 +714,7 @@ std::shared_ptr<const ChecksumList> ChecksumList::parse(const std::string& text)
 			words >> extra;
 
 			const int algo = algoName.empty() ? ELB_CHECKSUM_CRC32 :
-				elb_crc_algo_by_name(algoName.c_str() );
+				elb_checksum_algo_by_name(algoName.c_str() );
 
 			if( ( (phase != "WRITE") && (phase != "READ") ) || !extra.empty() || (algo < 0) ||
 				( !chunkWord.empty() && !parseChecksumListNum(chunkSizeStr, chunkSize) ) )
@@ -701,14 +749,13 @@ std::shared_ptr<const ChecksumList> ChecksumList::parse(const std::string& text)
 		const size_t offBlank = (lenBlank && (lenBlank != std::string::npos) ) ?
 			line.rfind(' ', lenBlank - 1) : std::string::npos;
 
-		size_t numDigits = 0; // (the algorithm's width)
-		std::string lineFormat;
+		const bool isBlake3 = (section->algo == ELB_CHECKSUM_BLAKE3);
+		size_t numDigits = isBlake3 ? 2 * elb_blake3_algo::DIGEST_BYTES : 0; // (the width)
+		const std::string lineFormat = std::string("not \"path offset length ") +
+			elb_checksum_algo_name(section->algo) + "\"";
 
 		elb_with_crc_algo(section->algo, [&](auto algo)
-		{
-			numDigits = sizeof(typename decltype(algo)::word) * 2;
-			lineFormat = std::string("not \"path offset length ") + algo.NAME + "\"";
-		});
+			{ numDigits = sizeof(typename decltype(algo)::word) * 2; } );
 
 		const bool is64 = (numDigits == 16);
 
@@ -737,20 +784,39 @@ std::shared_ptr<const ChecksumList> ChecksumList::parse(const std::string& text)
 		if(chunkIdx >= file.present.size() )
 		{
 			file.present.resize(chunkIdx + 1);
-			file.crcs.resize(chunkIdx + 1);
+
+			if(isBlake3)
+				file.digests.resize(8 * (chunkIdx + 1) );
+			else
+				file.crcs.resize(chunkIdx + 1);
 
 			if(is64)
 				file.crcsHi.resize(chunkIdx + 1);
 		}
 
-		const uint64_t crc = std::stoull(crcStr, NULL, 16);
-
 		file.path = line.substr(0, offBlank);
 		file.present[chunkIdx] = true;
-		file.crcs[chunkIdx] = (uint32_t)crc;
 
-		if(is64)
-			file.crcsHi[chunkIdx] = (uint32_t)(crc >> 32);
+		if(isBlake3)
+		{ // 32 bytes: word k holds bytes 4k .. 4k + 3, little-endian
+			for(unsigned b = 0; b < elb_blake3_algo::DIGEST_BYTES; b++)
+			{
+				const uint32_t byte = (uint32_t)std::stoul(crcStr.substr(2 * b, 2), NULL, 16);
+				uint32_t& word = file.digests[8 * chunkIdx + b / 4];
+
+				word = (word & ~(0xffu << (8 * (b % 4) ) ) ) | (byte << (8 * (b % 4) ) );
+			}
+		}
+		else
+		{
+			const uint64_t crc = std::stoull(crcStr, NULL, 16);
+
+			file.crcs[chunkIdx] = (uint32_t)crc;
+
+			if(is64)
+				file.crcsHi[chunkIdx] = (uint32_t)(crc >> 32);
+		}
+
 		section->numChunks++;
 
 		if(length != chunkSize)
@@ -775,8 +841,8 @@ void Manager::setChecksumList(std::shared_ptr<const ChecksumList> list)
 
 	if( (configChecksumAlgo != ELB_CHECKSUM_CRC32) && (configChecksumAlgo != list->algo) )
 		throw WorkerError(std::string("The checksum algorithm (--checksumalgo ") +
-			elb_crc_algo_name(configChecksumAlgo) + ") differs from the checksum list's (" +
-			elb_crc_algo_name(list->algo) + ").");
+			elb_checksum_algo_name(configChecksumAlgo) + ") differs from the checksum list's (" +
+			elb_checksum_algo_name(list->algo) + ").");
 
 	checkChecksumChunks(cfg, list->chunkShift, "the checksum list's chunk size");
 

@@ -46,6 +46,8 @@
 #include <stdint.h>
 #include <string.h>
 
+#include <string>
+
 #if defined(__CUDACC__)
 #define ELB_HD __host__ __device__ __forceinline__
 #define ELB_HD_MEMBER __host__ __device__ __forceinline__
@@ -456,6 +458,253 @@ inline int elb_crc_algo_by_name(const char* name)
 			{ if(!strcmp(crcAlgo.NAME, name) ) found = algo; } );
 
 	return found;
+}
+
+/* ---- BLAKE3 (--checksumalgo blake3) -------------------------------------------------------------
+ *
+ * The default BLAKE3 hash with a 256-bit output (what b3sum prints). A message is cut into 1 KiB
+ * chunks; chunk c is hashed with counter t = c into a 32-byte chaining value (CV), and CVs are
+ * joined by parent compressions in a binary tree whose left subtree of m >= 2 chunks holds
+ * 2^floor(log2(m - 1)) chunks. Every aligned run of 2^j chunks inside the message (chunk index a
+ * multiple of 2^j) is a node of that tree, unless it is the whole message, so runs can be hashed
+ * anywhere, in any order, and joined later. The root is the one compression that takes ROOT: the
+ * top parent, or the last block of a single-chunk message; its first 32 output bytes are the
+ * digest. Everything here is host and device code: the kernel, the host merge and the C ABI share
+ * it. */
+
+#define ELB_BLAKE3_CHUNK_SHIFT 10 /* 1 KiB chunks */
+#define ELB_BLAKE3_CHUNK_START 1u
+#define ELB_BLAKE3_CHUNK_END 2u
+#define ELB_BLAKE3_PARENT 4u
+#define ELB_BLAKE3_ROOT 8u
+
+/* ID: enum elb_checksum_algo; NAME: --checksumalgo and the list headers; LABEL: messages */
+struct elb_blake3_algo
+{
+	static constexpr int ID = 3;
+	static constexpr const char* NAME = "blake3";
+	static constexpr const char* LABEL = "BLAKE3";
+	static constexpr unsigned DIGEST_BYTES = 32;
+};
+
+/* the name of checksum algorithm algo (enum elb_checksum_algo: a CRC or BLAKE3; "" for none) */
+inline const char* elb_checksum_algo_name(int algo)
+{
+	return (algo == elb_blake3_algo::ID) ? elb_blake3_algo::NAME : elb_crc_algo_name(algo);
+}
+
+/* the ID of the checksum algorithm called name (--checksumalgo, list headers), -1 if none is */
+inline int elb_checksum_algo_by_name(const char* name)
+{
+	return !strcmp(name, elb_blake3_algo::NAME) ? elb_blake3_algo::ID : elb_crc_algo_by_name(name);
+}
+
+#define ELB_BLAKE3_IV0 0x6A09E667u
+#define ELB_BLAKE3_IV1 0xBB67AE85u
+#define ELB_BLAKE3_IV2 0x3C6EF372u
+#define ELB_BLAKE3_IV3 0xA54FF53Au
+#define ELB_BLAKE3_IV4 0x510E527Fu
+#define ELB_BLAKE3_IV5 0x9B05688Cu
+#define ELB_BLAKE3_IV6 0x1F83D9ABu
+#define ELB_BLAKE3_IV7 0x5BE0CD19u
+
+/* (on the device: 16 and 8 are byte permutes (PRMT), 12 and 7 funnel shifts) */
+ELB_HD uint32_t elb_blake3_rotr16(uint32_t x)
+{
+#if defined(__CUDA_ARCH__)
+	return __byte_perm(x, 0, 0x1032);
+#else
+	return (x >> 16) | (x << 16);
+#endif
+}
+
+ELB_HD uint32_t elb_blake3_rotr8(uint32_t x)
+{
+#if defined(__CUDA_ARCH__)
+	return __byte_perm(x, 0, 0x0321);
+#else
+	return (x >> 8) | (x << 24);
+#endif
+}
+
+ELB_HD uint32_t elb_blake3_rotr12(uint32_t x)
+{
+#if defined(__CUDA_ARCH__)
+	return __funnelshift_r(x, x, 12);
+#else
+	return (x >> 12) | (x << 20);
+#endif
+}
+
+ELB_HD uint32_t elb_blake3_rotr7(uint32_t x)
+{
+#if defined(__CUDA_ARCH__)
+	return __funnelshift_r(x, x, 7);
+#else
+	return (x >> 7) | (x << 25);
+#endif
+}
+
+#define ELB_BLAKE3_G(a, b, c, d, mx, my) \
+	do { \
+		a = a + b + (mx); d = elb_blake3_rotr16(d ^ a); c = c + d; b = elb_blake3_rotr12(b ^ c); \
+		a = a + b + (my); d = elb_blake3_rotr8(d ^ a); c = c + d; b = elb_blake3_rotr7(b ^ c); \
+	} while(0)
+
+/* one round; s0..s15: the message schedule of the round (the permutation applied r times) */
+#define ELB_BLAKE3_ROUND(m, s0, s1, s2, s3, s4, s5, s6, s7, s8, s9, s10, s11, s12, s13, s14, s15) \
+	do { \
+		ELB_BLAKE3_G(v0, v4, v8, v12, m[s0], m[s1]); \
+		ELB_BLAKE3_G(v1, v5, v9, v13, m[s2], m[s3]); \
+		ELB_BLAKE3_G(v2, v6, v10, v14, m[s4], m[s5]); \
+		ELB_BLAKE3_G(v3, v7, v11, v15, m[s6], m[s7]); \
+		ELB_BLAKE3_G(v0, v5, v10, v15, m[s8], m[s9]); \
+		ELB_BLAKE3_G(v1, v6, v11, v12, m[s10], m[s11]); \
+		ELB_BLAKE3_G(v2, v7, v8, v13, m[s12], m[s13]); \
+		ELB_BLAKE3_G(v3, v4, v9, v14, m[s14], m[s15]); \
+	} while(0)
+
+/* cv <- the first 8 output words of compressing the 16 message words m (little-endian) into cv,
+   with the 64-bit counter t, blockLen bytes and flags */
+ELB_HD void elb_blake3_compress(uint32_t cv[8], const uint32_t m[16], uint64_t t, uint32_t blockLen,
+	uint32_t flags)
+{
+	uint32_t v0 = cv[0], v1 = cv[1], v2 = cv[2], v3 = cv[3];
+	uint32_t v4 = cv[4], v5 = cv[5], v6 = cv[6], v7 = cv[7];
+	uint32_t v8 = ELB_BLAKE3_IV0, v9 = ELB_BLAKE3_IV1, v10 = ELB_BLAKE3_IV2, v11 = ELB_BLAKE3_IV3;
+	uint32_t v12 = (uint32_t)t, v13 = (uint32_t)(t >> 32), v14 = blockLen, v15 = flags;
+
+	ELB_BLAKE3_ROUND(m, 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15);
+	ELB_BLAKE3_ROUND(m, 2, 6, 3, 10, 7, 0, 4, 13, 1, 11, 12, 5, 9, 14, 15, 8);
+	ELB_BLAKE3_ROUND(m, 3, 4, 10, 12, 13, 2, 7, 14, 6, 5, 9, 0, 11, 15, 8, 1);
+	ELB_BLAKE3_ROUND(m, 10, 7, 12, 9, 14, 3, 13, 15, 4, 0, 11, 2, 5, 8, 1, 6);
+	ELB_BLAKE3_ROUND(m, 12, 13, 9, 11, 15, 10, 14, 8, 7, 2, 5, 3, 0, 1, 6, 4);
+	ELB_BLAKE3_ROUND(m, 9, 14, 11, 5, 8, 12, 15, 1, 13, 3, 0, 10, 2, 6, 4, 7);
+	ELB_BLAKE3_ROUND(m, 11, 15, 5, 0, 1, 9, 8, 6, 14, 10, 2, 12, 3, 4, 7, 13);
+
+	cv[0] = v0 ^ v8; cv[1] = v1 ^ v9; cv[2] = v2 ^ v10; cv[3] = v3 ^ v11;
+	cv[4] = v4 ^ v12; cv[5] = v5 ^ v13; cv[6] = v6 ^ v14; cv[7] = v7 ^ v15;
+}
+
+#undef ELB_BLAKE3_ROUND
+#undef ELB_BLAKE3_G
+
+ELB_HD void elb_blake3_iv(uint32_t cv[8])
+{
+	cv[0] = ELB_BLAKE3_IV0; cv[1] = ELB_BLAKE3_IV1; cv[2] = ELB_BLAKE3_IV2; cv[3] = ELB_BLAKE3_IV3;
+	cv[4] = ELB_BLAKE3_IV4; cv[5] = ELB_BLAKE3_IV5; cv[6] = ELB_BLAKE3_IV6; cv[7] = ELB_BLAKE3_IV7;
+}
+
+/* out <- the parent of left and right (with ROOT: the digest of the message they cover) */
+ELB_HD void elb_blake3_parent_cv(const uint32_t left[8], const uint32_t right[8], bool root,
+	uint32_t out[8])
+{
+	uint32_t m[16];
+
+	for(int i = 0; i < 8; i++)
+	{
+		m[i] = left[i];
+		m[i + 8] = right[i];
+	}
+
+	elb_blake3_iv(out);
+	elb_blake3_compress(out, m, 0, 64, ELB_BLAKE3_PARENT | (root ? ELB_BLAKE3_ROOT : 0) );
+}
+
+/* the CV of the chunk with counter t that holds the len <= 1024 bytes at data (host code; the
+   kernel loads its chunks itself); root: the chunk is the whole message, out is its digest */
+inline void elb_blake3_chunk_cv(const uint8_t* data, uint32_t len, uint64_t t, bool root,
+	uint32_t out[8])
+{
+	const uint32_t numBlocks = len ? (len + 63) / 64 : 1;
+
+	elb_blake3_iv(out);
+
+	for(uint32_t b = 0; b < numBlocks; b++)
+	{
+		const uint32_t blockLen = (b + 1 < numBlocks) ? 64 : (len - b * 64);
+		uint8_t bytes[64] = {};
+		uint32_t m[16];
+
+		memcpy(bytes, data + b * 64, blockLen);
+
+		for(int i = 0; i < 16; i++)
+			m[i] = (uint32_t)bytes[4 * i] | ( (uint32_t)bytes[4 * i + 1] << 8) |
+				( (uint32_t)bytes[4 * i + 2] << 16) | ( (uint32_t)bytes[4 * i + 3] << 24);
+
+		uint32_t flags = (b ? 0 : ELB_BLAKE3_CHUNK_START);
+
+		if(b + 1 == numBlocks)
+			flags |= ELB_BLAKE3_CHUNK_END | (root ? ELB_BLAKE3_ROOT : 0);
+
+		elb_blake3_compress(out, m, t, blockLen, flags);
+	}
+}
+
+/* log2 of the size in chunks of the largest aligned run that starts at chunk pos and ends at or
+   before chunk end (pos < end): the next run of the canonical cut of [pos, end) */
+ELB_HD unsigned elb_blake3_run_shift(uint64_t pos, uint64_t end)
+{
+	unsigned shift = 0;
+
+	while( (shift < 62) && !(pos & ( (2ULL << shift) - 1) ) && (pos + (2ULL << shift) <= end) )
+		shift++;
+
+	return shift;
+}
+
+/* the number of runs of the canonical cut of the chunks [begin, end): the maximal aligned runs,
+   left to right */
+ELB_HD uint64_t elb_blake3_num_runs(uint64_t begin, uint64_t end)
+{
+	uint64_t numRuns = 0;
+
+	for(uint64_t pos = begin; pos < end; numRuns++)
+		pos += 1ULL << elb_blake3_run_shift(pos, end);
+
+	return numRuns;
+}
+
+/* the chunks of a message of size bytes (0 bytes: one empty chunk) */
+ELB_HD uint64_t elb_blake3_num_chunks(uint64_t size)
+{
+	return size ? ( (size + 1023) >> ELB_BLAKE3_CHUNK_SHIFT) : 1;
+}
+
+/* the digest of a message of numChunks >= 2 chunks from the CVs of the runs of its fold cut (the
+   canonical cut of [0, numChunks), except that a power of two takes its two halves), in order:
+   joined from the right, the last join with ROOT. Returns false if numRuns does not fit. */
+inline bool elb_blake3_fold_cvs(const uint32_t (*runs)[8], uint64_t numRuns, uint64_t numChunks,
+	uint32_t out[8])
+{
+	const bool isPow2 = !(numChunks & (numChunks - 1) );
+	const uint64_t expected = isPow2 ? 2 : (uint64_t)__builtin_popcountll(numChunks);
+
+	if( (numChunks < 2) || (numRuns != expected) )
+		return false;
+
+	memcpy(out, runs[numRuns - 1], 32);
+
+	for(uint64_t i = numRuns - 1; i-- > 0; )
+		elb_blake3_parent_cv(runs[i], out, !i, out);
+
+	return true;
+}
+
+/* a digest (8 little-endian words) as the 64 lowercase hex digits of its 32 bytes */
+inline std::string elb_blake3_hex(const uint32_t digest[8])
+{
+	static const char digits[] = "0123456789abcdef";
+	std::string hex(64, '0');
+
+	for(int i = 0; i < 32; i++)
+	{
+		const uint8_t byte = (uint8_t)(digest[i / 4] >> (8 * (i % 4) ) );
+		hex[2 * i] = digits[byte >> 4];
+		hex[2 * i + 1] = digits[byte & 15];
+	}
+
+	return hex;
 }
 
 #endif /* ELB_PATTERNS_CUH_ */

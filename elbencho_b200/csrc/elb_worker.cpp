@@ -829,12 +829,23 @@ void Worker::setupChecksums()
 {
 	const bool readChecksum = cfg.checksums || shared->checksumList;
 	const unsigned chunkShift = cfg.checksumChunkShift ? cfg.checksumChunkShift : 64;
-	const uint64_t slotsPerDesc = (chunkShift == 64) ? 1 :
+	uint64_t slotsPerDesc = (chunkShift == 64) ? 1 :
 		std::max( (cfg.blockSize + ( (uint64_t)1 << chunkShift) - 1) >> chunkShift, (uint64_t)1);
 	size_t wordBytes = 0;
 
-	elb_with_crc_algo(cfg.checksumAlgo, [&](auto algo)
-		{ wordBytes = sizeof(typename decltype(algo)::word); } );
+	if(cfg.checksumAlgo == ELB_CHECKSUM_BLAKE3)
+	{ // a digest or CV per slot; whole files: the runs of a block of m chunks, 2 log2(m) + 1 at most
+		wordBytes = elb_blake3_algo::DIGEST_BYTES;
+
+		if(chunkShift == 64)
+		{
+			const uint64_t numChunks = elb_blake3_num_chunks(cfg.blockSize);
+			slotsPerDesc = 2 * (63 - __builtin_clzll(numChunks) ) + 1;
+		}
+	}
+	else
+		elb_with_crc_algo(cfg.checksumAlgo, [&](auto algo)
+			{ wordBytes = sizeof(typename decltype(algo)::word); } );
 
 	if(batches.empty() || ( (readChecksum == readStage.checksum) &&
 		(chunkShift == crcChunkShift) && (slotsPerDesc == crcSlotsPerDesc) &&
@@ -2224,6 +2235,13 @@ uint32_t Worker::fillStageDescs(Batch& batch, const GpuStage& stage, uint64_t& o
 		if(!stage.isRead && block.ioIsRead)
 			continue;
 
+		if(stage.checksum && (crcAlgo == ELB_CHECKSUM_BLAKE3) && ( (block.offset & 1023) ||
+			( ( (block.offset + block.len) & 1023) &&
+			(block.offset + block.len != blockFileSize(block) ) ) ) )
+			throw WorkerError("BLAKE3 checksums need blocks on 1 KiB boundaries. File: " +
+				blockFilePath(block) + "; Offset: " + std::to_string(block.offset) + "; Length: " +
+				std::to_string(block.len) );
+
 		if(stage.checksum && (crcChunkShift == 64) )
 			batch.hostShifts[numDescs] = blockFileSize(block) - block.offset - block.len;
 		else if(stage.checksum && (block.offset & ( ( (uint64_t)1 << crcChunkShift) - 1) ) )
@@ -2423,9 +2441,11 @@ void Worker::enqueueStage(Batch& batch, const GpuStage& stage, uint32_t numBlock
 	}
 
 	// (a write's checksum reads the device slot before its stage-out copy)
-	if(stage.checksum && elb_launch_crc(crcAlgo, batch.hostDescs, batch.hostShifts, numBlocks,
-		crcChunkShift, crcSlotsPerDesc, batch.devCrcs, batch.hostCrcs, batch.devDoneTicket,
-		batch.stream) )
+	if(stage.checksum && ( (crcAlgo == ELB_CHECKSUM_BLAKE3) ?
+		elb_launch_blake3(batch.hostDescs, batch.hostShifts, numBlocks, crcChunkShift,
+		crcSlotsPerDesc, batch.devCrcs, batch.hostCrcs, batch.stream) :
+		elb_launch_crc(crcAlgo, batch.hostDescs, batch.hostShifts, numBlocks, crcChunkShift,
+		crcSlotsPerDesc, batch.devCrcs, batch.hostCrcs, batch.devDoneTicket, batch.stream) ) )
 		throw WorkerError(std::string("GPU checksum failed. ") + elb_last_error() );
 
 	if( (stage.transfer == GpuStage::TRANSFER_COPY) && !stage.isRead)
@@ -2720,6 +2740,12 @@ void Worker::addBatchChecksums(const Batch& batch)
 	if(!cfg.checksums)
 		return;
 
+	if(crcAlgo == ELB_CHECKSUM_BLAKE3)
+	{
+		addBatchDigests(batch);
+		return;
+	}
+
 	for(size_t i = 0; i < batch.blocks.size(); i++)
 	{
 		const BlockRef& block = batch.blocks[i];
@@ -2744,6 +2770,150 @@ void Worker::addBatchChecksums(const Batch& batch)
 	}
 }
 
+/* --checksums --checksumalgo blake3: the slots of a batch whose blocks are done into the
+ * accumulator of each block's file: whole files, the block's runs (elb_blake3_chunks) into the
+ * file's run map, or its digest when the block is the whole file; chunks, one entry per chunk */
+void Worker::addBatchDigests(const Batch& batch)
+{
+	const uint32_t (*slots)[8] = (const uint32_t (*)[8])batch.hostCrcs;
+
+	for(size_t i = 0; i < batch.blocks.size(); i++)
+	{
+		const BlockRef& block = batch.blocks[i];
+		const uint64_t blockEnd = block.offset + block.len;
+		const uint64_t fileSize = blockFileSize(block);
+		ChecksumAcc& acc = checksumAccs.try_emplace(blockFileID(block), ChecksumAcc{block}).first->
+			second;
+
+		acc.numBytes += block.len;
+
+		if(crcChunkShift < 64)
+		{
+			const uint64_t chunkSize = (uint64_t)1 << crcChunkShift;
+
+			for(uint64_t pos = block.offset, slot = i * crcSlotsPerDesc; pos < blockEnd;
+				pos += chunkSize, slot++)
+			{
+				ChunkDigest chunk{pos, std::min(chunkSize, blockEnd - pos), {} };
+				memcpy(chunk.digest, slots[slot], sizeof(chunk.digest) );
+				acc.chunkDigests.push_back(chunk);
+			}
+
+			continue;
+		}
+
+		if(!block.offset && (blockEnd == fileSize) )
+		{
+			acc.blake3.addDigest(slots[i * crcSlotsPerDesc]);
+			continue;
+		}
+
+		const uint64_t first = block.offset >> ELB_BLAKE3_CHUNK_SHIFT;
+		const uint64_t end = (blockEnd + 1023) >> ELB_BLAKE3_CHUNK_SHIFT;
+		uint64_t slot = i * crcSlotsPerDesc;
+
+		for(uint64_t pos = first; pos < end; slot++)
+		{
+			const uint64_t numChunks = 1ULL << elb_blake3_run_shift(pos, end);
+
+			acc.blake3.add(pos, numChunks, slots[slot], elb_blake3_num_chunks(fileSize) );
+			pos += numChunks;
+		}
+	}
+}
+
+void Blake3Runs::add(uint64_t firstChunk, uint64_t numChunks, const uint32_t cv[8],
+	uint64_t fileChunks)
+{
+	if(isBroken)
+		return;
+
+	auto next = runs.lower_bound(firstChunk);
+
+	if(hasDigest || ( (next != runs.end() ) && (next->first < firstChunk + numChunks) ) ||
+		( (next != runs.begin() ) && (std::prev(next)->first + std::prev(next)->second.numChunks >
+		firstChunk) ) )
+	{ // a run that this phase hashed before: the file is not covered exactly once
+		isBroken = true;
+		runs.clear();
+		return;
+	}
+
+	Run run{numChunks, {} };
+	memcpy(run.cv, cv, sizeof(run.cv) );
+
+	for( ; ; )
+	{ // join with the aligned sibling while it is held, unless that makes the whole file
+		const bool isLeft = !(firstChunk & ( (run.numChunks << 1) - 1) );
+		const uint64_t siblingFirst = isLeft ? (firstChunk + run.numChunks) :
+			(firstChunk - run.numChunks);
+		const auto sibling = runs.find(siblingFirst);
+
+		if( (sibling == runs.end() ) || (sibling->second.numChunks != run.numChunks) ||
+			( (std::min(firstChunk, siblingFirst) == 0) && (2 * run.numChunks == fileChunks) ) )
+			break;
+
+		if(isLeft)
+			elb_blake3_parent_cv(run.cv, sibling->second.cv, false, run.cv);
+		else
+			elb_blake3_parent_cv(sibling->second.cv, run.cv, false, run.cv);
+
+		runs.erase(sibling);
+		firstChunk = std::min(firstChunk, siblingFirst);
+		run.numChunks *= 2;
+	}
+
+	runs.emplace(firstChunk, run);
+}
+
+void Blake3Runs::addDigest(const uint32_t fileDigest[8])
+{
+	if(hasDigest || !runs.empty() )
+		isBroken = true;
+
+	hasDigest = true;
+	memcpy(digest, fileDigest, sizeof(digest) );
+}
+
+void Blake3Runs::merge(const Blake3Runs& other, uint64_t fileChunks)
+{
+	if(other.isBroken)
+		isBroken = true;
+
+	if(other.hasDigest)
+		addDigest(other.digest);
+
+	for(const auto& entry : other.runs)
+		add(entry.first, entry.second.numChunks, entry.second.cv, fileChunks);
+}
+
+bool Blake3Runs::finish(uint64_t fileSize, uint32_t outDigest[8]) const
+{
+	if(isBroken)
+		return false;
+
+	if(hasDigest)
+	{
+		memcpy(outDigest, digest, sizeof(digest) );
+		return true;
+	}
+
+	std::vector<uint32_t> cvs;
+	uint64_t pos = 0;
+
+	for(const auto& entry : runs)
+	{ // (contiguous from chunk 0)
+		if(entry.first != pos)
+			return false;
+
+		cvs.insert(cvs.end(), entry.second.cv, entry.second.cv + 8);
+		pos += entry.second.numChunks;
+	}
+
+	return (pos == elb_blake3_num_chunks(fileSize) ) && elb_blake3_fold_cvs(
+		(const uint32_t (*)[8])cvs.data(), runs.size(), pos, outDigest);
+}
+
 /**
  * --checksumverify: compare the CRC of each chunk of a read batch with the list line of its file
  * and offset (blocks start at chunk boundaries, fillStageDescs). The file's list entry is looked up
@@ -2755,6 +2925,12 @@ void Worker::checkBatchChecksums(const Batch& batch)
 
 	if(!list || !readStage.checksum || (benchPhase != ELB_PHASE_READFILES) )
 		return;
+
+	if(crcAlgo == ELB_CHECKSUM_BLAKE3)
+	{
+		checkBatchDigests(batch);
+		return;
+	}
 
 	elb_with_crc_algo(crcAlgo, [&](auto algo)
 	{
@@ -2810,6 +2986,50 @@ void Worker::checkBatchChecksums(const Batch& batch)
 	});
 }
 
+/* --checksumverify with a blake3 list: checkBatchChecksums with 32-byte digests */
+void Worker::checkBatchDigests(const Batch& batch)
+{
+	const ChecksumList* list = shared->checksumList.get();
+	const uint32_t (*slots)[8] = (const uint32_t (*)[8])batch.hostCrcs;
+	const uint64_t chunkSize = (uint64_t)1 << crcChunkShift;
+
+	for(size_t i = 0; i < batch.blocks.size(); i++)
+	{
+		const BlockRef& block = batch.blocks[i];
+		const uint64_t blockEnd = block.offset + block.len;
+		auto fileIter = checksumListFiles.find(blockFileID(block) );
+
+		if(fileIter == checksumListFiles.end() )
+			fileIter = checksumListFiles.emplace(blockFileID(block),
+				list->findFile(blockFilePath(block) ) ).first;
+
+		const ChecksumList::File* file = fileIter->second;
+
+		for(uint64_t pos = block.offset, slot = i * crcSlotsPerDesc; pos < blockEnd;
+			pos += chunkSize, slot++)
+		{
+			const uint64_t len = std::min(chunkSize, blockEnd - pos);
+			const uint64_t chunkIdx = pos >> crcChunkShift;
+			const bool hasLine = file && file->hasLine(chunkIdx);
+
+			if(hasLine && (file->chunkLength(chunkIdx, chunkSize) == len) &&
+				!memcmp(&file->digests[chunkIdx * 8], slots[slot], elb_blake3_algo::DIGEST_BYTES) )
+			{
+				numChecksumChunksChecked++;
+				continue;
+			}
+
+			const std::string expected = hasLine ?
+				elb_blake3_hex(&file->digests[chunkIdx * 8]) : std::string("-");
+
+			throw WorkerError("Checksum verification failed. File: " + blockFilePath(block) +
+				"; Offset: " + std::to_string(pos) + "; Length: " + std::to_string(len) + "; "
+				"Expected " + elb_blake3_algo::LABEL + ": " + expected + "; Actual " +
+				elb_blake3_algo::LABEL + ": " + elb_blake3_hex(slots[slot]) );
+		}
+	}
+}
+
 /* --checksumverify: the paths of the files this worker checked in the phase */
 std::vector<std::string> Worker::getChecksumVerifiedFiles() const
 {
@@ -2835,7 +3055,7 @@ std::vector<FileChecksum> Worker::getFileChecksums() const
 	for(const auto& entry : checksumAccs)
 		checksums.push_back(FileChecksum{blockFilePath(entry.second.block),
 			blockFileSize(entry.second.block), entry.second.numBytes, entry.second.rawCrc,
-			entry.second.chunks});
+			entry.second.chunks, entry.second.blake3, entry.second.chunkDigests});
 
 	return checksums;
 }

@@ -130,6 +130,41 @@ struct ChunkChecksum
 	uint64_t rawCrc; // (elb_crc_chunks)
 };
 
+/* --checksumchunk --checksumalgo blake3: the digest of one chunk of a file that a phase moved */
+struct ChunkDigest
+{
+	uint64_t offset;
+	uint64_t length;
+	uint32_t digest[8];
+};
+
+/**
+ * --checksums --checksumalgo blake3, whole files: the runs of a file's 1 KiB chunks that a phase
+ * hashed (elb_blake3_chunks), by first chunk. A run is joined with its aligned sibling as soon as
+ * both are held, unless they make the whole file, so a sequential reader holds O(log n) runs. A
+ * run that arrives twice or overlaps a held one breaks the file (no digest). The kernel's digest of
+ * a block that is the whole file is held as such.
+ */
+struct Blake3Runs
+{
+	struct Run
+	{
+		uint64_t numChunks;
+		uint32_t cv[8];
+	};
+
+	std::map<uint64_t, Run> runs;
+	bool isBroken{false};
+	bool hasDigest{false};
+	uint32_t digest[8]{};
+
+	void add(uint64_t firstChunk, uint64_t numChunks, const uint32_t cv[8], uint64_t fileChunks);
+	void addDigest(const uint32_t fileDigest[8]);
+	void merge(const Blake3Runs& other, uint64_t fileChunks);
+	// the file's digest, if the runs make the file of fileSize bytes
+	bool finish(uint64_t fileSize, uint32_t outDigest[8]) const;
+};
+
 /* --checksums: what a worker moved of one file in a phase */
 struct FileChecksum
 {
@@ -138,13 +173,15 @@ struct FileChecksum
 	uint64_t numBytes{0}; // bytes of the blocks the phase moved
 	uint64_t rawCrc{0};   // XOR of the blocks' contributions (elb_crc_chunks)
 	std::vector<ChunkChecksum> chunks; // --checksumchunk: the chunks instead, in the order moved
+	Blake3Runs blake3;                 // blake3: the runs instead of rawCrc
+	std::vector<ChunkDigest> chunkDigests; // blake3 --checksumchunk: instead of chunks
 };
 
 /**
  * --checksumverify: the last section with a chunk size of a checksum list that --checksums
  * --checksumchunk wrote: "# phase WRITE|READ chunk <K> [algorithm]", then lines "path offset
- * length crc". One CRC (4 bytes, 8 for 64-bit algorithms) and one bit per chunk of each listed
- * file; lines shorter than K (a file's last chunk) keep their length aside.
+ * length crc". One CRC (4 bytes, 8 for 64-bit algorithms; a BLAKE3 digest: 32) and one bit per
+ * chunk of each listed file; lines shorter than K (a file's last chunk) keep their length aside.
  */
 struct ChecksumList
 {
@@ -153,6 +190,7 @@ struct ChecksumList
 		std::string path;
 		std::vector<uint32_t> crcs;   // the CRC by chunk index (64-bit algorithms: the low half)
 		std::vector<uint32_t> crcsHi; // 64-bit algorithms: the high half, else empty
+		std::vector<uint32_t> digests; // blake3: 8 words per chunk index instead of crcs
 		std::vector<bool> present;    // whether the chunk has a line
 
 		uint64_t crc(uint64_t chunkIdx) const
@@ -169,7 +207,7 @@ struct ChecksumList
 	};
 
 	unsigned chunkShift{0};
-	int algo{ELB_CHECKSUM_CRC32}; // elb_crc_algo::ID
+	int algo{ELB_CHECKSUM_CRC32}; // enum elb_checksum_algo
 	uint64_t numChunks{0};
 	std::map<std::string, File> files;
 
@@ -417,12 +455,14 @@ class Worker
 			uint64_t numBytes{0};
 			uint64_t rawCrc{0};
 			std::vector<ChunkChecksum> chunks; // --checksumchunk
+			Blake3Runs blake3;                 // blake3: instead of rawCrc
+			std::vector<ChunkDigest> chunkDigests; // blake3 --checksumchunk: instead of chunks
 		};
 		std::map<FileID, ChecksumAcc> checksumAccs;
 		unsigned crcChunkShift{64};    // the CRC launch's chunks (64: whole files), setupChecksums
 		uint64_t crcSlotsPerDesc{1};   // CRC slots per block
-		int crcAlgo{ELB_CHECKSUM_CRC32}; // the CRC launch's algorithm (elb_crc_algo::ID)
-		size_t crcWordBytes{4};          // bytes of a CRC slot
+		int crcAlgo{ELB_CHECKSUM_CRC32}; // the launch's algorithm (enum elb_checksum_algo)
+		size_t crcWordBytes{4};          // bytes of a slot (blake3: a 32-byte digest or CV)
 		/* --checksumverify: the list entry of each file the phase read (NULL: not listed) and the
 		   chunks that matched */
 		std::map<FileID, const ChecksumList::File*> checksumListFiles;
@@ -468,7 +508,9 @@ class Worker
 		void accountBatch(Batch& batch, uint64_t gpuUSecTotal);
 		uint64_t batchCrc(const Batch& batch, uint64_t slot) const;
 		void addBatchChecksums(const Batch& batch);
+		void addBatchDigests(const Batch& batch);
 		void checkBatchChecksums(const Batch& batch);
+		void checkBatchDigests(const Batch& batch);
 		void setupChecksums();
 		FileID blockFileID(const BlockRef& block) const;
 		uint64_t blockFileSize(const BlockRef& block) const;
@@ -552,6 +594,7 @@ class Manager
 		};
 		ChecksumReport getChecksumReport();
 		ChecksumReport getChunkChecksumReport();
+		ChecksumReport getChunkDigestReport();
 
 		/* --checksumverify: parse a checksum list and check the following read phases against
 		   it (throws WorkerError); the chunks and files the last phase checked */

@@ -12,8 +12,9 @@ from ._native import CONTENT_PATTERN, CONTENT_RANDOM, CONTENT_RANDOM_GRAIN  # no
 
 RANDALGO_SPLITMIX64 = 0
 
-# elb_checksum_algo by --checksumalgo name; crc64nvme slots are uint64, the others uint32
-CHECKSUM_ALGOS = {"crc32": 0, "crc32c": 1, "crc64nvme": 2}
+# elb_checksum_algo by --checksumalgo name; crc64nvme slots are uint64, the others uint32 (blake3
+# has entries of its own: blake3_chunks, blake3_parent, blake3_fold)
+CHECKSUM_ALGOS = {"crc32": 0, "crc32c": 1, "crc64nvme": 2, "blake3": 3}
 
 VERIFY_PATTERN = 0  # elb_verify_kind
 VERIFY_RANDOM = 1
@@ -387,3 +388,37 @@ def pack_block_descs(blocks):
         arr[i].fileOffset = off
         arr[i].blockCounter = ctr
     return bytes(arr)
+
+
+def blake3_chunks(pinned_descs_ptr, pinned_shifts_ptr, num_descs, chunk_shift, slots_per_desc,
+                  dev_digests_ptr, pinned_digests_ptr=0, dev_ticket_ptr=0, stream=0):
+    """BLAKE3 digests on the GPU, 32 bytes per slot (slot j of descriptor i at byte
+    32 * (i * slots_per_desc + j)). chunk_shift 64: the chaining values of the maximal aligned runs
+    of 1 KiB chunks of each block, left to right (the file's digest in slot 0 when the descriptor
+    is the whole file: offset 0 and shift 0), which blake3_parent and blake3_fold join;
+    chunk_shift 12..40: the digest of each chunk of 2**chunk_shift bytes of the block, each a
+    message of its own (pinned_shifts_ptr may then be 0). Descriptors must lie on 1 KiB (chunked:
+    chunk) boundaries, except at their file's end."""
+    _check(_native.load().elb_blake3_chunks(pinned_descs_ptr, pinned_shifts_ptr or None,
+                                            num_descs, chunk_shift, slots_per_desc,
+                                            dev_digests_ptr, pinned_digests_ptr or None,
+                                            dev_ticket_ptr or None, stream),
+           "elb_blake3_chunks")
+
+
+def blake3_parent(left, right, root=False):
+    """the BLAKE3 parent of two 32-byte chaining values (root: the digest of their message)"""
+    out = ctypes.create_string_buffer(32)
+    _native.load().elb_blake3_parent(bytes(left), bytes(right), int(bool(root)), out)
+    return out.raw
+
+
+def blake3_fold(runs, file_size):
+    """the BLAKE3 digest of a file of file_size bytes (more than 1 KiB) from the 32-byte chaining
+    values of its runs: the maximal aligned runs of its 1 KiB chunks, left to right, or the two
+    halves when the chunk count is a power of two"""
+    runs = [bytes(run) for run in runs]
+    out = ctypes.create_string_buffer(32)
+    _check(_native.load().elb_blake3_fold(b"".join(runs), len(runs), file_size, out),
+           "elb_blake3_fold")
+    return out.raw

@@ -116,7 +116,7 @@ class WorkerConfig:
     verify_report: bool = False       # --verifyreport: map bad blocks' damage, fail at phase end
     checksums: bool = False           # --checksums: each file's CRC per phase (checksums())
     checksum_chunk_shift: int = 0     # --checksumchunk: CRCs of 2**shift byte chunks (0: files)
-    checksum_algo: str = "crc32"      # --checksumalgo: "crc32", "crc32c" or "crc64nvme"
+    checksum_algo: str = "crc32"      # --checksumalgo: "crc32", "crc32c", "crc64nvme" or "blake3"
     serialize_buffered_writes: int = 0  # 0 auto, 1 on, 2 off (--writegate)
     staging_engine: int = 0           # 0 auto, 1 kernels move the data, 2 cudaMemcpyAsync
     no_gpu_numa_binding: bool = False  # --nogpunuma
@@ -439,7 +439,9 @@ class WorkerManager:
         """The last phase's files, merged over all workers and sorted by path:
         [(path, size, bytes_covered, crc32)], crc32 an int (zlib.crc32 of the file's first size
         bytes) or None if the phase did not cover them exactly once. With checksum_chunk_shift:
-        [(path, offset, length, crc32)] per chunk, sorted by path and offset."""
+        [(path, offset, length, crc32)] per chunk, sorted by path and offset. Other algorithms
+        give their CRC or digest as the int of its hex digits (blake3: "%064x" % value is the
+        digest as b3sum prints it)."""
         files = []
         for line in self.checksums_text().splitlines():
             path, size, covered, crc = line.rsplit(" ", 3)

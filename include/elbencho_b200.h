@@ -332,6 +332,30 @@ int elb_crc_chunks(int32_t algo, const elb_block_desc* descs, const uint64_t* sh
 uint64_t elb_crc_shift(int32_t algo, uint64_t crc, uint64_t n);
 uint64_t elb_crc_finish(int32_t algo, uint64_t rawCrc, uint64_t size);
 
+/* BLAKE3 digests (--checksumalgo blake3; the default 256-bit hash, as b3sum prints it). Slots are
+ * 32 bytes, slot j of descriptor i at devDigests + 32 * (i * slotsPerDesc + j).
+ * chunkShift 64 (whole files): with shifts[i] = the bytes from the block's end to its file's end,
+ * the slots take the chaining values of the maximal aligned runs of 1 KiB chunks of the block (file
+ * chunk c0 .. c1: the largest aligned power of two first, left to right), the subtrees of the
+ * file's BLAKE3 tree; a descriptor that is the whole file (offset 0, shift 0) takes the file's
+ * digest in slot 0 instead. elb_blake3_parent and elb_blake3_fold join runs into a file's digest.
+ * chunkShift 12..40: each chunk of 2^chunkShift bytes is a message of its own, and slot j takes
+ * the digest of the block's j-th chunk (shifts may be NULL). Descriptors must start on a 1 KiB
+ * (chunked: chunk) boundary and end on one or at their file's end; the call fails without
+ * launching otherwise, or if a descriptor needs more than slotsPerDesc slots. With hostDigests
+ * (pinned host memory), every slot the launch writes is also written there by the device; the host
+ * reads it after the stream's work is done. devTicket goes with hostDigests as in elb_crc_chunks
+ * and stays 0: the slots are final where they are made, so no last CTA joins or copies them. */
+int elb_blake3_chunks(const elb_block_desc* descs, const uint64_t* shifts, uint32_t numDescs,
+	unsigned chunkShift, uint64_t slotsPerDesc, void* devDigests, void* hostDigests,
+	unsigned* devTicket, void* stream);
+/* out <- the BLAKE3 parent of the 32-byte chaining values left and right (root: the digest) */
+void elb_blake3_parent(const uint8_t* left, const uint8_t* right, int root, uint8_t* out);
+/* out <- the BLAKE3 digest of a file of fileSize bytes (more than 1 KiB) from the 32-byte
+ * chaining values of its numRuns runs: the maximal aligned runs of its chunks, left to right, but
+ * the two halves when the chunk count is a power of two. Returns -1 if they do not fit. */
+int elb_blake3_fold(const uint8_t* runs, uint64_t numRuns, uint64_t fileSize, uint8_t* out);
+
 int elb_stage_copy(const elb_block_desc* descs, uint32_t numDescs, int hostToDevice,
 	int64_t hostDelta, uint64_t totalBytes, uint64_t maxBlockLen, void* stream);
 /* devResults[0..numDescs) <- {0, ~0} */
@@ -540,6 +564,7 @@ enum elb_checksum_algo
 	ELB_CHECKSUM_CRC32 = 0,     /* zlib, gzip, zip: polynomial 0xEDB88320, 32 bits */
 	ELB_CHECKSUM_CRC32C = 1,    /* Castagnoli (iSCSI, GCS, btrfs): 0x82F63B78, 32 bits */
 	ELB_CHECKSUM_CRC64NVME = 2, /* NVMe protection information guard: 0x9A6C9329AC4BC9B5, 64 bits */
+	ELB_CHECKSUM_BLAKE3 = 3,    /* BLAKE3-256 (b3sum), a tree hash over 1 KiB chunks */
 };
 
 /* elb_cfg::serializeBufferedWrites values */

@@ -1,11 +1,13 @@
 """Measure --checksumalgo on the GPU (one JSON line per measurement, each with the card's name, power
 limit and SM clock limit):
 
-1. the pinned host-to-device copy rate, and the CRC kernel of each algorithm (crc32, crc32c,
-   crc64nvme) over a 4 GiB resident window of 1 MiB and of 4 KiB blocks at K = 4 KiB / 64 KiB /
-   1 MiB (1 MiB blocks only) and whole files (CUDA events, median of the runs);
+1. the pinned host-to-device copy rate, and the checksum kernel of each algorithm (crc32, crc32c,
+   crc64nvme, blake3) over a 4 GiB resident window of 1 MiB and of 4 KiB blocks at K = 4 KiB /
+   64 KiB / 1 MiB (1 MiB blocks only) and whole files (CUDA events, median of the runs);
 2. sequential 1 MiB reads of a 16 GiB file in /dev/shm with 16 threads and --checksumverify at
-   K = 64 KiB, against a crc32 and a crc64nvme list of the file, alternating in one job.
+   K = 64 KiB, against a crc32, a crc64nvme and a blake3 list of the file, alternating in one job;
+3. sequential 4 KiB reads of the same file with 16 threads, without checksums and with whole-file
+   blake3 --checksums, alternating: the cost of the host merge of the BLAKE3 runs.
 
     python scripts/bench_checksum_algos.py [--size-gib 16] [--runs 3] [--dir /dev/shm]
 """
@@ -27,7 +29,7 @@ from elbencho_b200 import kernels  # noqa: E402
 from scripts.bench_checksums import SEED, descs_of, gpu_info, timed  # noqa: E402
 
 KiB, MiB, GiB = 1 << 10, 1 << 20, 1 << 30
-ALGOS = ("crc32", "crc32c", "crc64nvme")
+ALGOS = ("crc32", "crc32c", "crc64nvme", "blake3")
 
 
 def kernel_rates(runs, window):
@@ -53,6 +55,19 @@ def kernel_rates(runs, window):
             slots = 1 if shift == 64 else block >> shift
             chunk = "whole file" if shift == 64 else "K=%d KiB" % ((1 << shift) // KiB)
             for algo in ALGOS:
+                if algo == "blake3":
+                    # whole files: a slot per run, 2 log2(chunks per block) + 1 at most
+                    b3_slots = (2 * ((block // KiB).bit_length() - 1) + 1) if shift == 64 else slots
+                    digests = torch.zeros(n * b3_slots * 32, dtype=torch.uint8, device="cuda")
+                    host_digests = torch.zeros(n * b3_slots * 32, dtype=torch.uint8).pin_memory()
+                    ticket = torch.zeros(1, dtype=torch.int32, device="cuda")
+                    out["%s %s, %s" % (algo, chunk, label)] = window / GiB / timed(
+                        lambda: kernels.blake3_chunks(pinned_descs.data_ptr(), shifts.data_ptr(),
+                                                      n, shift, b3_slots, digests.data_ptr(),
+                                                      host_digests.data_ptr(), ticket.data_ptr(),
+                                                      stream), runs)
+                    del digests, host_digests
+                    continue
                 dtype = torch.int64 if algo == "crc64nvme" else torch.int32
                 crcs = torch.zeros(n * slots, dtype=dtype, device="cuda")
                 host_crcs = torch.zeros(n * slots, dtype=dtype).pin_memory()
@@ -85,6 +100,17 @@ def make_list(path, size, algo):
                 mgr.checksums_text())
 
 
+def whole_file_read_rate(path, size, checksums):
+    cfg = WorkerConfig(paths=[path], file_size=size, num_threads=16, block_size=4 * KiB,
+                       checksums=checksums, checksum_algo="blake3")
+    with WorkerManager(cfg) as mgr:
+        res = mgr.run_phase(BenchPhase.READFILES)
+        if checksums:
+            ((_, _, covered, digest),) = mgr.checksums()
+            assert covered == size and digest is not None
+    return round(res["ops_total"]["bytes"] / GiB / (res["last_finish_usec"] / 1e6), 3)
+
+
 def main():
     parser = argparse.ArgumentParser()
     parser.add_argument("--size-gib", type=int, default=16)
@@ -107,12 +133,18 @@ def main():
         with WorkerManager(WorkerConfig(paths=[path], block_size=MiB, file_size=size,
                                         num_threads=16, block_variance_percent=100)) as mgr:
             mgr.run_phase(BenchPhase.CREATEFILES)
-        lists = {algo: make_list(path, size, algo) for algo in ("crc32", "crc64nvme")}
+        lists = {algo: make_list(path, size, algo) for algo in ("crc32", "crc64nvme", "blake3")}
         for run in range(args.runs):
-            for algo in ("crc32", "crc64nvme"):
+            for algo in ("crc32", "crc64nvme", "blake3"):
                 rate = read_rate(path, size, lists[algo])
                 print(json.dumps({"gpu": info, "read": "seq 1 MiB, K=64 KiB, --checksumverify",
                                   "algo": algo, "run": run, "gib_per_s": rate}), flush=True)
+        for run in range(args.runs):
+            for checksums in (False, True):
+                rate = whole_file_read_rate(path, size, checksums)
+                print(json.dumps({"gpu": info, "read": "seq 4 KiB, whole file",
+                                  "checksums": "blake3" if checksums else "none", "run": run,
+                                  "gib_per_s": rate}), flush=True)
     finally:
         shutil.rmtree(workdir, ignore_errors=True)
 
