@@ -517,32 +517,16 @@ Manager::VerifyReport Manager::getVerifyReport()
 	return report;
 }
 
-/* the published CRC of algo of size bytes from their raw CRC, as lowercase hex digits of the
-   algorithm's width (8 or 16) */
-static std::string finishedCrcHex(int algo, uint64_t rawCrc, uint64_t size)
-{
-	char hex[17] = "";
-
-	elb_with_crc_algo(algo, [&](auto crcAlgo)
-	{
-		const auto crc = crcAlgo.finish( (typename decltype(crcAlgo)::word)rawCrc, size);
-		snprintf(hex, sizeof(hex), "%0*llx", (int)sizeof(crc) * 2, (unsigned long long)crc);
-	});
-
-	return hex;
-}
-
 /**
- * --checksums: the workers' accumulators merged by path (a file that several workers share has a
- * part in each): XOR of the raw CRCs, sum of the bytes. A file's CRC is complete when the phase
- * moved as many bytes of it as its size; the phase's block sources cover each byte once at most.
+ * --checksums: the workers' parts merged by path (a file that several workers share has a part in
+ * each). Whole files: the parts' sums merged and their bytes added; a file's value is complete when
+ * the phase moved as many bytes of it as its size, as the phase's block sources cover each byte once
+ * at most. --checksumchunk: one line per chunk that the phase moved, sorted by path and offset.
+ * Each file is reported as the phase computed it, even if a checksum list set since then changed
+ * the algorithm or the chunk size of the next phases.
  */
 Manager::ChecksumReport Manager::getChecksumReport()
 {
-	if(shared.cfg.checksumChunkShift)
-		return getChunkChecksumReport();
-
-	const bool isBlake3 = (shared.cfg.checksumAlgo == ELB_CHECKSUM_BLAKE3);
 	std::map<std::string, FileChecksum> files;
 
 	for(const std::unique_ptr<Worker>& worker : workers)
@@ -552,10 +536,12 @@ Manager::ChecksumReport Manager::getChecksumReport()
 
 			file.size = part.size;
 			file.numBytes += part.numBytes;
-			file.rawCrc ^= part.rawCrc;
-
-			if(isBlake3) // (blake3: the runs joined by the rule of the workers' maps)
-				file.blake3.merge(part.blake3, elb_blake3_num_chunks(part.size) );
+			file.algo = part.algo;
+			file.chunkShift = part.chunkShift;
+			file.whole.merge(part.whole, part.size);
+			file.chunks.insert(file.chunks.end(), part.chunks.begin(), part.chunks.end() );
+			file.chunkValues.insert(file.chunkValues.end(), part.chunkValues.begin(),
+				part.chunkValues.end() );
 		}
 
 	ChecksumReport report;
@@ -563,94 +549,37 @@ Manager::ChecksumReport Manager::getChecksumReport()
 	for(const auto& entry : files)
 	{
 		const FileChecksum& file = entry.second;
-		std::string crcStr = "-";
-		uint32_t digest[8];
+		const unsigned valueBytes = elb_checksum_value_bytes(file.algo);
 
-		if(isBlake3)
+		report.numFiles++;
+
+		if(file.chunkShift < 64)
 		{
-			if( (file.numBytes == file.size) && file.blake3.finish(file.size, digest) )
-			{
-				crcStr = elb_blake3_hex(digest);
-				report.numComplete++;
-			}
-		}
-		else if(file.numBytes == file.size)
-		{
-			crcStr = finishedCrcHex(shared.cfg.checksumAlgo, file.rawCrc, file.size);
-			report.numComplete++;
+			std::vector<size_t> order(file.chunks.size() );
+
+			for(size_t i = 0; i < order.size(); i++)
+				order[i] = i;
+
+			std::sort(order.begin(), order.end(), [&](size_t a, size_t b)
+				{ return file.chunks[a].offset < file.chunks[b].offset; } );
+
+			for(size_t i : order)
+				report.lines += entry.first + " " + std::to_string(file.chunks[i].offset) + " " +
+					std::to_string(file.chunks[i].length) + " " +
+					elb_checksum_hex(&file.chunkValues[i * valueBytes], valueBytes) + "\n";
+
+			report.numChunks += order.size();
+			continue;
 		}
 
+		uint8_t value[ELB_CHECKSUM_MAX_VALUE_BYTES];
+		const bool isComplete = (file.numBytes == file.size) &&
+			file.whole.finish(file.algo, file.size, value);
+
+		report.numComplete += isComplete;
 		report.lines += entry.first + " " + std::to_string(file.size) + " " +
-			std::to_string(file.numBytes) + " " + crcStr + "\n";
-		report.numFiles++;
-	}
-
-	return report;
-}
-
-/* --checksumchunk: one line per chunk that the last phase moved, sorted by path and offset */
-Manager::ChecksumReport Manager::getChunkChecksumReport()
-{
-	if(shared.cfg.checksumAlgo == ELB_CHECKSUM_BLAKE3)
-		return getChunkDigestReport();
-
-	std::map<std::string, std::vector<ChunkChecksum> > files;
-
-	for(const std::unique_ptr<Worker>& worker : workers)
-		for(const FileChecksum& part : worker->getFileChecksums() )
-		{
-			std::vector<ChunkChecksum>& chunks = files[part.path];
-			chunks.insert(chunks.end(), part.chunks.begin(), part.chunks.end() );
-		}
-
-	ChecksumReport report;
-
-	for(auto& entry : files)
-	{
-		std::vector<ChunkChecksum>& chunks = entry.second;
-
-		std::sort(chunks.begin(), chunks.end(),
-			[](const ChunkChecksum& a, const ChunkChecksum& b) { return a.offset < b.offset; } );
-
-		for(const ChunkChecksum& chunk : chunks)
-			report.lines += entry.first + " " + std::to_string(chunk.offset) + " " +
-				std::to_string(chunk.length) + " " +
-				finishedCrcHex(shared.cfg.checksumAlgo, chunk.rawCrc, chunk.length) + "\n";
-
-		report.numChunks += chunks.size();
-		report.numFiles++;
-	}
-
-	return report;
-}
-
-/* getChunkChecksumReport of --checksumalgo blake3: the chunks' digests */
-Manager::ChecksumReport Manager::getChunkDigestReport()
-{
-	std::map<std::string, std::vector<ChunkDigest> > files;
-
-	for(const std::unique_ptr<Worker>& worker : workers)
-		for(const FileChecksum& part : worker->getFileChecksums() )
-		{
-			std::vector<ChunkDigest>& chunks = files[part.path];
-			chunks.insert(chunks.end(), part.chunkDigests.begin(), part.chunkDigests.end() );
-		}
-
-	ChecksumReport report;
-
-	for(auto& entry : files)
-	{
-		std::vector<ChunkDigest>& chunks = entry.second;
-
-		std::sort(chunks.begin(), chunks.end(),
-			[](const ChunkDigest& a, const ChunkDigest& b) { return a.offset < b.offset; } );
-
-		for(const ChunkDigest& chunk : chunks)
-			report.lines += entry.first + " " + std::to_string(chunk.offset) + " " +
-				std::to_string(chunk.length) + " " + elb_blake3_hex(chunk.digest) + "\n";
-
-		report.numChunks += chunks.size();
-		report.numFiles++;
+			std::to_string(file.numBytes) + " " +
+			(isComplete ? elb_checksum_hex(value, valueBytes) : "-") + "\n";
 	}
 
 	return report;
@@ -664,6 +593,19 @@ static bool parseChecksumListNum(const std::string& str, uint64_t& outVal)
 		return false;
 
 	outVal = std::stoull(str);
+	return true;
+}
+
+/* a finished value of numBytes bytes from its hex digits, upper or lower case */
+static bool parseChecksumListValue(const std::string& str, unsigned numBytes, uint8_t* outValue)
+{
+	if( (str.size() != 2 * numBytes) ||
+		(str.find_first_not_of("0123456789abcdefABCDEF") != std::string::npos) )
+		return false;
+
+	for(unsigned i = 0; i < numBytes; i++)
+		outValue[i] = (uint8_t)std::stoul(str.substr(2 * i, 2), NULL, 16);
+
 	return true;
 }
 
@@ -733,6 +675,7 @@ std::shared_ptr<const ChecksumList> ChecksumList::parse(const std::string& text)
 			section = std::make_shared<ChecksumList>();
 			section->chunkShift = __builtin_ctzll(chunkSize);
 			section->algo = algo;
+			section->valueBytes = elb_checksum_value_bytes(algo);
 			list = section;
 			continue;
 		}
@@ -743,33 +686,24 @@ std::shared_ptr<const ChecksumList> ChecksumList::parse(const std::string& text)
 		if(!section)
 			continue; // (a line of a whole-file section)
 
-		const size_t crcBlank = line.rfind(' ');
-		const size_t lenBlank = (crcBlank && (crcBlank != std::string::npos) ) ?
-			line.rfind(' ', crcBlank - 1) : std::string::npos;
+		const size_t valueBlank = line.rfind(' ');
+		const size_t lenBlank = (valueBlank && (valueBlank != std::string::npos) ) ?
+			line.rfind(' ', valueBlank - 1) : std::string::npos;
 		const size_t offBlank = (lenBlank && (lenBlank != std::string::npos) ) ?
 			line.rfind(' ', lenBlank - 1) : std::string::npos;
-
-		const bool isBlake3 = (section->algo == ELB_CHECKSUM_BLAKE3);
-		size_t numDigits = isBlake3 ? 2 * elb_blake3_algo::DIGEST_BYTES : 0; // (the width)
 		const std::string lineFormat = std::string("not \"path offset length ") +
 			elb_checksum_algo_name(section->algo) + "\"";
-
-		elb_with_crc_algo(section->algo, [&](auto algo)
-			{ numDigits = sizeof(typename decltype(algo)::word) * 2; } );
-
-		const bool is64 = (numDigits == 16);
 
 		if( (offBlank == std::string::npos) || !offBlank)
 			fail(lineFormat);
 
-		const std::string crcStr = line.substr(crcBlank + 1);
 		const uint64_t chunkSize = 1ULL << section->chunkShift;
 		uint64_t offset, length;
+		uint8_t value[ELB_CHECKSUM_MAX_VALUE_BYTES];
 
 		if(!parseChecksumListNum(line.substr(offBlank + 1, lenBlank - offBlank - 1), offset) ||
-			!parseChecksumListNum(line.substr(lenBlank + 1, crcBlank - lenBlank - 1), length) ||
-			(crcStr.size() != numDigits) ||
-			(crcStr.find_first_not_of("0123456789abcdefABCDEF") != std::string::npos) )
+			!parseChecksumListNum(line.substr(lenBlank + 1, valueBlank - lenBlank - 1), length) ||
+			!parseChecksumListValue(line.substr(valueBlank + 1), section->valueBytes, value) )
 			fail(lineFormat);
 
 		if( (offset % chunkSize) || !length || (length > chunkSize) )
@@ -784,39 +718,12 @@ std::shared_ptr<const ChecksumList> ChecksumList::parse(const std::string& text)
 		if(chunkIdx >= file.present.size() )
 		{
 			file.present.resize(chunkIdx + 1);
-
-			if(isBlake3)
-				file.digests.resize(8 * (chunkIdx + 1) );
-			else
-				file.crcs.resize(chunkIdx + 1);
-
-			if(is64)
-				file.crcsHi.resize(chunkIdx + 1);
+			file.values.resize(section->valueBytes * (chunkIdx + 1) );
 		}
 
 		file.path = line.substr(0, offBlank);
 		file.present[chunkIdx] = true;
-
-		if(isBlake3)
-		{ // 32 bytes: word k holds bytes 4k .. 4k + 3, little-endian
-			for(unsigned b = 0; b < elb_blake3_algo::DIGEST_BYTES; b++)
-			{
-				const uint32_t byte = (uint32_t)std::stoul(crcStr.substr(2 * b, 2), NULL, 16);
-				uint32_t& word = file.digests[8 * chunkIdx + b / 4];
-
-				word = (word & ~(0xffu << (8 * (b % 4) ) ) ) | (byte << (8 * (b % 4) ) );
-			}
-		}
-		else
-		{
-			const uint64_t crc = std::stoull(crcStr, NULL, 16);
-
-			file.crcs[chunkIdx] = (uint32_t)crc;
-
-			if(is64)
-				file.crcsHi[chunkIdx] = (uint32_t)(crc >> 32);
-		}
-
+		memcpy(&file.values[section->valueBytes * chunkIdx], value, section->valueBytes);
 		section->numChunks++;
 
 		if(length != chunkSize)

@@ -306,6 +306,7 @@ struct elb_crc_algo
 {
 	typedef Word word;
 
+	static constexpr unsigned VALUE_BYTES = sizeof(Word); /* the finished CRC, big-endian */
 	static constexpr unsigned BITS = sizeof(Word) * 8;
 	static constexpr Word POLY = POLY_;
 	static constexpr Word ONE = (Word)1 << (BITS - 1); /* x^0 */
@@ -440,26 +441,6 @@ inline bool elb_with_crc_algo(int algo, F&& f)
 	}
 }
 
-/* the name of the algorithm with ID algo ("" for none) */
-inline const char* elb_crc_algo_name(int algo)
-{
-	const char* name = "";
-	elb_with_crc_algo(algo, [&](auto crcAlgo) { name = crcAlgo.NAME; } );
-	return name;
-}
-
-/* the ID of the algorithm called name (--checksumalgo, list headers), -1 if none is */
-inline int elb_crc_algo_by_name(const char* name)
-{
-	int found = -1;
-
-	for(int algo = 0; algo < ELB_CRC_NUM_ALGOS; algo++)
-		elb_with_crc_algo(algo, [&](auto crcAlgo)
-			{ if(!strcmp(crcAlgo.NAME, name) ) found = algo; } );
-
-	return found;
-}
-
 /* ---- BLAKE3 (--checksumalgo blake3) -------------------------------------------------------------
  *
  * The default BLAKE3 hash with a 256-bit output (what b3sum prints). A message is cut into 1 KiB
@@ -484,19 +465,71 @@ struct elb_blake3_algo
 	static constexpr int ID = 3;
 	static constexpr const char* NAME = "blake3";
 	static constexpr const char* LABEL = "BLAKE3";
-	static constexpr unsigned DIGEST_BYTES = 32;
+	static constexpr unsigned VALUE_BYTES = 32; /* the digest: 8 little-endian words */
 };
 
-/* the name of checksum algorithm algo (enum elb_checksum_algo: a CRC or BLAKE3; "" for none) */
-inline const char* elb_checksum_algo_name(int algo)
+/* the IDs run from 0 to BLAKE3's; no value is wider than a BLAKE3 digest (elb_checksum_value_bytes) */
+#define ELB_CHECKSUM_NUM_ALGOS (elb_blake3_algo::ID + 1)
+#define ELB_CHECKSUM_MAX_VALUE_BYTES elb_blake3_algo::VALUE_BYTES
+
+/* host code: f(the algorithm object of checksum algorithm ID algo, a CRC or BLAKE3); false (f not
+   called) for an unknown ID. A finished value is VALUE_BYTES bytes in the order they are printed. */
+template<class F>
+inline bool elb_with_checksum_algo(int algo, F&& f)
 {
-	return (algo == elb_blake3_algo::ID) ? elb_blake3_algo::NAME : elb_crc_algo_name(algo);
+	if(algo != elb_blake3_algo::ID)
+		return elb_with_crc_algo(algo, f);
+
+	f(elb_blake3_algo{});
+	return true;
 }
 
-/* the ID of the checksum algorithm called name (--checksumalgo, list headers), -1 if none is */
+/* the name of checksum algorithm algo (--checksumalgo, list headers; "" for none) */
+inline const char* elb_checksum_algo_name(int algo)
+{
+	const char* name = "";
+	elb_with_checksum_algo(algo, [&](auto checksumAlgo) { name = checksumAlgo.NAME; } );
+	return name;
+}
+
+/* the ID of the checksum algorithm called name, -1 if none is */
 inline int elb_checksum_algo_by_name(const char* name)
 {
-	return !strcmp(name, elb_blake3_algo::NAME) ? elb_blake3_algo::ID : elb_crc_algo_by_name(name);
+	for(int algo = 0; algo < ELB_CHECKSUM_NUM_ALGOS; algo++)
+		if(!strcmp(elb_checksum_algo_name(algo), name) )
+			return algo;
+
+	return -1;
+}
+
+/* the bytes of a finished value of checksum algorithm algo (0 for none) */
+inline unsigned elb_checksum_value_bytes(int algo)
+{
+	unsigned numBytes = 0;
+
+	elb_with_checksum_algo(algo, [&](auto checksumAlgo)
+	{
+		static_assert(decltype(checksumAlgo)::VALUE_BYTES <= ELB_CHECKSUM_MAX_VALUE_BYTES,
+			"a finished value must fit ELB_CHECKSUM_MAX_VALUE_BYTES");
+		numBytes = checksumAlgo.VALUE_BYTES;
+	});
+
+	return numBytes;
+}
+
+/* a finished value as the lowercase hex digits of its bytes */
+inline std::string elb_checksum_hex(const uint8_t* value, unsigned numBytes)
+{
+	static const char digits[] = "0123456789abcdef";
+	std::string hex(2 * numBytes, '0');
+
+	for(unsigned i = 0; i < numBytes; i++)
+	{
+		hex[2 * i] = digits[value[i] >> 4];
+		hex[2 * i + 1] = digits[value[i] & 15];
+	}
+
+	return hex;
 }
 
 #define ELB_BLAKE3_IV0 0x6A09E667u
@@ -689,22 +722,6 @@ inline bool elb_blake3_fold_cvs(const uint32_t (*runs)[8], uint64_t numRuns, uin
 		elb_blake3_parent_cv(runs[i], out, !i, out);
 
 	return true;
-}
-
-/* a digest (8 little-endian words) as the 64 lowercase hex digits of its 32 bytes */
-inline std::string elb_blake3_hex(const uint32_t digest[8])
-{
-	static const char digits[] = "0123456789abcdef";
-	std::string hex(64, '0');
-
-	for(int i = 0; i < 32; i++)
-	{
-		const uint8_t byte = (uint8_t)(digest[i / 4] >> (8 * (i % 4) ) );
-		hex[2 * i] = digits[byte >> 4];
-		hex[2 * i + 1] = digits[byte & 15];
-	}
-
-	return hex;
 }
 
 #endif /* ELB_PATTERNS_CUH_ */

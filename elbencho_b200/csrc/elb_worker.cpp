@@ -342,6 +342,7 @@ void Worker::resetStats() // Worker.h:92-110
 	numDamageBytesDropped = 0;
 	deferredVerifyError.clear();
 	checksumAccs.clear();
+	chunkValuesBatch = NULL;
 	checksumListFiles.clear();
 	numChecksumChunksChecked = 0;
 
@@ -819,11 +820,11 @@ void Worker::preparePhase()
 }
 
 /**
- * --checksums / --checksumverify: which stages take the CRC launch, in chunks of which size and of
- * which algorithm, and the batches' CRC slots. Runs after the rings are made and at the start of every write and read
- * phase, since a checksum list (elb_mgr_set_checksum_list) may be set between phases; a change
- * drops the batch graphs, which hold the launches of the old setup. Without either option it
- * allocates and changes nothing.
+ * --checksums / --checksumverify: which stages take the checksum launch, in chunks of which size
+ * and of which algorithm, and the batches' slots. Runs after the rings are made and at the start
+ * of every write and read phase, since a checksum list (elb_mgr_set_checksum_list) may be set
+ * between phases; a change drops the batch graphs, which hold the launches of the old setup.
+ * Without either option it allocates and changes nothing.
  */
 void Worker::setupChecksums()
 {
@@ -831,25 +832,16 @@ void Worker::setupChecksums()
 	const unsigned chunkShift = cfg.checksumChunkShift ? cfg.checksumChunkShift : 64;
 	uint64_t slotsPerDesc = (chunkShift == 64) ? 1 :
 		std::max( (cfg.blockSize + ( (uint64_t)1 << chunkShift) - 1) >> chunkShift, (uint64_t)1);
-	size_t wordBytes = 0;
 
-	if(cfg.checksumAlgo == ELB_CHECKSUM_BLAKE3)
-	{ // a digest or CV per slot; whole files: the runs of a block of m chunks, 2 log2(m) + 1 at most
-		wordBytes = elb_blake3_algo::DIGEST_BYTES;
-
-		if(chunkShift == 64)
-		{
-			const uint64_t numChunks = elb_blake3_num_chunks(cfg.blockSize);
-			slotsPerDesc = 2 * (63 - __builtin_clzll(numChunks) ) + 1;
-		}
+	if( (cfg.checksumAlgo == ELB_CHECKSUM_BLAKE3) && (chunkShift == 64) )
+	{ // whole files: the runs of a block of m chunks, 2 log2(m) + 1 at most
+		const uint64_t numChunks = elb_blake3_num_chunks(cfg.blockSize);
+		slotsPerDesc = 2 * (63 - __builtin_clzll(numChunks) ) + 1;
 	}
-	else
-		elb_with_crc_algo(cfg.checksumAlgo, [&](auto algo)
-			{ wordBytes = sizeof(typename decltype(algo)::word); } );
 
 	if(batches.empty() || ( (readChecksum == readStage.checksum) &&
-		(chunkShift == crcChunkShift) && (slotsPerDesc == crcSlotsPerDesc) &&
-		(cfg.checksumAlgo == crcAlgo) ) )
+		(chunkShift == checksumChunkShift) && (slotsPerDesc == checksumSlotsPerDesc) &&
+		(cfg.checksumAlgo == checksumAlgo) ) )
 		return;
 
 	std::shared_lock<std::shared_timed_mutex> allocLock(shared->gpuAllocMutex);
@@ -859,10 +851,10 @@ void Worker::setupChecksums()
 	/* --verifydirect: a write phase's checksums are those of the written bytes, so the read-back
 	   takes none, and must not share the read phase's batch graphs then */
 	verifyBackStage.useGraph = readStage.useGraph && !readChecksum;
-	crcChunkShift = chunkShift;
-	crcSlotsPerDesc = slotsPerDesc;
-	crcAlgo = cfg.checksumAlgo;
-	crcWordBytes = wordBytes;
+	checksumChunkShift = chunkShift;
+	checksumSlotsPerDesc = slotsPerDesc;
+	checksumAlgo = cfg.checksumAlgo;
+	checksumValueBytes = elb_checksum_value_bytes(checksumAlgo);
 
 	for(Batch& batch : batches)
 	{
@@ -870,15 +862,15 @@ void Worker::setupChecksums()
 			cudaGraphExecDestroy(batch.readGraphExec);
 		if(batch.writeGraphExec)
 			cudaGraphExecDestroy(batch.writeGraphExec);
-		if(batch.devCrcs)
-			cudaFree(batch.devCrcs);
-		if(batch.hostCrcs)
-			cudaFreeHost(batch.hostCrcs);
+		if(batch.devSums)
+			cudaFree(batch.devSums);
+		if(batch.hostSums)
+			cudaFreeHost(batch.hostSums);
 
 		batch.readGraphExec = NULL;
 		batch.writeGraphExec = NULL;
-		batch.devCrcs = NULL;
-		batch.hostCrcs = NULL;
+		batch.devSums = NULL;
+		batch.hostSums = NULL;
 
 		if(!readChecksum)
 			continue;
@@ -888,11 +880,11 @@ void Worker::setupChecksums()
 		if(!batch.hostShifts)
 			ELB_CUDA_CHECK(cudaHostAlloc( (void**)&batch.hostShifts, sizeof(uint64_t) * batchBlocks,
 				cudaHostAllocDefault), "Pinned checksum shift allocation");
-		ELB_CUDA_CHECK(cudaMalloc(&batch.devCrcs, crcWordBytes * numSlots),
+		ELB_CUDA_CHECK(cudaMalloc(&batch.devSums, checksumValueBytes * numSlots),
 			"GPU checksum allocation");
-		ELB_CUDA_CHECK(cudaHostAlloc(&batch.hostCrcs, crcWordBytes * numSlots,
+		ELB_CUDA_CHECK(cudaHostAlloc(&batch.hostSums, checksumValueBytes * numSlots,
 			cudaHostAllocDefault), "Pinned checksum allocation");
-		ELB_CUDA_CHECK(cudaMemsetAsync(batch.devCrcs, 0, crcWordBytes * numSlots,
+		ELB_CUDA_CHECK(cudaMemsetAsync(batch.devSums, 0, checksumValueBytes * numSlots,
 			batch.stream), "GPU checksum init");
 		ELB_CUDA_CHECK(cudaStreamSynchronize(batch.stream), "GPU checksum init");
 	}
@@ -1152,10 +1144,10 @@ void Worker::freeRings() // LocalWorker::cleanup (:1570-1641)
 			cudaFree(batch.devDoneTicket);
 		if(batch.hostShifts)
 			cudaFreeHost(batch.hostShifts);
-		if(batch.devCrcs)
-			cudaFree(batch.devCrcs);
-		if(batch.hostCrcs)
-			cudaFreeHost(batch.hostCrcs);
+		if(batch.devSums)
+			cudaFree(batch.devSums);
+		if(batch.hostSums)
+			cudaFreeHost(batch.hostSums);
 	}
 
 	batches.clear();
@@ -1241,9 +1233,9 @@ void Worker::abortInFlight()
 			// (a failed launch may have left the ticket or the armed results behind)
 			cudaMemsetAsync(batch.devDoneTicket, 0, sizeof(unsigned), batch.stream);
 			elb_launch_verify_init(batch.devResults, batchBlocks, batch.stream);
-			if(batch.devCrcs)
-				cudaMemsetAsync(batch.devCrcs, 0, crcWordBytes * batchBlocks * crcSlotsPerDesc,
-					batch.stream);
+			if(batch.devSums)
+				cudaMemsetAsync(batch.devSums, 0,
+					checksumValueBytes * batchBlocks * checksumSlotsPerDesc, batch.stream);
 			cudaStreamSynchronize(batch.stream);
 
 			batch.numIOPending = 0;
@@ -2235,19 +2227,19 @@ uint32_t Worker::fillStageDescs(Batch& batch, const GpuStage& stage, uint64_t& o
 		if(!stage.isRead && block.ioIsRead)
 			continue;
 
-		if(stage.checksum && (crcAlgo == ELB_CHECKSUM_BLAKE3) && ( (block.offset & 1023) ||
+		if(stage.checksum && (checksumAlgo == ELB_CHECKSUM_BLAKE3) && ( (block.offset & 1023) ||
 			( ( (block.offset + block.len) & 1023) &&
 			(block.offset + block.len != blockFileSize(block) ) ) ) )
 			throw WorkerError("BLAKE3 checksums need blocks on 1 KiB boundaries. File: " +
 				blockFilePath(block) + "; Offset: " + std::to_string(block.offset) + "; Length: " +
 				std::to_string(block.len) );
 
-		if(stage.checksum && (crcChunkShift == 64) )
+		if(stage.checksum && (checksumChunkShift == 64) )
 			batch.hostShifts[numDescs] = blockFileSize(block) - block.offset - block.len;
-		else if(stage.checksum && (block.offset & ( ( (uint64_t)1 << crcChunkShift) - 1) ) )
+		else if(stage.checksum && (block.offset & ( ( (uint64_t)1 << checksumChunkShift) - 1) ) )
 			throw WorkerError("Checksum chunks need blocks at multiples of the chunk size. "
 				"File: " + blockFilePath(block) + "; Offset: " + std::to_string(block.offset) +
-				"; Chunk size: " + std::to_string( (uint64_t)1 << crcChunkShift) );
+				"; Chunk size: " + std::to_string( (uint64_t)1 << checksumChunkShift) );
 
 		batch.hostDescs[numDescs++] = elb_block_desc{slotDevPtr(batch, i), block.len,
 			block.offset, descBlockCounter(stage.content, block)};
@@ -2441,11 +2433,12 @@ void Worker::enqueueStage(Batch& batch, const GpuStage& stage, uint32_t numBlock
 	}
 
 	// (a write's checksum reads the device slot before its stage-out copy)
-	if(stage.checksum && ( (crcAlgo == ELB_CHECKSUM_BLAKE3) ?
-		elb_launch_blake3(batch.hostDescs, batch.hostShifts, numBlocks, crcChunkShift,
-		crcSlotsPerDesc, batch.devCrcs, batch.hostCrcs, batch.stream) :
-		elb_launch_crc(crcAlgo, batch.hostDescs, batch.hostShifts, numBlocks, crcChunkShift,
-		crcSlotsPerDesc, batch.devCrcs, batch.hostCrcs, batch.devDoneTicket, batch.stream) ) )
+	if(stage.checksum && ( (checksumAlgo == ELB_CHECKSUM_BLAKE3) ?
+		elb_launch_blake3(batch.hostDescs, batch.hostShifts, numBlocks, checksumChunkShift,
+		checksumSlotsPerDesc, batch.devSums, batch.hostSums, batch.stream) :
+		elb_launch_crc(checksumAlgo, batch.hostDescs, batch.hostShifts, numBlocks,
+		checksumChunkShift, checksumSlotsPerDesc, batch.devSums, batch.hostSums,
+		batch.devDoneTicket, batch.stream) ) )
 		throw WorkerError(std::string("GPU checksum failed. ") + elb_last_error() );
 
 	if( (stage.transfer == GpuStage::TRANSFER_COPY) && !stage.isRead)
@@ -2465,6 +2458,9 @@ void Worker::gpuLaunchStage(Batch& batch, bool isRead)
 	const uint32_t numBlocks = fillStageDescs(batch, stage, numBytes);
 
 	batch.hadKernel = numBlocks && (stage.content.kind != elb_content::NONE);
+
+	if(chunkValuesBatch == &batch)
+		chunkValuesBatch = NULL; // (its checksum slots may change)
 
 	ELB_CUDA_CHECK(cudaEventRecord(batch.gpuStartEvent, batch.stream), "CUDA event record");
 
@@ -2726,98 +2722,94 @@ Worker::FileID Worker::blockFileID(const BlockRef& block) const
 		block.isTreeElem ? FileID(~0ULL, block.fileIndex) : FileID(block.dirIndex, block.fileIndex);
 }
 
-/* the raw CRC in host slot slot of a batch whose CRC launch is done */
-uint64_t Worker::batchCrc(const Batch& batch, uint64_t slot) const
+/* a finished CRC as its value bytes: big-endian, the order of its hex digits */
+template<class Word>
+static void storeCrcValue(Word crc, uint8_t* outValue)
 {
-	return (crcWordBytes == sizeof(uint64_t) ) ? ( (const uint64_t*)batch.hostCrcs)[slot] :
-		( (const uint32_t*)batch.hostCrcs)[slot];
+	for(unsigned b = 0; b < sizeof(Word); b++)
+		outValue[b] = (uint8_t)(crc >> (8 * (sizeof(Word) - 1 - b) ) );
 }
 
-/* --checksums: the CRC contributions of a batch whose blocks are done (no rwmix: descriptor i is
- * block i), into the accumulator of each block's file: XORed per file, or one entry per chunk */
+/**
+ * --checksumchunk: the finished value of each chunk of a batch whose checksum launch is done, at
+ * its slot's place (checksumValueBytes per slot). A BLAKE3 slot is the chunk's digest already. A
+ * CRC slot holds the chunk's raw CRC: a full chunk is finished by one XOR with the finish of a raw
+ * 0 of the chunk size, a short one (a file's last chunk) by Algo::finish. A read batch that is
+ * both checked and listed is finished once.
+ */
+const uint8_t* Worker::finishChunkValues(const Batch& batch)
+{
+	if(checksumAlgo == ELB_CHECKSUM_BLAKE3)
+		return (const uint8_t*)batch.hostSums;
+
+	if(chunkValuesBatch == &batch)
+		return chunkValues.data();
+
+	chunkValues.resize(checksumValueBytes * batchBlocks * checksumSlotsPerDesc);
+
+	elb_with_crc_algo(checksumAlgo, [&](auto algo)
+	{
+		typedef decltype(algo) Algo;
+		typedef typename Algo::word Word;
+
+		const uint64_t chunkSize = (uint64_t)1 << checksumChunkShift;
+		const Word fullChunkXor = Algo::finish(0, chunkSize);
+		const Word* rawCrcs = (const Word*)batch.hostSums;
+
+		for(size_t i = 0; i < batch.blocks.size(); i++)
+		{
+			const uint64_t blockEnd = batch.blocks[i].offset + batch.blocks[i].len;
+
+			for(uint64_t pos = batch.blocks[i].offset, slot = i * checksumSlotsPerDesc;
+				pos < blockEnd; pos += chunkSize, slot++)
+			{
+				const uint64_t len = std::min(chunkSize, blockEnd - pos);
+
+				storeCrcValue( (len == chunkSize) ? (Word)(rawCrcs[slot] ^ fullChunkXor) :
+					Algo::finish(rawCrcs[slot], len), &chunkValues[slot * sizeof(Word)]);
+			}
+		}
+	});
+
+	chunkValuesBatch = &batch;
+	return chunkValues.data();
+}
+
+/* --checksums: the slots of a batch whose blocks are done (no rwmix: descriptor i is block i),
+ * into what this worker moved of each block's file: whole files, the block's part; chunks, each
+ * chunk and its finished value */
 void Worker::addBatchChecksums(const Batch& batch)
 {
 	if(!cfg.checksums)
 		return;
 
-	if(crcAlgo == ELB_CHECKSUM_BLAKE3)
-	{
-		addBatchDigests(batch);
-		return;
-	}
+	const uint8_t* values = (checksumChunkShift < 64) ? finishChunkValues(batch) : NULL;
 
 	for(size_t i = 0; i < batch.blocks.size(); i++)
 	{
 		const BlockRef& block = batch.blocks[i];
-		ChecksumAcc& acc = checksumAccs.try_emplace(blockFileID(block), ChecksumAcc{block}).first->
-			second;
+		const uint64_t firstSlot = i * checksumSlotsPerDesc;
+		FileChecksum& file = checksumAccs.try_emplace(blockFileID(block), ChecksumAcc{block}).
+			first->second.file;
 
-		acc.numBytes += block.len;
+		file.numBytes += block.len;
 
-		if(crcChunkShift == 64)
+		if(!values)
 		{
-			acc.rawCrc ^= batchCrc(batch, i);
+			file.whole.add(checksumAlgo, (const uint8_t*)batch.hostSums +
+				firstSlot * checksumValueBytes, block.offset, block.len, blockFileSize(block) );
 			continue;
 		}
 
-		const uint64_t chunkSize = (uint64_t)1 << crcChunkShift;
+		const uint64_t chunkSize = (uint64_t)1 << checksumChunkShift;
 		const uint64_t blockEnd = block.offset + block.len;
 
-		for(uint64_t pos = block.offset, slot = i * crcSlotsPerDesc; pos < blockEnd;
-			pos += chunkSize, slot++)
-			acc.chunks.push_back(ChunkChecksum{pos, std::min(chunkSize, blockEnd - pos),
-				batchCrc(batch, slot)});
-	}
-}
-
-/* --checksums --checksumalgo blake3: the slots of a batch whose blocks are done into the
- * accumulator of each block's file: whole files, the block's runs (elb_blake3_chunks) into the
- * file's run map, or its digest when the block is the whole file; chunks, one entry per chunk */
-void Worker::addBatchDigests(const Batch& batch)
-{
-	const uint32_t (*slots)[8] = (const uint32_t (*)[8])batch.hostCrcs;
-
-	for(size_t i = 0; i < batch.blocks.size(); i++)
-	{
-		const BlockRef& block = batch.blocks[i];
-		const uint64_t blockEnd = block.offset + block.len;
-		const uint64_t fileSize = blockFileSize(block);
-		ChecksumAcc& acc = checksumAccs.try_emplace(blockFileID(block), ChecksumAcc{block}).first->
-			second;
-
-		acc.numBytes += block.len;
-
-		if(crcChunkShift < 64)
+		for(uint64_t pos = block.offset, slot = firstSlot; pos < blockEnd; pos += chunkSize, slot++)
 		{
-			const uint64_t chunkSize = (uint64_t)1 << crcChunkShift;
+			const uint8_t* value = values + slot * checksumValueBytes;
 
-			for(uint64_t pos = block.offset, slot = i * crcSlotsPerDesc; pos < blockEnd;
-				pos += chunkSize, slot++)
-			{
-				ChunkDigest chunk{pos, std::min(chunkSize, blockEnd - pos), {} };
-				memcpy(chunk.digest, slots[slot], sizeof(chunk.digest) );
-				acc.chunkDigests.push_back(chunk);
-			}
-
-			continue;
-		}
-
-		if(!block.offset && (blockEnd == fileSize) )
-		{
-			acc.blake3.addDigest(slots[i * crcSlotsPerDesc]);
-			continue;
-		}
-
-		const uint64_t first = block.offset >> ELB_BLAKE3_CHUNK_SHIFT;
-		const uint64_t end = (blockEnd + 1023) >> ELB_BLAKE3_CHUNK_SHIFT;
-		uint64_t slot = i * crcSlotsPerDesc;
-
-		for(uint64_t pos = first; pos < end; slot++)
-		{
-			const uint64_t numChunks = 1ULL << elb_blake3_run_shift(pos, end);
-
-			acc.blake3.add(pos, numChunks, slots[slot], elb_blake3_num_chunks(fileSize) );
-			pos += numChunks;
+			file.chunks.push_back(ChecksumChunk{pos, std::min(chunkSize, blockEnd - pos)});
+			file.chunkValues.insert(file.chunkValues.end(), value, value + checksumValueBytes);
 		}
 	}
 }
@@ -2914,10 +2906,61 @@ bool Blake3Runs::finish(uint64_t fileSize, uint32_t outDigest[8]) const
 		(const uint32_t (*)[8])cvs.data(), runs.size(), pos, outDigest);
 }
 
+void WholeFileChecksum::add(int algo, const void* slots, uint64_t offset, uint64_t len,
+	uint64_t fileSize)
+{
+	if(algo != ELB_CHECKSUM_BLAKE3)
+	{ // a CRC: the block's contribution
+		elb_with_crc_algo(algo, [&](auto crcAlgo)
+			{ rawCrc ^= *(const typename decltype(crcAlgo)::word*)slots; } );
+		return;
+	}
+
+	// BLAKE3: the block's runs (elb_blake3_chunks), or its digest when the block is the whole file
+	const uint32_t (*cvs)[8] = (const uint32_t (*)[8])slots;
+	const uint64_t endChunk = (offset + len + 1023) >> ELB_BLAKE3_CHUNK_SHIFT;
+
+	if(!offset && (offset + len == fileSize) )
+	{
+		blake3.addDigest(cvs[0]);
+		return;
+	}
+
+	for(uint64_t pos = offset >> ELB_BLAKE3_CHUNK_SHIFT; pos < endChunk; cvs++)
+	{
+		const uint64_t numChunks = 1ULL << elb_blake3_run_shift(pos, endChunk);
+
+		blake3.add(pos, numChunks, *cvs, elb_blake3_num_chunks(fileSize) );
+		pos += numChunks;
+	}
+}
+
+void WholeFileChecksum::merge(const WholeFileChecksum& other, uint64_t fileSize)
+{
+	rawCrc ^= other.rawCrc;
+	blake3.merge(other.blake3, elb_blake3_num_chunks(fileSize) );
+}
+
+bool WholeFileChecksum::finish(int algo, uint64_t fileSize, uint8_t* outValue) const
+{
+	if(algo != ELB_CHECKSUM_BLAKE3)
+		return elb_with_crc_algo(algo, [&](auto crcAlgo)
+			{ storeCrcValue(crcAlgo.finish( (typename decltype(crcAlgo)::word)rawCrc, fileSize),
+				outValue); } );
+
+	uint32_t digest[8];
+
+	if(!blake3.finish(fileSize, digest) )
+		return false;
+
+	memcpy(outValue, digest, sizeof(digest) ); // (little-endian words: the digest's bytes)
+	return true;
+}
+
 /**
- * --checksumverify: compare the CRC of each chunk of a read batch with the list line of its file
- * and offset (blocks start at chunk boundaries, fillStageDescs). The file's list entry is looked up
- * once per file and phase. The first chunk without a matching line fails the worker.
+ * --checksumverify: compare the finished value of each chunk of a read batch with the list line of
+ * its file and offset (blocks start at chunk boundaries, fillStageDescs). The file's list entry is
+ * looked up once per file and phase. The first chunk without a matching line fails the worker.
  */
 void Worker::checkBatchChecksums(const Batch& batch)
 {
@@ -2926,72 +2969,8 @@ void Worker::checkBatchChecksums(const Batch& batch)
 	if(!list || !readStage.checksum || (benchPhase != ELB_PHASE_READFILES) )
 		return;
 
-	if(crcAlgo == ELB_CHECKSUM_BLAKE3)
-	{
-		checkBatchDigests(batch);
-		return;
-	}
-
-	elb_with_crc_algo(crcAlgo, [&](auto algo)
-	{
-		typedef decltype(algo) Algo;
-
-		const uint64_t chunkSize = (uint64_t)1 << crcChunkShift;
-		const typename Algo::word fullChunkXor = Algo::finish(0, chunkSize);
-
-		for(size_t i = 0; i < batch.blocks.size(); i++)
-		{
-			const BlockRef& block = batch.blocks[i];
-			const uint64_t blockEnd = block.offset + block.len;
-			auto fileIter = checksumListFiles.find(blockFileID(block) );
-
-			if(fileIter == checksumListFiles.end() )
-				fileIter = checksumListFiles.emplace(blockFileID(block),
-					list->findFile(blockFilePath(block) ) ).first;
-
-			const ChecksumList::File* file = fileIter->second;
-
-			for(uint64_t pos = block.offset, slot = i * crcSlotsPerDesc; pos < blockEnd;
-				pos += chunkSize, slot++)
-			{
-				const uint64_t len = std::min(chunkSize, blockEnd - pos);
-				const typename Algo::word rawCrc = (typename Algo::word)batchCrc(batch, slot);
-				const typename Algo::word crc = (len == chunkSize) ? (rawCrc ^ fullChunkXor) :
-					Algo::finish(rawCrc, len);
-				const uint64_t chunkIdx = pos >> crcChunkShift;
-				const bool hasLine = file && file->hasLine(chunkIdx);
-
-				if(hasLine && (file->chunkLength(chunkIdx, chunkSize) == len) &&
-					(file->crc(chunkIdx) == crc) )
-				{
-					numChecksumChunksChecked++;
-					continue;
-				}
-
-				const int numDigits = (int)sizeof(crc) * 2;
-				char expected[17] = "-";
-				char actual[17];
-
-				if(hasLine)
-					snprintf(expected, sizeof(expected), "%0*llx", numDigits,
-						(unsigned long long)file->crc(chunkIdx) );
-				snprintf(actual, sizeof(actual), "%0*llx", numDigits, (unsigned long long)crc);
-
-				throw WorkerError("Checksum verification failed. File: " + blockFilePath(block) +
-					"; Offset: " + std::to_string(pos) + "; Length: " + std::to_string(len) + "; "
-					"Expected " + Algo::LABEL + ": " + expected + "; Actual " + Algo::LABEL + ": " +
-					actual);
-			}
-		}
-	});
-}
-
-/* --checksumverify with a blake3 list: checkBatchChecksums with 32-byte digests */
-void Worker::checkBatchDigests(const Batch& batch)
-{
-	const ChecksumList* list = shared->checksumList.get();
-	const uint32_t (*slots)[8] = (const uint32_t (*)[8])batch.hostCrcs;
-	const uint64_t chunkSize = (uint64_t)1 << crcChunkShift;
+	const uint8_t* values = finishChunkValues(batch);
+	const uint64_t chunkSize = (uint64_t)1 << checksumChunkShift;
 
 	for(size_t i = 0; i < batch.blocks.size(); i++)
 	{
@@ -3005,27 +2984,30 @@ void Worker::checkBatchDigests(const Batch& batch)
 
 		const ChecksumList::File* file = fileIter->second;
 
-		for(uint64_t pos = block.offset, slot = i * crcSlotsPerDesc; pos < blockEnd;
+		for(uint64_t pos = block.offset, slot = i * checksumSlotsPerDesc; pos < blockEnd;
 			pos += chunkSize, slot++)
 		{
 			const uint64_t len = std::min(chunkSize, blockEnd - pos);
-			const uint64_t chunkIdx = pos >> crcChunkShift;
-			const bool hasLine = file && file->hasLine(chunkIdx);
+			const uint64_t chunkIdx = pos >> checksumChunkShift;
+			const uint8_t* actual = values + slot * checksumValueBytes;
+			const uint8_t* expected = (file && file->hasLine(chunkIdx) ) ?
+				&file->values[chunkIdx * checksumValueBytes] : NULL;
 
-			if(hasLine && (file->chunkLength(chunkIdx, chunkSize) == len) &&
-				!memcmp(&file->digests[chunkIdx * 8], slots[slot], elb_blake3_algo::DIGEST_BYTES) )
+			if(expected && (file->chunkLength(chunkIdx, chunkSize) == len) &&
+				!memcmp(expected, actual, checksumValueBytes) )
 			{
 				numChecksumChunksChecked++;
 				continue;
 			}
 
-			const std::string expected = hasLine ?
-				elb_blake3_hex(&file->digests[chunkIdx * 8]) : std::string("-");
+			std::string label;
+			elb_with_checksum_algo(checksumAlgo, [&](auto algo) { label = algo.LABEL; } );
 
 			throw WorkerError("Checksum verification failed. File: " + blockFilePath(block) +
 				"; Offset: " + std::to_string(pos) + "; Length: " + std::to_string(len) + "; "
-				"Expected " + elb_blake3_algo::LABEL + ": " + expected + "; Actual " +
-				elb_blake3_algo::LABEL + ": " + elb_blake3_hex(slots[slot]) );
+				"Expected " + label + ": " +
+				(expected ? elb_checksum_hex(expected, checksumValueBytes) : "-") + "; Actual " +
+				label + ": " + elb_checksum_hex(actual, checksumValueBytes) );
 		}
 	}
 }
@@ -3053,9 +3035,13 @@ std::vector<FileChecksum> Worker::getFileChecksums() const
 	std::vector<FileChecksum> checksums;
 
 	for(const auto& entry : checksumAccs)
-		checksums.push_back(FileChecksum{blockFilePath(entry.second.block),
-			blockFileSize(entry.second.block), entry.second.numBytes, entry.second.rawCrc,
-			entry.second.chunks, entry.second.blake3, entry.second.chunkDigests});
+	{
+		checksums.push_back(entry.second.file);
+		checksums.back().path = blockFilePath(entry.second.block);
+		checksums.back().size = blockFileSize(entry.second.block);
+		checksums.back().algo = checksumAlgo;
+		checksums.back().chunkShift = checksumChunkShift;
+	}
 
 	return checksums;
 }

@@ -122,20 +122,11 @@ struct DamageRun
 	uint16_t firstSectorLo{0}; // where the block starts in the first sector (0: before it)
 };
 
-/* --checksumchunk: the CRC of one chunk of a file that a phase moved */
-struct ChunkChecksum
+/* --checksumchunk: one chunk of a file that a phase moved (its value: FileChecksum::chunkValues) */
+struct ChecksumChunk
 {
 	uint64_t offset;
 	uint64_t length;
-	uint64_t rawCrc; // (elb_crc_chunks)
-};
-
-/* --checksumchunk --checksumalgo blake3: the digest of one chunk of a file that a phase moved */
-struct ChunkDigest
-{
-	uint64_t offset;
-	uint64_t length;
-	uint32_t digest[8];
 };
 
 /**
@@ -165,36 +156,49 @@ struct Blake3Runs
 	bool finish(uint64_t fileSize, uint32_t outDigest[8]) const;
 };
 
+/**
+ * --checksums of whole files: what the blocks of one file that a phase moved add up to. A CRC
+ * XORs the blocks' raw contributions (elb_crc_chunks); BLAKE3 holds their runs (Blake3Runs).
+ */
+struct WholeFileChecksum
+{
+	uint64_t rawCrc{0};
+	Blake3Runs blake3;
+
+	// a block's slots of the whole-file launch of algo (enum elb_checksum_algo)
+	void add(int algo, const void* slots, uint64_t offset, uint64_t len, uint64_t fileSize);
+	void merge(const WholeFileChecksum& other, uint64_t fileSize);
+	// the file's finished value (elb_checksum_value_bytes), if the parts make the file
+	bool finish(int algo, uint64_t fileSize, uint8_t* outValue) const;
+};
+
 /* --checksums: what a worker moved of one file in a phase */
 struct FileChecksum
 {
 	std::string path; // as the worker opened the file
 	uint64_t size{0};     // the file's data set size
 	uint64_t numBytes{0}; // bytes of the blocks the phase moved
-	uint64_t rawCrc{0};   // XOR of the blocks' contributions (elb_crc_chunks)
-	std::vector<ChunkChecksum> chunks; // --checksumchunk: the chunks instead, in the order moved
-	Blake3Runs blake3;                 // blake3: the runs instead of rawCrc
-	std::vector<ChunkDigest> chunkDigests; // blake3 --checksumchunk: instead of chunks
+	int algo{ELB_CHECKSUM_CRC32}; // the phase's algorithm (enum elb_checksum_algo)
+	unsigned chunkShift{64};      // and its chunks (64: whole files)
+	WholeFileChecksum whole;           // whole files
+	std::vector<ChecksumChunk> chunks; // --checksumchunk: the chunks instead, in the order moved
+	std::vector<uint8_t> chunkValues;  // and their finished values, one after the other
 };
 
 /**
  * --checksumverify: the last section with a chunk size of a checksum list that --checksums
  * --checksumchunk wrote: "# phase WRITE|READ chunk <K> [algorithm]", then lines "path offset
- * length crc". One CRC (4 bytes, 8 for 64-bit algorithms; a BLAKE3 digest: 32) and one bit per
- * chunk of each listed file; lines shorter than K (a file's last chunk) keep their length aside.
+ * length value". One finished value (4 bytes for the 32-bit CRCs, 8 for CRC-64/NVME, 32 for
+ * BLAKE3) and one bit per chunk of each listed file; lines shorter than K (a file's last chunk)
+ * keep their length aside.
  */
 struct ChecksumList
 {
 	struct File
 	{
 		std::string path;
-		std::vector<uint32_t> crcs;   // the CRC by chunk index (64-bit algorithms: the low half)
-		std::vector<uint32_t> crcsHi; // 64-bit algorithms: the high half, else empty
-		std::vector<uint32_t> digests; // blake3: 8 words per chunk index instead of crcs
-		std::vector<bool> present;    // whether the chunk has a line
-
-		uint64_t crc(uint64_t chunkIdx) const
-			{ return crcs[chunkIdx] | (crcsHi.empty() ? 0 : (uint64_t)crcsHi[chunkIdx] << 32); }
+		std::vector<uint8_t> values; // the finished value by chunk index (valueBytes each)
+		std::vector<bool> present;   // whether the chunk has a line
 		std::map<uint64_t, uint64_t> shortLengths; // chunk index -> length of lines shorter than K
 
 		bool hasLine(uint64_t chunkIdx) const
@@ -208,6 +212,7 @@ struct ChecksumList
 
 	unsigned chunkShift{0};
 	int algo{ELB_CHECKSUM_CRC32}; // enum elb_checksum_algo
+	unsigned valueBytes{4};       // elb_checksum_value_bytes(algo)
 	uint64_t numChunks{0};
 	std::map<std::string, File> files;
 
@@ -244,7 +249,7 @@ struct GpuStage
 	elb_content content; // what the write fills or the read verifies (NONE: the blocks only move)
 	bool useGraph;    // replay full batches from a CUDA graph (one launch per batch anyway under
 	                  // kernel staging)
-	bool checksum;    // --checksums: each block's CRC contribution from its device slot
+	bool checksum;    // --checksums, a checksum list: the checksum launch over the device slots
 };
 
 /* a batch: a contiguous slice of the rings plus everything its GPU stage needs */
@@ -269,11 +274,12 @@ struct Batch
 	elb_verify_result* hostResults{NULL}; // pinned
 	unsigned* devDoneTicket{NULL};
 
-	/* --checksums: bytes from each block's end to its file's end (pinned, read by the CRC kernel)
-	   and the blocks' CRC contributions, published to pinned memory by the kernel's last CTA */
+	/* --checksums, a checksum list: bytes from each block's end to its file's end (pinned, read by
+	   the checksum kernel) and the blocks' slots (a raw CRC, a BLAKE3 CV or digest), which the
+	   kernel publishes to pinned memory */
 	uint64_t* hostShifts{NULL};
-	void* devCrcs{NULL};  // zero, re-zeroed by the kernel (the algorithm's word per slot)
-	void* hostCrcs{NULL};
+	void* devSums{NULL};  // zero, re-zeroed by the kernel (the algorithm's value bytes per slot)
+	void* hostSums{NULL};
 
 	// aio state
 	std::vector<struct iocb> iocbs;
@@ -446,23 +452,21 @@ class Worker
 		uint64_t numDamageBytesDropped{0};
 		std::string deferredVerifyError;
 
-		/* --checksums: the XOR of the CRC contributions and the bytes of each file this worker
-		   moved in the phase, by numeric file identity; paths are resolved at the phase end */
+		/* --checksums: what this worker moved of each file in the phase, by numeric file identity,
+		   with a block of the file; paths and sizes are resolved at the phase end */
 		typedef std::pair<uint64_t, uint64_t> FileID; // (blockFileID)
 		struct ChecksumAcc
 		{
-			BlockRef block; // (a block of the file, for its path)
-			uint64_t numBytes{0};
-			uint64_t rawCrc{0};
-			std::vector<ChunkChecksum> chunks; // --checksumchunk
-			Blake3Runs blake3;                 // blake3: instead of rawCrc
-			std::vector<ChunkDigest> chunkDigests; // blake3 --checksumchunk: instead of chunks
+			BlockRef block; // (a block of the file, for its path and size)
+			FileChecksum file;
 		};
 		std::map<FileID, ChecksumAcc> checksumAccs;
-		unsigned crcChunkShift{64};    // the CRC launch's chunks (64: whole files), setupChecksums
-		uint64_t crcSlotsPerDesc{1};   // CRC slots per block
-		int crcAlgo{ELB_CHECKSUM_CRC32}; // the launch's algorithm (enum elb_checksum_algo)
-		size_t crcWordBytes{4};          // bytes of a slot (blake3: a 32-byte digest or CV)
+		unsigned checksumChunkShift{64};  // the checksum launch's chunks (64: whole files)
+		uint64_t checksumSlotsPerDesc{1}; // its slots per block
+		int checksumAlgo{ELB_CHECKSUM_CRC32}; // its algorithm (enum elb_checksum_algo)
+		unsigned checksumValueBytes{4};   // bytes of a slot and of a finished value
+		std::vector<uint8_t> chunkValues; // finishChunkValues: of the batch being retired
+		const Batch* chunkValuesBatch{NULL}; // the batch they are of (NULL: none since its launch)
 		/* --checksumverify: the list entry of each file the phase read (NULL: not listed) and the
 		   chunks that matched */
 		std::map<FileID, const ChecksumList::File*> checksumListFiles;
@@ -506,11 +510,9 @@ class Worker
 			bool oneFilePerBatch = false);
 		void verifyWrittenBatch(Batch& batch);
 		void accountBatch(Batch& batch, uint64_t gpuUSecTotal);
-		uint64_t batchCrc(const Batch& batch, uint64_t slot) const;
+		const uint8_t* finishChunkValues(const Batch& batch);
 		void addBatchChecksums(const Batch& batch);
-		void addBatchDigests(const Batch& batch);
 		void checkBatchChecksums(const Batch& batch);
-		void checkBatchDigests(const Batch& batch);
 		void setupChecksums();
 		FileID blockFileID(const BlockRef& block) const;
 		uint64_t blockFileSize(const BlockRef& block) const;
@@ -586,15 +588,13 @@ class Manager
 		/* --checksums: each file of the last phase, merged over all workers */
 		struct ChecksumReport
 		{
-			std::string lines; // "<path> <size> <bytes covered> <crc or ->\n", sorted by path;
-			                   // --checksumchunk: "<path> <offset> <length> <crc>\n" per chunk
+			std::string lines; // "<path> <size> <bytes covered> <value or ->\n", sorted by path;
+			                   // --checksumchunk: "<path> <offset> <length> <value>\n" per chunk
 			uint64_t numFiles{0};
-			uint64_t numComplete{0}; // files with a CRC
+			uint64_t numComplete{0}; // files with a value
 			uint64_t numChunks{0};   // --checksumchunk
 		};
 		ChecksumReport getChecksumReport();
-		ChecksumReport getChunkChecksumReport();
-		ChecksumReport getChunkDigestReport();
 
 		/* --checksumverify: parse a checksum list and check the following read phases against
 		   it (throws WorkerError); the chunks and files the last phase checked */
