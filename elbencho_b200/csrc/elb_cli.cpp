@@ -1126,6 +1126,16 @@ void ProgArgs::checkArgs()
 		throw ProgError("No benchmark phase selected. Try \"--help\".");
 }
 
+void ProgArgs::ABIConfig::useGPU0IfNone()
+{
+	if(!gpuIDs.empty() )
+		return;
+
+	gpuIDs.push_back(0);
+	cfg.gpuIDs = gpuIDs.data();
+	cfg.numGPUIDs = 1;
+}
+
 void ProgArgs::toABIConfig(ABIConfig& out) const
 {
 	memset(&out.cfg, 0, sizeof(out.cfg) );

@@ -11,6 +11,7 @@
 
 #include <stdint.h>
 
+#include <functional>
 #include <map>
 #include <memory>
 #include <ostream>
@@ -191,6 +192,10 @@ class ProgArgs
 			std::vector<int32_t> gpuIDs;
 			std::vector<int32_t> cpuCores;
 			std::vector<int32_t> numaZones;
+
+			/* GPU 0 if the config names none ("all" or master mode), for the expected totals of
+			   a phase, which do not depend on the GPUs */
+			void useGPU0IfNone();
 		};
 		void toABIConfig(ABIConfig& out) const;
 
@@ -271,6 +276,51 @@ namespace stats
 		const elb_phase_results& res, uint64_t phaseID, const std::string& isoStartDate); // :2429-2723
 	void printDryRunPhaseInfo(const ProgArgs& progArgs, int benchPhase, uint64_t entriesPerThread,
 		uint64_t bytesPerThread, std::ostream& out); // :2850-2876
+
+	/* local time now: "2026-01-01T00:00:00+0000", or "2026-01-01T00:00:00.000+0000" withMillis */
+	std::string isoDateNow(bool withMillis);
+
+	/* Statistics::printPhaseResults (:1568-1632): one phase's results on the console and in
+	 * --resfile, --csvfile and --jsonfile; without worker elapsed times a "Skipping stats print"
+	 * line instead. @isoStartDate the phase start, for CSV and JSON. */
+	void writePhaseResults(const ProgArgs& progArgs, int benchPhase, const elb_phase_results& res,
+		const std::vector<uint64_t>& elapsedUSecVec, const std::string& isoStartDate,
+		uint64_t phaseID,
+		const std::vector<std::pair<uint64_t, std::string> >* svcCompletionMS = NULL);
+
+	/* a --livecsv row after its ISO Date, Label, Phase and RuntimeMS columns; an empty string
+	 * leaves a column empty */
+	struct LiveCSVRow
+	{
+		std::string rank, mixType, percentDone, doneBytes, mibPerSec, iopsPerSec, entries,
+			entriesPerSec, latEntriesUSec, latIOUSec, numActive, cpuPercent, service;
+	};
+
+	/* the "Total" rows of one --livecsv update, one per mix type */
+	void addLiveCSVTotalRows(const ProgArgs& progArgs, const elb_liveops liveOps[2],
+		const elb_liveops oldLiveOps[2], const elb_livelat& liveLat, uint64_t intervalUSec,
+		bool isRWMixPhase, uint64_t expectedEntries, uint64_t expectedBytes, uint64_t numActive,
+		uint64_t cpuPercent, std::vector<LiveCSVRow>& rows);
+
+	/* --livecsvex: the rows of one worker or service, one per mix type, without per-second and
+	 * latency values */
+	void addLiveCSVRankRows(const ProgArgs& progArgs, size_t rank, const elb_liveops ops[2],
+		bool isRWMixPhase, uint64_t expectedEntries, uint64_t expectedBytes,
+		const std::string& numActive, const std::string& cpuPercent, const std::string& service,
+		std::vector<LiveCSVRow>& rows);
+
+	/* Statistics::prepLiveCSVFile + printLiveStatsCSV (:2944-3230): appends the rows of one update
+	 * to the --livecsv file or writes them to stdout; the header goes into an empty file, or once
+	 * to stdout */
+	class LiveCSVWriter
+	{
+		public:
+			void write(const ProgArgs& progArgs, int benchPhase, uint64_t elapsedMS,
+				const std::vector<LiveCSVRow>& rows);
+
+		private:
+			bool headerPrinted{false};
+	};
 }
 
 /* size of the first existing file / block device if cfg->fileSize is 0 (ProgArgs.cpp:2071-2210) */
@@ -278,6 +328,12 @@ uint64_t detectFileSize(const elb_cfg* abiCfg);
 
 /* Coordinator::waitForUserDefinedStartTime (Coordinator.cpp:149-158) */
 void waitForUserDefinedStartTime(const ProgArgs& progArgs);
+
+/* Coordinator::runBenchmarks (Coordinator.cpp:298-374): each iteration runs the enabled phases
+ * through runPhase, each phase followed by the sync and dropcaches phases; between two phases the
+ * --phasedelay sleep, then betweenPhases (if set) */
+void runPhaseSequence(const ProgArgs& progArgs, const std::function<void(int)>& runPhase,
+	const std::function<void()>& betweenPhases);
 
 /* expected entries/bytes per worker (WorkerManager::getPhaseNumEntriesAndBytes, :333-487) */
 class TreeManifest;

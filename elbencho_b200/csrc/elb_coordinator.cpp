@@ -1,20 +1,19 @@
 /*
  * Coordinator: what the reference's main() + Coordinator do for a local run
  * (source/Main.cpp:13-68, source/Coordinator.cpp:31-142 main, :248-272 runBenchmarkPhase,
- * :298-374 runBenchmarks, :380-413 runSyncAndDropCaches, :418-440 signal handling) on top of the
- * native manager, plus the live statistics loop (source/Statistics.cpp:180-300, 1232-1345).
+ * :298-413 runBenchmarks + runSyncAndDropCaches as runPhaseSequence, which the distributed master
+ * shares, :418-440 signal handling) on top of the native manager, plus the live statistics loop
+ * (source/Statistics.cpp:180-300, 1232-1345).
  *
  * Exported as elb_cli_main(argc, argv) so that the tiny elbencho-b200 executable, tests and any
  * embedding program share one implementation.
  */
 #include <signal.h>
 #include <sys/ioctl.h>
-#include <sys/stat.h>
 #include <time.h>
 #include <unistd.h>
 
 #include <fstream>
-#include <iomanip>
 #include <iostream>
 #include <sstream>
 
@@ -31,30 +30,6 @@ static void interruptSignalHandler(int signal) // Coordinator.cpp:418-440
 {
 	(void)signal;
 	gotUserInterruptSignal = 1;
-}
-
-static std::string isoDateNow(bool withMillis)
-{
-	struct timespec now;
-	clock_gettime(CLOCK_REALTIME, &now);
-
-	struct tm localTimeInfo;
-	localtime_r(&now.tv_sec, &localTimeInfo);
-
-	char dateBuf[64];
-	char zoneBuf[16];
-	strftime(dateBuf, sizeof(dateBuf), "%FT%T", &localTimeInfo);
-	strftime(zoneBuf, sizeof(zoneBuf), "%z", &localTimeInfo);
-
-	std::ostringstream out;
-	out << dateBuf;
-
-	if(withMillis)
-		out << "." << std::setfill('0') << std::setw(3) << (now.tv_nsec / 1000000);
-
-	out << zoneBuf;
-
-	return out.str();
 }
 
 std::string stats::elapsedSecToHumanStr(uint64_t elapsedSec) // UnitTk::elapsedSecToHumanStr
@@ -86,10 +61,8 @@ class Coordinator
 		CPUUtil liveCpuUtil;
 		uint64_t phaseCounter{0};
 
-		void runBenchmarks();
 		void runBenchmarkPhase(int benchPhase);
-		void runSyncAndDropCaches();
-		bool liveCSVHeaderPrinted{false};
+		stats::LiveCSVWriter liveCSV;
 		bool isPhaseTimeExpired{false}; // WorkersSharedData::isPhaseTimeExpired
 		void printLiveStatsCSV(int benchPhase, const elb_liveops liveOps[2],
 			const elb_liveops oldLiveOps[2], const elb_livelat& liveLat, uint64_t intervalUSec,
@@ -98,7 +71,6 @@ class Coordinator
 		void printLiveStatsLine(int benchPhase, const elb_liveops liveOps[2],
 			const elb_liveops oldLiveOps[2], uint64_t intervalUSec, size_t numWorkersDone,
 			uint64_t elapsedSec);
-		void printPhaseResultsEverywhere(int benchPhase, const std::string& isoStartDate);
 		void writeVerifyReportSection(int benchPhase);
 		void writeChecksumSection(int benchPhase);
 		void printChecksumVerifyLine(int benchPhase);
@@ -110,13 +82,7 @@ void Coordinator::printDryRunInfo()
 {
 	ProgArgs::ABIConfig abiConfig;
 	progArgs.toABIConfig(abiConfig);
-
-	if(abiConfig.gpuIDs.empty() )
-	{ // "all" or master mode: the GPU list does not matter for the expected totals
-		abiConfig.gpuIDs.push_back(0);
-		abiConfig.cfg.gpuIDs = abiConfig.gpuIDs.data();
-		abiConfig.cfg.numGPUIDs = 1;
-	}
+	abiConfig.useGPU0IfNone();
 
 	abiConfig.cfg.fileSize = detectFileSize(&abiConfig.cfg);
 
@@ -213,199 +179,33 @@ void Coordinator::printLiveStatsLine(int benchPhase, const elb_liveops liveOps[2
 	std::cout << lineStr << std::flush;
 }
 
-/* Statistics::prepLiveCSVFile + printLiveStatsCSV (:2944-3113): one "Total" line per interval
- * (plus a "Read" line in rwmix phases) with the aggregate of all local workers */
+/* Statistics::printLiveStatsCSV (:2944-3225): the "Total" rows of all local workers and, with
+ * --livecsvex, one row per worker with its totals so far */
 void Coordinator::printLiveStatsCSV(int benchPhase, const elb_liveops liveOps[2],
 	const elb_liveops oldLiveOps[2], const elb_livelat& liveLat, uint64_t intervalUSec,
 	size_t numWorkersDone, uint64_t expectedEntries, uint64_t expectedBytes, uint64_t elapsedMS)
 {
-	const bool toStdout = (progArgs.liveCSVFilePath == "stdout");
-	std::ofstream fileStream;
-	bool printHeaders = toStdout ? !liveCSVHeaderPrinted : false;
-
-	if(!toStdout)
-	{
-		struct stat statBuf;
-		printHeaders = (stat(progArgs.liveCSVFilePath.c_str(), &statBuf) != 0) ||
-			!statBuf.st_size;
-
-		fileStream.open(progArgs.liveCSVFilePath, std::ofstream::app);
-
-		if(!fileStream)
-			throw ProgError("Unable to open live stats csv file: " + progArgs.liveCSVFilePath);
-	}
-
-	std::ostream& out = toStdout ? std::cout : fileStream;
-
-	if(printHeaders)
-		out << "ISO Date,Label,Phase,RuntimeMS,Rank,MixType,Done%,DoneBytes,MiB/s,IOPS,Entries,"
-			"Entries/s,Lat Ent us,Lat IO us,Active,CPU,Service," << std::endl;
-
-	liveCSVHeaderPrinted = true;
-
 	const bool isRWMixPhase = (liveOps[1].numBytesDone || liveOps[1].numEntriesDone);
-	const bool isDirMode = (progArgs.benchPathType == ELB_PATH_DIR);
-	const std::string isoDate = isoDateNow(true);
-	const std::string phaseName = stats::phaseName(benchPhase, progArgs);
-	std::string label = progArgs.benchLabel;
-	std::replace(label.begin(), label.end(), ',', ' ');
+	const size_t numWorkers = manager->workers.size();
+	std::vector<stats::LiveCSVRow> rows;
 
 	liveCpuUtil.update();
 
-	auto perSec = [&](uint64_t newVal, uint64_t oldVal)
-		{ return intervalUSec ? perSecFromUSec(newVal - oldVal, intervalUSec) : 0; };
-	auto percentDone = [&](const elb_liveops& ops)
-	{
-		uint64_t percent = 0;
+	stats::addLiveCSVTotalRows(progArgs, liveOps, oldLiveOps, liveLat, intervalUSec, isRWMixPhase,
+		expectedEntries, expectedBytes, numWorkers - numWorkersDone,
+		liveCpuUtil.getCPUUtilPercent(), rows);
 
-		if(expectedBytes)
-			percent = (100 * ops.numBytesDone) / expectedBytes;
-		else
-		if(expectedEntries)
-			percent = (100 * ops.numEntriesDone) / expectedEntries;
-
-		return std::min(percent, (uint64_t)100);
-	};
-	auto avg = [](uint64_t sum, uint64_t num) { return num ? (sum / num) : 0; };
-
-	for(int mixIdx = 0; mixIdx < (isRWMixPhase ? 2 : 1); mixIdx++)
-	{
-		const elb_liveops& ops = liveOps[mixIdx];
-		const elb_liveops& oldOps = oldLiveOps[mixIdx];
-
-		out << isoDate << "," << label << "," << phaseName << "," << elapsedMS << "," <<
-			"Total" << "," << (isRWMixPhase ? (mixIdx ? "Read" : "Write") : "") << "," <<
-			percentDone(ops) << "," << ops.numBytesDone << "," <<
-			(perSec(ops.numBytesDone, oldOps.numBytesDone) / (1024 * 1024) ) << "," <<
-			perSec(ops.numIOPSDone, oldOps.numIOPSDone) << "," <<
-			(isDirMode ? ops.numEntriesDone : 0) << "," <<
-			(isDirMode ? perSec(ops.numEntriesDone, oldOps.numEntriesDone) : 0) << "," <<
-			(mixIdx ? avg(liveLat.avgEntriesLatReadMixMicrosSecsSum,
-				liveLat.numAvgEntriesLatReadMixValues) :
-				avg(liveLat.avgEntriesLatMicroSecsSum, liveLat.numAvgEntriesLatValues) ) << "," <<
-			(mixIdx ? avg(liveLat.avgIOLatReadMixMicroSecsSum, liveLat.numAvgIOLatReadMixValues) :
-				avg(liveLat.avgIOLatMicroSecsSum, liveLat.numAvgIOLatValues) ) << "," <<
-			(manager->workers.size() - numWorkersDone) << "," <<
-			liveCpuUtil.getCPUUtilPercent() << "," << "" << "," << std::endl;
-	}
-
-	if(!progArgs.useExtendedLiveCSV)
-		return;
-
-	/* --livecsvex: one more line per worker with its totals so far; no per-second and latency
-	   values there (Statistics.cpp:3116-3225) */
-	const size_t numWorkers = manager->workers.size();
-	const uint64_t bytesPerWorker = numWorkers ? (expectedBytes / numWorkers) : 0;
-	const uint64_t entriesPerWorker = numWorkers ? (expectedEntries / numWorkers) : 0;
-
-	for(size_t workerIdx = 0; workerIdx < numWorkers; workerIdx++)
-	{
-		const elb_liveops workerOps[2] = { manager->workers[workerIdx]->getLiveOps(),
-			manager->workers[workerIdx]->getLiveOpsReadMix() };
-
-		for(int mixIdx = 0; mixIdx < (isRWMixPhase ? 2 : 1); mixIdx++)
+	if(progArgs.useExtendedLiveCSV)
+		for(size_t workerIdx = 0; workerIdx < numWorkers; workerIdx++)
 		{
-			const elb_liveops& ops = workerOps[mixIdx];
-			uint64_t workerPercentDone = 0;
+			const elb_liveops workerOps[2] = { manager->workers[workerIdx]->getLiveOps(),
+				manager->workers[workerIdx]->getLiveOpsReadMix() };
 
-			if(bytesPerWorker)
-				workerPercentDone = (100 * ops.numBytesDone) / bytesPerWorker;
-			else
-			if(entriesPerWorker)
-				workerPercentDone = (100 * ops.numEntriesDone) / entriesPerWorker;
-
-			out << isoDate << "," << label << "," << phaseName << "," << elapsedMS << "," <<
-				workerIdx << "," << (isRWMixPhase ? (mixIdx ? "Read" : "Write") : "") << "," <<
-				std::min(workerPercentDone, (uint64_t)100) << "," << ops.numBytesDone << "," <<
-				"" << "," << "" << "," << (isDirMode ? ops.numEntriesDone : 0) << "," <<
-				"" << "," << "" << "," << "" << "," << ",,," << std::endl;
-		}
-	}
-}
-
-/* Statistics::printPhaseResults (:1568-1632): console + optional txt/csv/json files */
-void Coordinator::printPhaseResultsEverywhere(int benchPhase, const std::string& isoStartDate)
-{
-	elb_phase_results res;
-	manager->getPhaseResults(res);
-
-	std::vector<uint64_t> elapsedUSecVec;
-	for(const std::unique_ptr<Worker>& worker : manager->workers)
-		if(worker->getElapsedUSec() )
-			elapsedUSecVec.push_back(worker->getElapsedUSec() );
-
-	const bool haveResults = !elapsedUSecVec.empty();
-
-	if(!haveResults)
-		std::cout << "Skipping stats print due to unavailable worker results." << std::endl;
-	else
-		stats::printPhaseResults(progArgs, benchPhase, res, elapsedUSecVec, std::cout);
-
-	if(!progArgs.resFilePath.empty() )
-	{
-		std::ofstream fileStream(progArgs.resFilePath, std::ofstream::app);
-
-		if(!fileStream)
-			std::cerr << "ERROR: Opening results file failed: " << progArgs.resFilePath <<
-				std::endl;
-		else
-		{
-			if(!haveResults)
-				fileStream << "Skipping stats print due to unavailable worker results." <<
-					std::endl;
-			else
-				stats::printPhaseResults(progArgs, benchPhase, res, elapsedUSecVec, fileStream);
-
-			fileStream << std::endl;
-		}
-	}
-
-	if(haveResults && !progArgs.csvFilePath.empty() )
-	{
-		std::vector<std::string> labels, values;
-		stats::csvLabelsAndValues(progArgs, benchPhase, res, isoDateNow(false), labels, values);
-
-		// labels line only for a new/empty file (Coordinator.cpp checkCSVFileCompatibility)
-		bool needLabels = !progArgs.noCSVLabels;
-		{
-			std::ifstream existing(progArgs.csvFilePath);
-			if(existing && (existing.peek() != std::ifstream::traits_type::eof() ) )
-				needLabels = false;
+			stats::addLiveCSVRankRows(progArgs, workerIdx, workerOps, isRWMixPhase,
+				expectedEntries / numWorkers, expectedBytes / numWorkers, "", "", "", rows);
 		}
 
-		std::ofstream fileStream(progArgs.csvFilePath, std::ofstream::app);
-
-		if(!fileStream)
-			std::cerr << "ERROR: Opening results CSV file failed: " << progArgs.csvFilePath <<
-				std::endl;
-		else
-		{
-			auto joinCSV = [](const std::vector<std::string>& vec)
-			{
-				std::string line;
-				for(size_t i = 0; i < vec.size(); i++)
-					line += (i ? "," : "") + vec[i];
-				return line;
-			};
-
-			if(needLabels)
-				fileStream << joinCSV(labels) << std::endl;
-
-			fileStream << joinCSV(values) << std::endl;
-		}
-	}
-
-	if(haveResults && !progArgs.jsonFilePath.empty() )
-	{
-		std::ofstream fileStream(progArgs.jsonFilePath, std::ofstream::app);
-
-		if(!fileStream)
-			std::cerr << "ERROR: Opening results JSON file failed: " << progArgs.jsonFilePath <<
-				std::endl;
-		else
-			fileStream << stats::phaseResultsJSON(progArgs, benchPhase, res, phaseCounter,
-				isoStartDate) << std::endl;
-	}
+	liveCSV.write(progArgs, benchPhase, elapsedMS, rows);
 }
 
 /* --verifyreport: after each phase that verified data (a read, or a write with --verifydirect),
@@ -485,7 +285,7 @@ void Coordinator::runBenchmarkPhase(int benchPhase)
 	if(isPhaseTimeExpired)
 		throw ProgTimeLimit();
 
-	const std::string isoStartDate = isoDateNow(true);
+	const std::string isoStartDate = stats::isoDateNow(true);
 	const Clock::time_point phaseStartT = Clock::now();
 
 	phaseCounter++;
@@ -502,7 +302,6 @@ void Coordinator::runBenchmarkPhase(int benchPhase)
 		(isatty(STDOUT_FILENO) || getenv("ELB_FORCE_LIVESTATS") );
 	const bool writeLiveCSV = !progArgs.liveCSVFilePath.empty();
 	const bool showLive = showLiveLine || writeLiveCSV;
-	const bool useLiveReduce = (manager->getNumGPUs() >= 2);
 
 	uint64_t expectedEntries = 0, expectedBytes = 0; // of all local workers, for "Done%"
 	manager->getExpectedTotals(benchPhase, expectedEntries, expectedBytes);
@@ -526,35 +325,17 @@ void Coordinator::runBenchmarkPhase(int benchPhase)
 		if(progArgs.timeLimitSecs && (elapsedSec >= progArgs.timeLimitSecs) )
 		{ // WorkerManager::checkPhaseTimeLimit (:109-128): friendly interruption, results stay
 			isPhaseTimeExpired = true;
-			std::unique_lock<std::mutex> lock(manager->shared.mutex);
-			for(Worker* worker : manager->shared.workers)
-				worker->interruptExecution();
+			manager->interruptWorkers();
 		}
 
 		if(!showLive)
 			continue;
 
-		elb_liveops liveOps[2] = {};
+		elb_liveops liveOps[2];
 		elb_livelat liveLat = {};
 		size_t numWorkersDone;
 
-		if(useLiveReduce)
-		{ // workers on several GPUs: per-GPU partial sums, reduced over NVLink by NCCL
-			elb_live_snapshot snapshot;
-			manager->getLiveSnapshot(snapshot);
-			liveOps[0] = snapshot.ops;
-			liveOps[1] = snapshot.opsReadMix;
-			liveLat = snapshot.lat;
-		}
-		else
-			for(const std::unique_ptr<Worker>& worker : manager->workers)
-			{
-				liveOpsAdd(liveOps[0], worker->getLiveOps() );
-				liveOpsAdd(liveOps[1], worker->getLiveOpsReadMix() );
-
-				if(writeLiveCSV)
-					worker->getAndResetLiveLatency(liveLat);
-			}
+		manager->getLiveOps(liveOps, writeLiveCSV ? &liveLat : NULL);
 
 		{
 			std::unique_lock<std::mutex> lock(manager->shared.mutex);
@@ -619,20 +400,21 @@ void Coordinator::runBenchmarkPhase(int benchPhase)
 		throw ProgError("Worker encountered error"); // WorkerManager.cpp:54-58
 	}
 
-	if( (benchPhase != ELB_PHASE_SYNC) && (benchPhase != ELB_PHASE_DROPCACHES) )
-	{
-		printPhaseResultsEverywhere(benchPhase, isoStartDate);
-		writeVerifyReportSection(benchPhase);
-		writeChecksumSection(benchPhase);
-		printChecksumVerifyLine(benchPhase);
-	}
-	else
+	elb_phase_results res;
+	manager->getPhaseResults(res);
+
+	if( (benchPhase == ELB_PHASE_SYNC) || (benchPhase == ELB_PHASE_DROPCACHES) )
 	{ // (sync and dropcache phases print only their elapsed time)
-		elb_phase_results res;
-		manager->getPhaseResults(res);
 		std::vector<uint64_t> elapsedUSecVec(1, res.lastFinishUSec);
 		stats::printPhaseResults(progArgs, benchPhase, res, elapsedUSecVec, std::cout);
+		return;
 	}
+
+	stats::writePhaseResults(progArgs, benchPhase, res, manager->getElapsedUSecVec(), isoStartDate,
+		phaseCounter);
+	writeVerifyReportSection(benchPhase);
+	writeChecksumSection(benchPhase);
+	printChecksumVerifyLine(benchPhase);
 }
 
 void waitForUserDefinedStartTime(const ProgArgs& progArgs) // Coordinator.cpp:149-158
@@ -651,16 +433,8 @@ void waitForUserDefinedStartTime(const ProgArgs& progArgs) // Coordinator.cpp:14
 		usleep(1000);
 }
 
-void Coordinator::runSyncAndDropCaches() // Coordinator.cpp:380-413
-{
-	if(progArgs.runSyncPhase)
-		runBenchmarkPhase(ELB_PHASE_SYNC);
-
-	if(progArgs.runDropCachesPhase)
-		runBenchmarkPhase(ELB_PHASE_DROPCACHES);
-}
-
-void Coordinator::runBenchmarks() // Coordinator.cpp:298-374
+void runPhaseSequence(const ProgArgs& progArgs, const std::function<void(int)>& runPhase,
+	const std::function<void()>& betweenPhases)
 {
 	struct BenchPhaseConfig { int benchPhase; bool runPhase; };
 
@@ -679,6 +453,15 @@ void Coordinator::runBenchmarks() // Coordinator.cpp:298-374
 		if(phaseConfig.runPhase)
 			enabledPhases.push_back(phaseConfig.benchPhase);
 
+	auto runSyncAndDropCaches = [&]() // Coordinator.cpp:380-413
+	{
+		if(progArgs.runSyncPhase)
+			runPhase(ELB_PHASE_SYNC);
+
+		if(progArgs.runDropCachesPhase)
+			runPhase(ELB_PHASE_DROPCACHES);
+	};
+
 	for(uint64_t iterationIndex = 0; iterationIndex < progArgs.iterations; iterationIndex++)
 	{
 		if(progArgs.iterations > 1)
@@ -691,12 +474,18 @@ void Coordinator::runBenchmarks() // Coordinator.cpp:298-374
 
 		for(size_t phaseIdx = 0; phaseIdx < enabledPhases.size(); phaseIdx++)
 		{
-			runBenchmarkPhase(enabledPhases[phaseIdx] );
+			runPhase(enabledPhases[phaseIdx] );
 
 			runSyncAndDropCaches();
 
-			if( (phaseIdx < (enabledPhases.size() - 1) ) && progArgs.nextPhaseDelaySecs)
+			if(phaseIdx == (enabledPhases.size() - 1) )
+				continue;
+
+			if(progArgs.nextPhaseDelaySecs)
 				sleep( (unsigned)progArgs.nextPhaseDelaySecs);
+
+			if(betweenPhases)
+				betweenPhases();
 		}
 	}
 }
@@ -780,7 +569,8 @@ int Coordinator::main() // Coordinator.cpp:31-142
 
 		waitForUserDefinedStartTime(progArgs);
 
-		runBenchmarks();
+		runPhaseSequence(progArgs, [this](int benchPhase) { runBenchmarkPhase(benchPhase); },
+			nullptr);
 
 		manager.reset();
 	}

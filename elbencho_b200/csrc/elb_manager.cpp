@@ -125,8 +125,7 @@ Manager::~Manager()
 			std::unique_lock<std::mutex> lock(shared.mutex);
 			shared.currentBenchPhase = ELB_PHASE_TERMINATE;
 			shared.currentBenchSeq++;
-			for(Worker* worker : shared.workers)
-				worker->interruptExecution();
+			interruptWorkersLocked();
 			shared.condition.notify_all();
 		}
 
@@ -145,6 +144,47 @@ void Manager::getLiveSnapshot(elb_live_snapshot& out)
 		liveStatsReducer.reset(new LiveStatsReducer(*this) );
 
 	liveStatsReducer->snapshot(out);
+}
+
+void Manager::getLiveOps(elb_liveops outLiveOps[2], elb_livelat* outLiveLat, bool exactSums)
+{
+	outLiveOps[0] = outLiveOps[1] = elb_liveops{};
+
+	if(outLiveLat)
+		*outLiveLat = elb_livelat{};
+
+	if(!exactSums && (getNumGPUs() >= 2) )
+	{ // workers on several GPUs: per-GPU partial sums, reduced over NVLink by NCCL
+		elb_live_snapshot snapshot;
+		getLiveSnapshot(snapshot);
+		outLiveOps[0] = snapshot.ops;
+		outLiveOps[1] = snapshot.opsReadMix;
+
+		if(outLiveLat)
+			*outLiveLat = snapshot.lat;
+
+		return;
+	}
+
+	for(const std::unique_ptr<Worker>& worker : workers)
+	{
+		liveOpsAdd(outLiveOps[0], worker->getLiveOps() );
+		liveOpsAdd(outLiveOps[1], worker->getLiveOpsReadMix() );
+
+		if(outLiveLat)
+			worker->getAndResetLiveLatency(*outLiveLat);
+	}
+}
+
+std::vector<uint64_t> Manager::getElapsedUSecVec() const
+{
+	std::vector<uint64_t> elapsedUSecVec;
+
+	for(const std::unique_ptr<Worker>& worker : workers)
+		if(worker->getElapsedUSec() )
+			elapsedUSecVec.push_back(worker->getElapsedUSec() );
+
+	return elapsedUSecVec;
 }
 
 size_t Manager::getNumGPUs() const
@@ -383,8 +423,7 @@ int Manager::waitForWorkersDone(int timeoutMS)
 	{
 		if(shared.numWorkersDoneWithError)
 		{ // a worker failed: ask the others to stop and wait for them (:54-58)
-			for(Worker* worker : shared.workers)
-				worker->interruptExecution();
+			interruptWorkersLocked();
 
 			while(shared.numWorkersDone < numWorkersTotal)
 				shared.condition.wait_for(lock, std::chrono::milliseconds(100) );
@@ -408,12 +447,25 @@ int Manager::waitForWorkersDone(int timeoutMS)
 	}
 }
 
+/* WorkerManager::checkPhaseTimeLimit (WorkerManager.cpp:109-128): a friendly interruption */
+void Manager::interruptWorkers()
+{
+	std::unique_lock<std::mutex> lock(shared.mutex);
+
+	interruptWorkersLocked();
+}
+
+void Manager::interruptWorkersLocked()
+{
+	for(Worker* worker : shared.workers)
+		worker->interruptExecution();
+}
+
 void Manager::interruptAndNotifyWorkers() // WorkerManager.cpp:75-90
 {
 	std::unique_lock<std::mutex> lock(shared.mutex);
 
-	for(Worker* worker : shared.workers)
-		worker->interruptExecution();
+	interruptWorkersLocked();
 
 	shared.currentBenchPhase = ELB_PHASE_TERMINATE;
 	shared.currentBenchSeq++;
@@ -1446,15 +1498,7 @@ int elb_mgr_run_phase(elb_mgr* m, int benchPhase)
 
 int elb_mgr_live_ops(elb_mgr* m, elb_liveops out[2])
 {
-	out[0] = elb_liveops{};
-	out[1] = elb_liveops{};
-
-	for(const std::unique_ptr<elb::Worker>& worker : m->impl->workers)
-	{
-		elb::liveOpsAdd(out[0], worker->getLiveOps() );
-		elb::liveOpsAdd(out[1], worker->getLiveOpsReadMix() );
-	}
-
+	m->impl->getLiveOps(out, NULL, true);
 	return 0;
 }
 

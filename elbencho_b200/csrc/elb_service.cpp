@@ -774,8 +774,7 @@ class Service
 		HttpResponse handleInterruptPhase(const HttpRequest& request);
 		void resetManager();
 		void collectErrHistory();
-		void putCommonStats(JsonTree& tree, bool isFinal,
-			const elb_live_snapshot* liveSnapshot = NULL);
+		void putCommonStats(JsonTree& tree, bool isFinal, const elb_liveops liveOps[2]);
 };
 
 void Service::resetManager()
@@ -830,26 +829,13 @@ static void histogramFromTree(const JsonTree& tree, const std::string& prefix, e
 }
 
 /* common part of /status and /benchresult (Statistics.cpp:1350-1405, 2728-2804) */
-void Service::putCommonStats(JsonTree& tree, bool isFinal, const elb_live_snapshot* liveSnapshot)
+void Service::putCommonStats(JsonTree& tree, bool isFinal, const elb_liveops liveOps[2])
 {
-	elb_liveops liveOps[2] = {};
 	size_t numWorkersDone = 0, numWorkersDoneWithError = 0;
 	bool stoneWallTriggered = false;
 
 	if(manager)
 	{
-		if(liveSnapshot)
-		{
-			liveOps[0] = liveSnapshot->ops;
-			liveOps[1] = liveSnapshot->opsReadMix;
-		}
-		else
-			for(const std::unique_ptr<Worker>& worker : manager->workers)
-			{
-				liveOpsAdd(liveOps[0], worker->getLiveOps() );
-				liveOpsAdd(liveOps[1], worker->getLiveOpsReadMix() );
-			}
-
 		std::unique_lock<std::mutex> lock(manager->shared.mutex);
 		numWorkersDoneWithError = manager->shared.numWorkersDoneWithError;
 		/* (the reference counts workers with error separately from numWorkersDone,
@@ -887,11 +873,11 @@ HttpResponse Service::handleStatus()
 
 	/* workers on several GPUs: per-GPU partial sums reduced over NVLink by NCCL
 	   (LiveStatsReducer); final results always come from the exact per-worker values */
-	elb_live_snapshot liveSnapshot;
-	const bool useLiveReduce = manager && (manager->getNumGPUs() >= 2);
+	elb_liveops liveOps[2] = {};
+	elb_livelat liveLat = {};
 
-	if(useLiveReduce)
-		manager->getLiveSnapshot(liveSnapshot);
+	if(manager)
+		manager->getLiveOps(liveOps, &liveLat);
 
 	/* phase time limit: the master polls /status every few hundred ms, so this is where the
 	   service notices the expiry and asks its workers to finish (friendly interruption, the
@@ -899,27 +885,14 @@ HttpResponse Service::handleStatus()
 	if(manager && progArgs.timeLimitSecs && (currentPhase != ELB_PHASE_IDLE) &&
 		( (uint64_t)std::chrono::duration_cast<std::chrono::seconds>(
 			Clock::now() - phaseStartT).count() >= progArgs.timeLimitSecs) )
-	{
-		std::unique_lock<std::mutex> lock(manager->shared.mutex);
+		manager->interruptWorkers();
 
-		for(Worker* worker : manager->shared.workers)
-			worker->interruptExecution();
-	}
-
-	putCommonStats(tree, false, useLiveReduce ? &liveSnapshot : NULL);
+	putCommonStats(tree, false, liveOps);
 
 	liveCpuUtil.update();
 	tree.put("CPUUtil", liveCpuUtil.getCPUUtilPercent() );
 	tree.put("ElapsedSecs", (uint64_t)std::chrono::duration_cast<std::chrono::seconds>(
 		Clock::now() - phaseStartT).count() );
-
-	elb_livelat liveLat = {};
-	if(useLiveReduce)
-		liveLat = liveSnapshot.lat;
-	else
-	if(manager)
-		for(const std::unique_ptr<Worker>& worker : manager->workers)
-			worker->getAndResetLiveLatency(liveLat);
 
 	tree.put("NumIOLatUSec", liveLat.numAvgIOLatValues);
 	tree.put("SumIOLatUSec", liveLat.avgIOLatMicroSecsSum);
@@ -953,7 +926,10 @@ HttpResponse Service::handleBenchResult()
 		return response;
 	}
 
-	putCommonStats(tree, true);
+	elb_liveops liveOps[2];
+	manager->getLiveOps(liveOps, NULL, true);
+
+	putCommonStats(tree, true, liveOps);
 
 	elb_phase_results res;
 	manager->getPhaseResults(res);
@@ -989,10 +965,7 @@ HttpResponse Service::handleBenchResult()
 	tree.put("ErrorHistory", errHistory);
 
 	// show results when running in foreground (HTTPServiceSWS.cpp:241)
-	std::vector<uint64_t> elapsedUSecVec;
-	for(const std::unique_ptr<Worker>& worker : manager->workers)
-		if(worker->getElapsedUSec() )
-			elapsedUSecVec.push_back(worker->getElapsedUSec() );
+	const std::vector<uint64_t> elapsedUSecVec = manager->getElapsedUSecVec();
 
 	if(!elapsedUSecVec.empty() )
 	{
@@ -1128,13 +1101,8 @@ HttpResponse Service::handlePreparePhase(const HttpRequest& request)
 
 		checkAuthorization(request);
 
-		time_t currentTime = time(NULL);
-		struct tm localTimeInfo;
-		localtime_r(&currentTime, &localTimeInfo);
-		char dateBuf[64];
-		strftime(dateBuf, sizeof(dateBuf), "%FT%T%z", &localTimeInfo);
-
-		std::cout << "Preparing new benchmark phase... (ISO DATE: " << dateBuf << ")" << std::endl;
+		std::cout << "Preparing new benchmark phase... (ISO DATE: " << stats::isoDateNow(false) <<
+			")" << std::endl;
 
 		JsonTree recvTree = JsonTree::parse(request.body);
 
@@ -1862,7 +1830,6 @@ class Master
 		void initHosts();
 		void prepareRemotePhases();
 		void runPhase(int benchPhase);
-		void runSyncAndDropCaches();
 		void interruptAll(bool quit);
 		void waitForServicesReady();
 		void rotateHosts();
@@ -1870,7 +1837,7 @@ class Master
 		void printLiveStatsCSV(int benchPhase, elb_liveops oldLiveOps[2],
 			Clock::time_point& lastT, const Clock::time_point& phaseStartT,
 			uint64_t expectedEntries, uint64_t expectedBytes);
-		bool liveCSVHeaderPrinted{false};
+		stats::LiveCSVWriter liveCSV;
 		bool isPhaseTimeExpired{false};
 };
 
@@ -2001,15 +1968,9 @@ void Master::runPhase(int benchPhase)
 	const bool isRWMixConfig = (progArgs.rwMixReadPercent || progArgs.numRWMixReadThreads) &&
 		(benchPhase == ELB_PHASE_CREATEFILES);
 
-	phaseCounter++;
+	const std::string isoStartDate = stats::isoDateNow(true);
 
-	char isoBuf[64];
-	{
-		time_t nowSecs = time(NULL);
-		struct tm localTimeInfo;
-		localtime_r(&nowSecs, &localTimeInfo);
-		strftime(isoBuf, sizeof(isoBuf), "%FT%T.000%z", &localTimeInfo);
-	}
+	phaseCounter++;
 
 	for(RemoteHost& remote : hosts)
 	{
@@ -2253,79 +2214,22 @@ void Master::runPhase(int benchPhase)
 	res.cpuUtilStoneWallPercent = (uint32_t)(cpuStoneWallSum / hosts.size() );
 	res.cpuUtilPercent = (uint32_t)(cpuLastDoneSum / hosts.size() );
 
-	if(allElapsedUSec.empty() )
-		std::cout << "Skipping stats print due to unavailable worker results." << std::endl;
-	else
+	// --svcelapsed: slowest thread of each service (Statistics.cpp:2093-2108)
+	std::vector<std::pair<uint64_t, std::string> > svcCompletionMS;
+
+	for(const RemoteHost& remote : hosts)
 	{
-		// --svcelapsed: slowest thread of each service (Statistics.cpp:2093-2108)
-		std::vector<std::pair<uint64_t, std::string> > svcCompletionMS;
+		uint64_t slowestThreadUSec = 0;
 
-		for(const RemoteHost& remote : hosts)
-		{
-			uint64_t slowestThreadUSec = 0;
+		for(uint64_t elapsedUSec : remote.elapsedUSecVec)
+			slowestThreadUSec = std::max(slowestThreadUSec, elapsedUSec);
 
-			for(uint64_t elapsedUSec : remote.elapsedUSecVec)
-				slowestThreadUSec = std::max(slowestThreadUSec, elapsedUSec);
-
-			svcCompletionMS.push_back(std::make_pair(slowestThreadUSec / 1000,
-				remote.host + ":" + std::to_string(remote.port) ) );
-		}
-
-		stats::printPhaseResults(progArgs, benchPhase, res, allElapsedUSec, std::cout,
-			&svcCompletionMS);
-
-		if(!progArgs.resFilePath.empty() )
-		{
-			std::ofstream fileStream(progArgs.resFilePath, std::ofstream::app);
-			stats::printPhaseResults(progArgs, benchPhase, res, allElapsedUSec, fileStream,
-				&svcCompletionMS);
-			fileStream << std::endl;
-		}
-
-		if(!progArgs.csvFilePath.empty() )
-		{
-			std::vector<std::string> labels, values;
-			stats::csvLabelsAndValues(progArgs, benchPhase, res, isoBuf, labels, values);
-
-			bool needLabels = !progArgs.noCSVLabels;
-			{
-				std::ifstream existing(progArgs.csvFilePath);
-				if(existing && (existing.peek() != std::ifstream::traits_type::eof() ) )
-					needLabels = false;
-			}
-
-			std::ofstream fileStream(progArgs.csvFilePath, std::ofstream::app);
-
-			auto joinCSV = [](const std::vector<std::string>& vec)
-			{
-				std::string line;
-				for(size_t i = 0; i < vec.size(); i++)
-					line += (i ? "," : "") + vec[i];
-				return line;
-			};
-
-			if(needLabels)
-				fileStream << joinCSV(labels) << std::endl;
-
-			fileStream << joinCSV(values) << std::endl;
-		}
-
-		if(!progArgs.jsonFilePath.empty() )
-		{
-			std::ofstream fileStream(progArgs.jsonFilePath, std::ofstream::app);
-			fileStream << stats::phaseResultsJSON(progArgs, benchPhase, res, phaseCounter,
-				isoBuf) << std::endl;
-		}
+		svcCompletionMS.push_back(std::make_pair(slowestThreadUSec / 1000,
+			remote.host + ":" + std::to_string(remote.port) ) );
 	}
-}
 
-void Master::runSyncAndDropCaches()
-{
-	if(progArgs.runSyncPhase)
-		runPhase(ELB_PHASE_SYNC);
-
-	if(progArgs.runDropCachesPhase)
-		runPhase(ELB_PHASE_DROPCACHES);
+	stats::writePhaseResults(progArgs, benchPhase, res, allElapsedUSec, isoStartDate, phaseCounter,
+		&svcCompletionMS);
 }
 
 /* Coordinator::waitForServicesReady (Coordinator.cpp:160-230): GET /status on every service until
@@ -2378,13 +2282,7 @@ void Master::getExpectedTotals(int benchPhase, uint64_t& outEntries, uint64_t& o
 	{
 		ProgArgs::ABIConfig abiConfig;
 		progArgs.toABIConfig(abiConfig);
-
-		if(abiConfig.gpuIDs.empty() )
-		{
-			abiConfig.gpuIDs.push_back(0);
-			abiConfig.cfg.gpuIDs = abiConfig.gpuIDs.data();
-			abiConfig.cfg.numGPUIDs = 1;
-		}
+		abiConfig.useGPU0IfNone();
 
 		abiConfig.cfg.pathType = progArgs.benchPathType; // (as reported by the services)
 		abiConfig.cfg.treeFilePath = NULL;
@@ -2402,39 +2300,18 @@ void Master::getExpectedTotals(int benchPhase, uint64_t& outEntries, uint64_t& o
 	catch(std::exception& e) { }
 }
 
-/* Statistics::printLiveStatsCSV in a distributed run (Statistics.cpp:3017-3230): a "Total" line
- * per update (plus a "Read" line in rwmix phases) and, with --livecsvex, one line per service
- * with its threads left, CPU utilisation and host name */
+/* Statistics::printLiveStatsCSV in a distributed run (Statistics.cpp:3017-3230): the "Total" rows
+ * of all services and, with --livecsvex, one row per service with its threads left, CPU
+ * utilisation and host name */
 void Master::printLiveStatsCSV(int benchPhase, elb_liveops oldLiveOps[2], Clock::time_point& lastT,
 	const Clock::time_point& phaseStartT, uint64_t expectedEntries, uint64_t expectedBytes)
 {
-	const bool toStdout = (progArgs.liveCSVFilePath == "stdout");
-	std::ofstream fileStream;
-	bool printHeaders = toStdout ? !liveCSVHeaderPrinted : false;
-
-	if(!toStdout)
-	{
-		struct stat statBuf;
-		printHeaders = (stat(progArgs.liveCSVFilePath.c_str(), &statBuf) != 0) ||
-			!statBuf.st_size;
-
-		fileStream.open(progArgs.liveCSVFilePath, std::ofstream::app);
-
-		if(!fileStream)
-			throw ProgError("Unable to open live stats csv file: " + progArgs.liveCSVFilePath);
-	}
-
-	std::ostream& out = toStdout ? std::cout : fileStream;
-
-	if(printHeaders)
-		out << "ISO Date,Label,Phase,RuntimeMS,Rank,MixType,Done%,DoneBytes,MiB/s,IOPS,Entries,"
-			"Entries/s,Lat Ent us,Lat IO us,Active,CPU,Service," << std::endl;
-
-	liveCSVHeaderPrinted = true;
-
 	elb_liveops liveOps[2] = {};
 	elb_livelat liveLat = {};
 	uint64_t numThreadsLeft = 0, cpuSum = 0;
+
+	auto threadsLeft = [&](const RemoteHost& remote)
+		{ return progArgs.numThreads - std::min(progArgs.numThreads, (uint64_t)remote.numWorkersDone); };
 
 	for(RemoteHost& remote : hosts)
 	{
@@ -2445,93 +2322,37 @@ void Master::printLiveStatsCSV(int benchPhase, elb_liveops oldLiveOps[2], Clock:
 		liveLat.numAvgEntriesLatValues += remote.liveLat.numAvgEntriesLatValues;
 		liveLat.avgEntriesLatMicroSecsSum += remote.liveLat.avgEntriesLatMicroSecsSum;
 		remote.liveLat = elb_livelat{};
-		numThreadsLeft += progArgs.numThreads - std::min(progArgs.numThreads,
-			(uint64_t)remote.numWorkersDone);
+		numThreadsLeft += threadsLeft(remote);
 		cpuSum += remote.cpuUtilLive;
 	}
 
 	const Clock::time_point nowT = Clock::now();
-	const uint64_t intervalUSec =
-		std::chrono::duration_cast<std::chrono::microseconds>(nowT - lastT).count();
-	const uint64_t elapsedMS =
-		std::chrono::duration_cast<std::chrono::milliseconds>(nowT - phaseStartT).count();
 	const bool isRWMixPhase = (liveOps[1].numBytesDone || liveOps[1].numEntriesDone);
-	const bool isDirMode = (progArgs.benchPathType == ELB_PATH_DIR);
-	const std::string phaseName = stats::phaseName(benchPhase, progArgs);
-	std::string label = progArgs.benchLabel;
-	std::replace(label.begin(), label.end(), ',', ' ');
+	std::vector<stats::LiveCSVRow> rows;
 
-	char isoBuf[64];
-	{
-		struct timeval timeVal;
-		gettimeofday(&timeVal, NULL);
-		struct tm localTimeInfo;
-		localtime_r(&timeVal.tv_sec, &localTimeInfo);
-		char dateBuf[32], zoneBuf[16];
-		strftime(dateBuf, sizeof(dateBuf), "%FT%T", &localTimeInfo);
-		strftime(zoneBuf, sizeof(zoneBuf), "%z", &localTimeInfo);
-		snprintf(isoBuf, sizeof(isoBuf), "%s.%03d%s", dateBuf, (int)(timeVal.tv_usec / 1000),
-			zoneBuf);
-	}
+	stats::addLiveCSVTotalRows(progArgs, liveOps, oldLiveOps, liveLat,
+		std::chrono::duration_cast<std::chrono::microseconds>(nowT - lastT).count(), isRWMixPhase,
+		expectedEntries, expectedBytes, numThreadsLeft, hosts.empty() ? 0 : (cpuSum / hosts.size() ),
+		rows);
 
-	auto perSec = [&](uint64_t newVal, uint64_t oldVal)
-		{ return intervalUSec ? perSecFromUSec(newVal - oldVal, intervalUSec) : 0; };
-	auto percentDone = [](const elb_liveops& ops, uint64_t bytesTotal, uint64_t entriesTotal)
-	{
-		uint64_t percent = 0;
+	if(progArgs.useExtendedLiveCSV)
+		for(size_t hostIdx = 0; hostIdx < hosts.size(); hostIdx++)
+		{
+			const RemoteHost& remote = hosts[hostIdx];
+			const elb_liveops remoteOps[2] = {remote.liveOps, remote.liveOpsReadMix};
 
-		if(bytesTotal)
-			percent = (100 * ops.numBytesDone) / bytesTotal;
-		else
-		if(entriesTotal)
-			percent = (100 * ops.numEntriesDone) / entriesTotal;
+			stats::addLiveCSVRankRows(progArgs, hostIdx, remoteOps, isRWMixPhase,
+				expectedEntries / hosts.size(), expectedBytes / hosts.size(),
+				std::to_string(threadsLeft(remote) ), std::to_string(remote.cpuUtilLive),
+				remote.host + ":" + std::to_string(remote.port), rows);
+		}
 
-		return std::min(percent, (uint64_t)100);
-	};
-	auto avg = [](uint64_t sum, uint64_t num) { return num ? (sum / num) : 0; };
+	liveCSV.write(progArgs, benchPhase,
+		std::chrono::duration_cast<std::chrono::milliseconds>(nowT - phaseStartT).count(), rows);
 
-	for(int mixIdx = 0; mixIdx < (isRWMixPhase ? 2 : 1); mixIdx++)
-	{
-		const elb_liveops& ops = liveOps[mixIdx];
-
-		out << isoBuf << "," << label << "," << phaseName << "," << elapsedMS << "," <<
-			"Total" << "," << (isRWMixPhase ? (mixIdx ? "Read" : "Write") : "") << "," <<
-			percentDone(ops, expectedBytes, expectedEntries) << "," << ops.numBytesDone << "," <<
-			(perSec(ops.numBytesDone, oldLiveOps[mixIdx].numBytesDone) / (1024 * 1024) ) << "," <<
-			perSec(ops.numIOPSDone, oldLiveOps[mixIdx].numIOPSDone) << "," <<
-			(isDirMode ? ops.numEntriesDone : 0) << "," <<
-			(isDirMode ? perSec(ops.numEntriesDone, oldLiveOps[mixIdx].numEntriesDone) : 0) <<
-			"," << (mixIdx ? 0 : avg(liveLat.avgEntriesLatMicroSecsSum,
-				liveLat.numAvgEntriesLatValues) ) << "," <<
-			(mixIdx ? 0 : avg(liveLat.avgIOLatMicroSecsSum, liveLat.numAvgIOLatValues) ) << "," <<
-			numThreadsLeft << "," << (hosts.empty() ? 0 : (cpuSum / hosts.size() ) ) << "," <<
-			"" << "," << std::endl;
-
-		oldLiveOps[mixIdx] = ops;
-	}
-
+	oldLiveOps[0] = liveOps[0];
+	oldLiveOps[1] = liveOps[1];
 	lastT = nowT;
-
-	if(!progArgs.useExtendedLiveCSV)
-		return;
-
-	for(size_t hostIdx = 0; hostIdx < hosts.size(); hostIdx++)
-	{
-		const RemoteHost& remote = hosts[hostIdx];
-		const elb_liveops remoteOps[2] = {remote.liveOps, remote.liveOpsReadMix};
-
-		for(int mixIdx = 0; mixIdx < (isRWMixPhase ? 2 : 1); mixIdx++)
-			out << isoBuf << "," << label << "," << phaseName << "," << elapsedMS << "," <<
-				hostIdx << "," << (isRWMixPhase ? (mixIdx ? "Read" : "Write") : "") << "," <<
-				percentDone(remoteOps[mixIdx], expectedBytes / hosts.size(),
-					expectedEntries / hosts.size() ) << "," <<
-				remoteOps[mixIdx].numBytesDone << "," << "" << "," << "" << "," <<
-				(isDirMode ? remoteOps[mixIdx].numEntriesDone : 0) << "," << "" << "," << "" <<
-				"," << "" << "," <<
-				(progArgs.numThreads - std::min(progArgs.numThreads,
-					(uint64_t)remote.numWorkersDone) ) << "," << remote.cpuUtilLive << "," <<
-				remote.host << ":" << remote.port << "," << std::endl;
-	}
 }
 
 /* Coordinator::rotateHosts (Coordinator.cpp:382-404) + ProgArgs::rotateHosts (:4137-4144): between
@@ -2561,44 +2382,8 @@ int Master::run()
 
 		waitForUserDefinedStartTime(progArgs);
 
-		struct BenchPhaseConfig { int benchPhase; bool runPhase; };
-
-		const BenchPhaseConfig allBenchPhases[] =
-		{
-			{ELB_PHASE_CREATEDIRS, progArgs.runCreateDirsPhase},
-			{ELB_PHASE_CREATEFILES, progArgs.runCreateFilesPhase},
-			{ELB_PHASE_STATFILES, progArgs.runStatFilesPhase},
-			{ELB_PHASE_READFILES, progArgs.runReadPhase},
-			{ELB_PHASE_DELETEFILES, progArgs.runDeleteFilesPhase},
-			{ELB_PHASE_DELETEDIRS, progArgs.runDeleteDirsPhase},
-		};
-
-		for(uint64_t iterationIndex = 0; iterationIndex < progArgs.iterations; iterationIndex++)
-		{
-			if(progArgs.iterations > 1)
-				std::cout << "[Starting iteration " << (iterationIndex + 1) << " of " <<
-					progArgs.iterations << "...]" << std::endl;
-
-			stats::printPhaseResultsTableHeader(std::cout);
-
-			runSyncAndDropCaches();
-
-			bool isFirstPhase = true;
-
-			for(const BenchPhaseConfig& phaseConfig : allBenchPhases)
-			{
-				if(!phaseConfig.runPhase)
-					continue;
-
-				if(!isFirstPhase)
-					rotateHosts();
-
-				isFirstPhase = false;
-
-				runPhase(phaseConfig.benchPhase);
-				runSyncAndDropCaches();
-			}
-		}
+		runPhaseSequence(progArgs, [this](int benchPhase) { runPhase(benchPhase); },
+			[this]() { rotateHosts(); });
 	}
 	catch(ProgTimeLimit& e)
 	{ // a user-defined time limit, not an error

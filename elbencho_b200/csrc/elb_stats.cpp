@@ -1,13 +1,19 @@
 /*
  * Statistics output in the reference's formats (see elb_cli.h): console table
  * (source/Statistics.cpp:1546-1562, 1771-2140, 2325-2400), CSV columns (:2151-2323 +
- * ProgArgs::getAsStringVec ProgArgs.cpp:3865-3912), JSON (:2429-2723), dry run (:2850-2876).
+ * ProgArgs::getAsStringVec ProgArgs.cpp:3865-3912), JSON (:2429-2723), dry run (:2850-2876), and
+ * the results and live CSV files that local and distributed runs write with them (:1568-1632,
+ * 2944-3230).
  */
 #include <stdio.h>
+#include <sys/stat.h>
+#include <time.h>
 
 #include <algorithm>
 #include <cmath>
+#include <fstream>
 #include <iomanip>
+#include <iostream>
 #include <sstream>
 
 #include "elb_cli.h"
@@ -727,6 +733,233 @@ void printDryRunPhaseInfo(const ProgArgs& progArgs, int benchPhase, uint64_t ent
 	out << "* Bytes total:        " << bytesTotal << " | " <<
 		(bytesTotal / (1024 * 1024) ) << " MiB" " | " <<
 		(bytesTotal / (1024 * 1024 * 1024) ) << " GiB" << std::endl;
+}
+
+std::string isoDateNow(bool withMillis)
+{
+	struct timespec now;
+	clock_gettime(CLOCK_REALTIME, &now);
+
+	struct tm localTimeInfo;
+	localtime_r(&now.tv_sec, &localTimeInfo);
+
+	char dateBuf[64];
+	char zoneBuf[16];
+	strftime(dateBuf, sizeof(dateBuf), "%FT%T", &localTimeInfo);
+	strftime(zoneBuf, sizeof(zoneBuf), "%z", &localTimeInfo);
+
+	std::ostringstream out;
+	out << dateBuf;
+
+	if(withMillis)
+		out << "." << std::setfill('0') << std::setw(3) << (now.tv_nsec / 1000000);
+
+	out << zoneBuf;
+
+	return out.str();
+}
+
+void writePhaseResults(const ProgArgs& progArgs, int benchPhase, const elb_phase_results& res,
+	const std::vector<uint64_t>& elapsedUSecVec, const std::string& isoStartDate, uint64_t phaseID,
+	const std::vector<std::pair<uint64_t, std::string> >* svcCompletionMS)
+{
+	const bool haveResults = !elapsedUSecVec.empty();
+	const char* skipLine = "Skipping stats print due to unavailable worker results.";
+
+	if(!haveResults)
+		std::cout << skipLine << std::endl;
+	else
+		printPhaseResults(progArgs, benchPhase, res, elapsedUSecVec, std::cout, svcCompletionMS);
+
+	if(!progArgs.resFilePath.empty() )
+	{
+		std::ofstream fileStream(progArgs.resFilePath, std::ofstream::app);
+
+		if(!fileStream)
+			std::cerr << "ERROR: Opening results file failed: " << progArgs.resFilePath <<
+				std::endl;
+		else
+		{
+			if(!haveResults)
+				fileStream << skipLine << std::endl;
+			else
+				printPhaseResults(progArgs, benchPhase, res, elapsedUSecVec, fileStream,
+					svcCompletionMS);
+
+			fileStream << std::endl;
+		}
+	}
+
+	if(!haveResults)
+		return;
+
+	if(!progArgs.csvFilePath.empty() )
+	{
+		std::vector<std::string> labels, values;
+		csvLabelsAndValues(progArgs, benchPhase, res, isoStartDate, labels, values);
+
+		// labels line only for a new/empty file (Coordinator.cpp checkCSVFileCompatibility)
+		bool needLabels = !progArgs.noCSVLabels;
+		{
+			std::ifstream existing(progArgs.csvFilePath);
+			if(existing && (existing.peek() != std::ifstream::traits_type::eof() ) )
+				needLabels = false;
+		}
+
+		std::ofstream fileStream(progArgs.csvFilePath, std::ofstream::app);
+
+		if(!fileStream)
+			std::cerr << "ERROR: Opening results CSV file failed: " << progArgs.csvFilePath <<
+				std::endl;
+		else
+		{
+			auto joinCSV = [](const std::vector<std::string>& vec)
+			{
+				std::string line;
+				for(size_t i = 0; i < vec.size(); i++)
+					line += (i ? "," : "") + vec[i];
+				return line;
+			};
+
+			if(needLabels)
+				fileStream << joinCSV(labels) << std::endl;
+
+			fileStream << joinCSV(values) << std::endl;
+		}
+	}
+
+	if(!progArgs.jsonFilePath.empty() )
+	{
+		std::ofstream fileStream(progArgs.jsonFilePath, std::ofstream::app);
+
+		if(!fileStream)
+			std::cerr << "ERROR: Opening results JSON file failed: " << progArgs.jsonFilePath <<
+				std::endl;
+		else
+			fileStream << phaseResultsJSON(progArgs, benchPhase, res, phaseID, isoStartDate) <<
+				std::endl;
+	}
+}
+
+/* "Done%" of a live row: of the expected bytes, or of the expected entries if no bytes */
+static uint64_t livePercentDone(const elb_liveops& ops, uint64_t expectedEntries,
+	uint64_t expectedBytes)
+{
+	uint64_t percent = 0;
+
+	if(expectedBytes)
+		percent = (100 * ops.numBytesDone) / expectedBytes;
+	else
+	if(expectedEntries)
+		percent = (100 * ops.numEntriesDone) / expectedEntries;
+
+	return std::min(percent, (uint64_t)100);
+}
+
+static const char* liveMixType(bool isRWMixPhase, int mixIdx)
+{
+	return isRWMixPhase ? (mixIdx ? "Read" : "Write") : "";
+}
+
+void addLiveCSVTotalRows(const ProgArgs& progArgs, const elb_liveops liveOps[2],
+	const elb_liveops oldLiveOps[2], const elb_livelat& liveLat, uint64_t intervalUSec,
+	bool isRWMixPhase, uint64_t expectedEntries, uint64_t expectedBytes, uint64_t numActive,
+	uint64_t cpuPercent, std::vector<LiveCSVRow>& rows)
+{
+	const bool isDirMode = (progArgs.benchPathType == ELB_PATH_DIR);
+
+	auto perSec = [&](uint64_t newVal, uint64_t oldVal)
+		{ return intervalUSec ? perSecFromUSec(newVal - oldVal, intervalUSec) : 0; };
+	auto avg = [](uint64_t sum, uint64_t num) { return num ? (sum / num) : 0; };
+
+	const uint64_t latEntriesUSec[2] = {
+		avg(liveLat.avgEntriesLatMicroSecsSum, liveLat.numAvgEntriesLatValues),
+		avg(liveLat.avgEntriesLatReadMixMicrosSecsSum, liveLat.numAvgEntriesLatReadMixValues) };
+	const uint64_t latIOUSec[2] = {
+		avg(liveLat.avgIOLatMicroSecsSum, liveLat.numAvgIOLatValues),
+		avg(liveLat.avgIOLatReadMixMicroSecsSum, liveLat.numAvgIOLatReadMixValues) };
+
+	for(int mixIdx = 0; mixIdx < (isRWMixPhase ? 2 : 1); mixIdx++)
+	{
+		const elb_liveops& ops = liveOps[mixIdx];
+		const elb_liveops& oldOps = oldLiveOps[mixIdx];
+
+		LiveCSVRow row;
+		row.rank = "Total";
+		row.mixType = liveMixType(isRWMixPhase, mixIdx);
+		row.percentDone = num(livePercentDone(ops, expectedEntries, expectedBytes) );
+		row.doneBytes = num(ops.numBytesDone);
+		row.mibPerSec = num(perSec(ops.numBytesDone, oldOps.numBytesDone) / (1024 * 1024) );
+		row.iopsPerSec = num(perSec(ops.numIOPSDone, oldOps.numIOPSDone) );
+		row.entries = num(isDirMode ? ops.numEntriesDone : 0);
+		row.entriesPerSec = num(isDirMode ? perSec(ops.numEntriesDone, oldOps.numEntriesDone) : 0);
+		row.latEntriesUSec = num(latEntriesUSec[mixIdx] );
+		row.latIOUSec = num(latIOUSec[mixIdx] );
+		row.numActive = num(numActive);
+		row.cpuPercent = num(cpuPercent);
+		rows.push_back(row);
+	}
+}
+
+void addLiveCSVRankRows(const ProgArgs& progArgs, size_t rank, const elb_liveops ops[2],
+	bool isRWMixPhase, uint64_t expectedEntries, uint64_t expectedBytes,
+	const std::string& numActive, const std::string& cpuPercent, const std::string& service,
+	std::vector<LiveCSVRow>& rows)
+{
+	const bool isDirMode = (progArgs.benchPathType == ELB_PATH_DIR);
+
+	for(int mixIdx = 0; mixIdx < (isRWMixPhase ? 2 : 1); mixIdx++)
+	{
+		LiveCSVRow row;
+		row.rank = num(rank);
+		row.mixType = liveMixType(isRWMixPhase, mixIdx);
+		row.percentDone = num(livePercentDone(ops[mixIdx], expectedEntries, expectedBytes) );
+		row.doneBytes = num(ops[mixIdx].numBytesDone);
+		row.entries = num(isDirMode ? ops[mixIdx].numEntriesDone : 0);
+		row.numActive = numActive;
+		row.cpuPercent = cpuPercent;
+		row.service = service;
+		rows.push_back(row);
+	}
+}
+
+void LiveCSVWriter::write(const ProgArgs& progArgs, int benchPhase, uint64_t elapsedMS,
+	const std::vector<LiveCSVRow>& rows)
+{
+	const bool toStdout = (progArgs.liveCSVFilePath == "stdout");
+	std::ofstream fileStream;
+	bool printHeader = !headerPrinted;
+
+	if(!toStdout)
+	{
+		struct stat statBuf;
+		printHeader = (stat(progArgs.liveCSVFilePath.c_str(), &statBuf) != 0) || !statBuf.st_size;
+
+		fileStream.open(progArgs.liveCSVFilePath, std::ofstream::app);
+
+		if(!fileStream)
+			throw ProgError("Unable to open live stats csv file: " + progArgs.liveCSVFilePath);
+	}
+
+	std::ostream& out = toStdout ? std::cout : fileStream;
+
+	if(printHeader)
+		out << "ISO Date,Label,Phase,RuntimeMS,Rank,MixType,Done%,DoneBytes,MiB/s,IOPS,Entries,"
+			"Entries/s,Lat Ent us,Lat IO us,Active,CPU,Service," << std::endl;
+
+	headerPrinted = true;
+
+	std::string label = progArgs.benchLabel;
+	std::replace(label.begin(), label.end(), ',', ' ');
+
+	const std::string rowStart = isoDateNow(true) + "," + label + "," +
+		phaseName(benchPhase, progArgs) + "," + num(elapsedMS) + ",";
+
+	for(const LiveCSVRow& row : rows)
+		out << rowStart << row.rank << "," << row.mixType << "," << row.percentDone << "," <<
+			row.doneBytes << "," << row.mibPerSec << "," << row.iopsPerSec << "," << row.entries <<
+			"," << row.entriesPerSec << "," << row.latEntriesUSec << "," << row.latIOUSec << "," <<
+			row.numActive << "," << row.cpuPercent << "," << row.service << "," << std::endl;
 }
 
 } // namespace stats

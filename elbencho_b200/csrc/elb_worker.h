@@ -569,10 +569,18 @@ class Manager
 		std::string getLiveReduceInfo();
 		size_t getNumGPUs() const; // distinct GPUs of the workers
 
+		/* live ops of all workers, [1] of the rwmix reads; outLiveLat (if set) takes their live
+		   latency. Workers on several GPUs: the snapshot, unless exactSums asks for per-worker
+		   sums */
+		void getLiveOps(elb_liveops outLiveOps[2], elb_livelat* outLiveLat,
+			bool exactSums = false);
+
 		void startNextPhase(int benchPhase);
 		int waitForWorkersDone(int timeoutMS); // 1 done, 0 timeout, <0 error
+		void interruptWorkers(); // ask all workers to end the phase early; its results stay
 		void interruptAndNotifyWorkers();
 		void getPhaseResults(elb_phase_results& out);
+		std::vector<uint64_t> getElapsedUSecVec() const; // the non-zero ones of the workers
 		void getExpectedTotals(int benchPhase, uint64_t& outEntries, uint64_t& outBytes);
 
 		/* --verifyreport: the damaged extents of the last phase, merged over all workers */
@@ -608,6 +616,7 @@ class Manager
 		std::mutex lastErrorMutex;
 
 	private:
+		void interruptWorkersLocked(); // (shared.mutex held)
 		void prepareBenchPathFDs();
 		void prepareFilesForPhase(int benchPhase);
 		void closeBenchPathFDs();
