@@ -40,6 +40,7 @@ CONTENT_RANDOM_GRAIN = 3
 class Cfg(ctypes.Structure):
     _fields_ = [
         ("structSize", c_u32),
+        ("dedupeChunkShift", ctypes.c_int32),
         ("paths", ctypes.POINTER(ctypes.c_char_p)),
         ("numPaths", c_u32),
         ("pathType", c_i32),
@@ -258,6 +259,10 @@ SIGNATURES = {
                                          _VP]),
     "elb_blake3_parent": (None, [_VP, _VP, ctypes.c_int, _VP]),
     "elb_blake3_fold": (ctypes.c_int, [_VP, c_u64, c_u64, _VP]),
+    "elb_dedupe_insert": (ctypes.c_int, [_VP, c_u32, ctypes.c_uint, c_u64, _VP, _VP, c_u64, _VP,
+                                         _VP, _VP]),
+    "elb_dedupe_merge": (ctypes.c_int, [_VP, c_u64, _VP, c_u64, _VP, _VP]),
+    "elb_dedupe_zero_digest": (ctypes.c_int, [ctypes.c_uint, _VP]),
     "elb_damage_map": (ctypes.c_int, [_VP, c_u32, ctypes.c_int, c_u64, ctypes.c_uint,
                                       ctypes.c_uint, ctypes.c_uint, _VP, c_u64, _VP]),
     "elb_stage_copy": (ctypes.c_int, [_VP, c_u32, ctypes.c_int, ctypes.c_int64, c_u64, c_u64,
@@ -327,6 +332,8 @@ SIGNATURES = {
     "elb_mgr_set_checksum_list": (ctypes.c_int, [_VP, ctypes.c_char_p, c_u64]),
     "elb_mgr_checksum_verify_counts": (ctypes.c_int, [_VP, ctypes.POINTER(c_u64),
                                                       ctypes.POINTER(c_u64)]),
+    "elb_mgr_dedupe_stats": (ctypes.c_int, [_VP, ctypes.POINTER(c_u64), ctypes.POINTER(c_u64),
+                                            ctypes.POINTER(c_u64)]),
     "elb_mgr_num_workers": (c_u32, [_VP]),
     "elb_mgr_worker": (_VP, [_VP, c_u32]),
     "elb_mgr_last_error": (ctypes.c_char_p, [_VP]),

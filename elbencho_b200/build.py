@@ -17,6 +17,7 @@ LIB_PATH = os.path.join(PKG_DIR, "libelbencho_b200.so")
 SOURCES = [
     "elb_kernels.cu",
     "elb_capi_kernels.cu",
+    "elb_dedupe.cu",
     "elb_config.cpp",
     "elb_cufile.cpp",
     "elb_worker.cpp",

@@ -592,6 +592,98 @@ int elb_blake3_fold(const uint8_t* runs, uint64_t numRuns, uint64_t fileSize, ui
 	return 0;
 }
 
+/* the table checks of elb_dedupe_insert and elb_dedupe_merge */
+static bool dedupeTableArgsValid(const char* what, void* table, uint64_t tableEntries,
+	elb_dedupe_counters* devCounters)
+{
+	if(!tableEntries || (tableEntries & (tableEntries - 1) ) )
+	{
+		elb_set_last_error(std::string(what) + ": table size " + std::to_string(tableEntries) +
+			" is not a power of two");
+		return false;
+	}
+
+	if(!table || !devCounters)
+	{
+		elb_set_last_error(std::string(what) + ": NULL table or counters");
+		return false;
+	}
+
+	return true;
+}
+
+int elb_dedupe_insert(const elb_block_desc* descs, uint32_t numDescs, unsigned chunkShift,
+	uint64_t slotsPerDesc, const void* devDigests, void* table, uint64_t tableEntries,
+	elb_dedupe_counters* devCounters, const uint8_t* zeroDigest, void* stream)
+{
+	const char* what = "elb_dedupe_insert";
+
+	if(!dedupeTableArgsValid(what, table, tableEntries, devCounters) )
+		return -1;
+
+	if( (numDescs && (!descs || !devDigests) ) || !zeroDigest)
+	{
+		elb_set_last_error(std::string(what) + ": NULL descriptor, digest or zero digest array");
+		return -1;
+	}
+
+	if( (chunkShift < ELB_DEDUPE_MIN_CHUNK_SHIFT) || (chunkShift > ELB_DEDUPE_MAX_CHUNK_SHIFT) )
+	{
+		elb_set_last_error(std::string(what) + ": chunk shift " + std::to_string(chunkShift) +
+			" is not in [" + std::to_string(ELB_DEDUPE_MIN_CHUNK_SHIFT) + ", " +
+			std::to_string(ELB_DEDUPE_MAX_CHUNK_SHIFT) + "]");
+		return -1;
+	}
+
+	if(elb_launch_dedupe_insert(descs, numDescs, chunkShift, slotsPerDesc, devDigests, table,
+		tableEntries, devCounters, zeroDigest, (cudaStream_t)stream) )
+	{
+		elb_set_last_error(std::string("elb_") + elb_last_error() );
+		return -1;
+	}
+
+	return 0;
+}
+
+int elb_dedupe_merge(const void* srcEntries, uint64_t numSrcEntries, void* table,
+	uint64_t tableEntries, elb_dedupe_counters* devCounters, void* stream)
+{
+	const char* what = "elb_dedupe_merge";
+
+	if(!dedupeTableArgsValid(what, table, tableEntries, devCounters) )
+		return -1;
+
+	if(numSrcEntries && !srcEntries)
+	{
+		elb_set_last_error(std::string(what) + ": NULL source entries");
+		return -1;
+	}
+
+	if(elb_launch_dedupe_merge(srcEntries, numSrcEntries, table, tableEntries, devCounters,
+		(cudaStream_t)stream) )
+	{
+		elb_set_last_error(std::string("elb_") + elb_last_error() );
+		return -1;
+	}
+
+	return 0;
+}
+
+int elb_dedupe_zero_digest(unsigned chunkShift, uint8_t* out)
+{
+	if( (chunkShift < ELB_DEDUPE_MIN_CHUNK_SHIFT) || (chunkShift > ELB_DEDUPE_MAX_CHUNK_SHIFT) ||
+		!out)
+	{
+		elb_set_last_error("elb_dedupe_zero_digest: chunk shift " + std::to_string(chunkShift) +
+			" is not in [" + std::to_string(ELB_DEDUPE_MIN_CHUNK_SHIFT) + ", " +
+			std::to_string(ELB_DEDUPE_MAX_CHUNK_SHIFT) + "], or NULL output");
+		return -1;
+	}
+
+	elb_dedupe_zero_chunk_digest(chunkShift, out);
+	return 0;
+}
+
 int elb_stage_copy(const elb_block_desc* descs, uint32_t numDescs, int hostToDevice,
 	int64_t hostDelta, uint64_t totalBytes, uint64_t maxBlockLen, void* stream)
 {

@@ -148,6 +148,13 @@ static const OptDef optDefs[] =
 		"with the name, and crc64nvme CRCs have 16 hex digits instead of 8. A list's own "
 		"algorithm is used for --checksumverify. Requires --checksums or --checksumverify. "
 		"(Default: crc32) [b200]"},
+	{"dedupestats", 0, Opt_BYTES, &ProgArgs::dedupeStatsChunkSize, Wire_NONE, "Chunk size of dedupe "
+		"statistics: every write and read phase counts the chunks of this size (a power of two from "
+		"4K to 1G that the block size is a multiple of) that it moved, the distinct ones by their "
+		"BLAKE3 digest (hashed and counted on the GPU) and the ones of zero bytes, over all files "
+		"and threads, and prints \"Dedupe: <N> chunks of <K>, <D> distinct, <Z> zero: <N/D>:1\". "
+		"A file's short last chunk counts as a chunk of its own length. Cannot be used with "
+		"--rand, --norandalign, --infloop, --rwmixpct, --rwmixthr or --hosts. [b200]"},
 	{"rwmixpct", 0, Opt_U64, &ProgArgs::rwMixReadPercent, Wire_REF, "Percentage of blocks that "
 		"should be read in a write phase."},
 	{"rwmixthr", 0, Opt_U64, &ProgArgs::numRWMixReadThreads, Wire_REF, "Number of threads that "
@@ -1030,6 +1037,41 @@ void ProgArgs::checkArgs()
 				"\"--norandalign\"");
 	}
 
+	if(dedupeStatsChunkSize)
+	{ // (each chunk of the data set exactly once, in one direction, on this host)
+		if( (dedupeStatsChunkSize < (1ULL << ELB_CHECKSUM_MIN_CHUNK_SHIFT) ) ||
+			(dedupeStatsChunkSize > (1ULL << ELB_CHECKSUM_MAX_CHUNK_SHIFT) ) ||
+			(dedupeStatsChunkSize & (dedupeStatsChunkSize - 1) ) )
+			throw ProgError("Option \"--dedupestats\" must be a power of two from 4K to 1G");
+
+		/* (as the config: a block reduced to the file size is the whole file, whose last chunk may
+		   be short) */
+		const uint64_t fileBlockSize = (fileSize && (blockSize > fileSize) ) ? fileSize : blockSize;
+
+		if( (fileBlockSize % dedupeStatsChunkSize) && (fileBlockSize != fileSize) )
+			throw ProgError("The block size (" + std::to_string(blockSize) + ") must be a multiple "
+				"of \"--dedupestats\" (" + std::to_string(dedupeStatsChunkSize) + ")");
+
+		if(useRandomUnaligned)
+			throw ProgError("Option \"--dedupestats\" cannot be used together with "
+				"\"--norandalign\"");
+
+		if(useRandomOffsets)
+			throw ProgError("Option \"--dedupestats\" cannot be used together with \"--rand\"");
+
+		if(doInfiniteIOLoop)
+			throw ProgError("Option \"--dedupestats\" cannot be used together with \"--infloop\"");
+
+		if(rwMixReadPercent)
+			throw ProgError("Option \"--dedupestats\" cannot be used together with \"--rwmixpct\"");
+
+		if(numRWMixReadThreads)
+			throw ProgError("Option \"--dedupestats\" cannot be used together with \"--rwmixthr\"");
+
+		if(!hosts.empty() )
+			throw ProgError("Option \"--dedupestats\" cannot be used together with \"--hosts\"");
+	}
+
 	if(!checksumAlgoName.empty() )
 	{
 		if(checksumsPath.empty() && checksumVerifyPath.empty() )
@@ -1199,6 +1241,7 @@ void ProgArgs::toABIConfig(ABIConfig& out) const
 		checksumChunkSize ? __builtin_ctzll(checksumChunkSize) : 0;
 	cfg.checksumAlgo = checksumList ? checksumList->algo : checksumAlgoName.empty() ?
 		ELB_CHECKSUM_CRC32 : elb_checksum_algo_by_name(checksumAlgoName.c_str() );
+	cfg.dedupeChunkShift = dedupeStatsChunkSize ? __builtin_ctzll(dedupeStatsChunkSize) : 0;
 	cfg.serializeBufferedWrites = neverSerializeBufferedWrites ? ELB_WRITEGATE_OFF :
 		(serializeBufferedWrites ? ELB_WRITEGATE_ON : ELB_WRITEGATE_AUTO);
 	cfg.noGPUNumaBinding = noGPUNumaBinding;

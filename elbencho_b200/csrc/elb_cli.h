@@ -94,6 +94,7 @@ class ProgArgs
 		uint64_t checksumChunkSize{0}; // --checksumchunk
 		std::string checksumVerifyPath; // --checksumverify
 		std::string checksumAlgoName; // --checksumalgo
+		uint64_t dedupeStatsChunkSize{0}; // --dedupestats
 		std::shared_ptr<const ChecksumList> checksumList; // --checksumverify, parsed by checkArgs
 		uint64_t rwMixReadPercent{0};
 		bool hasUserSetRWMixPercent{false};

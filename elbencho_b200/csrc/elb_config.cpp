@@ -4,6 +4,7 @@
  * (reference source/ProgArgs.cpp:1041-1671).
  */
 #include "elb_host.h"
+#include "elb_internal.h"
 
 #include <fstream>
 
@@ -234,6 +235,30 @@ Config Config::fromABI(const elb_cfg* cfg)
 		throw WorkerError("Checksums (--checksums) cannot be used together with rwmix (a phase in "
 			"both directions).");
 
+	if(cfg->dedupeChunkShift && ( (cfg->dedupeChunkShift < ELB_DEDUPE_MIN_CHUNK_SHIFT) ||
+		(cfg->dedupeChunkShift > ELB_DEDUPE_MAX_CHUNK_SHIFT) ) )
+		throw WorkerError("The dedupe chunk shift (" + std::to_string(cfg->dedupeChunkShift) +
+			") is not in [" + std::to_string(ELB_DEDUPE_MIN_CHUNK_SHIFT) + ", " +
+			std::to_string(ELB_DEDUPE_MAX_CHUNK_SHIFT) + "].");
+
+	c.dedupeChunkShift = (cfg->dedupeChunkShift > 0) ? (unsigned)cfg->dedupeChunkShift : 0;
+
+	if(c.dedupeChunkShift && c.useRandomOffsets)
+		throw WorkerError("Dedupe stats (--dedupestats) cannot be used together with random "
+			"offsets: they need every chunk of a file exactly once.");
+
+	if(c.dedupeChunkShift && c.doInfiniteIOLoop)
+		throw WorkerError("Dedupe stats (--dedupestats) cannot be used together with an infinite "
+			"I/O loop (--infloop).");
+
+	if(c.dedupeChunkShift && (c.rwMixReadPercent || c.numRWMixReadThreads) )
+		throw WorkerError("Dedupe stats (--dedupestats) cannot be used together with rwmix (a "
+			"phase in both directions).");
+
+	if(c.dedupeChunkShift && c.useRandomUnaligned)
+		throw WorkerError("Dedupe stats (--dedupestats) cannot be used together with unaligned "
+			"random offsets (--norandalign).");
+
 	if(c.verifyDamageReport && !c.integrityCheckSalt)
 		throw WorkerError("A verify report (--verifyreport) requires data verification (--verify "
 			"or --verifyrand).");
@@ -310,6 +335,13 @@ Config Config::fromABI(const elb_cfg* cfg)
 		(c.blockSize != c.fileSize) )
 		throw WorkerError("Option \"--checksumalgo\" blake3 requires a block size that is a "
 			"multiple of 1K");
+
+	// (a block reduced to the file size is the whole file: its last chunk may be short)
+	if(c.dedupeChunkShift && (c.blockSize % (1ULL << c.dedupeChunkShift) ) &&
+		(c.blockSize != c.fileSize) )
+		throw WorkerError("The block size (" + std::to_string(c.blockSize) + ") is not a multiple "
+			"of the dedupe chunk size (--dedupestats) (" +
+			std::to_string(1ULL << c.dedupeChunkShift) + ").");
 
 	if( (c.checksumAlgo == ELB_CHECKSUM_BLAKE3) && c.useRandomUnaligned)
 		throw WorkerError("Option \"--checksumalgo\" blake3 cannot be used together with "

@@ -74,6 +74,7 @@ class Coordinator
 		void writeVerifyReportSection(int benchPhase);
 		void writeChecksumSection(int benchPhase);
 		void printChecksumVerifyLine(int benchPhase);
+		void printDedupeLine(int benchPhase);
 		void printDryRunInfo();
 };
 
@@ -278,6 +279,31 @@ void Coordinator::printChecksumVerifyLine(int benchPhase)
 		" files: " << progArgs.checksumVerifyPath << std::endl;
 }
 
+/* --dedupestats: after each write and read phase that succeeded, its counts and their ratio */
+void Coordinator::printDedupeLine(int benchPhase)
+{
+	if(!progArgs.dedupeStatsChunkSize ||
+		( (benchPhase != ELB_PHASE_CREATEFILES) && (benchPhase != ELB_PHASE_READFILES) ) )
+		return;
+
+	uint64_t numChunks, numDistinct, numZero;
+
+	try
+	{
+		manager->getDedupeStats(numChunks, numDistinct, numZero);
+	}
+	catch(const WorkerError& e)
+	{
+		throw ProgError(e.what() );
+	}
+
+	char ratio[32];
+	snprintf(ratio, sizeof(ratio), "%.2f", numDistinct ? (double)numChunks / numDistinct : 1.0);
+
+	std::cout << "Dedupe: " << numChunks << " chunks of " << progArgs.dedupeStatsChunkSize << ", " <<
+		numDistinct << " distinct, " << numZero << " zero: " << ratio << ":1" << std::endl;
+}
+
 /* Coordinator::runBenchmarkPhase (:248-272) + Statistics live loop (:1284-1345) */
 void Coordinator::runBenchmarkPhase(int benchPhase)
 {
@@ -415,6 +441,7 @@ void Coordinator::runBenchmarkPhase(int benchPhase)
 	writeVerifyReportSection(benchPhase);
 	writeChecksumSection(benchPhase);
 	printChecksumVerifyLine(benchPhase);
+	printDedupeLine(benchPhase);
 }
 
 void waitForUserDefinedStartTime(const ProgArgs& progArgs) // Coordinator.cpp:149-158

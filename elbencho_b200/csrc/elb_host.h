@@ -1005,6 +1005,7 @@ struct Config
 	unsigned checksumChunkShift{0}; // --checksumchunk / the checksum list's (0: whole files),
 	                                // ELB_CHECKSUM_MIN/MAX_CHUNK_SHIFT
 	int checksumAlgo{ELB_CHECKSUM_CRC32}; // --checksumalgo / the checksum list's (elb_crc_algo::ID)
+	unsigned dedupeChunkShift{0}; // --dedupestats: chunks of 2^shift bytes (0: off), 12..30
 	int serializeBufferedWrites{ELB_WRITEGATE_AUTO};
 	int stagingEngine{ELB_STAGING_AUTO};
 	bool noGPUNumaBinding{false};

@@ -105,7 +105,20 @@ int elb_launch_crc(int algo, const elb_block_desc* descs, const uint64_t* shifts
 int elb_launch_blake3(const elb_block_desc* descs, const uint64_t* shifts, uint32_t numDescs,
 	unsigned chunkShift, uint64_t slotsPerDesc, void* devDigests, void* hostDigests,
 	cudaStream_t stream);
+/* --dedupestats (elb_dedupe.cu; elb_dedupe_insert, elb_dedupe_merge): descs must be host- and
+   device-readable, the host checks them and sizes the grid from their lengths. zeroDigest is the
+   BLAKE3 of one chunk of zero bytes (elb_dedupe_zero_chunk_digest). */
+#define ELB_DEDUPE_MAX_PROBES 4096 /* a longer probe sequence sets elb_dedupe_counters::overflow */
+#define ELB_DEDUPE_MIN_CHUNK_SHIFT 12 /* 4 KiB .. 1 GiB chunks */
+#define ELB_DEDUPE_MAX_CHUNK_SHIFT 30
+int elb_launch_dedupe_insert(const elb_block_desc* descs, uint32_t numDescs, unsigned chunkShift,
+	uint64_t slotsPerDesc, const void* devDigests, void* table, uint64_t tableEntries,
+	elb_dedupe_counters* devCounters, const uint8_t zeroDigest[32], cudaStream_t stream);
+int elb_launch_dedupe_merge(const void* srcEntries, uint64_t numSrcEntries, void* table,
+	uint64_t tableEntries, elb_dedupe_counters* devCounters, cudaStream_t stream);
+void elb_dedupe_zero_chunk_digest(unsigned chunkShift, uint8_t out[32]); // chunkShift 12..30
 int elb_kernels_warmup();
 uint64_t elb_get_num_kernel_launches();
+void elb_count_kernel_launch(); // (launches of the kernels outside elb_kernels.cu)
 
 #endif /* ELB_INTERNAL_H_ */

@@ -2371,3 +2371,8 @@ uint64_t elb_get_num_kernel_launches()
 {
 	return gNumKernelLaunches.load(std::memory_order_relaxed);
 }
+
+void elb_count_kernel_launch()
+{
+	gNumKernelLaunches.fetch_add(1, std::memory_order_relaxed);
+}

@@ -133,6 +133,7 @@ Manager::~Manager()
 			thread.join();
 	}
 
+	freeDedupeTables();
 	closeBenchPathFDs();
 }
 
@@ -384,6 +385,7 @@ void Manager::prepareFilesForPhase(int benchPhase)
 void Manager::startNextPhase(int benchPhase)
 {
 	prepareFilesForPhase(benchPhase);
+	prepareDedupeTables(benchPhase);
 
 	std::unique_lock<std::mutex> lock(shared.mutex);
 
@@ -833,6 +835,308 @@ void Manager::getChecksumVerifyCounts(uint64_t& outNumChunks, uint64_t& outNumFi
 	}
 
 	outNumFiles = paths.size();
+}
+
+/* --dedupestats: the K-chunks the worker of the given rank can move in a phase, capped by the
+ * data set's. Sequential file mode: its share of the paths' blocks as FileSeqSource cuts them, the
+ * standard share, or the last data set thread's with the remainder; no block spans two files, so a
+ * block holds at most ceil(blockSize / K) chunks. Strided access: the whole data set. Dir mode:
+ * its own files. Custom tree mode: the whole tree, since the shares can be uneven. */
+static uint64_t dedupeWorkerChunkBound(const Config& cfg, const TreeManifest& customTree,
+	uint64_t rank)
+{
+	const unsigned shift = cfg.dedupeChunkShift;
+	const uint64_t chunkSize = (uint64_t)1 << shift;
+	const uint64_t fileChunks = (cfg.fileSize + chunkSize - 1) >> shift;
+
+	if( (cfg.pathType == ELB_PATH_DIR) && customTree.isLoaded)
+		return (customTree.getNumFileBytes() >> shift) + customTree.getNumFiles();
+
+	if(cfg.pathType == ELB_PATH_DIR)
+		return std::max(cfg.numDirs, (uint64_t)1) * cfg.numFiles * fileChunks;
+
+	const uint64_t totalChunks = (uint64_t)cfg.paths.size() * fileChunks;
+
+	if(cfg.useStridedAccess || !cfg.blockSize)
+		return totalChunks;
+
+	const uint64_t blockChunks = (cfg.blockSize + chunkSize - 1) >> shift;
+	const uint64_t numBlocksTotal = (uint64_t)cfg.paths.size() *
+		( (cfg.fileSize + cfg.blockSize - 1) / cfg.blockSize);
+	const uint64_t numThreads = cfg.numDataSetThreads;
+	const uint64_t standardNumBlocks = numBlocksTotal / numThreads;
+	const uint64_t numBlocks = (rank == numThreads - 1) ?
+		(numBlocksTotal - standardNumBlocks * (numThreads - 1) ) : standardNumBlocks;
+
+	return std::min(totalChunks, numBlocks * blockChunks);
+}
+
+/* the K-chunks that the whole data set of a phase has (custom tree mode: the tree; dir mode: no
+ * cap beyond the workers' own files) */
+static uint64_t dedupeDataSetChunks(const Config& cfg, const TreeManifest& customTree)
+{
+	const unsigned shift = cfg.dedupeChunkShift;
+
+	if( (cfg.pathType == ELB_PATH_DIR) && customTree.isLoaded)
+		return (customTree.getNumFileBytes() >> shift) + customTree.getNumFiles();
+
+	if(cfg.pathType == ELB_PATH_DIR)
+		return ~0ULL;
+
+	return (uint64_t)cfg.paths.size() * ( (cfg.fileSize + ( (uint64_t)1 << shift) - 1) >> shift);
+}
+
+static void checkDedupeCuda(int gpuID, cudaError_t res, const char* what)
+{
+	if(res != cudaSuccess)
+		throw WorkerError(std::string(what) + " failed. GPU ID: " + std::to_string(gpuID) +
+			"; CUDA Error: " + cudaGetErrorString(res) );
+}
+
+/**
+ * --dedupestats: before a write or read phase, one fingerprint table per GPU, cleared. A table
+ * has the next power of two at or above twice the chunks that the GPU's workers can move (the
+ * first GPU's: all of the phase's chunks, as the others are merged into it), so its load stays at
+ * or below 0.5. Fails before any I/O if the tables need more than half of a GPU's free memory.
+ */
+void Manager::prepareDedupeTables(int benchPhase)
+{
+	const Config& cfg = shared.cfg;
+
+	if(!cfg.dedupeChunkShift ||
+		( (benchPhase != ELB_PHASE_CREATEFILES) && (benchPhase != ELB_PHASE_READFILES) ) )
+		return;
+
+	if(dedupeZeroDigestShift != cfg.dedupeChunkShift)
+	{
+		elb_dedupe_zero_chunk_digest(cfg.dedupeChunkShift, shared.dedupeZeroDigest);
+		dedupeZeroDigestShift = cfg.dedupeChunkShift;
+	}
+
+	/* the GPUs of the workers, the first worker's first, and the chunks their workers can move;
+	   the first GPU takes all of the phase's chunks, as the others are merged into it */
+	const uint64_t dataSetChunks = dedupeDataSetChunks(cfg, shared.customTree);
+	std::vector<std::pair<int, uint64_t> > gpuChunks;
+	uint64_t phaseChunks = 0;
+
+	for(const std::unique_ptr<Worker>& worker : workers)
+	{
+		const uint64_t workerChunks = dedupeWorkerChunkBound(cfg, shared.customTree,
+			worker->getRank() );
+		auto iter = std::find_if(gpuChunks.begin(), gpuChunks.end(),
+			[&](const std::pair<int, uint64_t>& gpu) { return gpu.first == worker->getGPUID(); } );
+
+		if(iter == gpuChunks.end() )
+			gpuChunks.emplace_back(worker->getGPUID(), workerChunks);
+		else
+			iter->second += workerChunks;
+
+		phaseChunks += workerChunks;
+	}
+
+	std::vector<DedupeTable> tables;
+
+	for(size_t i = 0; i < gpuChunks.size(); i++)
+	{
+		const uint64_t numChunks = std::min(dataSetChunks, !i ? phaseChunks : gpuChunks[i].second);
+		uint64_t numEntries = 1024;
+
+		while(numEntries < 2 * numChunks)
+			numEntries *= 2;
+
+		DedupeTable table;
+		table.gpuID = gpuChunks[i].first;
+		table.numEntries = numEntries;
+		tables.push_back(table);
+	}
+
+	int prevDevice = 0;
+	cudaGetDevice(&prevDevice);
+
+	std::shared_lock<std::shared_timed_mutex> allocLock(shared.gpuAllocMutex);
+	bool replaced = false;
+
+	try
+	{
+		for(DedupeTable& table : tables)
+		{ // all checks first: a failing phase leaves the tables as they were
+			const uint64_t numBytes = table.numEntries * 16 + sizeof(elb_dedupe_counters);
+			uint64_t heldBytes = 0;
+			size_t freeBytes = 0, totalBytes = 0;
+
+			for(const DedupeTable& oldTable : shared.dedupeTables)
+				if(oldTable.gpuID == table.gpuID)
+					heldBytes = oldTable.numEntries * 16 + sizeof(elb_dedupe_counters);
+
+			checkDedupeCuda(table.gpuID, cudaSetDevice(table.gpuID), "Setting CUDA device");
+			checkDedupeCuda(table.gpuID, cudaMemGetInfo(&freeBytes, &totalBytes),
+				"GPU memory query");
+
+			if(numBytes > (freeBytes + heldBytes) / 2)
+				throw WorkerError("Dedupe stats (--dedupestats) need " + std::to_string(numBytes) +
+					" bytes of GPU memory for the chunk table of GPU " +
+					std::to_string(table.gpuID) + ", more than half of its " +
+					std::to_string(freeBytes + heldBytes) + " free bytes. Use a larger chunk "
+					"size.");
+		}
+
+		// keep the tables of the same size, free the others, then make the missing ones
+		for(DedupeTable& table : tables)
+			for(DedupeTable& oldTable : shared.dedupeTables)
+				if( (oldTable.gpuID == table.gpuID) && (oldTable.numEntries == table.numEntries) )
+					std::swap(oldTable, table);
+
+		freeDedupeTables();
+		shared.dedupeTables = tables;
+		replaced = true;
+
+		for(DedupeTable& table : shared.dedupeTables)
+		{
+			checkDedupeCuda(table.gpuID, cudaSetDevice(table.gpuID), "Setting CUDA device");
+
+			if(!table.entries)
+			{
+				checkDedupeCuda(table.gpuID, cudaMalloc(&table.counters,
+					sizeof(elb_dedupe_counters) ), "GPU dedupe counter allocation");
+				checkDedupeCuda(table.gpuID, cudaMalloc(&table.entries, table.numEntries * 16),
+					"GPU dedupe table allocation");
+			}
+
+			/* on a stream of its own: the legacy default stream would wait for the caller's work
+			   there */
+			cudaStream_t stream;
+			checkDedupeCuda(table.gpuID, cudaStreamCreateWithFlags(&stream,
+				cudaStreamNonBlocking), "CUDA stream creation");
+			cudaError_t clearRes = cudaMemsetAsync(table.entries, 0, table.numEntries * 16, stream);
+			if(clearRes == cudaSuccess)
+				clearRes = cudaMemsetAsync(table.counters, 0, sizeof(elb_dedupe_counters), stream);
+			if(clearRes == cudaSuccess)
+				clearRes = cudaStreamSynchronize(stream);
+			cudaStreamDestroy(stream);
+			checkDedupeCuda(table.gpuID, clearRes, "GPU dedupe table clear");
+		}
+	}
+	catch(...)
+	{
+		if(replaced)
+			freeDedupeTables(); // (a failed allocation: no table is left half made)
+
+		cudaSetDevice(prevDevice);
+		throw;
+	}
+
+	cudaSetDevice(prevDevice);
+}
+
+/* the tables and their counters (the workers must not use them any more) */
+void Manager::freeDedupeTables()
+{
+	for(DedupeTable& table : shared.dedupeTables)
+	{
+		cudaSetDevice(table.gpuID);
+
+		if(table.entries)
+			cudaFree(table.entries);
+		if(table.counters)
+			cudaFree(table.counters);
+	}
+
+	shared.dedupeTables.clear();
+}
+
+void Manager::getDedupeStats(uint64_t& outNumChunks, uint64_t& outNumDistinct,
+	uint64_t& outNumZero)
+{
+	outNumChunks = 0;
+	outNumDistinct = 0;
+	outNumZero = 0;
+
+	if(shared.dedupeTables.empty() )
+		return;
+
+	const DedupeTable& first = shared.dedupeTables[0];
+	std::vector<elb_dedupe_counters> counters(shared.dedupeTables.size() );
+	int prevDevice = 0;
+	cudaGetDevice(&prevDevice);
+
+	std::shared_lock<std::shared_timed_mutex> allocLock(shared.gpuAllocMutex);
+
+	cudaStream_t stream = NULL;
+	void* piece = NULL;
+	cudaError_t res = cudaSetDevice(first.gpuID);
+
+	if(res == cudaSuccess)
+		res = cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking);
+
+	/* the other GPUs' tables, peer to peer in pieces of at most 2^20 entries (16 MiB), merged into
+	   the first GPU's; merging twice adds nothing, so this may run again for the same phase */
+	uint64_t pieceEntries = 0;
+
+	for(size_t i = 1; i < shared.dedupeTables.size(); i++)
+		pieceEntries = std::max(pieceEntries,
+			std::min(shared.dedupeTables[i].numEntries, (uint64_t)1 << 20) );
+
+	if( (res == cudaSuccess) && pieceEntries)
+		res = cudaMalloc(&piece, pieceEntries * 16);
+
+	for(size_t i = 1; (res == cudaSuccess) && (i < shared.dedupeTables.size() ); i++)
+	{
+		const DedupeTable& table = shared.dedupeTables[i];
+
+		for(uint64_t offset = 0; (res == cudaSuccess) && (offset < table.numEntries);
+			offset += pieceEntries)
+		{
+			const uint64_t numEntries = std::min(pieceEntries, table.numEntries - offset);
+
+			// (unified addressing: the copy goes peer to peer)
+			res = cudaMemcpyAsync(piece, (char*)table.entries + offset * 16, numEntries * 16,
+				cudaMemcpyDefault, stream);
+
+			if( (res == cudaSuccess) && elb_launch_dedupe_merge(piece, numEntries, first.entries,
+				first.numEntries, first.counters, stream) )
+			{
+				if(stream)
+					cudaStreamSynchronize(stream);
+				if(piece)
+					cudaFree(piece);
+				cudaStreamDestroy(stream);
+				cudaSetDevice(prevDevice);
+				throw WorkerError(std::string("GPU dedupe merge failed. ") + elb_last_error() );
+			}
+		}
+	}
+
+	for(size_t i = 0; (res == cudaSuccess) && (i < shared.dedupeTables.size() ); i++)
+		res = cudaMemcpyAsync(&counters[i], shared.dedupeTables[i].counters,
+			sizeof(elb_dedupe_counters), cudaMemcpyDefault, stream);
+
+	if(stream)
+	{
+		const cudaError_t syncRes = cudaStreamSynchronize(stream);
+		res = (res == cudaSuccess) ? syncRes : res;
+	}
+
+	if(piece)
+		cudaFree(piece);
+	if(stream)
+		cudaStreamDestroy(stream);
+
+	cudaSetDevice(prevDevice);
+
+	checkDedupeCuda(first.gpuID, res, "GPU dedupe counter read");
+
+	for(size_t i = 0; i < counters.size(); i++)
+	{
+		if(counters[i].overflow)
+			throw WorkerError("Dedupe stats (--dedupestats): the chunk table of GPU " +
+				std::to_string(shared.dedupeTables[i].gpuID) + " ran past its probe bound of " +
+				std::to_string(ELB_DEDUPE_MAX_PROBES) + " entries; the counts are void.");
+
+		outNumChunks += counters[i].numChunks;
+		outNumZero += counters[i].numZero;
+	}
+
+	outNumDistinct = counters[0].numDistinct;
 }
 
 /* Statistics::generatePhaseResults (Statistics.cpp:1641-1764) */
@@ -1619,6 +1923,34 @@ int elb_mgr_checksum_verify_counts(elb_mgr* m, uint64_t* outNumChunks, uint64_t*
 	}
 
 	m->impl->getChecksumVerifyCounts(*outNumChunks, *outNumFiles);
+	return 0;
+}
+
+int elb_mgr_dedupe_stats(elb_mgr* m, uint64_t* outNumChunks, uint64_t* outNumDistinct,
+	uint64_t* outNumZero)
+{
+	if(!m || !outNumChunks || !outNumDistinct || !outNumZero)
+	{
+		elb_set_last_error("elb_mgr_dedupe_stats: NULL argument");
+		return -1;
+	}
+
+	if(!m->impl->shared.cfg.dedupeChunkShift)
+	{
+		elb_set_last_error("elb_mgr_dedupe_stats: dedupe stats are off (elb_cfg::dedupeChunkShift)");
+		return -1;
+	}
+
+	try
+	{
+		m->impl->getDedupeStats(*outNumChunks, *outNumDistinct, *outNumZero);
+	}
+	catch(std::exception& e)
+	{
+		elb_set_last_error(e.what() );
+		return -1;
+	}
+
 	return 0;
 }
 

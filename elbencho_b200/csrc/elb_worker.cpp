@@ -821,10 +821,12 @@ void Worker::preparePhase()
 
 /**
  * --checksums / --checksumverify: which stages take the checksum launch, in chunks of which size
- * and of which algorithm, and the batches' slots. Runs after the rings are made and at the start
- * of every write and read phase, since a checksum list (elb_mgr_set_checksum_list) may be set
- * between phases; a change drops the batch graphs, which hold the launches of the old setup.
- * Without either option it allocates and changes nothing.
+ * and of which algorithm, and the batches' slots. --dedupestats: the table the stages insert into
+ * and where the digests come from, the checksum launch's slots when it hashes BLAKE3 at the same
+ * chunk size, else the batch's own. Runs after the rings are made and at the start of every write
+ * and read phase, since a checksum list (elb_mgr_set_checksum_list) may be set and the manager may
+ * make new tables between phases; a change drops the batch graphs, which hold the launches of the
+ * old setup. Without these options it allocates and changes nothing.
  */
 void Worker::setupChecksums()
 {
@@ -839,18 +841,41 @@ void Worker::setupChecksums()
 		slotsPerDesc = 2 * (63 - __builtin_clzll(numChunks) ) + 1;
 	}
 
+	DedupeTable table;
+
+	for(const DedupeTable& gpuTable : shared->dedupeTables)
+		if(cfg.dedupeChunkShift && (gpuTable.gpuID == gpuID) )
+			table = gpuTable;
+
+	const bool dedupe = (table.entries != NULL);
+	const bool dedupeUsesSums = dedupe && (cfg.checksumAlgo == ELB_CHECKSUM_BLAKE3) &&
+		(chunkShift == cfg.dedupeChunkShift);
+	const bool dedupeNeedsOwnSums = dedupe && !(dedupeUsesSums && cfg.checksums);
+	const uint64_t dedupeSlots = !dedupe ? 1 : std::max( (cfg.blockSize +
+		( (uint64_t)1 << cfg.dedupeChunkShift) - 1) >> cfg.dedupeChunkShift, (uint64_t)1);
+
 	if(batches.empty() || ( (readChecksum == readStage.checksum) &&
 		(chunkShift == checksumChunkShift) && (slotsPerDesc == checksumSlotsPerDesc) &&
-		(cfg.checksumAlgo == checksumAlgo) ) )
+		(cfg.checksumAlgo == checksumAlgo) && (dedupe == readStage.dedupe) &&
+		(table.entries == dedupeTable.entries) && (table.numEntries == dedupeTable.numEntries) &&
+		(table.counters == dedupeTable.counters) && (dedupeSlots == dedupeSlotsPerDesc) &&
+		( (dedupeUsesSums && readChecksum) == dedupeUsesReadSums) ) )
 		return;
 
 	std::shared_lock<std::shared_timed_mutex> allocLock(shared->gpuAllocMutex);
 
 	writeStage.checksum = cfg.checksums;
 	readStage.checksum = readChecksum;
-	/* --verifydirect: a write phase's checksums are those of the written bytes, so the read-back
-	   takes none, and must not share the read phase's batch graphs then */
-	verifyBackStage.useGraph = readStage.useGraph && !readChecksum;
+	writeStage.dedupe = dedupe;
+	readStage.dedupe = dedupe;
+	verifyBackStage.dedupe = false;
+	/* --verifydirect: a write phase's checksums and dedupe counts are those of the written bytes,
+	   so the read-back takes none, and must not share the read phase's batch graphs then */
+	verifyBackStage.useGraph = readStage.useGraph && !readChecksum && !dedupe;
+	dedupeTable = table;
+	dedupeSlotsPerDesc = dedupeSlots;
+	dedupeUsesWriteSums = dedupeUsesSums && cfg.checksums;
+	dedupeUsesReadSums = dedupeUsesSums && readChecksum;
 	checksumChunkShift = chunkShift;
 	checksumSlotsPerDesc = slotsPerDesc;
 	checksumAlgo = cfg.checksumAlgo;
@@ -866,11 +891,18 @@ void Worker::setupChecksums()
 			cudaFree(batch.devSums);
 		if(batch.hostSums)
 			cudaFreeHost(batch.hostSums);
+		if(batch.devDedupeSums)
+			cudaFree(batch.devDedupeSums);
 
 		batch.readGraphExec = NULL;
 		batch.writeGraphExec = NULL;
 		batch.devSums = NULL;
 		batch.hostSums = NULL;
+		batch.devDedupeSums = NULL;
+
+		if(dedupeNeedsOwnSums)
+			ELB_CUDA_CHECK(cudaMalloc(&batch.devDedupeSums, elb_checksum_value_bytes(
+				ELB_CHECKSUM_BLAKE3) * batchBlocks * dedupeSlots), "GPU dedupe digest allocation");
 
 		if(!readChecksum)
 			continue;
@@ -1146,6 +1178,8 @@ void Worker::freeRings() // LocalWorker::cleanup (:1570-1641)
 			cudaFreeHost(batch.hostShifts);
 		if(batch.devSums)
 			cudaFree(batch.devSums);
+		if(batch.devDedupeSums)
+			cudaFree(batch.devDedupeSums);
 		if(batch.hostSums)
 			cudaFreeHost(batch.hostSums);
 	}
@@ -1889,6 +1923,8 @@ void Worker::rwPhase()
 
 		rwBlocksPipelined(source, isRead);
 	}
+
+	checkDedupeOverflow();
 }
 
 /**
@@ -2441,8 +2477,52 @@ void Worker::enqueueStage(Batch& batch, const GpuStage& stage, uint32_t numBlock
 		batch.devDoneTicket, batch.stream) ) )
 		throw WorkerError(std::string("GPU checksum failed. ") + elb_last_error() );
 
+	if(stage.dedupe)
+		enqueueDedupeInsert(batch, stage, numBlocks);
+
 	if( (stage.transfer == GpuStage::TRANSFER_COPY) && !stage.isRead)
 		enqueueStageCopies(batch, false, true);
+}
+
+/* --dedupestats: the digests of the batch's chunks (those of the checksum launch just enqueued when
+ * it hashes BLAKE3 at the same chunk size, else an own BLAKE3 launch into device-only slots) into
+ * the table of this worker's GPU. Nothing is copied or waited for: the counters are read at the
+ * end of the phase. */
+void Worker::enqueueDedupeInsert(Batch& batch, const GpuStage& stage, uint32_t numBlocks)
+{
+	const bool usesSums = stage.checksum &&
+		(stage.isRead ? dedupeUsesReadSums : dedupeUsesWriteSums);
+	void* digests = usesSums ? batch.devSums : batch.devDedupeSums;
+	const uint64_t slotsPerDesc = usesSums ? checksumSlotsPerDesc : dedupeSlotsPerDesc;
+
+	if(!usesSums && elb_launch_blake3(batch.hostDescs, NULL, numBlocks, cfg.dedupeChunkShift,
+		slotsPerDesc, digests, NULL, batch.stream) )
+		throw WorkerError(std::string("GPU dedupe digests failed. ") + elb_last_error() );
+
+	if(elb_launch_dedupe_insert(batch.hostDescs, numBlocks, cfg.dedupeChunkShift, slotsPerDesc,
+		digests, dedupeTable.entries, dedupeTable.numEntries, dedupeTable.counters,
+		shared->dedupeZeroDigest, batch.stream) )
+		throw WorkerError(std::string("GPU dedupe insert failed. ") + elb_last_error() );
+}
+
+/* --dedupestats: the phase fails if the table of this worker's GPU ran past its probe bound (a
+ * guard: a table is sized for a load of at most 0.5) */
+void Worker::checkDedupeOverflow()
+{
+	if(!readStage.dedupe || batches.empty() )
+		return;
+
+	uint32_t overflow = 0;
+
+	ELB_CUDA_CHECK(cudaMemcpyAsync(&overflow, &dedupeTable.counters->overflow, sizeof(overflow),
+		cudaMemcpyDeviceToHost, batches[0].stream), "GPU dedupe counter read");
+	ELB_CUDA_CHECK(cudaStreamSynchronize(batches[0].stream), "GPU dedupe counter read");
+
+	if(overflow)
+		throw WorkerError("Dedupe stats (--dedupestats): the chunk table of GPU " +
+			std::to_string(gpuID) + " (" + std::to_string(dedupeTable.numEntries) + " entries) "
+			"ran past its probe bound of " + std::to_string(ELB_DEDUPE_MAX_PROBES) + " entries; "
+			"the counts are void.");
 }
 
 /**
@@ -2481,6 +2561,9 @@ void Worker::gpuLaunchStage(Batch& batch, bool isRead)
 		numKernelLaunches++;
 	if(numBlocks && stage.checksum)
 		numKernelLaunches++;
+	if(numBlocks && stage.dedupe) // (the insert, and the BLAKE3 launch unless it shares one)
+		numKernelLaunches += (stage.checksum &&
+			(stage.isRead ? dedupeUsesReadSums : dedupeUsesWriteSums) ) ? 1 : 2;
 
 	if(stage.transfer != GpuStage::TRANSFER_NONE)
 		(isRead ? numH2DBytes : numD2HBytes) += numBytes;

@@ -52,6 +52,16 @@ class Worker;
 
 struct ChecksumList;
 
+/* --dedupestats: the fingerprint table of one GPU (elb_dedupe_insert) and its counters, made and
+ * cleared by the manager at the start of every write and read phase, shared by the GPU's workers */
+struct DedupeTable
+{
+	int gpuID{-1};
+	void* entries{NULL};    // numEntries entries of 16 bytes
+	uint64_t numEntries{0}; // a power of two
+	elb_dedupe_counters* counters{NULL};
+};
+
 /* WorkersSharedData (reference source/workers/WorkersSharedData.h:33-107): phase barrier and
  * done counters. The reference's boost uuid bench ID becomes a sequence number. */
 struct Shared
@@ -75,6 +85,8 @@ struct Shared
 
 	TreeManifest customTree; // --treefile, parsed once by the manager (ProgArgs::loadCustomTreeFile)
 	std::shared_ptr<const ChecksumList> checksumList; // --checksumverify (set between phases)
+	std::vector<DedupeTable> dedupeTables; // --dedupestats: one per GPU, the first worker's first
+	uint8_t dedupeZeroDigest[32]{};        // --dedupestats: the BLAKE3 of a chunk of zero bytes
 
 	/* workers hold this shared while they allocate / free device memory or instantiate graphs;
 	   the live stats reducer holds it exclusively while its collective is in flight, because a
@@ -250,6 +262,7 @@ struct GpuStage
 	bool useGraph;    // replay full batches from a CUDA graph (one launch per batch anyway under
 	                  // kernel staging)
 	bool checksum;    // --checksums, a checksum list: the checksum launch over the device slots
+	bool dedupe;      // --dedupestats: the chunks' digests go into the GPU's fingerprint table
 };
 
 /* a batch: a contiguous slice of the rings plus everything its GPU stage needs */
@@ -280,6 +293,9 @@ struct Batch
 	uint64_t* hostShifts{NULL};
 	void* devSums{NULL};  // zero, re-zeroed by the kernel (the algorithm's value bytes per slot)
 	void* hostSums{NULL};
+	/* --dedupestats without a BLAKE3 checksum launch of its chunk size: the chunks' digests, 32
+	   bytes per slot (device only) */
+	void* devDedupeSums{NULL};
 
 	// aio state
 	std::vector<struct iocb> iocbs;
@@ -471,6 +487,12 @@ class Worker
 		   chunks that matched */
 		std::map<FileID, const ChecksumList::File*> checksumListFiles;
 		uint64_t numChecksumChunksChecked{0};
+		/* --dedupestats: the table of this worker's GPU, the slots of the digests its inserts read
+		   and whether a stage's checksum launch writes them (BLAKE3 at the same chunk size) */
+		DedupeTable dedupeTable;
+		uint64_t dedupeSlotsPerDesc{1};
+		bool dedupeUsesWriteSums{false};
+		bool dedupeUsesReadSums{false};
 
 		// accounting
 		std::atomic<uint64_t> numH2DBytes{0};
@@ -514,6 +536,8 @@ class Worker
 		void addBatchChecksums(const Batch& batch);
 		void checkBatchChecksums(const Batch& batch);
 		void setupChecksums();
+		void enqueueDedupeInsert(Batch& batch, const GpuStage& stage, uint32_t numBlocks);
+		void checkDedupeOverflow();
 		FileID blockFileID(const BlockRef& block) const;
 		uint64_t blockFileSize(const BlockRef& block) const;
 		void gpuLaunchStage(Batch& batch, bool isRead);
@@ -609,6 +633,12 @@ class Manager
 		void setChecksumList(std::shared_ptr<const ChecksumList> list);
 		void getChecksumVerifyCounts(uint64_t& outNumChunks, uint64_t& outNumFiles);
 
+		/* --dedupestats: the chunks, distinct chunks and zero chunks of the last write or read
+		   phase over all GPUs (merges the other GPUs' tables into the first's; throws WorkerError
+		   if a table ran past its probe bound) */
+		void getDedupeStats(uint64_t& outNumChunks, uint64_t& outNumDistinct,
+			uint64_t& outNumZero);
+
 		Shared shared;
 		std::vector<std::unique_ptr<Worker> > workers;
 		std::vector<std::thread> threads;
@@ -623,6 +653,9 @@ class Manager
 		bool pathFDsOpenedForWrite{false};
 		bool hadCreateFilesPhase{false}; // (size check of read-only runs, ProgArgs.cpp:2099)
 		int configChecksumAlgo{ELB_CHECKSUM_CRC32}; // elb_cfg::checksumAlgo (a list's may replace it)
+		unsigned dedupeZeroDigestShift{0}; // the chunk shift of shared.dedupeZeroDigest (0: none)
+		void prepareDedupeTables(int benchPhase);
+		void freeDedupeTables();
 		std::unique_ptr<LiveStatsReducer> liveStatsReducer; // created on first use
 		std::mutex liveStatsReducerMutex;
 };

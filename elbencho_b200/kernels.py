@@ -422,3 +422,48 @@ def blake3_fold(runs, file_size):
     _check(_native.load().elb_blake3_fold(b"".join(runs), len(runs), file_size, out),
            "elb_blake3_fold")
     return out.raw
+
+
+# ---- --dedupestats: a set of chunk fingerprints (BLAKE3 digests) in device memory ----
+
+DEDUPE_ENTRY_BYTES = 16     # a table entry: the digest's first 16 bytes, bit 0 set (0: empty)
+DEDUPE_COUNTERS_BYTES = 32  # elb_dedupe_counters: chunks, distinct, zero (u64), overflow (u32)
+DEDUPE_MAX_PROBES = 4096
+
+
+def dedupe_zero_digest(chunk_shift):
+    """the BLAKE3 digest of 2**chunk_shift zero bytes (chunk_shift 12..30), computed on the host"""
+    out = ctypes.create_string_buffer(32)
+    _check(_native.load().elb_dedupe_zero_digest(chunk_shift, out), "elb_dedupe_zero_digest")
+    return out.raw
+
+
+def dedupe_insert(pinned_descs_ptr, num_descs, chunk_shift, slots_per_desc, dev_digests_ptr,
+                  dev_table_ptr, table_entries, dev_counters_ptr, zero_digest=None, stream=0):
+    """Insert the chunk digests of blake3_chunks (the same descriptors and slots, chunk_shift
+    12..30) into a table of table_entries (a power of two) 16-byte entries, zero when empty, and
+    count them in the 32-byte counters at dev_counters_ptr (chunks, distinct, zero chunks,
+    overflow). zero_digest: the digest that counts as a zero chunk (default: that of chunk_shift)."""
+    if zero_digest is None:
+        zero_digest = dedupe_zero_digest(chunk_shift)
+    _check(_native.load().elb_dedupe_insert(pinned_descs_ptr or None, num_descs, chunk_shift,
+                                            slots_per_desc, dev_digests_ptr or None,
+                                            dev_table_ptr or None, table_entries,
+                                            dev_counters_ptr or None, bytes(zero_digest), stream),
+           "elb_dedupe_insert")
+
+
+def dedupe_merge(dev_src_entries_ptr, num_src_entries, dev_table_ptr, table_entries,
+                 dev_counters_ptr, stream=0):
+    """Insert the non-empty entries of another table (num_src_entries entries in device memory of
+    the table's GPU) into the table; counts the entries newly taken as distinct."""
+    _check(_native.load().elb_dedupe_merge(dev_src_entries_ptr or None, num_src_entries,
+                                           dev_table_ptr or None, table_entries,
+                                           dev_counters_ptr or None, stream),
+           "elb_dedupe_merge")
+
+
+def dedupe_counters(raw):
+    """(chunks, distinct, zero, overflow) from the 32 bytes of elb_dedupe_counters"""
+    import struct
+    return struct.unpack("<QQQI4x", bytes(raw))

@@ -117,6 +117,7 @@ class WorkerConfig:
     checksums: bool = False           # --checksums: each file's CRC per phase (checksums())
     checksum_chunk_shift: int = 0     # --checksumchunk: CRCs of 2**shift byte chunks (0: files)
     checksum_algo: str = "crc32"      # --checksumalgo: "crc32", "crc32c", "crc64nvme" or "blake3"
+    dedupe_chunk: int = 0             # --dedupestats bytes (a power of two 4K..1G; 0 = off)
     serialize_buffered_writes: int = 0  # 0 auto, 1 on, 2 off (--writegate)
     staging_engine: int = 0           # 0 auto, 1 kernels move the data, 2 cudaMemcpyAsync
     no_gpu_numa_binding: bool = False  # --nogpunuma
@@ -137,6 +138,10 @@ class WorkerConfig:
         cfg.rankOffset = self.rank_offset
         cfg.numDataSetThreads = self.num_dataset_threads
         cfg.checksumChunkShift = self.checksum_chunk_shift
+        chunk = self.dedupe_chunk
+        # (not a power of two: a shift that the library rejects)
+        cfg.dedupeChunkShift = (0 if not chunk else chunk.bit_length() - 1
+                                if not chunk & (chunk - 1) else -1)
         cfg.blockSize = self.block_size
         cfg.fileSize = self.file_size
         cfg.ioDepth = self.io_depth
@@ -434,6 +439,14 @@ class WorkerManager:
                                                     ctypes.byref(files)) != 0:
             raise WorkerError(_native.last_error())
         return chunks.value, files.value
+
+    def dedupe_stats(self):
+        """--dedupestats: (chunks, distinct chunks, zero chunks) of the last write or read phase,
+        over all workers and GPUs."""
+        vals = [ctypes.c_uint64(0) for _ in range(3)]
+        if self._lib.elb_mgr_dedupe_stats(self._h, *[ctypes.byref(v) for v in vals]) != 0:
+            raise WorkerError(_native.last_error())
+        return tuple(v.value for v in vals)
 
     def checksums(self):
         """The last phase's files, merged over all workers and sorted by path:

@@ -356,6 +356,41 @@ void elb_blake3_parent(const uint8_t* left, const uint8_t* right, int root, uint
  * the two halves when the chunk count is a power of two. Returns -1 if they do not fit. */
 int elb_blake3_fold(const uint8_t* runs, uint64_t numRuns, uint64_t fileSize, uint8_t* out);
 
+/* --dedupestats: the counters of one fingerprint table (device memory, zero at the start) */
+typedef struct elb_dedupe_counters
+{
+	uint64_t numChunks;   /* chunks inserted (N) */
+	uint64_t numDistinct; /* entries newly taken: distinct chunks (D) */
+	uint64_t numZero;     /* chunks whose digest is that of a chunk of zero bytes (Z) */
+	uint32_t overflow;    /* nonzero: a probe sequence ran past its bound, the counts are void */
+	uint32_t reserved;
+} elb_dedupe_counters;
+
+/* --dedupestats: insert the chunk digests of elb_blake3_chunks (chunkShift 12..30, the same
+ * descriptors and slots: descriptor i has ceil(len_i / 2^chunkShift) chunks, the digest of chunk j
+ * in devDigests + 32 * (i * slotsPerDesc + j)) into a fingerprint table of tableEntries (a power
+ * of two) 16-byte entries in device memory, all 0 when empty. A key is the digest's first 16 bytes
+ * with bit 0 set, the home entry comes from bytes 8..15 and probing is linear. Adds to
+ * devCounters: every chunk to numChunks, every key that took a new entry to numDistinct, every
+ * digest equal to zeroDigest (32 bytes on the host, elb_dedupe_zero_digest) to numZero. A probe
+ * sequence longer than 4096 entries (or the table) sets overflow and drops the chunk. Reads no
+ * slot past a descriptor's chunks. descs must be pinned host memory: the host checks them and
+ * sizes the grid from their lengths, the device reads them. Fails without launching for a table
+ * size that is not a power of two, NULL pointers, a chunkShift outside 12..30, a descriptor off a
+ * chunk boundary or one with more chunks than slotsPerDesc. */
+int elb_dedupe_insert(const elb_block_desc* descs, uint32_t numDescs, unsigned chunkShift,
+	uint64_t slotsPerDesc, const void* devDigests, void* table, uint64_t tableEntries,
+	elb_dedupe_counters* devCounters, const uint8_t* zeroDigest, void* stream);
+/* --dedupestats: insert the non-empty entries of numSrcEntries entries at srcEntries (device
+ * memory of the table's device, e.g. a peer copy of another GPU's table) into the table; adds the
+ * entries newly taken to devCounters->numDistinct and sets overflow as elb_dedupe_insert does.
+ * Fails without launching for a table size that is not a power of two or NULL pointers. */
+int elb_dedupe_merge(const void* srcEntries, uint64_t numSrcEntries, void* table,
+	uint64_t tableEntries, elb_dedupe_counters* devCounters, void* stream);
+/* out (32 bytes) <- the BLAKE3 digest of 2^chunkShift zero bytes (chunkShift 12..30), computed on
+ * the host. Returns -1 for another chunkShift. */
+int elb_dedupe_zero_digest(unsigned chunkShift, uint8_t* out);
+
 int elb_stage_copy(const elb_block_desc* descs, uint32_t numDescs, int hostToDevice,
 	int64_t hostDelta, uint64_t totalBytes, uint64_t maxBlockLen, void* stream);
 /* devResults[0..numDescs) <- {0, ~0} */
@@ -381,6 +416,11 @@ uint32_t elb_phase_results_struct_size(void);
 typedef struct elb_cfg
 {
 	uint32_t structSize; /* = sizeof(elb_cfg), for ABI checking */
+	/* --dedupestats: every write and read phase counts the chunks of 2^shift file bytes (12..30)
+	 * it moved, the distinct ones by BLAKE3 digest and the zero ones (elb_mgr_dedupe_stats);
+	 * 0 = off. Rejects random offsets, infinite loops and rwmix. It takes the 4 bytes of padding in
+	 * front of paths: no other field moves. */
+	int32_t dedupeChunkShift;
 
 	/* bench paths (ProgArgs benchPathsVec / benchPathType) */
 	const char* const* paths;
@@ -836,6 +876,13 @@ int64_t elb_mgr_checksums(elb_mgr* m, char* outBuf, uint64_t outBufLen);
 int elb_mgr_set_checksum_list(elb_mgr* m, const char* text, uint64_t len);
 /* --checksumverify: the chunks the last phase checked and the files they belong to */
 int elb_mgr_checksum_verify_counts(elb_mgr* m, uint64_t* outNumChunks, uint64_t* outNumFiles);
+/* --dedupestats (elb_cfg::dedupeChunkShift): of the last write or read phase, the chunks it moved
+ * (N), the distinct ones by BLAKE3 digest (D) and those of zero bytes (Z), over all workers and
+ * GPUs of the manager. A file's short last chunk is a chunk of its own length and never a zero
+ * chunk. All 0 before the first such phase. Returns -1 if --dedupestats is off, or if a table ran
+ * past its probe bound (elb_last_error), else 0. */
+int elb_mgr_dedupe_stats(elb_mgr* m, uint64_t* outNumChunks, uint64_t* outNumDistinct,
+	uint64_t* outNumZero);
 
 uint32_t elb_mgr_num_workers(elb_mgr* m);
 elb_worker* elb_mgr_worker(elb_mgr* m, uint32_t localIdx);
