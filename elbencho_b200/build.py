@@ -18,6 +18,7 @@ SOURCES = [
     "elb_kernels.cu",
     "elb_capi_kernels.cu",
     "elb_dedupe.cu",
+    "elb_compress.cu",
     "elb_config.cpp",
     "elb_cufile.cpp",
     "elb_worker.cpp",

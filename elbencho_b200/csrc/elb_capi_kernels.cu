@@ -684,6 +684,36 @@ int elb_dedupe_zero_digest(unsigned chunkShift, uint8_t* out)
 	return 0;
 }
 
+int elb_lz4_chunks(const elb_block_desc* descs, uint32_t numDescs, unsigned chunkShift,
+	uint64_t slotsPerDesc, elb_compress_counters* devCounters, uint32_t* devSizes, void* devOut,
+	void* stream)
+{
+	const char* what = "elb_lz4_chunks";
+
+	if( (numDescs && !descs) || !devCounters)
+	{
+		elb_set_last_error(std::string(what) + ": NULL descriptor array or counters");
+		return -1;
+	}
+
+	if( (chunkShift < ELB_COMPRESS_MIN_CHUNK_SHIFT) || (chunkShift > ELB_COMPRESS_MAX_CHUNK_SHIFT) )
+	{
+		elb_set_last_error(std::string(what) + ": chunk shift " + std::to_string(chunkShift) +
+			" is not in [" + std::to_string(ELB_COMPRESS_MIN_CHUNK_SHIFT) + ", " +
+			std::to_string(ELB_COMPRESS_MAX_CHUNK_SHIFT) + "]");
+		return -1;
+	}
+
+	if(elb_launch_lz4_chunks(descs, numDescs, chunkShift, slotsPerDesc, devCounters, devSizes,
+		devOut, (cudaStream_t)stream) )
+	{
+		elb_set_last_error(std::string("elb_") + elb_last_error() );
+		return -1;
+	}
+
+	return 0;
+}
+
 int elb_stage_copy(const elb_block_desc* descs, uint32_t numDescs, int hostToDevice,
 	int64_t hostDelta, uint64_t totalBytes, uint64_t maxBlockLen, void* stream)
 {

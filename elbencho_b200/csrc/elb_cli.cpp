@@ -155,6 +155,14 @@ static const OptDef optDefs[] =
 		"and threads, and prints \"Dedupe: <N> chunks of <K>, <D> distinct, <Z> zero: <N/D>:1\". "
 		"A file's short last chunk counts as a chunk of its own length. Cannot be used with "
 		"--rand, --norandalign, --infloop, --rwmixpct, --rwmixthr or --hosts. [b200]"},
+	{"compressstats", 0, Opt_BYTES, &ProgArgs::compressStatsChunkSize, Wire_NONE, "Chunk size of "
+		"compression statistics: every write and read phase compresses each chunk of this size (a "
+		"power of two from 4K to 1M that the block size is a multiple of) that it moved into one LZ4 "
+		"block on the GPU, and prints \"Compress: <N> chunks of <K>, <U> incompressible: <B> bytes "
+		"to <S>: <B/S>:1\", where S counts a chunk that does not shrink at its own length. A file's "
+		"short last chunk is a chunk of its own length. The parse is greedy and simpler than the "
+		"lz4 tool's, so its ratio is not lz4's. Cannot be used with --norandalign, --rwmixpct, "
+		"--rwmixthr or --hosts. [b200]"},
 	{"rwmixpct", 0, Opt_U64, &ProgArgs::rwMixReadPercent, Wire_REF, "Percentage of blocks that "
 		"should be read in a write phase."},
 	{"rwmixthr", 0, Opt_U64, &ProgArgs::numRWMixReadThreads, Wire_REF, "Number of threads that "
@@ -1070,6 +1078,35 @@ void ProgArgs::checkArgs()
 
 		if(!hosts.empty() )
 			throw ProgError("Option \"--dedupestats\" cannot be used together with \"--hosts\"");
+	}
+
+	if(compressStatsChunkSize)
+	{
+		if( (compressStatsChunkSize < (1ULL << ELB_COMPRESS_MIN_CHUNK_SHIFT) ) ||
+			(compressStatsChunkSize > (1ULL << ELB_COMPRESS_MAX_CHUNK_SHIFT) ) ||
+			(compressStatsChunkSize & (compressStatsChunkSize - 1) ) )
+			throw ProgError("Option \"--compressstats\" must be a power of two from 4K to 1M");
+
+		/* (as the manager: a block reduced to the file size is the whole file, whose last chunk
+		   may be short) */
+		const uint64_t fileBlockSize = (fileSize && (blockSize > fileSize) ) ? fileSize : blockSize;
+
+		if( (fileBlockSize % compressStatsChunkSize) && (fileBlockSize != fileSize) )
+			throw ProgError("The block size (" + std::to_string(blockSize) + ") must be a multiple "
+				"of \"--compressstats\" (" + std::to_string(compressStatsChunkSize) + ")");
+
+		if(useRandomUnaligned)
+			throw ProgError("Option \"--compressstats\" cannot be used together with "
+				"\"--norandalign\"");
+
+		if(rwMixReadPercent)
+			throw ProgError("Option \"--compressstats\" cannot be used together with \"--rwmixpct\"");
+
+		if(numRWMixReadThreads)
+			throw ProgError("Option \"--compressstats\" cannot be used together with \"--rwmixthr\"");
+
+		if(!hosts.empty() )
+			throw ProgError("Option \"--compressstats\" cannot be used together with \"--hosts\"");
 	}
 
 	if(!checksumAlgoName.empty() )

@@ -75,6 +75,7 @@ class Coordinator
 		void writeChecksumSection(int benchPhase);
 		void printChecksumVerifyLine(int benchPhase);
 		void printDedupeLine(int benchPhase);
+		void printCompressLine(int benchPhase);
 		void printDryRunInfo();
 };
 
@@ -304,6 +305,41 @@ void Coordinator::printDedupeLine(int benchPhase)
 		numDistinct << " distinct, " << numZero << " zero: " << ratio << ":1" << std::endl;
 }
 
+/* --compressstats: "Compress: <N> chunks of <K>, <U> incompressible: <B> bytes to <S>: <B/S>:1",
+   the ratio 1.00 when no bytes were moved */
+static std::string formatCompressLine(uint64_t chunkSize, const elb_compress_counters& counters)
+{
+	char ratio[32];
+	snprintf(ratio, sizeof(ratio), "%.2f", counters.numBytesStored ?
+		(double)counters.numBytesIn / counters.numBytesStored : 1.0);
+
+	return "Compress: " + std::to_string(counters.numChunks) + " chunks of " +
+		std::to_string(chunkSize) + ", " + std::to_string(counters.numIncompressible) +
+		" incompressible: " + std::to_string(counters.numBytesIn) + " bytes to " +
+		std::to_string(counters.numBytesStored) + ": " + ratio + ":1";
+}
+
+/* --compressstats: after each write and read phase that succeeded, its counts and their ratio */
+void Coordinator::printCompressLine(int benchPhase)
+{
+	if(!progArgs.compressStatsChunkSize ||
+		( (benchPhase != ELB_PHASE_CREATEFILES) && (benchPhase != ELB_PHASE_READFILES) ) )
+		return;
+
+	elb_compress_counters counters;
+
+	try
+	{
+		manager->getCompressStats(counters);
+	}
+	catch(const WorkerError& e)
+	{
+		throw ProgError(e.what() );
+	}
+
+	std::cout << formatCompressLine(progArgs.compressStatsChunkSize, counters) << std::endl;
+}
+
 /* Coordinator::runBenchmarkPhase (:248-272) + Statistics live loop (:1284-1345) */
 void Coordinator::runBenchmarkPhase(int benchPhase)
 {
@@ -442,6 +478,7 @@ void Coordinator::runBenchmarkPhase(int benchPhase)
 	writeChecksumSection(benchPhase);
 	printChecksumVerifyLine(benchPhase);
 	printDedupeLine(benchPhase);
+	printCompressLine(benchPhase);
 }
 
 void waitForUserDefinedStartTime(const ProgArgs& progArgs) // Coordinator.cpp:149-158
@@ -570,6 +607,9 @@ int Coordinator::main() // Coordinator.cpp:31-142
 
 		if(progArgs.checksumList)
 			manager->setChecksumList(progArgs.checksumList);
+
+		if(progArgs.compressStatsChunkSize)
+			manager->setCompressStats(__builtin_ctzll(progArgs.compressStatsChunkSize) );
 
 		/* workers on several GPUs: create the NCCL communicators of the statistics reduce now,
 		   while the workers are idle (and before any result output) */
@@ -704,6 +744,27 @@ extern "C" int64_t elb_format_value(int kind, uint64_t value, double percentage,
 			elb_set_last_error("elb_format_value: invalid kind " + std::to_string(kind) );
 			return -1;
 	}
+
+	if(outBuf && outBufLen)
+	{
+		const size_t copyLen = std::min( (size_t)(outBufLen - 1), text.size() );
+		memcpy(outBuf, text.data(), copyLen);
+		outBuf[copyLen] = 0;
+	}
+
+	return (int64_t)text.size();
+}
+
+extern "C" int64_t elb_format_compress_line(uint64_t chunkSize,
+	const elb_compress_counters* counters, char* outBuf, uint64_t outBufLen)
+{
+	if(!counters)
+	{
+		elb_set_last_error("elb_format_compress_line: NULL counters");
+		return -1;
+	}
+
+	const std::string text = elb::formatCompressLine(chunkSize, *counters);
 
 	if(outBuf && outBufLen)
 	{

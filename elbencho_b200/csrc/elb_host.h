@@ -1006,6 +1006,7 @@ struct Config
 	                                // ELB_CHECKSUM_MIN/MAX_CHUNK_SHIFT
 	int checksumAlgo{ELB_CHECKSUM_CRC32}; // --checksumalgo / the checksum list's (elb_crc_algo::ID)
 	unsigned dedupeChunkShift{0}; // --dedupestats: chunks of 2^shift bytes (0: off), 12..30
+	unsigned compressChunkShift{0}; // --compressstats (elb_mgr_set_compress_stats): 0 off, 12..20
 	int serializeBufferedWrites{ELB_WRITEGATE_AUTO};
 	int stagingEngine{ELB_STAGING_AUTO};
 	bool noGPUNumaBinding{false};

@@ -117,6 +117,13 @@ int elb_launch_dedupe_insert(const elb_block_desc* descs, uint32_t numDescs, uns
 int elb_launch_dedupe_merge(const void* srcEntries, uint64_t numSrcEntries, void* table,
 	uint64_t tableEntries, elb_dedupe_counters* devCounters, cudaStream_t stream);
 void elb_dedupe_zero_chunk_digest(unsigned chunkShift, uint8_t out[32]); // chunkShift 12..30
+/* --compressstats (elb_compress.cu; elb_lz4_chunks): descs must be host- and device-readable, the
+   host checks them and sizes the grid from their lengths. devSizes and devOut may be NULL. */
+#define ELB_COMPRESS_MIN_CHUNK_SHIFT 12 /* 4 KiB .. 1 MiB chunks */
+#define ELB_COMPRESS_MAX_CHUNK_SHIFT 20
+int elb_launch_lz4_chunks(const elb_block_desc* descs, uint32_t numDescs, unsigned chunkShift,
+	uint64_t slotsPerDesc, elb_compress_counters* devCounters, uint32_t* devSizes, void* devOut,
+	cudaStream_t stream);
 int elb_kernels_warmup();
 uint64_t elb_get_num_kernel_launches();
 void elb_count_kernel_launch(); // (launches of the kernels outside elb_kernels.cu)

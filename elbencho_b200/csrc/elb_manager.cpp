@@ -134,6 +134,7 @@ Manager::~Manager()
 	}
 
 	freeDedupeTables();
+	freeCompressCounters();
 	closeBenchPathFDs();
 }
 
@@ -386,6 +387,7 @@ void Manager::startNextPhase(int benchPhase)
 {
 	prepareFilesForPhase(benchPhase);
 	prepareDedupeTables(benchPhase);
+	prepareCompressCounters(benchPhase);
 
 	std::unique_lock<std::mutex> lock(shared.mutex);
 
@@ -886,7 +888,7 @@ static uint64_t dedupeDataSetChunks(const Config& cfg, const TreeManifest& custo
 	return (uint64_t)cfg.paths.size() * ( (cfg.fileSize + ( (uint64_t)1 << shift) - 1) >> shift);
 }
 
-static void checkDedupeCuda(int gpuID, cudaError_t res, const char* what)
+static void checkGpuCall(int gpuID, cudaError_t res, const char* what)
 {
 	if(res != cudaSuccess)
 		throw WorkerError(std::string(what) + " failed. GPU ID: " + std::to_string(gpuID) +
@@ -968,8 +970,8 @@ void Manager::prepareDedupeTables(int benchPhase)
 				if(oldTable.gpuID == table.gpuID)
 					heldBytes = oldTable.numEntries * 16 + sizeof(elb_dedupe_counters);
 
-			checkDedupeCuda(table.gpuID, cudaSetDevice(table.gpuID), "Setting CUDA device");
-			checkDedupeCuda(table.gpuID, cudaMemGetInfo(&freeBytes, &totalBytes),
+			checkGpuCall(table.gpuID, cudaSetDevice(table.gpuID), "Setting CUDA device");
+			checkGpuCall(table.gpuID, cudaMemGetInfo(&freeBytes, &totalBytes),
 				"GPU memory query");
 
 			if(numBytes > (freeBytes + heldBytes) / 2)
@@ -992,20 +994,20 @@ void Manager::prepareDedupeTables(int benchPhase)
 
 		for(DedupeTable& table : shared.dedupeTables)
 		{
-			checkDedupeCuda(table.gpuID, cudaSetDevice(table.gpuID), "Setting CUDA device");
+			checkGpuCall(table.gpuID, cudaSetDevice(table.gpuID), "Setting CUDA device");
 
 			if(!table.entries)
 			{
-				checkDedupeCuda(table.gpuID, cudaMalloc(&table.counters,
+				checkGpuCall(table.gpuID, cudaMalloc(&table.counters,
 					sizeof(elb_dedupe_counters) ), "GPU dedupe counter allocation");
-				checkDedupeCuda(table.gpuID, cudaMalloc(&table.entries, table.numEntries * 16),
+				checkGpuCall(table.gpuID, cudaMalloc(&table.entries, table.numEntries * 16),
 					"GPU dedupe table allocation");
 			}
 
 			/* on a stream of its own: the legacy default stream would wait for the caller's work
 			   there */
 			cudaStream_t stream;
-			checkDedupeCuda(table.gpuID, cudaStreamCreateWithFlags(&stream,
+			checkGpuCall(table.gpuID, cudaStreamCreateWithFlags(&stream,
 				cudaStreamNonBlocking), "CUDA stream creation");
 			cudaError_t clearRes = cudaMemsetAsync(table.entries, 0, table.numEntries * 16, stream);
 			if(clearRes == cudaSuccess)
@@ -1013,7 +1015,7 @@ void Manager::prepareDedupeTables(int benchPhase)
 			if(clearRes == cudaSuccess)
 				clearRes = cudaStreamSynchronize(stream);
 			cudaStreamDestroy(stream);
-			checkDedupeCuda(table.gpuID, clearRes, "GPU dedupe table clear");
+			checkGpuCall(table.gpuID, clearRes, "GPU dedupe table clear");
 		}
 	}
 	catch(...)
@@ -1123,7 +1125,7 @@ void Manager::getDedupeStats(uint64_t& outNumChunks, uint64_t& outNumDistinct,
 
 	cudaSetDevice(prevDevice);
 
-	checkDedupeCuda(first.gpuID, res, "GPU dedupe counter read");
+	checkGpuCall(first.gpuID, res, "GPU dedupe counter read");
 
 	for(size_t i = 0; i < counters.size(); i++)
 	{
@@ -1137,6 +1139,135 @@ void Manager::getDedupeStats(uint64_t& outNumChunks, uint64_t& outNumDistinct,
 	}
 
 	outNumDistinct = counters[0].numDistinct;
+}
+
+void Manager::setCompressStats(unsigned chunkShift)
+{
+	Config& cfg = shared.cfg;
+
+	if(chunkShift && ( (chunkShift < ELB_COMPRESS_MIN_CHUNK_SHIFT) ||
+		(chunkShift > ELB_COMPRESS_MAX_CHUNK_SHIFT) ) )
+		throw WorkerError("The compress chunk shift (" + std::to_string(chunkShift) + ") is not in "
+			"[" + std::to_string(ELB_COMPRESS_MIN_CHUNK_SHIFT) + ", " +
+			std::to_string(ELB_COMPRESS_MAX_CHUNK_SHIFT) + "].");
+
+	// (a block reduced to the file size is the whole file: its last chunk may be short)
+	if(chunkShift && (cfg.blockSize % (1ULL << chunkShift) ) && (cfg.blockSize != cfg.fileSize) )
+		throw WorkerError("The block size (" + std::to_string(cfg.blockSize) + ") is not a multiple "
+			"of the compress chunk size (--compressstats) (" + std::to_string(1ULL << chunkShift) +
+			").");
+
+	if(chunkShift && cfg.useRandomUnaligned)
+		throw WorkerError("Compress stats (--compressstats) cannot be used together with unaligned "
+			"random offsets (--norandalign).");
+
+	if(chunkShift && (cfg.rwMixReadPercent || cfg.numRWMixReadThreads) )
+		throw WorkerError("Compress stats (--compressstats) cannot be used together with rwmix (a "
+			"phase in both directions).");
+
+	cfg.compressChunkShift = chunkShift;
+}
+
+/* --compressstats: before a write or read phase, the counters of every GPU of the workers, made
+ * when first needed and cleared */
+void Manager::prepareCompressCounters(int benchPhase)
+{
+	if(!shared.cfg.compressChunkShift ||
+		( (benchPhase != ELB_PHASE_CREATEFILES) && (benchPhase != ELB_PHASE_READFILES) ) )
+		return;
+
+	int prevDevice = 0;
+	cudaGetDevice(&prevDevice);
+
+	std::shared_lock<std::shared_timed_mutex> allocLock(shared.gpuAllocMutex);
+
+	try
+	{
+		for(const std::unique_ptr<Worker>& worker : workers)
+			if(std::none_of(shared.compressCounters.begin(), shared.compressCounters.end(),
+				[&](const CompressCounters& gpu) { return gpu.gpuID == worker->getGPUID(); } ) )
+			{
+				CompressCounters gpu;
+				gpu.gpuID = worker->getGPUID();
+				checkGpuCall(gpu.gpuID, cudaSetDevice(gpu.gpuID), "Setting CUDA device");
+				checkGpuCall(gpu.gpuID, cudaMalloc(&gpu.counters, sizeof(elb_compress_counters) ),
+					"GPU compress counter allocation");
+				shared.compressCounters.push_back(gpu);
+			}
+
+		for(const CompressCounters& gpu : shared.compressCounters)
+		{ // (on a stream of its own: the legacy default stream would wait for the caller's work)
+			cudaStream_t stream;
+			checkGpuCall(gpu.gpuID, cudaSetDevice(gpu.gpuID), "Setting CUDA device");
+			checkGpuCall(gpu.gpuID, cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking),
+				"CUDA stream creation");
+			cudaError_t clearRes = cudaMemsetAsync(gpu.counters, 0, sizeof(elb_compress_counters),
+				stream);
+			if(clearRes == cudaSuccess)
+				clearRes = cudaStreamSynchronize(stream);
+			cudaStreamDestroy(stream);
+			checkGpuCall(gpu.gpuID, clearRes, "GPU compress counter clear");
+		}
+	}
+	catch(...)
+	{
+		cudaSetDevice(prevDevice);
+		throw;
+	}
+
+	cudaSetDevice(prevDevice);
+}
+
+/* the counters (the workers must not use them any more) */
+void Manager::freeCompressCounters()
+{
+	for(CompressCounters& gpu : shared.compressCounters)
+	{
+		cudaSetDevice(gpu.gpuID);
+		cudaFree(gpu.counters);
+	}
+
+	shared.compressCounters.clear();
+}
+
+void Manager::getCompressStats(elb_compress_counters& out)
+{
+	out = elb_compress_counters{};
+
+	int prevDevice = 0;
+	cudaGetDevice(&prevDevice);
+
+	std::shared_lock<std::shared_timed_mutex> allocLock(shared.gpuAllocMutex);
+
+	for(const CompressCounters& gpu : shared.compressCounters)
+	{
+		elb_compress_counters counters;
+		cudaStream_t stream = NULL;
+		cudaError_t res = cudaSetDevice(gpu.gpuID);
+
+		if(res == cudaSuccess)
+			res = cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking);
+		if(res == cudaSuccess)
+			res = cudaMemcpyAsync(&counters, gpu.counters, sizeof(counters), cudaMemcpyDeviceToHost,
+				stream);
+		if(res == cudaSuccess)
+			res = cudaStreamSynchronize(stream);
+		if(stream)
+			cudaStreamDestroy(stream);
+
+		if(res != cudaSuccess)
+		{
+			cudaSetDevice(prevDevice);
+			checkGpuCall(gpu.gpuID, res, "GPU compress counter read");
+		}
+
+		out.numChunks += counters.numChunks;
+		out.numBytesIn += counters.numBytesIn;
+		out.numBytesStored += counters.numBytesStored;
+		out.numIncompressible += counters.numIncompressible;
+	}
+
+	cudaSetDevice(prevDevice);
 }
 
 /* Statistics::generatePhaseResults (Statistics.cpp:1641-1764) */
@@ -1951,6 +2082,62 @@ int elb_mgr_dedupe_stats(elb_mgr* m, uint64_t* outNumChunks, uint64_t* outNumDis
 		return -1;
 	}
 
+	return 0;
+}
+
+int elb_mgr_set_compress_stats(elb_mgr* m, unsigned chunkShift)
+{
+	if(!m)
+	{
+		elb_set_last_error("elb_mgr_set_compress_stats: NULL manager");
+		return -1;
+	}
+
+	try
+	{
+		m->impl->setCompressStats(chunkShift);
+	}
+	catch(std::exception& e)
+	{
+		elb_set_last_error(e.what() );
+		return -1;
+	}
+
+	return 0;
+}
+
+int elb_mgr_compress_stats(elb_mgr* m, uint64_t* outNumChunks, uint64_t* outNumBytesIn,
+	uint64_t* outNumBytesStored, uint64_t* outNumIncompressible)
+{
+	if(!m || !outNumChunks || !outNumBytesIn || !outNumBytesStored || !outNumIncompressible)
+	{
+		elb_set_last_error("elb_mgr_compress_stats: NULL argument");
+		return -1;
+	}
+
+	if(!m->impl->shared.cfg.compressChunkShift)
+	{
+		elb_set_last_error("elb_mgr_compress_stats: compress stats are off "
+			"(elb_mgr_set_compress_stats)");
+		return -1;
+	}
+
+	elb_compress_counters counters;
+
+	try
+	{
+		m->impl->getCompressStats(counters);
+	}
+	catch(std::exception& e)
+	{
+		elb_set_last_error(e.what() );
+		return -1;
+	}
+
+	*outNumChunks = counters.numChunks;
+	*outNumBytesIn = counters.numBytesIn;
+	*outNumBytesStored = counters.numBytesStored;
+	*outNumIncompressible = counters.numIncompressible;
 	return 0;
 }
 

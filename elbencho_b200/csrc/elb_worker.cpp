@@ -823,10 +823,12 @@ void Worker::preparePhase()
  * --checksums / --checksumverify: which stages take the checksum launch, in chunks of which size
  * and of which algorithm, and the batches' slots. --dedupestats: the table the stages insert into
  * and where the digests come from, the checksum launch's slots when it hashes BLAKE3 at the same
- * chunk size, else the batch's own. Runs after the rings are made and at the start of every write
- * and read phase, since a checksum list (elb_mgr_set_checksum_list) may be set and the manager may
- * make new tables between phases; a change drops the batch graphs, which hold the launches of the
- * old setup. Without these options it allocates and changes nothing.
+ * chunk size, else the batch's own. --compressstats: the chunk size and counters of the stages'
+ * LZ4 launch. Runs after the rings are made and at the start of every write and read phase, since
+ * a checksum list (elb_mgr_set_checksum_list) or the LZ4 chunk size (elb_mgr_set_compress_stats)
+ * may be set and the manager may make new tables between phases; a change drops the batch graphs,
+ * which hold the launches of the old setup. Without these options it allocates and changes
+ * nothing.
  */
 void Worker::setupChecksums()
 {
@@ -854,12 +856,21 @@ void Worker::setupChecksums()
 	const uint64_t dedupeSlots = !dedupe ? 1 : std::max( (cfg.blockSize +
 		( (uint64_t)1 << cfg.dedupeChunkShift) - 1) >> cfg.dedupeChunkShift, (uint64_t)1);
 
+	elb_compress_counters* lz4Counters = NULL;
+
+	for(const CompressCounters& gpuCounters : shared->compressCounters)
+		if(cfg.compressChunkShift && (gpuCounters.gpuID == gpuID) )
+			lz4Counters = gpuCounters.counters;
+
+	const unsigned lz4ChunkShift = lz4Counters ? cfg.compressChunkShift : 0;
+
 	if(batches.empty() || ( (readChecksum == readStage.checksum) &&
 		(chunkShift == checksumChunkShift) && (slotsPerDesc == checksumSlotsPerDesc) &&
 		(cfg.checksumAlgo == checksumAlgo) && (dedupe == readStage.dedupe) &&
 		(table.entries == dedupeTable.entries) && (table.numEntries == dedupeTable.numEntries) &&
 		(table.counters == dedupeTable.counters) && (dedupeSlots == dedupeSlotsPerDesc) &&
-		( (dedupeUsesSums && readChecksum) == dedupeUsesReadSums) ) )
+		( (dedupeUsesSums && readChecksum) == dedupeUsesReadSums) &&
+		(lz4ChunkShift == compressChunkShift) && (lz4Counters == compressCounters) ) )
 		return;
 
 	std::shared_lock<std::shared_timed_mutex> allocLock(shared->gpuAllocMutex);
@@ -869,9 +880,17 @@ void Worker::setupChecksums()
 	writeStage.dedupe = dedupe;
 	readStage.dedupe = dedupe;
 	verifyBackStage.dedupe = false;
-	/* --verifydirect: a write phase's checksums and dedupe counts are those of the written bytes,
-	   so the read-back takes none, and must not share the read phase's batch graphs then */
-	verifyBackStage.useGraph = readStage.useGraph && !readChecksum && !dedupe;
+	writeStage.compress = (lz4ChunkShift != 0);
+	readStage.compress = (lz4ChunkShift != 0);
+	verifyBackStage.compress = false;
+	/* --verifydirect: a write phase's checksums, dedupe and compress counts are those of the
+	   written bytes, so the read-back takes none, and must not share the read phase's batch graphs
+	   then */
+	verifyBackStage.useGraph = readStage.useGraph && !readChecksum && !dedupe && !lz4ChunkShift;
+	compressChunkShift = lz4ChunkShift;
+	compressCounters = lz4Counters;
+	compressSlotsPerDesc = !lz4ChunkShift ? 1 : std::max( (cfg.blockSize +
+		( (uint64_t)1 << lz4ChunkShift) - 1) >> lz4ChunkShift, (uint64_t)1);
 	dedupeTable = table;
 	dedupeSlotsPerDesc = dedupeSlots;
 	dedupeUsesWriteSums = dedupeUsesSums && cfg.checksums;
@@ -2480,6 +2499,11 @@ void Worker::enqueueStage(Batch& batch, const GpuStage& stage, uint32_t numBlock
 	if(stage.dedupe)
 		enqueueDedupeInsert(batch, stage, numBlocks);
 
+	// (--compressstats: nothing is copied or waited for, the counters are read after the phase)
+	if(stage.compress && elb_launch_lz4_chunks(batch.hostDescs, numBlocks, compressChunkShift,
+		compressSlotsPerDesc, compressCounters, NULL, NULL, batch.stream) )
+		throw WorkerError(std::string("GPU compress stats failed. ") + elb_last_error() );
+
 	if( (stage.transfer == GpuStage::TRANSFER_COPY) && !stage.isRead)
 		enqueueStageCopies(batch, false, true);
 }
@@ -2564,6 +2588,8 @@ void Worker::gpuLaunchStage(Batch& batch, bool isRead)
 	if(numBlocks && stage.dedupe) // (the insert, and the BLAKE3 launch unless it shares one)
 		numKernelLaunches += (stage.checksum &&
 			(stage.isRead ? dedupeUsesReadSums : dedupeUsesWriteSums) ) ? 1 : 2;
+	if(numBlocks && stage.compress)
+		numKernelLaunches++;
 
 	if(stage.transfer != GpuStage::TRANSFER_NONE)
 		(isRead ? numH2DBytes : numD2HBytes) += numBytes;

@@ -62,6 +62,14 @@ struct DedupeTable
 	elb_dedupe_counters* counters{NULL};
 };
 
+/* --compressstats: the LZ4 counters of one GPU (elb_lz4_chunks), made by the manager when first
+ * needed and cleared at the start of every write and read phase, shared by the GPU's workers */
+struct CompressCounters
+{
+	int gpuID{-1};
+	elb_compress_counters* counters{NULL};
+};
+
 /* WorkersSharedData (reference source/workers/WorkersSharedData.h:33-107): phase barrier and
  * done counters. The reference's boost uuid bench ID becomes a sequence number. */
 struct Shared
@@ -87,6 +95,7 @@ struct Shared
 	std::shared_ptr<const ChecksumList> checksumList; // --checksumverify (set between phases)
 	std::vector<DedupeTable> dedupeTables; // --dedupestats: one per GPU, the first worker's first
 	uint8_t dedupeZeroDigest[32]{};        // --dedupestats: the BLAKE3 of a chunk of zero bytes
+	std::vector<CompressCounters> compressCounters; // --compressstats: one per GPU
 
 	/* workers hold this shared while they allocate / free device memory or instantiate graphs;
 	   the live stats reducer holds it exclusively while its collective is in flight, because a
@@ -263,6 +272,7 @@ struct GpuStage
 	                  // kernel staging)
 	bool checksum;    // --checksums, a checksum list: the checksum launch over the device slots
 	bool dedupe;      // --dedupestats: the chunks' digests go into the GPU's fingerprint table
+	bool compress;    // --compressstats: the LZ4 launch over the chunks, into the GPU's counters
 };
 
 /* a batch: a contiguous slice of the rings plus everything its GPU stage needs */
@@ -493,6 +503,11 @@ class Worker
 		uint64_t dedupeSlotsPerDesc{1};
 		bool dedupeUsesWriteSums{false};
 		bool dedupeUsesReadSums{false};
+		/* --compressstats: the chunk shift and counters that the stages' LZ4 launches use (0: none)
+		   and their slots per descriptor */
+		unsigned compressChunkShift{0};
+		elb_compress_counters* compressCounters{NULL};
+		uint64_t compressSlotsPerDesc{1};
 
 		// accounting
 		std::atomic<uint64_t> numH2DBytes{0};
@@ -639,6 +654,13 @@ class Manager
 		void getDedupeStats(uint64_t& outNumChunks, uint64_t& outNumDistinct,
 			uint64_t& outNumZero);
 
+		/* --compressstats: from the next write or read phase on, the LZ4 counts of chunks of
+		   2^chunkShift bytes (0: off); throws WorkerError for a shift outside 12..20 or a config
+		   it cannot be used with */
+		void setCompressStats(unsigned chunkShift);
+		/* --compressstats: the counters of the last write or read phase, summed over all GPUs */
+		void getCompressStats(elb_compress_counters& out);
+
 		Shared shared;
 		std::vector<std::unique_ptr<Worker> > workers;
 		std::vector<std::thread> threads;
@@ -656,6 +678,8 @@ class Manager
 		unsigned dedupeZeroDigestShift{0}; // the chunk shift of shared.dedupeZeroDigest (0: none)
 		void prepareDedupeTables(int benchPhase);
 		void freeDedupeTables();
+		void prepareCompressCounters(int benchPhase);
+		void freeCompressCounters();
 		std::unique_ptr<LiveStatsReducer> liveStatsReducer; // created on first use
 		std::mutex liveStatsReducerMutex;
 };

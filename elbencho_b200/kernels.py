@@ -467,3 +467,42 @@ def dedupe_counters(raw):
     """(chunks, distinct, zero, overflow) from the 32 bytes of elb_dedupe_counters"""
     import struct
     return struct.unpack("<QQQI4x", bytes(raw))
+
+
+# ---- --compressstats: one LZ4 block per chunk ----
+
+COMPRESS_COUNTERS_BYTES = 32  # elb_compress_counters: chunks, bytes in, bytes stored, incompressible
+
+
+def lz4_out_slot_bytes(chunk_shift):
+    """the bytes of one output slot of lz4_chunks (ELB_LZ4_OUT_SLOT_BYTES)"""
+    return (1 << chunk_shift) + (1 << chunk_shift) // 255 + 16
+
+
+def lz4_chunks(pinned_descs_ptr, num_descs, chunk_shift, slots_per_desc, dev_counters_ptr,
+               dev_sizes_ptr=0, dev_out_ptr=0, stream=0):
+    """Compress each chunk of 2**chunk_shift bytes (12..20) of the descriptors into one LZ4 block
+    and add it to the 32-byte counters at dev_counters_ptr (compress_counters). If given, the
+    block size of chunk j of descriptor i goes to the uint32 at dev_sizes_ptr + 4 * (i *
+    slots_per_desc + j), and its bytes to dev_out_ptr + (i * slots_per_desc + j) *
+    lz4_out_slot_bytes(chunk_shift)."""
+    _check(_native.load().elb_lz4_chunks(pinned_descs_ptr or None, num_descs, chunk_shift,
+                                         slots_per_desc, dev_counters_ptr or None,
+                                         dev_sizes_ptr or None, dev_out_ptr or None, stream),
+           "elb_lz4_chunks")
+
+
+def compress_counters(raw):
+    """(chunks, bytes in, bytes stored, incompressible) from the 32 bytes of elb_compress_counters"""
+    import struct
+    return struct.unpack("<QQQQ", bytes(raw))
+
+
+def compress_line(chunk_size, chunks, bytes_in, bytes_stored, incompressible):
+    """the console line of --compressstats for these counts"""
+    counters = (ctypes.c_uint64 * 4)(chunks, bytes_in, bytes_stored, incompressible)
+    buf = ctypes.create_string_buffer(256)
+    lib = _native.load()
+    if lib.elb_format_compress_line(chunk_size, counters, buf, len(buf)) < 0:
+        raise KernelError("elb_format_compress_line failed: %s" % _native.last_error())
+    return buf.value.decode()

@@ -118,6 +118,7 @@ class WorkerConfig:
     checksum_chunk_shift: int = 0     # --checksumchunk: CRCs of 2**shift byte chunks (0: files)
     checksum_algo: str = "crc32"      # --checksumalgo: "crc32", "crc32c", "crc64nvme" or "blake3"
     dedupe_chunk: int = 0             # --dedupestats bytes (a power of two 4K..1G; 0 = off)
+    compress_chunk: int = 0           # --compressstats bytes (a power of two 4K..1M; 0 = off)
     serialize_buffered_writes: int = 0  # 0 auto, 1 on, 2 off (--writegate)
     staging_engine: int = 0           # 0 auto, 1 kernels move the data, 2 cudaMemcpyAsync
     no_gpu_numa_binding: bool = False  # --nogpunuma
@@ -289,6 +290,14 @@ class WorkerManager:
         self._h = self._lib.elb_mgr_create(ctypes.byref(cfg))
         if not self._h:
             raise WorkerError(_native.last_error())
+        chunk = config.compress_chunk
+        if chunk:
+            # (not a power of two: a shift that the library rejects)
+            shift = chunk.bit_length() - 1 if not chunk & (chunk - 1) else 0xffffffff
+            if self._lib.elb_mgr_set_compress_stats(self._h, shift) != 0:
+                err = _native.last_error()
+                self.close()
+                raise WorkerError(err)
 
     def close(self):
         if self._h:
@@ -445,6 +454,14 @@ class WorkerManager:
         over all workers and GPUs."""
         vals = [ctypes.c_uint64(0) for _ in range(3)]
         if self._lib.elb_mgr_dedupe_stats(self._h, *[ctypes.byref(v) for v in vals]) != 0:
+            raise WorkerError(_native.last_error())
+        return tuple(v.value for v in vals)
+
+    def compress_stats(self):
+        """--compressstats: (chunks, bytes, bytes stored, incompressible chunks) of the last write or
+        read phase, over all workers and GPUs; the ratio is bytes / bytes stored."""
+        vals = [ctypes.c_uint64(0) for _ in range(4)]
+        if self._lib.elb_mgr_compress_stats(self._h, *[ctypes.byref(v) for v in vals]) != 0:
             raise WorkerError(_native.last_error())
         return tuple(v.value for v in vals)
 

@@ -391,6 +391,34 @@ int elb_dedupe_merge(const void* srcEntries, uint64_t numSrcEntries, void* table
  * the host. Returns -1 for another chunkShift. */
 int elb_dedupe_zero_digest(unsigned chunkShift, uint8_t* out);
 
+/* --compressstats: the LZ4 counters of one GPU (device memory, zero at the start) */
+typedef struct elb_compress_counters
+{
+	uint64_t numChunks;         /* chunks compressed (N) */
+	uint64_t numBytesIn;        /* the sum of their lengths (B) */
+	uint64_t numBytesStored;    /* the sum of min(LZ4 block size, chunk length) (S) */
+	uint64_t numIncompressible; /* chunks whose LZ4 block is not shorter than the chunk (U) */
+} elb_compress_counters;
+
+/* the bytes of one output slot of elb_lz4_chunks for chunks of 2^chunkShift bytes */
+#define ELB_LZ4_OUT_SLOT_BYTES(chunkShift) \
+	( (1ULL << (chunkShift) ) + ( (1ULL << (chunkShift) ) / 255) + 16)
+
+/* --compressstats: compress every chunk of 2^chunkShift bytes (12..20) of the descriptors into one
+ * LZ4 block each, by the greedy parse of DESIGN.md "--compressstats" (a 4096-entry hash table of
+ * the most recent position, no backward extension, the last 5 bytes literals). Descriptor i has
+ * ceil(len_i / 2^chunkShift) chunks, chunk j being its bytes [j * 2^chunkShift, min((j + 1) *
+ * 2^chunkShift, len_i)). Adds to devCounters (device memory) every chunk, its length, min(block
+ * size, length) and whether the block did not shrink. If not NULL, devSizes[i * slotsPerDesc + j]
+ * (uint32) gets the LZ4 block size of chunk j of descriptor i, and devOut + (i * slotsPerDesc + j)
+ * * ELB_LZ4_OUT_SLOT_BYTES(chunkShift) its bytes. descs must be pinned host memory: the host checks
+ * them and sizes the grid from their lengths, the device reads them. Fails without launching for a
+ * chunkShift outside 12..20, NULL pointers, a descriptor off a chunk boundary of the file or one
+ * with more chunks than slotsPerDesc. */
+int elb_lz4_chunks(const elb_block_desc* descs, uint32_t numDescs, unsigned chunkShift,
+	uint64_t slotsPerDesc, elb_compress_counters* devCounters, uint32_t* devSizes, void* devOut,
+	void* stream);
+
 int elb_stage_copy(const elb_block_desc* descs, uint32_t numDescs, int hostToDevice,
 	int64_t hostDelta, uint64_t totalBytes, uint64_t maxBlockLen, void* stream);
 /* devResults[0..numDescs) <- {0, ~0} */
@@ -724,6 +752,11 @@ uint64_t elb_per_sec_from_usec(uint64_t totalValue, uint64_t elapsedUSec);
  * text length (text truncated to outBufLen - 1), -1 on error. */
 int64_t elb_format_value(int kind, uint64_t value, double percentage, const elb_histogram* histo,
 	char* outBuf, uint64_t outBufLen);
+/* --compressstats: the console line of a phase's counters for chunks of chunkSize bytes, "Compress:
+ * <N> chunks of <K>, <U> incompressible: <B> bytes to <S>: <B/S>:1" (the ratio with two decimals,
+ * 1.00 when S is 0). Returns the text length (text truncated to outBufLen - 1), -1 on error. */
+int64_t elb_format_compress_line(uint64_t chunkSize, const elb_compress_counters* counters,
+	char* outBuf, uint64_t outBufLen);
 /* UnitTk::numHumanToBytesBinary (toolkits/UnitTk.cpp:18-76): "4k", "1M", "64G"; 0 ok, -1 error */
 int elb_num_human_to_bytes(const char* numHuman, uint64_t* outBytes);
 
@@ -883,6 +916,18 @@ int elb_mgr_checksum_verify_counts(elb_mgr* m, uint64_t* outNumChunks, uint64_t*
  * past its probe bound (elb_last_error), else 0. */
 int elb_mgr_dedupe_stats(elb_mgr* m, uint64_t* outNumChunks, uint64_t* outNumDistinct,
 	uint64_t* outNumZero);
+/* --compressstats: from the next write or read phase on, compress every chunk of 2^chunkShift file
+ * bytes (12..20) that a phase moves with elb_lz4_chunks and count it (elb_mgr_compress_stats);
+ * 0 turns it off. Returns -1 (elb_last_error) for another chunkShift, or if the config has a block
+ * size that is not a multiple of the chunk size (after a block larger than the file is reduced to
+ * the file size), unaligned random offsets or rwmix. */
+int elb_mgr_set_compress_stats(elb_mgr* m, unsigned chunkShift);
+/* --compressstats: of the last write or read phase, the chunks it moved (N), their bytes (B), the
+ * sum of min(LZ4 block size, chunk length) (S) and the chunks whose block did not shrink (U), over
+ * all workers and GPUs of the manager. All 0 before the first such phase. Returns -1 if
+ * --compressstats is off (elb_last_error), else 0. */
+int elb_mgr_compress_stats(elb_mgr* m, uint64_t* outNumChunks, uint64_t* outNumBytesIn,
+	uint64_t* outNumBytesStored, uint64_t* outNumIncompressible);
 
 uint32_t elb_mgr_num_workers(elb_mgr* m);
 elb_worker* elb_mgr_worker(elb_mgr* m, uint32_t localIdx);
