@@ -19,6 +19,7 @@ SOURCES = [
     "elb_capi_kernels.cu",
     "elb_dedupe.cu",
     "elb_compress.cu",
+    "elb_reduce.cu",
     "elb_config.cpp",
     "elb_cufile.cpp",
     "elb_worker.cpp",

@@ -714,6 +714,138 @@ int elb_lz4_chunks(const elb_block_desc* descs, uint32_t numDescs, unsigned chun
 	return 0;
 }
 
+/* the table checks of elb_reduce_insert, _merge and _sum */
+static bool reduceTableArgsValid(const char* what, const void* table, uint64_t tableEntries,
+	const void* devCounters)
+{
+	if(!tableEntries || (tableEntries & (tableEntries - 1) ) )
+	{
+		elb_set_last_error(std::string(what) + ": table size " + std::to_string(tableEntries) +
+			" is not a power of two");
+		return false;
+	}
+
+	if(!table || !devCounters)
+	{
+		elb_set_last_error(std::string(what) + ": NULL table or counters");
+		return false;
+	}
+
+	return true;
+}
+
+/* the chunk shift check of elb_reduce_insert and _lz4 */
+static bool reduceChunkShiftValid(const char* what, unsigned chunkShift)
+{
+	if( (chunkShift < ELB_COMPRESS_MIN_CHUNK_SHIFT) || (chunkShift > ELB_COMPRESS_MAX_CHUNK_SHIFT) )
+	{
+		elb_set_last_error(std::string(what) + ": chunk shift " + std::to_string(chunkShift) +
+			" is not in [" + std::to_string(ELB_COMPRESS_MIN_CHUNK_SHIFT) + ", " +
+			std::to_string(ELB_COMPRESS_MAX_CHUNK_SHIFT) + "]");
+		return false;
+	}
+
+	return true;
+}
+
+int elb_reduce_insert(const elb_block_desc* descs, uint32_t numDescs, unsigned chunkShift,
+	uint64_t slotsPerDesc, const void* devDigests, void* table, uint64_t tableEntries,
+	elb_reduce_counters* devCounters, uint64_t* devMarks, void* stream)
+{
+	const char* what = "elb_reduce_insert";
+
+	if(!reduceTableArgsValid(what, table, tableEntries, devCounters) ||
+		!reduceChunkShiftValid(what, chunkShift) )
+		return -1;
+
+	if(numDescs && (!descs || !devDigests || !devMarks) )
+	{
+		elb_set_last_error(std::string(what) + ": NULL descriptor, digest or mark array");
+		return -1;
+	}
+
+	if(elb_launch_reduce_insert(descs, numDescs, chunkShift, slotsPerDesc, devDigests, table,
+		tableEntries, devCounters, devMarks, (cudaStream_t)stream) )
+	{
+		elb_set_last_error(std::string("elb_") + elb_last_error() );
+		return -1;
+	}
+
+	return 0;
+}
+
+int elb_reduce_lz4(const elb_block_desc* descs, uint32_t numDescs, unsigned chunkShift,
+	uint64_t slotsPerDesc, const uint64_t* devMarks, void* devPayloads, void* stream)
+{
+	const char* what = "elb_reduce_lz4";
+
+	if(!reduceChunkShiftValid(what, chunkShift) )
+		return -1;
+
+	if(numDescs && (!descs || !devMarks || !devPayloads) )
+	{
+		elb_set_last_error(std::string(what) + ": NULL descriptor, mark or payload array");
+		return -1;
+	}
+
+	if(elb_launch_reduce_lz4(descs, numDescs, chunkShift, slotsPerDesc, devMarks, devPayloads,
+		(cudaStream_t)stream) )
+	{
+		elb_set_last_error(std::string("elb_") + elb_last_error() );
+		return -1;
+	}
+
+	return 0;
+}
+
+int elb_reduce_merge(const void* srcEntries, const void* srcPayloads, uint64_t numSrcEntries,
+	void* table, void* payloads, uint64_t tableEntries, elb_reduce_counters* devCounters,
+	void* stream)
+{
+	const char* what = "elb_reduce_merge";
+
+	if(!reduceTableArgsValid(what, table, tableEntries, devCounters) )
+		return -1;
+
+	if(!payloads || (numSrcEntries && (!srcEntries || !srcPayloads) ) )
+	{
+		elb_set_last_error(std::string(what) + ": NULL payloads or source entries");
+		return -1;
+	}
+
+	if(elb_launch_reduce_merge(srcEntries, srcPayloads, numSrcEntries, table, payloads,
+		tableEntries, devCounters, (cudaStream_t)stream) )
+	{
+		elb_set_last_error(std::string("elb_") + elb_last_error() );
+		return -1;
+	}
+
+	return 0;
+}
+
+int elb_reduce_sum(const void* table, const void* payloads, uint64_t tableEntries,
+	elb_reduce_counters* devCounters, void* stream)
+{
+	const char* what = "elb_reduce_sum";
+
+	if(!reduceTableArgsValid(what, table, tableEntries, devCounters) )
+		return -1;
+
+	if(!payloads)
+	{
+		elb_set_last_error(std::string(what) + ": NULL payloads");
+		return -1;
+	}
+
+	if(elb_launch_reduce_sum(table, payloads, tableEntries, devCounters, (cudaStream_t)stream) )
+	{
+		elb_set_last_error(std::string("elb_") + elb_last_error() );
+		return -1;
+	}
+
+	return 0;
+}
+
 int elb_stage_copy(const elb_block_desc* descs, uint32_t numDescs, int hostToDevice,
 	int64_t hostDelta, uint64_t totalBytes, uint64_t maxBlockLen, void* stream)
 {

@@ -163,6 +163,16 @@ static const OptDef optDefs[] =
 		"short last chunk is a chunk of its own length. The parse is greedy and simpler than the "
 		"lz4 tool's, so its ratio is not lz4's. Cannot be used with --norandalign, --rwmixpct, "
 		"--rwmixthr or --hosts. [b200]"},
+	{"reducestats", 0, Opt_BYTES, &ProgArgs::reduceStatsChunkSize, Wire_NONE, "Chunk size of data "
+		"reduction statistics: every write and read phase counts the chunks of this size (a power "
+		"of two from 4K to 1M that the block size is a multiple of) that it moved, finds the "
+		"distinct ones by BLAKE3 digest as --dedupestats does and compresses each distinct chunk "
+		"once into one LZ4 block as --compressstats does, all on the GPU. It prints \"Reduce: <N> "
+		"chunks of <K>, <D> distinct: <B> bytes, <U> distinct bytes stored as <S>: dedupe "
+		"<B/U>:1, compress <U/S>:1, total <B/S>:1\", where U counts each distinct chunk once and "
+		"S stores it as min(LZ4 size, length): what storage that deduplicates and compresses "
+		"would keep. A file's short last chunk is a chunk of its own length. Cannot be used with "
+		"--rand, --norandalign, --infloop, --rwmixpct, --rwmixthr or --hosts. [b200]"},
 	{"rwmixpct", 0, Opt_U64, &ProgArgs::rwMixReadPercent, Wire_REF, "Percentage of blocks that "
 		"should be read in a write phase."},
 	{"rwmixthr", 0, Opt_U64, &ProgArgs::numRWMixReadThreads, Wire_REF, "Number of threads that "
@@ -1107,6 +1117,41 @@ void ProgArgs::checkArgs()
 
 		if(!hosts.empty() )
 			throw ProgError("Option \"--compressstats\" cannot be used together with \"--hosts\"");
+	}
+
+	if(reduceStatsChunkSize)
+	{
+		if( (reduceStatsChunkSize < (1ULL << ELB_COMPRESS_MIN_CHUNK_SHIFT) ) ||
+			(reduceStatsChunkSize > (1ULL << ELB_COMPRESS_MAX_CHUNK_SHIFT) ) ||
+			(reduceStatsChunkSize & (reduceStatsChunkSize - 1) ) )
+			throw ProgError("Option \"--reducestats\" must be a power of two from 4K to 1M");
+
+		/* (as the manager: a block reduced to the file size is the whole file, whose last chunk
+		   may be short) */
+		const uint64_t fileBlockSize = (fileSize && (blockSize > fileSize) ) ? fileSize : blockSize;
+
+		if( (fileBlockSize % reduceStatsChunkSize) && (fileBlockSize != fileSize) )
+			throw ProgError("The block size (" + std::to_string(blockSize) + ") must be a multiple "
+				"of \"--reducestats\" (" + std::to_string(reduceStatsChunkSize) + ")");
+
+		if(useRandomUnaligned)
+			throw ProgError("Option \"--reducestats\" cannot be used together with "
+				"\"--norandalign\"");
+
+		if(useRandomOffsets)
+			throw ProgError("Option \"--reducestats\" cannot be used together with \"--rand\"");
+
+		if(doInfiniteIOLoop)
+			throw ProgError("Option \"--reducestats\" cannot be used together with \"--infloop\"");
+
+		if(rwMixReadPercent)
+			throw ProgError("Option \"--reducestats\" cannot be used together with \"--rwmixpct\"");
+
+		if(numRWMixReadThreads)
+			throw ProgError("Option \"--reducestats\" cannot be used together with \"--rwmixthr\"");
+
+		if(!hosts.empty() )
+			throw ProgError("Option \"--reducestats\" cannot be used together with \"--hosts\"");
 	}
 
 	if(!checksumAlgoName.empty() )

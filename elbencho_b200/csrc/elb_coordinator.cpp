@@ -76,6 +76,7 @@ class Coordinator
 		void printChecksumVerifyLine(int benchPhase);
 		void printDedupeLine(int benchPhase);
 		void printCompressLine(int benchPhase);
+		void printReduceLine(int benchPhase);
 		void printDryRunInfo();
 };
 
@@ -340,6 +341,49 @@ void Coordinator::printCompressLine(int benchPhase)
 	std::cout << formatCompressLine(progArgs.compressStatsChunkSize, counters) << std::endl;
 }
 
+/* a ratio of the --reducestats line: two decimals, 1.00 when den is 0 */
+static std::string formatReduceRatio(uint64_t num, uint64_t den)
+{
+	char ratio[32];
+	snprintf(ratio, sizeof(ratio), "%.2f", den ? (double)num / den : 1.0);
+	return ratio;
+}
+
+/* --reducestats: "Reduce: <N> chunks of <K>, <D> distinct: <B> bytes, <U> distinct bytes stored as
+   <S>: dedupe <B/U>:1, compress <U/S>:1, total <B/S>:1" */
+static std::string formatReduceLine(uint64_t chunkSize, const elb_reduce_counters& counters)
+{
+	return "Reduce: " + std::to_string(counters.numChunks) + " chunks of " +
+		std::to_string(chunkSize) + ", " + std::to_string(counters.numDistinct) + " distinct: " +
+		std::to_string(counters.numBytes) + " bytes, " +
+		std::to_string(counters.numBytesDistinct) + " distinct bytes stored as " +
+		std::to_string(counters.numBytesStored) + ": dedupe " +
+		formatReduceRatio(counters.numBytes, counters.numBytesDistinct) + ":1, compress " +
+		formatReduceRatio(counters.numBytesDistinct, counters.numBytesStored) + ":1, total " +
+		formatReduceRatio(counters.numBytes, counters.numBytesStored) + ":1";
+}
+
+/* --reducestats: after each write and read phase that succeeded, its counts and their ratios */
+void Coordinator::printReduceLine(int benchPhase)
+{
+	if(!progArgs.reduceStatsChunkSize ||
+		( (benchPhase != ELB_PHASE_CREATEFILES) && (benchPhase != ELB_PHASE_READFILES) ) )
+		return;
+
+	elb_reduce_counters counters;
+
+	try
+	{
+		manager->getReduceStats(counters);
+	}
+	catch(const WorkerError& e)
+	{
+		throw ProgError(e.what() );
+	}
+
+	std::cout << formatReduceLine(progArgs.reduceStatsChunkSize, counters) << std::endl;
+}
+
 /* Coordinator::runBenchmarkPhase (:248-272) + Statistics live loop (:1284-1345) */
 void Coordinator::runBenchmarkPhase(int benchPhase)
 {
@@ -479,6 +523,7 @@ void Coordinator::runBenchmarkPhase(int benchPhase)
 	printChecksumVerifyLine(benchPhase);
 	printDedupeLine(benchPhase);
 	printCompressLine(benchPhase);
+	printReduceLine(benchPhase);
 }
 
 void waitForUserDefinedStartTime(const ProgArgs& progArgs) // Coordinator.cpp:149-158
@@ -610,6 +655,9 @@ int Coordinator::main() // Coordinator.cpp:31-142
 
 		if(progArgs.compressStatsChunkSize)
 			manager->setCompressStats(__builtin_ctzll(progArgs.compressStatsChunkSize) );
+
+		if(progArgs.reduceStatsChunkSize)
+			manager->setReduceStats(__builtin_ctzll(progArgs.reduceStatsChunkSize) );
 
 		/* workers on several GPUs: create the NCCL communicators of the statistics reduce now,
 		   while the workers are idle (and before any result output) */
@@ -765,6 +813,27 @@ extern "C" int64_t elb_format_compress_line(uint64_t chunkSize,
 	}
 
 	const std::string text = elb::formatCompressLine(chunkSize, *counters);
+
+	if(outBuf && outBufLen)
+	{
+		const size_t copyLen = std::min( (size_t)(outBufLen - 1), text.size() );
+		memcpy(outBuf, text.data(), copyLen);
+		outBuf[copyLen] = 0;
+	}
+
+	return (int64_t)text.size();
+}
+
+extern "C" int64_t elb_format_reduce_line(uint64_t chunkSize, const elb_reduce_counters* counters,
+	char* outBuf, uint64_t outBufLen)
+{
+	if(!counters)
+	{
+		elb_set_last_error("elb_format_reduce_line: NULL counters");
+		return -1;
+	}
+
+	const std::string text = elb::formatReduceLine(chunkSize, *counters);
 
 	if(outBuf && outBufLen)
 	{

@@ -1007,6 +1007,7 @@ struct Config
 	int checksumAlgo{ELB_CHECKSUM_CRC32}; // --checksumalgo / the checksum list's (elb_crc_algo::ID)
 	unsigned dedupeChunkShift{0}; // --dedupestats: chunks of 2^shift bytes (0: off), 12..30
 	unsigned compressChunkShift{0}; // --compressstats (elb_mgr_set_compress_stats): 0 off, 12..20
+	unsigned reduceChunkShift{0}; // --reducestats (elb_mgr_set_reduce_stats): 0 off, 12..20
 	int serializeBufferedWrites{ELB_WRITEGATE_AUTO};
 	int stagingEngine{ELB_STAGING_AUTO};
 	bool noGPUNumaBinding{false};

@@ -124,6 +124,19 @@ void elb_dedupe_zero_chunk_digest(unsigned chunkShift, uint8_t out[32]); // chun
 int elb_launch_lz4_chunks(const elb_block_desc* descs, uint32_t numDescs, unsigned chunkShift,
 	uint64_t slotsPerDesc, elb_compress_counters* devCounters, uint32_t* devSizes, void* devOut,
 	cudaStream_t stream);
+/* --reducestats (elb_reduce.cu; elb_reduce_insert, _lz4, _merge, _sum): descs must be host- and
+   device-readable, the host checks them and sizes the grid from their lengths. Chunk shifts are
+   those of --compressstats. */
+int elb_launch_reduce_insert(const elb_block_desc* descs, uint32_t numDescs, unsigned chunkShift,
+	uint64_t slotsPerDesc, const void* devDigests, void* table, uint64_t tableEntries,
+	elb_reduce_counters* devCounters, uint64_t* devMarks, cudaStream_t stream);
+int elb_launch_reduce_lz4(const elb_block_desc* descs, uint32_t numDescs, unsigned chunkShift,
+	uint64_t slotsPerDesc, const uint64_t* devMarks, void* payloads, cudaStream_t stream);
+int elb_launch_reduce_merge(const void* srcEntries, const void* srcPayloads,
+	uint64_t numSrcEntries, void* table, void* payloads, uint64_t tableEntries,
+	elb_reduce_counters* devCounters, cudaStream_t stream);
+int elb_launch_reduce_sum(const void* table, const void* payloads, uint64_t tableEntries,
+	elb_reduce_counters* devCounters, cudaStream_t stream);
 int elb_kernels_warmup();
 uint64_t elb_get_num_kernel_launches();
 void elb_count_kernel_launch(); // (launches of the kernels outside elb_kernels.cu)

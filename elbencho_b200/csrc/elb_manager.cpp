@@ -135,6 +135,7 @@ Manager::~Manager()
 
 	freeDedupeTables();
 	freeCompressCounters();
+	freeReduceTables();
 	closeBenchPathFDs();
 }
 
@@ -388,6 +389,7 @@ void Manager::startNextPhase(int benchPhase)
 	prepareFilesForPhase(benchPhase);
 	prepareDedupeTables(benchPhase);
 	prepareCompressCounters(benchPhase);
+	prepareReduceTables(benchPhase);
 
 	std::unique_lock<std::mutex> lock(shared.mutex);
 
@@ -839,15 +841,14 @@ void Manager::getChecksumVerifyCounts(uint64_t& outNumChunks, uint64_t& outNumFi
 	outNumFiles = paths.size();
 }
 
-/* --dedupestats: the K-chunks the worker of the given rank can move in a phase, capped by the
- * data set's. Sequential file mode: its share of the paths' blocks as FileSeqSource cuts them, the
- * standard share, or the last data set thread's with the remainder; no block spans two files, so a
- * block holds at most ceil(blockSize / K) chunks. Strided access: the whole data set. Dir mode:
+/* --dedupestats, --reducestats: the K-chunks the worker of the given rank can move in a phase,
+ * capped by the data set's. Sequential file mode: its share of the paths' blocks as FileSeqSource
+ * cuts them, the standard share, or the last data set thread's with the remainder; no block spans
+ * two files, so a block holds at most ceil(blockSize / K) chunks. Strided access: the whole data set. Dir mode:
  * its own files. Custom tree mode: the whole tree, since the shares can be uneven. */
 static uint64_t dedupeWorkerChunkBound(const Config& cfg, const TreeManifest& customTree,
-	uint64_t rank)
+	uint64_t rank, unsigned shift)
 {
-	const unsigned shift = cfg.dedupeChunkShift;
 	const uint64_t chunkSize = (uint64_t)1 << shift;
 	const uint64_t fileChunks = (cfg.fileSize + chunkSize - 1) >> shift;
 
@@ -875,9 +876,9 @@ static uint64_t dedupeWorkerChunkBound(const Config& cfg, const TreeManifest& cu
 
 /* the K-chunks that the whole data set of a phase has (custom tree mode: the tree; dir mode: no
  * cap beyond the workers' own files) */
-static uint64_t dedupeDataSetChunks(const Config& cfg, const TreeManifest& customTree)
+static uint64_t dedupeDataSetChunks(const Config& cfg, const TreeManifest& customTree,
+	unsigned shift)
 {
-	const unsigned shift = cfg.dedupeChunkShift;
 
 	if( (cfg.pathType == ELB_PATH_DIR) && customTree.isLoaded)
 		return (customTree.getNumFileBytes() >> shift) + customTree.getNumFiles();
@@ -895,11 +896,49 @@ static void checkGpuCall(int gpuID, cudaError_t res, const char* what)
 			"; CUDA Error: " + cudaGetErrorString(res) );
 }
 
+/* --dedupestats, --reducestats: the GPUs of the workers, the first worker's first, and the
+ * entries of each GPU's table of chunks of 2^chunkShift bytes: the next power of two at or above
+ * twice the chunks that the GPU's workers can move (the first GPU's: all of the phase's chunks, as
+ * the others are merged into it), so its load stays at or below 0.5 */
+std::vector<std::pair<int, uint64_t> > Manager::chunkTableSizes(unsigned chunkShift)
+{
+	const Config& cfg = shared.cfg;
+	const uint64_t dataSetChunks = dedupeDataSetChunks(cfg, shared.customTree, chunkShift);
+	std::vector<std::pair<int, uint64_t> > gpuChunks;
+	uint64_t phaseChunks = 0;
+
+	for(const std::unique_ptr<Worker>& worker : workers)
+	{
+		const uint64_t workerChunks = dedupeWorkerChunkBound(cfg, shared.customTree,
+			worker->getRank(), chunkShift);
+		auto iter = std::find_if(gpuChunks.begin(), gpuChunks.end(),
+			[&](const std::pair<int, uint64_t>& gpu) { return gpu.first == worker->getGPUID(); } );
+
+		if(iter == gpuChunks.end() )
+			gpuChunks.emplace_back(worker->getGPUID(), workerChunks);
+		else
+			iter->second += workerChunks;
+
+		phaseChunks += workerChunks;
+	}
+
+	for(size_t i = 0; i < gpuChunks.size(); i++)
+	{
+		const uint64_t numChunks = std::min(dataSetChunks, !i ? phaseChunks : gpuChunks[i].second);
+		uint64_t numEntries = 1024;
+
+		while(numEntries < 2 * numChunks)
+			numEntries *= 2;
+
+		gpuChunks[i].second = numEntries;
+	}
+
+	return gpuChunks;
+}
+
 /**
- * --dedupestats: before a write or read phase, one fingerprint table per GPU, cleared. A table
- * has the next power of two at or above twice the chunks that the GPU's workers can move (the
- * first GPU's: all of the phase's chunks, as the others are merged into it), so its load stays at
- * or below 0.5. Fails before any I/O if the tables need more than half of a GPU's free memory.
+ * --dedupestats: before a write or read phase, one fingerprint table per GPU of chunkTableSizes,
+ * cleared. Fails before any I/O if the tables need more than half of a GPU's free memory.
  */
 void Manager::prepareDedupeTables(int benchPhase)
 {
@@ -915,40 +954,13 @@ void Manager::prepareDedupeTables(int benchPhase)
 		dedupeZeroDigestShift = cfg.dedupeChunkShift;
 	}
 
-	/* the GPUs of the workers, the first worker's first, and the chunks their workers can move;
-	   the first GPU takes all of the phase's chunks, as the others are merged into it */
-	const uint64_t dataSetChunks = dedupeDataSetChunks(cfg, shared.customTree);
-	std::vector<std::pair<int, uint64_t> > gpuChunks;
-	uint64_t phaseChunks = 0;
-
-	for(const std::unique_ptr<Worker>& worker : workers)
-	{
-		const uint64_t workerChunks = dedupeWorkerChunkBound(cfg, shared.customTree,
-			worker->getRank() );
-		auto iter = std::find_if(gpuChunks.begin(), gpuChunks.end(),
-			[&](const std::pair<int, uint64_t>& gpu) { return gpu.first == worker->getGPUID(); } );
-
-		if(iter == gpuChunks.end() )
-			gpuChunks.emplace_back(worker->getGPUID(), workerChunks);
-		else
-			iter->second += workerChunks;
-
-		phaseChunks += workerChunks;
-	}
-
 	std::vector<DedupeTable> tables;
 
-	for(size_t i = 0; i < gpuChunks.size(); i++)
+	for(const std::pair<int, uint64_t>& gpuEntries : chunkTableSizes(cfg.dedupeChunkShift) )
 	{
-		const uint64_t numChunks = std::min(dataSetChunks, !i ? phaseChunks : gpuChunks[i].second);
-		uint64_t numEntries = 1024;
-
-		while(numEntries < 2 * numChunks)
-			numEntries *= 2;
-
 		DedupeTable table;
-		table.gpuID = gpuChunks[i].first;
-		table.numEntries = numEntries;
+		table.gpuID = gpuEntries.first;
+		table.numEntries = gpuEntries.second;
 		tables.push_back(table);
 	}
 
@@ -1268,6 +1280,268 @@ void Manager::getCompressStats(elb_compress_counters& out)
 	}
 
 	cudaSetDevice(prevDevice);
+}
+
+void Manager::setReduceStats(unsigned chunkShift)
+{
+	Config& cfg = shared.cfg;
+
+	if(chunkShift && ( (chunkShift < ELB_COMPRESS_MIN_CHUNK_SHIFT) ||
+		(chunkShift > ELB_COMPRESS_MAX_CHUNK_SHIFT) ) )
+		throw WorkerError("The reduce chunk shift (" + std::to_string(chunkShift) + ") is not in "
+			"[" + std::to_string(ELB_COMPRESS_MIN_CHUNK_SHIFT) + ", " +
+			std::to_string(ELB_COMPRESS_MAX_CHUNK_SHIFT) + "].");
+
+	// (a block reduced to the file size is the whole file: its last chunk may be short)
+	if(chunkShift && (cfg.blockSize % (1ULL << chunkShift) ) && (cfg.blockSize != cfg.fileSize) )
+		throw WorkerError("The block size (" + std::to_string(cfg.blockSize) + ") is not a multiple "
+			"of the reduce chunk size (--reducestats) (" + std::to_string(1ULL << chunkShift) +
+			").");
+
+	if(chunkShift && cfg.useRandomOffsets)
+		throw WorkerError("Reduce stats (--reducestats) cannot be used together with random "
+			"offsets (--rand).");
+
+	if(chunkShift && cfg.doInfiniteIOLoop)
+		throw WorkerError("Reduce stats (--reducestats) cannot be used together with an infinite "
+			"I/O loop (--infloop).");
+
+	if(chunkShift && cfg.useRandomUnaligned)
+		throw WorkerError("Reduce stats (--reducestats) cannot be used together with unaligned "
+			"random offsets (--norandalign).");
+
+	if(chunkShift && (cfg.rwMixReadPercent || cfg.numRWMixReadThreads) )
+		throw WorkerError("Reduce stats (--reducestats) cannot be used together with rwmix (a "
+			"phase in both directions).");
+
+	cfg.reduceChunkShift = chunkShift;
+}
+
+/**
+ * --reducestats: before a write or read phase, one reduce table per GPU of chunkTableSizes, its
+ * keys, payloads and counters cleared. Fails before any I/O if the tables need more than half of a
+ * GPU's free memory.
+ */
+void Manager::prepareReduceTables(int benchPhase)
+{
+	const Config& cfg = shared.cfg;
+	const uint64_t entryBytes = 16 + ELB_REDUCE_PAYLOAD_BYTES;
+
+	if(!cfg.reduceChunkShift ||
+		( (benchPhase != ELB_PHASE_CREATEFILES) && (benchPhase != ELB_PHASE_READFILES) ) )
+		return;
+
+	std::vector<ReduceTable> tables;
+
+	for(const std::pair<int, uint64_t>& gpuEntries : chunkTableSizes(cfg.reduceChunkShift) )
+	{
+		ReduceTable table;
+		table.gpuID = gpuEntries.first;
+		table.numEntries = gpuEntries.second;
+		tables.push_back(table);
+	}
+
+	int prevDevice = 0;
+	cudaGetDevice(&prevDevice);
+
+	std::shared_lock<std::shared_timed_mutex> allocLock(shared.gpuAllocMutex);
+	bool replaced = false;
+
+	try
+	{
+		for(ReduceTable& table : tables)
+		{ // all checks first: a failing phase leaves the tables as they were
+			const uint64_t numBytes = table.numEntries * entryBytes + sizeof(elb_reduce_counters);
+			uint64_t heldBytes = 0;
+			size_t freeBytes = 0, totalBytes = 0;
+
+			for(const ReduceTable& oldTable : shared.reduceTables)
+				if(oldTable.gpuID == table.gpuID)
+					heldBytes = oldTable.numEntries * entryBytes + sizeof(elb_reduce_counters);
+
+			checkGpuCall(table.gpuID, cudaSetDevice(table.gpuID), "Setting CUDA device");
+			checkGpuCall(table.gpuID, cudaMemGetInfo(&freeBytes, &totalBytes),
+				"GPU memory query");
+
+			if(numBytes > (freeBytes + heldBytes) / 2)
+				throw WorkerError("Reduce stats (--reducestats) need " + std::to_string(numBytes) +
+					" bytes of GPU memory for the chunk table of GPU " +
+					std::to_string(table.gpuID) + ", more than half of its " +
+					std::to_string(freeBytes + heldBytes) + " free bytes. Use a larger chunk "
+					"size.");
+		}
+
+		// keep the tables of the same size, free the others, then make the missing ones
+		for(ReduceTable& table : tables)
+			for(ReduceTable& oldTable : shared.reduceTables)
+				if( (oldTable.gpuID == table.gpuID) && (oldTable.numEntries == table.numEntries) )
+					std::swap(oldTable, table);
+
+		freeReduceTables();
+		shared.reduceTables = tables;
+		replaced = true;
+
+		for(ReduceTable& table : shared.reduceTables)
+		{
+			checkGpuCall(table.gpuID, cudaSetDevice(table.gpuID), "Setting CUDA device");
+
+			if(!table.entries)
+			{
+				checkGpuCall(table.gpuID, cudaMalloc(&table.counters,
+					sizeof(elb_reduce_counters) ), "GPU reduce counter allocation");
+				checkGpuCall(table.gpuID, cudaMalloc(&table.entries, table.numEntries * entryBytes),
+					"GPU reduce table allocation");
+				table.payloads = (char*)table.entries + table.numEntries * 16;
+			}
+
+			// (on a stream of its own: the legacy default stream would wait for the caller's work)
+			cudaStream_t stream;
+			checkGpuCall(table.gpuID, cudaStreamCreateWithFlags(&stream,
+				cudaStreamNonBlocking), "CUDA stream creation");
+			cudaError_t clearRes = cudaMemsetAsync(table.entries, 0, table.numEntries * entryBytes,
+				stream);
+			if(clearRes == cudaSuccess)
+				clearRes = cudaMemsetAsync(table.counters, 0, sizeof(elb_reduce_counters), stream);
+			if(clearRes == cudaSuccess)
+				clearRes = cudaStreamSynchronize(stream);
+			cudaStreamDestroy(stream);
+			checkGpuCall(table.gpuID, clearRes, "GPU reduce table clear");
+		}
+	}
+	catch(...)
+	{
+		if(replaced)
+			freeReduceTables(); // (a failed allocation: no table is left half made)
+
+		cudaSetDevice(prevDevice);
+		throw;
+	}
+
+	cudaSetDevice(prevDevice);
+}
+
+/* the tables and their counters (the workers must not use them any more) */
+void Manager::freeReduceTables()
+{
+	for(ReduceTable& table : shared.reduceTables)
+	{
+		cudaSetDevice(table.gpuID);
+
+		if(table.entries)
+			cudaFree(table.entries);
+		if(table.counters)
+			cudaFree(table.counters);
+	}
+
+	shared.reduceTables.clear();
+}
+
+void Manager::getReduceStats(elb_reduce_counters& out)
+{
+	out = elb_reduce_counters{};
+
+	if(shared.reduceTables.empty() )
+		return;
+
+	const ReduceTable& first = shared.reduceTables[0];
+	std::vector<elb_reduce_counters> counters(shared.reduceTables.size() );
+	int prevDevice = 0;
+	cudaGetDevice(&prevDevice);
+
+	std::shared_lock<std::shared_timed_mutex> allocLock(shared.gpuAllocMutex);
+
+	cudaStream_t stream = NULL;
+	void* piece = NULL;
+	cudaError_t res = cudaSetDevice(first.gpuID);
+	bool launchFailed = false;
+
+	if(res == cudaSuccess)
+		res = cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking);
+
+	/* the other GPUs' tables, peer to peer in pieces of at most 2^20 keys and their payloads
+	   (24 MiB), merged into the first GPU's; merging twice adds nothing, so this may run again
+	   for the same phase */
+	uint64_t pieceEntries = 0;
+
+	for(size_t i = 1; i < shared.reduceTables.size(); i++)
+		pieceEntries = std::max(pieceEntries,
+			std::min(shared.reduceTables[i].numEntries, (uint64_t)1 << 20) );
+
+	if( (res == cudaSuccess) && pieceEntries)
+		res = cudaMalloc(&piece, pieceEntries * (16 + ELB_REDUCE_PAYLOAD_BYTES) );
+
+	void* piecePayloads = (char*)piece + pieceEntries * 16;
+
+	for(size_t i = 1; (res == cudaSuccess) && !launchFailed && (i < shared.reduceTables.size() );
+		i++)
+	{
+		const ReduceTable& table = shared.reduceTables[i];
+
+		for(uint64_t offset = 0; (res == cudaSuccess) && !launchFailed &&
+			(offset < table.numEntries); offset += pieceEntries)
+		{
+			const uint64_t numEntries = std::min(pieceEntries, table.numEntries - offset);
+
+			// (unified addressing: the copies go peer to peer)
+			res = cudaMemcpyAsync(piece, (char*)table.entries + offset * 16, numEntries * 16,
+				cudaMemcpyDefault, stream);
+			if(res == cudaSuccess)
+				res = cudaMemcpyAsync(piecePayloads, (char*)table.payloads +
+					offset * ELB_REDUCE_PAYLOAD_BYTES, numEntries * ELB_REDUCE_PAYLOAD_BYTES,
+					cudaMemcpyDefault, stream);
+
+			launchFailed = (res == cudaSuccess) && elb_launch_reduce_merge(piece, piecePayloads,
+				numEntries, first.entries, first.payloads, first.numEntries, first.counters,
+				stream);
+		}
+	}
+
+	// D, U and S of the merged table, summed anew each time
+	if( (res == cudaSuccess) && !launchFailed)
+		res = cudaMemsetAsync(&first.counters->numDistinct, 0, 3 * sizeof(uint64_t), stream);
+	if( (res == cudaSuccess) && !launchFailed)
+		launchFailed = elb_launch_reduce_sum(first.entries, first.payloads, first.numEntries,
+			first.counters, stream);
+
+	for(size_t i = 0; (res == cudaSuccess) && !launchFailed &&
+		(i < shared.reduceTables.size() ); i++)
+		res = cudaMemcpyAsync(&counters[i], shared.reduceTables[i].counters,
+			sizeof(elb_reduce_counters), cudaMemcpyDefault, stream);
+
+	const std::string launchError = launchFailed ? elb_last_error() : "";
+
+	if(stream)
+	{
+		const cudaError_t syncRes = cudaStreamSynchronize(stream);
+		res = (res == cudaSuccess) ? syncRes : res;
+	}
+
+	if(piece)
+		cudaFree(piece);
+	if(stream)
+		cudaStreamDestroy(stream);
+
+	cudaSetDevice(prevDevice);
+
+	if(launchFailed)
+		throw WorkerError("GPU reduce merge failed. " + launchError);
+
+	checkGpuCall(first.gpuID, res, "GPU reduce counter read");
+
+	for(size_t i = 0; i < counters.size(); i++)
+	{
+		if(counters[i].overflow)
+			throw WorkerError("Reduce stats (--reducestats): the chunk table of GPU " +
+				std::to_string(shared.reduceTables[i].gpuID) + " ran past its probe bound of " +
+				std::to_string(ELB_DEDUPE_MAX_PROBES) + " entries; the counts are void.");
+
+		out.numChunks += counters[i].numChunks;
+		out.numBytes += counters[i].numBytes;
+	}
+
+	out.numDistinct = counters[0].numDistinct;
+	out.numBytesDistinct = counters[0].numBytesDistinct;
+	out.numBytesStored = counters[0].numBytesStored;
 }
 
 /* Statistics::generatePhaseResults (Statistics.cpp:1641-1764) */
@@ -2138,6 +2412,63 @@ int elb_mgr_compress_stats(elb_mgr* m, uint64_t* outNumChunks, uint64_t* outNumB
 	*outNumBytesIn = counters.numBytesIn;
 	*outNumBytesStored = counters.numBytesStored;
 	*outNumIncompressible = counters.numIncompressible;
+	return 0;
+}
+
+int elb_mgr_set_reduce_stats(elb_mgr* m, unsigned chunkShift)
+{
+	if(!m)
+	{
+		elb_set_last_error("elb_mgr_set_reduce_stats: NULL manager");
+		return -1;
+	}
+
+	try
+	{
+		m->impl->setReduceStats(chunkShift);
+	}
+	catch(std::exception& e)
+	{
+		elb_set_last_error(e.what() );
+		return -1;
+	}
+
+	return 0;
+}
+
+int elb_mgr_reduce_stats(elb_mgr* m, uint64_t* outNumChunks, uint64_t* outNumDistinct,
+	uint64_t* outNumBytes, uint64_t* outNumBytesDistinct, uint64_t* outNumBytesStored)
+{
+	if(!m || !outNumChunks || !outNumDistinct || !outNumBytes || !outNumBytesDistinct ||
+		!outNumBytesStored)
+	{
+		elb_set_last_error("elb_mgr_reduce_stats: NULL argument");
+		return -1;
+	}
+
+	if(!m->impl->shared.cfg.reduceChunkShift)
+	{
+		elb_set_last_error("elb_mgr_reduce_stats: reduce stats are off (elb_mgr_set_reduce_stats)");
+		return -1;
+	}
+
+	elb_reduce_counters counters;
+
+	try
+	{
+		m->impl->getReduceStats(counters);
+	}
+	catch(std::exception& e)
+	{
+		elb_set_last_error(e.what() );
+		return -1;
+	}
+
+	*outNumChunks = counters.numChunks;
+	*outNumDistinct = counters.numDistinct;
+	*outNumBytes = counters.numBytes;
+	*outNumBytesDistinct = counters.numBytesDistinct;
+	*outNumBytesStored = counters.numBytesStored;
 	return 0;
 }
 

@@ -824,11 +824,13 @@ void Worker::preparePhase()
  * and of which algorithm, and the batches' slots. --dedupestats: the table the stages insert into
  * and where the digests come from, the checksum launch's slots when it hashes BLAKE3 at the same
  * chunk size, else the batch's own. --compressstats: the chunk size and counters of the stages'
- * LZ4 launch. Runs after the rings are made and at the start of every write and read phase, since
- * a checksum list (elb_mgr_set_checksum_list) or the LZ4 chunk size (elb_mgr_set_compress_stats)
- * may be set and the manager may make new tables between phases; a change drops the batch graphs,
- * which hold the launches of the old setup. Without these options it allocates and changes
- * nothing.
+ * LZ4 launch. --reducestats: the table the stages insert into, where the digests come from (as
+ * for --dedupestats, or the dedupe launch's own at the same chunk size) and the batches' marks.
+ * Runs after the rings are made and at the start of every write and read phase, since a checksum
+ * list (elb_mgr_set_checksum_list) or the LZ4 or reduce chunk size (elb_mgr_set_compress_stats,
+ * elb_mgr_set_reduce_stats) may be set and the manager may make new tables between phases; a
+ * change drops the batch graphs, which hold the launches of the old setup. Without these options
+ * it allocates and changes nothing.
  */
 void Worker::setupChecksums()
 {
@@ -864,13 +866,34 @@ void Worker::setupChecksums()
 
 	const unsigned lz4ChunkShift = lz4Counters ? cfg.compressChunkShift : 0;
 
+	ReduceTable rTable;
+
+	for(const ReduceTable& gpuTable : shared->reduceTables)
+		if(cfg.reduceChunkShift && (gpuTable.gpuID == gpuID) )
+			rTable = gpuTable;
+
+	const bool reduce = (rTable.entries != NULL);
+	const bool reduceUsesSums = reduce && (cfg.checksumAlgo == ELB_CHECKSUM_BLAKE3) &&
+		(chunkShift == cfg.reduceChunkShift);
+	const bool reduceUsesDedupe = reduce && dedupe &&
+		(cfg.dedupeChunkShift == cfg.reduceChunkShift);
+	const bool reduceNeedsOwnSums = reduce && !(reduceUsesSums && cfg.checksums) &&
+		!reduceUsesDedupe;
+	const uint64_t reduceSlots = !reduce ? 1 : std::max( (cfg.blockSize +
+		( (uint64_t)1 << cfg.reduceChunkShift) - 1) >> cfg.reduceChunkShift, (uint64_t)1);
+
 	if(batches.empty() || ( (readChecksum == readStage.checksum) &&
 		(chunkShift == checksumChunkShift) && (slotsPerDesc == checksumSlotsPerDesc) &&
 		(cfg.checksumAlgo == checksumAlgo) && (dedupe == readStage.dedupe) &&
 		(table.entries == dedupeTable.entries) && (table.numEntries == dedupeTable.numEntries) &&
 		(table.counters == dedupeTable.counters) && (dedupeSlots == dedupeSlotsPerDesc) &&
 		( (dedupeUsesSums && readChecksum) == dedupeUsesReadSums) &&
-		(lz4ChunkShift == compressChunkShift) && (lz4Counters == compressCounters) ) )
+		(lz4ChunkShift == compressChunkShift) && (lz4Counters == compressCounters) &&
+		(reduce == readStage.reduce) && (rTable.entries == reduceTable.entries) &&
+		(rTable.numEntries == reduceTable.numEntries) &&
+		(rTable.counters == reduceTable.counters) && (reduceSlots == reduceSlotsPerDesc) &&
+		( (reduceUsesSums && readChecksum) == reduceUsesReadSums) &&
+		(reduceUsesDedupe == reduceUsesDedupeSums) ) )
 		return;
 
 	std::shared_lock<std::shared_timed_mutex> allocLock(shared->gpuAllocMutex);
@@ -883,10 +906,19 @@ void Worker::setupChecksums()
 	writeStage.compress = (lz4ChunkShift != 0);
 	readStage.compress = (lz4ChunkShift != 0);
 	verifyBackStage.compress = false;
-	/* --verifydirect: a write phase's checksums, dedupe and compress counts are those of the
-	   written bytes, so the read-back takes none, and must not share the read phase's batch graphs
-	   then */
-	verifyBackStage.useGraph = readStage.useGraph && !readChecksum && !dedupe && !lz4ChunkShift;
+	writeStage.reduce = reduce;
+	readStage.reduce = reduce;
+	verifyBackStage.reduce = false;
+	/* --verifydirect: a write phase's checksums, dedupe, compress and reduce counts are those of
+	   the written bytes, so the read-back takes none, and must not share the read phase's batch
+	   graphs then */
+	verifyBackStage.useGraph = readStage.useGraph && !readChecksum && !dedupe && !lz4ChunkShift &&
+		!reduce;
+	reduceTable = rTable;
+	reduceSlotsPerDesc = reduceSlots;
+	reduceUsesWriteSums = reduceUsesSums && cfg.checksums;
+	reduceUsesReadSums = reduceUsesSums && readChecksum;
+	reduceUsesDedupeSums = reduceUsesDedupe;
 	compressChunkShift = lz4ChunkShift;
 	compressCounters = lz4Counters;
 	compressSlotsPerDesc = !lz4ChunkShift ? 1 : std::max( (cfg.blockSize +
@@ -912,16 +944,30 @@ void Worker::setupChecksums()
 			cudaFreeHost(batch.hostSums);
 		if(batch.devDedupeSums)
 			cudaFree(batch.devDedupeSums);
+		if(batch.devReduceSums)
+			cudaFree(batch.devReduceSums);
+		if(batch.devReduceMarks)
+			cudaFree(batch.devReduceMarks);
 
 		batch.readGraphExec = NULL;
 		batch.writeGraphExec = NULL;
 		batch.devSums = NULL;
 		batch.hostSums = NULL;
 		batch.devDedupeSums = NULL;
+		batch.devReduceSums = NULL;
+		batch.devReduceMarks = NULL;
 
 		if(dedupeNeedsOwnSums)
 			ELB_CUDA_CHECK(cudaMalloc(&batch.devDedupeSums, elb_checksum_value_bytes(
 				ELB_CHECKSUM_BLAKE3) * batchBlocks * dedupeSlots), "GPU dedupe digest allocation");
+
+		if(reduceNeedsOwnSums)
+			ELB_CUDA_CHECK(cudaMalloc(&batch.devReduceSums, elb_checksum_value_bytes(
+				ELB_CHECKSUM_BLAKE3) * batchBlocks * reduceSlots), "GPU reduce digest allocation");
+
+		if(reduce)
+			ELB_CUDA_CHECK(cudaMalloc( (void**)&batch.devReduceMarks, sizeof(uint64_t) *
+				batchBlocks * reduceSlots), "GPU reduce mark allocation");
 
 		if(!readChecksum)
 			continue;
@@ -1199,6 +1245,10 @@ void Worker::freeRings() // LocalWorker::cleanup (:1570-1641)
 			cudaFree(batch.devSums);
 		if(batch.devDedupeSums)
 			cudaFree(batch.devDedupeSums);
+		if(batch.devReduceSums)
+			cudaFree(batch.devReduceSums);
+		if(batch.devReduceMarks)
+			cudaFree(batch.devReduceMarks);
 		if(batch.hostSums)
 			cudaFreeHost(batch.hostSums);
 	}
@@ -1944,6 +1994,7 @@ void Worker::rwPhase()
 	}
 
 	checkDedupeOverflow();
+	checkReduceOverflow();
 }
 
 /**
@@ -2504,6 +2555,9 @@ void Worker::enqueueStage(Batch& batch, const GpuStage& stage, uint32_t numBlock
 		compressSlotsPerDesc, compressCounters, NULL, NULL, batch.stream) )
 		throw WorkerError(std::string("GPU compress stats failed. ") + elb_last_error() );
 
+	if(stage.reduce)
+		enqueueReduce(batch, stage, numBlocks);
+
 	if( (stage.transfer == GpuStage::TRANSFER_COPY) && !stage.isRead)
 		enqueueStageCopies(batch, false, true);
 }
@@ -2549,6 +2603,54 @@ void Worker::checkDedupeOverflow()
 			"the counts are void.");
 }
 
+/* --reducestats: the digests of the batch's chunks (those of the checksum launch when it hashes
+ * BLAKE3 at the same chunk size, else those of the dedupe launch at the same chunk size, else an
+ * own BLAKE3 launch into device-only slots) into the reduce table of this worker's GPU, then the
+ * LZ4 launch over the chunks whose keys took a new entry. Nothing is copied or waited for: the
+ * table is read at the end of the phase. */
+void Worker::enqueueReduce(Batch& batch, const GpuStage& stage, uint32_t numBlocks)
+{
+	const bool usesSums = stage.checksum &&
+		(stage.isRead ? reduceUsesReadSums : reduceUsesWriteSums);
+	const bool usesDedupeSums = !usesSums && stage.dedupe && reduceUsesDedupeSums;
+	void* digests = usesSums ? batch.devSums :
+		usesDedupeSums ? batch.devDedupeSums : batch.devReduceSums;
+	const uint64_t slotsPerDesc = usesSums ? checksumSlotsPerDesc : reduceSlotsPerDesc;
+
+	if(!usesSums && !usesDedupeSums && elb_launch_blake3(batch.hostDescs, NULL, numBlocks,
+		cfg.reduceChunkShift, slotsPerDesc, digests, NULL, batch.stream) )
+		throw WorkerError(std::string("GPU reduce digests failed. ") + elb_last_error() );
+
+	if(elb_launch_reduce_insert(batch.hostDescs, numBlocks, cfg.reduceChunkShift, slotsPerDesc,
+		digests, reduceTable.entries, reduceTable.numEntries, reduceTable.counters,
+		batch.devReduceMarks, batch.stream) )
+		throw WorkerError(std::string("GPU reduce insert failed. ") + elb_last_error() );
+
+	if(elb_launch_reduce_lz4(batch.hostDescs, numBlocks, cfg.reduceChunkShift, slotsPerDesc,
+		batch.devReduceMarks, reduceTable.payloads, batch.stream) )
+		throw WorkerError(std::string("GPU reduce compression failed. ") + elb_last_error() );
+}
+
+/* --reducestats: the phase fails if the table of this worker's GPU ran past its probe bound (a
+ * guard: a table is sized for a load of at most 0.5) */
+void Worker::checkReduceOverflow()
+{
+	if(!readStage.reduce || batches.empty() )
+		return;
+
+	uint32_t overflow = 0;
+
+	ELB_CUDA_CHECK(cudaMemcpyAsync(&overflow, &reduceTable.counters->overflow, sizeof(overflow),
+		cudaMemcpyDeviceToHost, batches[0].stream), "GPU reduce counter read");
+	ELB_CUDA_CHECK(cudaStreamSynchronize(batches[0].stream), "GPU reduce counter read");
+
+	if(overflow)
+		throw WorkerError("Reduce stats (--reducestats): the chunk table of GPU " +
+			std::to_string(gpuID) + " (" + std::to_string(reduceTable.numEntries) + " entries) "
+			"ran past its probe bound of " + std::to_string(ELB_DEDUPE_MAX_PROBES) + " entries; "
+			"the counts are void.");
+}
+
 /**
  * GPU stage of a batch, write (fill + stage-out, LocalWorker.cpp:1249-1265) or read (stage-in +
  * verify, :1311-1319; the reference verifies on the CPU), between the batch's stage events. A
@@ -2590,6 +2692,10 @@ void Worker::gpuLaunchStage(Batch& batch, bool isRead)
 			(stage.isRead ? dedupeUsesReadSums : dedupeUsesWriteSums) ) ? 1 : 2;
 	if(numBlocks && stage.compress)
 		numKernelLaunches++;
+	if(numBlocks && stage.reduce) // (insert and LZ4, and the BLAKE3 launch unless it shares one)
+		numKernelLaunches += ( (stage.checksum &&
+			(stage.isRead ? reduceUsesReadSums : reduceUsesWriteSums) ) ||
+			(stage.dedupe && reduceUsesDedupeSums) ) ? 2 : 3;
 
 	if(stage.transfer != GpuStage::TRANSFER_NONE)
 		(isRead ? numH2DBytes : numD2HBytes) += numBytes;

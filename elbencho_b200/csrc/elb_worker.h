@@ -62,6 +62,18 @@ struct DedupeTable
 	elb_dedupe_counters* counters{NULL};
 };
 
+/* --reducestats: the reduce table of one GPU (elb_reduce_insert): the keys as in DedupeTable, the
+ * payloads after them in the same allocation, and its counters; made and cleared by the manager at
+ * the start of every write and read phase, shared by the GPU's workers */
+struct ReduceTable
+{
+	int gpuID{-1};
+	void* entries{NULL};    // numEntries keys of 16 bytes, then numEntries payloads of 8 bytes
+	void* payloads{NULL};   // (entries + 16 * numEntries)
+	uint64_t numEntries{0}; // a power of two
+	elb_reduce_counters* counters{NULL};
+};
+
 /* --compressstats: the LZ4 counters of one GPU (elb_lz4_chunks), made by the manager when first
  * needed and cleared at the start of every write and read phase, shared by the GPU's workers */
 struct CompressCounters
@@ -96,6 +108,7 @@ struct Shared
 	std::vector<DedupeTable> dedupeTables; // --dedupestats: one per GPU, the first worker's first
 	uint8_t dedupeZeroDigest[32]{};        // --dedupestats: the BLAKE3 of a chunk of zero bytes
 	std::vector<CompressCounters> compressCounters; // --compressstats: one per GPU
+	std::vector<ReduceTable> reduceTables; // --reducestats: one per GPU, the first worker's first
 
 	/* workers hold this shared while they allocate / free device memory or instantiate graphs;
 	   the live stats reducer holds it exclusively while its collective is in flight, because a
@@ -273,6 +286,8 @@ struct GpuStage
 	bool checksum;    // --checksums, a checksum list: the checksum launch over the device slots
 	bool dedupe;      // --dedupestats: the chunks' digests go into the GPU's fingerprint table
 	bool compress;    // --compressstats: the LZ4 launch over the chunks, into the GPU's counters
+	bool reduce;      // --reducestats: the chunks' digests into the GPU's reduce table, the new
+	                  // ones compressed
 };
 
 /* a batch: a contiguous slice of the rings plus everything its GPU stage needs */
@@ -306,6 +321,10 @@ struct Batch
 	/* --dedupestats without a BLAKE3 checksum launch of its chunk size: the chunks' digests, 32
 	   bytes per slot (device only) */
 	void* devDedupeSums{NULL};
+	/* --reducestats: the chunks' digests when no other launch hashes BLAKE3 at its chunk size,
+	   and every slot's mark (elb_reduce_insert), 8 bytes per slot (device only) */
+	void* devReduceSums{NULL};
+	uint64_t* devReduceMarks{NULL};
 
 	// aio state
 	std::vector<struct iocb> iocbs;
@@ -508,6 +527,14 @@ class Worker
 		unsigned compressChunkShift{0};
 		elb_compress_counters* compressCounters{NULL};
 		uint64_t compressSlotsPerDesc{1};
+		/* --reducestats: the table of this worker's GPU, the slots of the digests and marks of its
+		   launches, whether a stage's checksum launch writes the digests (BLAKE3 at the same chunk
+		   size), else whether the dedupe launch's own digests are those (the same chunk size) */
+		ReduceTable reduceTable;
+		uint64_t reduceSlotsPerDesc{1};
+		bool reduceUsesWriteSums{false};
+		bool reduceUsesReadSums{false};
+		bool reduceUsesDedupeSums{false};
 
 		// accounting
 		std::atomic<uint64_t> numH2DBytes{0};
@@ -553,6 +580,8 @@ class Worker
 		void setupChecksums();
 		void enqueueDedupeInsert(Batch& batch, const GpuStage& stage, uint32_t numBlocks);
 		void checkDedupeOverflow();
+		void enqueueReduce(Batch& batch, const GpuStage& stage, uint32_t numBlocks);
+		void checkReduceOverflow();
 		FileID blockFileID(const BlockRef& block) const;
 		uint64_t blockFileSize(const BlockRef& block) const;
 		void gpuLaunchStage(Batch& batch, bool isRead);
@@ -661,6 +690,15 @@ class Manager
 		/* --compressstats: the counters of the last write or read phase, summed over all GPUs */
 		void getCompressStats(elb_compress_counters& out);
 
+		/* --reducestats: from the next write or read phase on, the reduce counts of chunks of
+		   2^chunkShift bytes (0: off); throws WorkerError for a shift outside 12..20 or a config
+		   it cannot be used with */
+		void setReduceStats(unsigned chunkShift);
+		/* --reducestats: N, B, D, U and S of the last write or read phase over all GPUs (merges the
+		   other GPUs' tables into the first's; throws WorkerError if a table ran past its probe
+		   bound) */
+		void getReduceStats(elb_reduce_counters& out);
+
 		Shared shared;
 		std::vector<std::unique_ptr<Worker> > workers;
 		std::vector<std::thread> threads;
@@ -680,6 +718,9 @@ class Manager
 		void freeDedupeTables();
 		void prepareCompressCounters(int benchPhase);
 		void freeCompressCounters();
+		std::vector<std::pair<int, uint64_t> > chunkTableSizes(unsigned chunkShift);
+		void prepareReduceTables(int benchPhase);
+		void freeReduceTables();
 		std::unique_ptr<LiveStatsReducer> liveStatsReducer; // created on first use
 		std::mutex liveStatsReducerMutex;
 };

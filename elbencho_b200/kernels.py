@@ -506,3 +506,72 @@ def compress_line(chunk_size, chunks, bytes_in, bytes_stored, incompressible):
     if lib.elb_format_compress_line(chunk_size, counters, buf, len(buf)) < 0:
         raise KernelError("elb_format_compress_line failed: %s" % _native.last_error())
     return buf.value.decode()
+
+
+# ---- --reducestats: each distinct chunk stored once, compressed ----
+
+REDUCE_PAYLOAD_BYTES = 8    # a payload entry: u32 length, u32 min(LZ4 size, length)
+REDUCE_COUNTERS_BYTES = 48  # elb_reduce_counters: chunks, bytes, distinct, distinct bytes, stored
+                            # (u64), overflow (u32)
+REDUCE_NOT_NEW = (1 << 64) - 1  # the mark of a slot that took no entry
+
+
+def reduce_insert(pinned_descs_ptr, num_descs, chunk_shift, slots_per_desc, dev_digests_ptr,
+                  dev_table_ptr, table_entries, dev_counters_ptr, dev_marks_ptr, stream=0):
+    """Insert the chunk digests of blake3_chunks (the same descriptors and slots, chunk_shift
+    12..20) into a table of table_entries (a power of two) 16-byte entries, zero when empty, as
+    dedupe_insert does; add the chunks and their bytes to the 48-byte counters and set their
+    overflow flag past the probe bound. The uint64 at dev_marks_ptr + 8 * slot gets the entry the
+    slot's key newly took, else REDUCE_NOT_NEW."""
+    _check(_native.load().elb_reduce_insert(pinned_descs_ptr or None, num_descs, chunk_shift,
+                                            slots_per_desc, dev_digests_ptr or None,
+                                            dev_table_ptr or None, table_entries,
+                                            dev_counters_ptr or None, dev_marks_ptr or None,
+                                            stream),
+           "elb_reduce_insert")
+
+
+def reduce_lz4(pinned_descs_ptr, num_descs, chunk_shift, slots_per_desc, dev_marks_ptr,
+               dev_payloads_ptr, stream=0):
+    """Compress each chunk whose mark (reduce_insert) is an entry e by the parse of lz4_chunks and
+    write (length, min(size, length)) as two uint32 to dev_payloads_ptr + 8 * e."""
+    _check(_native.load().elb_reduce_lz4(pinned_descs_ptr or None, num_descs, chunk_shift,
+                                         slots_per_desc, dev_marks_ptr or None,
+                                         dev_payloads_ptr or None, stream),
+           "elb_reduce_lz4")
+
+
+def reduce_merge(dev_src_entries_ptr, dev_src_payloads_ptr, num_src_entries, dev_table_ptr,
+                 dev_payloads_ptr, table_entries, dev_counters_ptr, stream=0):
+    """Insert the non-empty entries of another table into the table; a key that takes a new entry
+    brings its payload."""
+    _check(_native.load().elb_reduce_merge(dev_src_entries_ptr or None,
+                                           dev_src_payloads_ptr or None, num_src_entries,
+                                           dev_table_ptr or None, dev_payloads_ptr or None,
+                                           table_entries, dev_counters_ptr or None, stream),
+           "elb_reduce_merge")
+
+
+def reduce_sum(dev_table_ptr, dev_payloads_ptr, table_entries, dev_counters_ptr, stream=0):
+    """Add the table's keys, their lengths and stored sizes to the counters' distinct, distinct
+    bytes and stored fields."""
+    _check(_native.load().elb_reduce_sum(dev_table_ptr or None, dev_payloads_ptr or None,
+                                         table_entries, dev_counters_ptr or None, stream),
+           "elb_reduce_sum")
+
+
+def reduce_counters(raw):
+    """(chunks, bytes, distinct, distinct bytes, stored, overflow) from the 48 bytes of
+    elb_reduce_counters"""
+    import struct
+    return struct.unpack("<QQQQQI4x", bytes(raw))
+
+
+def reduce_line(chunk_size, chunks, distinct, bytes_in, distinct_bytes, stored):
+    """the console line of --reducestats for these counts"""
+    counters = (ctypes.c_uint64 * 6)(chunks, bytes_in, distinct, distinct_bytes, stored, 0)
+    buf = ctypes.create_string_buffer(384)
+    lib = _native.load()
+    if lib.elb_format_reduce_line(chunk_size, counters, buf, len(buf)) < 0:
+        raise KernelError("elb_format_reduce_line failed: %s" % _native.last_error())
+    return buf.value.decode()

@@ -119,6 +119,7 @@ class WorkerConfig:
     checksum_algo: str = "crc32"      # --checksumalgo: "crc32", "crc32c", "crc64nvme" or "blake3"
     dedupe_chunk: int = 0             # --dedupestats bytes (a power of two 4K..1G; 0 = off)
     compress_chunk: int = 0           # --compressstats bytes (a power of two 4K..1M; 0 = off)
+    reduce_chunk: int = 0             # --reducestats bytes (a power of two 4K..1M; 0 = off)
     serialize_buffered_writes: int = 0  # 0 auto, 1 on, 2 off (--writegate)
     staging_engine: int = 0           # 0 auto, 1 kernels move the data, 2 cudaMemcpyAsync
     no_gpu_numa_binding: bool = False  # --nogpunuma
@@ -298,6 +299,13 @@ class WorkerManager:
                 err = _native.last_error()
                 self.close()
                 raise WorkerError(err)
+        chunk = config.reduce_chunk
+        if chunk:
+            shift = chunk.bit_length() - 1 if not chunk & (chunk - 1) else 0xffffffff
+            if self._lib.elb_mgr_set_reduce_stats(self._h, shift) != 0:
+                err = _native.last_error()
+                self.close()
+                raise WorkerError(err)
 
     def close(self):
         if self._h:
@@ -462,6 +470,15 @@ class WorkerManager:
         read phase, over all workers and GPUs; the ratio is bytes / bytes stored."""
         vals = [ctypes.c_uint64(0) for _ in range(4)]
         if self._lib.elb_mgr_compress_stats(self._h, *[ctypes.byref(v) for v in vals]) != 0:
+            raise WorkerError(_native.last_error())
+        return tuple(v.value for v in vals)
+
+    def reduce_stats(self):
+        """--reducestats: (chunks N, distinct chunks D, bytes B, distinct bytes U, stored bytes S)
+        of the last write or read phase, over all workers and GPUs; the dedupe ratio is B / U, the
+        compress ratio U / S and the total B / S."""
+        vals = [ctypes.c_uint64(0) for _ in range(5)]
+        if self._lib.elb_mgr_reduce_stats(self._h, *[ctypes.byref(v) for v in vals]) != 0:
             raise WorkerError(_native.last_error())
         return tuple(v.value for v in vals)
 

@@ -419,6 +419,55 @@ int elb_lz4_chunks(const elb_block_desc* descs, uint32_t numDescs, unsigned chun
 	uint64_t slotsPerDesc, elb_compress_counters* devCounters, uint32_t* devSizes, void* devOut,
 	void* stream);
 
+/* --reducestats: the counters of one GPU's reduce table (device memory, zero at the start) */
+typedef struct elb_reduce_counters
+{
+	uint64_t numChunks;        /* chunks inserted (N) */
+	uint64_t numBytes;         /* the sum of their lengths (B) */
+	uint64_t numDistinct;      /* elb_reduce_sum: the table's keys (D) */
+	uint64_t numBytesDistinct; /* elb_reduce_sum: the sum of their chunks' lengths (U) */
+	uint64_t numBytesStored;   /* elb_reduce_sum: the sum of min(LZ4 size, length) of them (S) */
+	uint32_t overflow;         /* nonzero: a probe sequence ran past its bound, the counts are void */
+	uint32_t reserved;
+} elb_reduce_counters;
+
+/* --reducestats: a reduce table is a fingerprint table of elb_dedupe_insert's layout (tableEntries
+ * 16-byte keys, a power of two, all 0 when empty) with a parallel array of tableEntries payloads of
+ * ELB_REDUCE_PAYLOAD_BYTES: entry e's {uint32 length, uint32 min(LZ4 size, length)} at payloads +
+ * 8 * e. The mark of a slot (uint64) is the entry its key newly took, or ELB_REDUCE_NOT_NEW. */
+#define ELB_REDUCE_PAYLOAD_BYTES 8
+#define ELB_REDUCE_NOT_NEW 0xffffffffffffffffULL
+/* --reducestats: insert the chunk digests of elb_blake3_chunks (chunkShift 12..20, the same
+ * descriptors and slots) into the keys of a reduce table as elb_dedupe_insert does, and write the
+ * mark of every chunk's slot to devMarks[i * slotsPerDesc + j]. Adds every chunk to numChunks and
+ * its length to numBytes of devCounters; a probe sequence longer than 4096 entries (or the table)
+ * sets overflow and marks the chunk not new. descs must be pinned host memory. Fails without
+ * launching for a table size that is not a power of two, NULL pointers, a chunkShift outside
+ * 12..20, a descriptor off a chunk boundary or one with more chunks than slotsPerDesc. */
+int elb_reduce_insert(const elb_block_desc* descs, uint32_t numDescs, unsigned chunkShift,
+	uint64_t slotsPerDesc, const void* devDigests, void* table, uint64_t tableEntries,
+	elb_reduce_counters* devCounters, uint64_t* devMarks, void* stream);
+/* --reducestats: compress every chunk whose mark in devMarks (elb_reduce_insert, the same
+ * descriptors and slots) is an entry e into one LZ4 block by the parse of elb_lz4_chunks, and write
+ * {length, min(block size, length)} to payload e at devPayloads. A chunk marked not new is not
+ * compressed. Fails without launching for NULL pointers, a chunkShift outside 12..20, a descriptor
+ * off a chunk boundary or one with more chunks than slotsPerDesc. */
+int elb_reduce_lz4(const elb_block_desc* descs, uint32_t numDescs, unsigned chunkShift,
+	uint64_t slotsPerDesc, const uint64_t* devMarks, void* devPayloads, void* stream);
+/* --reducestats: insert the non-empty keys of numSrcEntries entries at srcEntries, with their
+ * payloads at srcPayloads (device memory of the table's device, e.g. peer copies of another GPU's
+ * table), into the reduce table; a key that takes a new entry brings its payload. Sets overflow as
+ * elb_reduce_insert does. Fails without launching for a table size that is not a power of two or
+ * NULL pointers. */
+int elb_reduce_merge(const void* srcEntries, const void* srcPayloads, uint64_t numSrcEntries,
+	void* table, void* payloads, uint64_t tableEntries, elb_reduce_counters* devCounters,
+	void* stream);
+/* --reducestats: add the keys of a reduce table to devCounters->numDistinct, the lengths of their
+ * payloads to numBytesDistinct and their stored sizes to numBytesStored. Fails without launching
+ * for a table size that is not a power of two or NULL pointers. */
+int elb_reduce_sum(const void* table, const void* payloads, uint64_t tableEntries,
+	elb_reduce_counters* devCounters, void* stream);
+
 int elb_stage_copy(const elb_block_desc* descs, uint32_t numDescs, int hostToDevice,
 	int64_t hostDelta, uint64_t totalBytes, uint64_t maxBlockLen, void* stream);
 /* devResults[0..numDescs) <- {0, ~0} */
@@ -757,6 +806,12 @@ int64_t elb_format_value(int kind, uint64_t value, double percentage, const elb_
  * 1.00 when S is 0). Returns the text length (text truncated to outBufLen - 1), -1 on error. */
 int64_t elb_format_compress_line(uint64_t chunkSize, const elb_compress_counters* counters,
 	char* outBuf, uint64_t outBufLen);
+/* --reducestats: the console line of a phase's counters for chunks of chunkSize bytes, "Reduce: <N>
+ * chunks of <K>, <D> distinct: <B> bytes, <U> distinct bytes stored as <S>: dedupe <B/U>:1,
+ * compress <U/S>:1, total <B/S>:1" (each ratio with two decimals, 1.00 when its denominator is 0).
+ * Returns the text length (text truncated to outBufLen - 1), -1 on error. */
+int64_t elb_format_reduce_line(uint64_t chunkSize, const elb_reduce_counters* counters,
+	char* outBuf, uint64_t outBufLen);
 /* UnitTk::numHumanToBytesBinary (toolkits/UnitTk.cpp:18-76): "4k", "1M", "64G"; 0 ok, -1 error */
 int elb_num_human_to_bytes(const char* numHuman, uint64_t* outBytes);
 
@@ -928,6 +983,20 @@ int elb_mgr_set_compress_stats(elb_mgr* m, unsigned chunkShift);
  * --compressstats is off (elb_last_error), else 0. */
 int elb_mgr_compress_stats(elb_mgr* m, uint64_t* outNumChunks, uint64_t* outNumBytesIn,
 	uint64_t* outNumBytesStored, uint64_t* outNumIncompressible);
+/* --reducestats: from the next write or read phase on, put every chunk of 2^chunkShift file bytes
+ * (12..20) that a phase moves into a reduce table per GPU (elb_reduce_insert) and compress each
+ * distinct one once (elb_reduce_lz4); 0 turns it off. Returns -1 (elb_last_error) for another
+ * chunkShift, or if the config has a block size that is not a multiple of the chunk size (after a
+ * block larger than the file is reduced to the file size), random or unaligned random offsets, an
+ * infinite loop or rwmix. */
+int elb_mgr_set_reduce_stats(elb_mgr* m, unsigned chunkShift);
+/* --reducestats: of the last write or read phase, the chunks it moved (N), the distinct ones (D),
+ * the bytes of all (B), the bytes of the distinct ones each counted once (U) and the sum of their
+ * min(LZ4 block size, length) (S), over all workers and GPUs of the manager (merges the other GPUs'
+ * tables into the first's). All 0 before the first such phase. Returns -1 if --reducestats is off
+ * or a table ran past its probe bound (elb_last_error), else 0. */
+int elb_mgr_reduce_stats(elb_mgr* m, uint64_t* outNumChunks, uint64_t* outNumDistinct,
+	uint64_t* outNumBytes, uint64_t* outNumBytesDistinct, uint64_t* outNumBytesStored);
 
 uint32_t elb_mgr_num_workers(elb_mgr* m);
 elb_worker* elb_mgr_worker(elb_mgr* m, uint32_t localIdx);
