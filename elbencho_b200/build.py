@@ -20,6 +20,7 @@ SOURCES = [
     "elb_dedupe.cu",
     "elb_compress.cu",
     "elb_reduce.cu",
+    "elb_cdc.cu",
     "elb_config.cpp",
     "elb_cufile.cpp",
     "elb_worker.cpp",

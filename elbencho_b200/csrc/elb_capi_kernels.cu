@@ -846,6 +846,71 @@ int elb_reduce_sum(const void* table, const void* payloads, uint64_t tableEntrie
 	return 0;
 }
 
+/* the mean chunk size check of elb_cdc_cut and _hash_insert */
+static bool cdcAvgShiftValid(const char* what, unsigned avgShift)
+{
+	if( (avgShift < ELB_CDC_MIN_AVG_SHIFT) || (avgShift > ELB_CDC_MAX_AVG_SHIFT) )
+	{
+		elb_set_last_error(std::string(what) + ": mean chunk shift " + std::to_string(avgShift) +
+			" is not in [" + std::to_string(ELB_CDC_MIN_AVG_SHIFT) + ", " +
+			std::to_string(ELB_CDC_MAX_AVG_SHIFT) + "]");
+		return false;
+	}
+
+	return true;
+}
+
+int elb_cdc_cut(const elb_block_desc* descs, uint32_t numDescs, unsigned avgShift,
+	uint64_t slotsPerDesc, uint32_t* devCounts, uint64_t* devEnds, void* stream)
+{
+	const char* what = "elb_cdc_cut";
+
+	if(!cdcAvgShiftValid(what, avgShift) )
+		return -1;
+
+	if(numDescs && (!descs || !devCounts || !devEnds) )
+	{
+		elb_set_last_error(std::string(what) + ": NULL descriptor, count or end array");
+		return -1;
+	}
+
+	if(elb_launch_cdc_cut(descs, numDescs, avgShift, slotsPerDesc, devCounts, devEnds,
+		(cudaStream_t)stream) )
+	{
+		elb_set_last_error(std::string("elb_") + elb_last_error() );
+		return -1;
+	}
+
+	return 0;
+}
+
+int elb_cdc_hash_insert(const elb_block_desc* descs, uint32_t numDescs, unsigned avgShift,
+	uint64_t slotsPerDesc, const uint32_t* devCounts, const uint64_t* devEnds, void* devDigests,
+	void* table, void* payloads, uint64_t tableEntries, elb_reduce_counters* devCounters,
+	void* stream)
+{
+	const char* what = "elb_cdc_hash_insert";
+
+	if(!reduceTableArgsValid(what, table, tableEntries, devCounters) ||
+		!cdcAvgShiftValid(what, avgShift) )
+		return -1;
+
+	if(!payloads || (numDescs && (!descs || !devCounts || !devEnds) ) )
+	{
+		elb_set_last_error(std::string(what) + ": NULL payloads, descriptor, count or end array");
+		return -1;
+	}
+
+	if(elb_launch_cdc_hash_insert(descs, numDescs, avgShift, slotsPerDesc, devCounts, devEnds,
+		devDigests, table, payloads, tableEntries, devCounters, (cudaStream_t)stream) )
+	{
+		elb_set_last_error(std::string("elb_") + elb_last_error() );
+		return -1;
+	}
+
+	return 0;
+}
+
 int elb_stage_copy(const elb_block_desc* descs, uint32_t numDescs, int hostToDevice,
 	int64_t hostDelta, uint64_t totalBytes, uint64_t maxBlockLen, void* stream)
 {

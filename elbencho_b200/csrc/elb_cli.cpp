@@ -173,6 +173,16 @@ static const OptDef optDefs[] =
 		"S stores it as min(LZ4 size, length): what storage that deduplicates and compresses "
 		"would keep. A file's short last chunk is a chunk of its own length. Cannot be used with "
 		"--rand, --norandalign, --infloop, --rwmixpct, --rwmixthr or --hosts. [b200]"},
+	{"cdcstats", 0, Opt_BYTES, &ProgArgs::cdcStatsAvgSize, Wire_NONE, "Mean chunk size of "
+		"content-defined chunking statistics: every write and read phase cuts each block it moved "
+		"into chunks of MIN = AVG/4 to MAX = 4*AVG bytes where a rolling gear hash of the last 64 "
+		"bytes chooses the cut, as deduplicating backup tools do (AVG a power of two from 4K to "
+		"256K), finds the distinct chunks by BLAKE3 digest, all on the GPU, and prints \"CDC: <N> "
+		"chunks of <MIN> to <MAX> bytes, mean <B/N>, <D> distinct: <B> bytes, <U> distinct bytes: "
+		"<B/U>:1\", where U counts each distinct chunk once. Unlike --dedupestats, it finds "
+		"duplicates at any offset. Each block is chunked on its own from its first byte. The block "
+		"size must be at least MAX. Cannot be used with --rand, --norandalign, --infloop, "
+		"--rwmixpct, --rwmixthr or --hosts. [b200]"},
 	{"rwmixpct", 0, Opt_U64, &ProgArgs::rwMixReadPercent, Wire_REF, "Percentage of blocks that "
 		"should be read in a write phase."},
 	{"rwmixthr", 0, Opt_U64, &ProgArgs::numRWMixReadThreads, Wire_REF, "Number of threads that "
@@ -1152,6 +1162,40 @@ void ProgArgs::checkArgs()
 
 		if(!hosts.empty() )
 			throw ProgError("Option \"--reducestats\" cannot be used together with \"--hosts\"");
+	}
+
+	if(cdcStatsAvgSize)
+	{
+		if( (cdcStatsAvgSize < (1ULL << ELB_CDC_MIN_AVG_SHIFT) ) ||
+			(cdcStatsAvgSize > (1ULL << ELB_CDC_MAX_AVG_SHIFT) ) ||
+			(cdcStatsAvgSize & (cdcStatsAvgSize - 1) ) )
+			throw ProgError("Option \"--cdcstats\" must be a power of two from 4K to 256K");
+
+		// (as the manager: a block reduced to the file size is the whole file)
+		const uint64_t fileBlockSize = (fileSize && (blockSize > fileSize) ) ? fileSize : blockSize;
+
+		if(fileBlockSize < 4 * cdcStatsAvgSize)
+			throw ProgError("The block size (" + std::to_string(fileBlockSize) + ") must be at "
+				"least the largest chunk of \"--cdcstats\" (" +
+				std::to_string(4 * cdcStatsAvgSize) + ")");
+
+		if(useRandomUnaligned)
+			throw ProgError("Option \"--cdcstats\" cannot be used together with \"--norandalign\"");
+
+		if(useRandomOffsets)
+			throw ProgError("Option \"--cdcstats\" cannot be used together with \"--rand\"");
+
+		if(doInfiniteIOLoop)
+			throw ProgError("Option \"--cdcstats\" cannot be used together with \"--infloop\"");
+
+		if(rwMixReadPercent)
+			throw ProgError("Option \"--cdcstats\" cannot be used together with \"--rwmixpct\"");
+
+		if(numRWMixReadThreads)
+			throw ProgError("Option \"--cdcstats\" cannot be used together with \"--rwmixthr\"");
+
+		if(!hosts.empty() )
+			throw ProgError("Option \"--cdcstats\" cannot be used together with \"--hosts\"");
 	}
 
 	if(!checksumAlgoName.empty() )

@@ -97,6 +97,7 @@ class ProgArgs
 		uint64_t dedupeStatsChunkSize{0}; // --dedupestats
 		uint64_t compressStatsChunkSize{0}; // --compressstats
 		uint64_t reduceStatsChunkSize{0}; // --reducestats
+		uint64_t cdcStatsAvgSize{0}; // --cdcstats
 		std::shared_ptr<const ChecksumList> checksumList; // --checksumverify, parsed by checkArgs
 		uint64_t rwMixReadPercent{0};
 		bool hasUserSetRWMixPercent{false};

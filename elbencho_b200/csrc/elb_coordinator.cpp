@@ -77,6 +77,7 @@ class Coordinator
 		void printDedupeLine(int benchPhase);
 		void printCompressLine(int benchPhase);
 		void printReduceLine(int benchPhase);
+		void printCdcLine(int benchPhase);
 		void printDryRunInfo();
 };
 
@@ -384,6 +385,39 @@ void Coordinator::printReduceLine(int benchPhase)
 	std::cout << formatReduceLine(progArgs.reduceStatsChunkSize, counters) << std::endl;
 }
 
+/* --cdcstats: "CDC: <N> chunks of <MIN> to <MAX> bytes, mean <B/N>, <D> distinct: <B> bytes, <U>
+   distinct bytes: <B/U>:1" for a mean chunk size of avgSize */
+static std::string formatCdcLine(uint64_t avgSize, const elb_reduce_counters& counters)
+{
+	return "CDC: " + std::to_string(counters.numChunks) + " chunks of " +
+		std::to_string(avgSize / 4) + " to " + std::to_string(avgSize * 4) + " bytes, mean " +
+		std::to_string(counters.numChunks ? counters.numBytes / counters.numChunks : 0) + ", " +
+		std::to_string(counters.numDistinct) + " distinct: " + std::to_string(counters.numBytes) +
+		" bytes, " + std::to_string(counters.numBytesDistinct) + " distinct bytes: " +
+		formatReduceRatio(counters.numBytes, counters.numBytesDistinct) + ":1";
+}
+
+/* --cdcstats: after each write and read phase that succeeded, its counts and their ratio */
+void Coordinator::printCdcLine(int benchPhase)
+{
+	if(!progArgs.cdcStatsAvgSize ||
+		( (benchPhase != ELB_PHASE_CREATEFILES) && (benchPhase != ELB_PHASE_READFILES) ) )
+		return;
+
+	elb_reduce_counters counters;
+
+	try
+	{
+		manager->getCdcStats(counters);
+	}
+	catch(const WorkerError& e)
+	{
+		throw ProgError(e.what() );
+	}
+
+	std::cout << formatCdcLine(progArgs.cdcStatsAvgSize, counters) << std::endl;
+}
+
 /* Coordinator::runBenchmarkPhase (:248-272) + Statistics live loop (:1284-1345) */
 void Coordinator::runBenchmarkPhase(int benchPhase)
 {
@@ -524,6 +558,7 @@ void Coordinator::runBenchmarkPhase(int benchPhase)
 	printDedupeLine(benchPhase);
 	printCompressLine(benchPhase);
 	printReduceLine(benchPhase);
+	printCdcLine(benchPhase);
 }
 
 void waitForUserDefinedStartTime(const ProgArgs& progArgs) // Coordinator.cpp:149-158
@@ -658,6 +693,9 @@ int Coordinator::main() // Coordinator.cpp:31-142
 
 		if(progArgs.reduceStatsChunkSize)
 			manager->setReduceStats(__builtin_ctzll(progArgs.reduceStatsChunkSize) );
+
+		if(progArgs.cdcStatsAvgSize)
+			manager->setCdcStats(__builtin_ctzll(progArgs.cdcStatsAvgSize) );
 
 		/* workers on several GPUs: create the NCCL communicators of the statistics reduce now,
 		   while the workers are idle (and before any result output) */
@@ -834,6 +872,27 @@ extern "C" int64_t elb_format_reduce_line(uint64_t chunkSize, const elb_reduce_c
 	}
 
 	const std::string text = elb::formatReduceLine(chunkSize, *counters);
+
+	if(outBuf && outBufLen)
+	{
+		const size_t copyLen = std::min( (size_t)(outBufLen - 1), text.size() );
+		memcpy(outBuf, text.data(), copyLen);
+		outBuf[copyLen] = 0;
+	}
+
+	return (int64_t)text.size();
+}
+
+extern "C" int64_t elb_format_cdc_line(uint64_t avgSize, const elb_reduce_counters* counters,
+	char* outBuf, uint64_t outBufLen)
+{
+	if(!counters)
+	{
+		elb_set_last_error("elb_format_cdc_line: NULL counters");
+		return -1;
+	}
+
+	const std::string text = elb::formatCdcLine(avgSize, *counters);
 
 	if(outBuf && outBufLen)
 	{

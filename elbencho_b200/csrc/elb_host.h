@@ -1008,6 +1008,7 @@ struct Config
 	unsigned dedupeChunkShift{0}; // --dedupestats: chunks of 2^shift bytes (0: off), 12..30
 	unsigned compressChunkShift{0}; // --compressstats (elb_mgr_set_compress_stats): 0 off, 12..20
 	unsigned reduceChunkShift{0}; // --reducestats (elb_mgr_set_reduce_stats): 0 off, 12..20
+	unsigned cdcAvgShift{0}; // --cdcstats (elb_mgr_set_cdc_stats): mean chunk 2^shift, 0 off, 12..18
 	int serializeBufferedWrites{ELB_WRITEGATE_AUTO};
 	int stagingEngine{ELB_STAGING_AUTO};
 	bool noGPUNumaBinding{false};

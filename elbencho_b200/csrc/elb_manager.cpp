@@ -135,7 +135,8 @@ Manager::~Manager()
 
 	freeDedupeTables();
 	freeCompressCounters();
-	freeReduceTables();
+	freeReduceTables(shared.reduceTables);
+	freeReduceTables(shared.cdcTables);
 	closeBenchPathFDs();
 }
 
@@ -389,7 +390,10 @@ void Manager::startNextPhase(int benchPhase)
 	prepareFilesForPhase(benchPhase);
 	prepareDedupeTables(benchPhase);
 	prepareCompressCounters(benchPhase);
-	prepareReduceTables(benchPhase);
+	prepareReduceTables(shared.reduceTables, shared.cfg.reduceChunkShift,
+		"Reduce stats (--reducestats)", benchPhase);
+	prepareReduceTables(shared.cdcTables, shared.cfg.cdcAvgShift ? shared.cfg.cdcAvgShift - 2 : 0,
+		"CDC stats (--cdcstats)", benchPhase);
 
 	std::unique_lock<std::mutex> lock(shared.mutex);
 
@@ -1317,23 +1321,60 @@ void Manager::setReduceStats(unsigned chunkShift)
 	cfg.reduceChunkShift = chunkShift;
 }
 
-/**
- * --reducestats: before a write or read phase, one reduce table per GPU of chunkTableSizes, its
- * keys, payloads and counters cleared. Fails before any I/O if the tables need more than half of a
- * GPU's free memory.
- */
-void Manager::prepareReduceTables(int benchPhase)
+void Manager::setCdcStats(unsigned avgShift)
 {
-	const Config& cfg = shared.cfg;
+	Config& cfg = shared.cfg;
+
+	if(avgShift && ( (avgShift < ELB_CDC_MIN_AVG_SHIFT) || (avgShift > ELB_CDC_MAX_AVG_SHIFT) ) )
+		throw WorkerError("The CDC mean chunk shift (" + std::to_string(avgShift) + ") is not in "
+			"[" + std::to_string(ELB_CDC_MIN_AVG_SHIFT) + ", " +
+			std::to_string(ELB_CDC_MAX_AVG_SHIFT) + "].");
+
+	// (below the largest chunk, every block would be one chunk at most: block dedupe)
+	const uint64_t fileBlockSize = (cfg.fileSize && (cfg.blockSize > cfg.fileSize) ) ?
+		cfg.fileSize : cfg.blockSize;
+
+	if(avgShift && (fileBlockSize < (4ULL << avgShift) ) )
+		throw WorkerError("The block size (" + std::to_string(fileBlockSize) + ") is below the "
+			"largest CDC chunk (--cdcstats) (" + std::to_string(4ULL << avgShift) + ").");
+
+	if(avgShift && cfg.useRandomOffsets)
+		throw WorkerError("CDC stats (--cdcstats) cannot be used together with random offsets "
+			"(--rand).");
+
+	if(avgShift && cfg.doInfiniteIOLoop)
+		throw WorkerError("CDC stats (--cdcstats) cannot be used together with an infinite I/O "
+			"loop (--infloop).");
+
+	if(avgShift && cfg.useRandomUnaligned)
+		throw WorkerError("CDC stats (--cdcstats) cannot be used together with unaligned random "
+			"offsets (--norandalign).");
+
+	if(avgShift && (cfg.rwMixReadPercent || cfg.numRWMixReadThreads) )
+		throw WorkerError("CDC stats (--cdcstats) cannot be used together with rwmix (a phase in "
+			"both directions).");
+
+	cfg.cdcAvgShift = avgShift;
+}
+
+/**
+ * --reducestats, --cdcstats: before a write or read phase, one reduce table per GPU of
+ * chunkTableSizes for chunks of at least 2^chunkShift bytes (0: the option is off) into
+ * sharedTables, its keys, payloads and counters cleared. Fails before any I/O if the tables need
+ * more than half of a GPU's free memory; what names the option in messages.
+ */
+void Manager::prepareReduceTables(std::vector<ReduceTable>& sharedTables, unsigned chunkShift,
+	const char* what, int benchPhase)
+{
 	const uint64_t entryBytes = 16 + ELB_REDUCE_PAYLOAD_BYTES;
 
-	if(!cfg.reduceChunkShift ||
+	if(!chunkShift ||
 		( (benchPhase != ELB_PHASE_CREATEFILES) && (benchPhase != ELB_PHASE_READFILES) ) )
 		return;
 
 	std::vector<ReduceTable> tables;
 
-	for(const std::pair<int, uint64_t>& gpuEntries : chunkTableSizes(cfg.reduceChunkShift) )
+	for(const std::pair<int, uint64_t>& gpuEntries : chunkTableSizes(chunkShift) )
 	{
 		ReduceTable table;
 		table.gpuID = gpuEntries.first;
@@ -1355,7 +1396,7 @@ void Manager::prepareReduceTables(int benchPhase)
 			uint64_t heldBytes = 0;
 			size_t freeBytes = 0, totalBytes = 0;
 
-			for(const ReduceTable& oldTable : shared.reduceTables)
+			for(const ReduceTable& oldTable : sharedTables)
 				if(oldTable.gpuID == table.gpuID)
 					heldBytes = oldTable.numEntries * entryBytes + sizeof(elb_reduce_counters);
 
@@ -1364,7 +1405,7 @@ void Manager::prepareReduceTables(int benchPhase)
 				"GPU memory query");
 
 			if(numBytes > (freeBytes + heldBytes) / 2)
-				throw WorkerError("Reduce stats (--reducestats) need " + std::to_string(numBytes) +
+				throw WorkerError(std::string(what) + " need " + std::to_string(numBytes) +
 					" bytes of GPU memory for the chunk table of GPU " +
 					std::to_string(table.gpuID) + ", more than half of its " +
 					std::to_string(freeBytes + heldBytes) + " free bytes. Use a larger chunk "
@@ -1373,15 +1414,15 @@ void Manager::prepareReduceTables(int benchPhase)
 
 		// keep the tables of the same size, free the others, then make the missing ones
 		for(ReduceTable& table : tables)
-			for(ReduceTable& oldTable : shared.reduceTables)
+			for(ReduceTable& oldTable : sharedTables)
 				if( (oldTable.gpuID == table.gpuID) && (oldTable.numEntries == table.numEntries) )
 					std::swap(oldTable, table);
 
-		freeReduceTables();
-		shared.reduceTables = tables;
+		freeReduceTables(sharedTables);
+		sharedTables = tables;
 		replaced = true;
 
-		for(ReduceTable& table : shared.reduceTables)
+		for(ReduceTable& table : sharedTables)
 		{
 			checkGpuCall(table.gpuID, cudaSetDevice(table.gpuID), "Setting CUDA device");
 
@@ -1411,7 +1452,7 @@ void Manager::prepareReduceTables(int benchPhase)
 	catch(...)
 	{
 		if(replaced)
-			freeReduceTables(); // (a failed allocation: no table is left half made)
+			freeReduceTables(sharedTables); // (a failed allocation: no table is left half made)
 
 		cudaSetDevice(prevDevice);
 		throw;
@@ -1421,9 +1462,9 @@ void Manager::prepareReduceTables(int benchPhase)
 }
 
 /* the tables and their counters (the workers must not use them any more) */
-void Manager::freeReduceTables()
+void Manager::freeReduceTables(std::vector<ReduceTable>& sharedTables)
 {
-	for(ReduceTable& table : shared.reduceTables)
+	for(ReduceTable& table : sharedTables)
 	{
 		cudaSetDevice(table.gpuID);
 
@@ -1433,18 +1474,32 @@ void Manager::freeReduceTables()
 			cudaFree(table.counters);
 	}
 
-	shared.reduceTables.clear();
+	sharedTables.clear();
 }
 
 void Manager::getReduceStats(elb_reduce_counters& out)
 {
+	sumReduceTables(shared.reduceTables, "Reduce stats (--reducestats)", out);
+}
+
+/* --cdcstats: the counts of the CDC tables, summed as the reduce tables are; U is also in S */
+void Manager::getCdcStats(elb_reduce_counters& out)
+{
+	sumReduceTables(shared.cdcTables, "CDC stats (--cdcstats)", out);
+}
+
+/* --reducestats, --cdcstats: N and B of all tables of sharedTables, and D, U and S of the first
+ * after the others are merged into it (what names the option in messages) */
+void Manager::sumReduceTables(std::vector<ReduceTable>& sharedTables, const char* what,
+	elb_reduce_counters& out)
+{
 	out = elb_reduce_counters{};
 
-	if(shared.reduceTables.empty() )
+	if(sharedTables.empty() )
 		return;
 
-	const ReduceTable& first = shared.reduceTables[0];
-	std::vector<elb_reduce_counters> counters(shared.reduceTables.size() );
+	const ReduceTable& first = sharedTables[0];
+	std::vector<elb_reduce_counters> counters(sharedTables.size() );
 	int prevDevice = 0;
 	cudaGetDevice(&prevDevice);
 
@@ -1463,19 +1518,19 @@ void Manager::getReduceStats(elb_reduce_counters& out)
 	   for the same phase */
 	uint64_t pieceEntries = 0;
 
-	for(size_t i = 1; i < shared.reduceTables.size(); i++)
+	for(size_t i = 1; i < sharedTables.size(); i++)
 		pieceEntries = std::max(pieceEntries,
-			std::min(shared.reduceTables[i].numEntries, (uint64_t)1 << 20) );
+			std::min(sharedTables[i].numEntries, (uint64_t)1 << 20) );
 
 	if( (res == cudaSuccess) && pieceEntries)
 		res = cudaMalloc(&piece, pieceEntries * (16 + ELB_REDUCE_PAYLOAD_BYTES) );
 
 	void* piecePayloads = (char*)piece + pieceEntries * 16;
 
-	for(size_t i = 1; (res == cudaSuccess) && !launchFailed && (i < shared.reduceTables.size() );
+	for(size_t i = 1; (res == cudaSuccess) && !launchFailed && (i < sharedTables.size() );
 		i++)
 	{
-		const ReduceTable& table = shared.reduceTables[i];
+		const ReduceTable& table = sharedTables[i];
 
 		for(uint64_t offset = 0; (res == cudaSuccess) && !launchFailed &&
 			(offset < table.numEntries); offset += pieceEntries)
@@ -1504,8 +1559,8 @@ void Manager::getReduceStats(elb_reduce_counters& out)
 			first.counters, stream);
 
 	for(size_t i = 0; (res == cudaSuccess) && !launchFailed &&
-		(i < shared.reduceTables.size() ); i++)
-		res = cudaMemcpyAsync(&counters[i], shared.reduceTables[i].counters,
+		(i < sharedTables.size() ); i++)
+		res = cudaMemcpyAsync(&counters[i], sharedTables[i].counters,
 			sizeof(elb_reduce_counters), cudaMemcpyDefault, stream);
 
 	const std::string launchError = launchFailed ? elb_last_error() : "";
@@ -1531,8 +1586,8 @@ void Manager::getReduceStats(elb_reduce_counters& out)
 	for(size_t i = 0; i < counters.size(); i++)
 	{
 		if(counters[i].overflow)
-			throw WorkerError("Reduce stats (--reducestats): the chunk table of GPU " +
-				std::to_string(shared.reduceTables[i].gpuID) + " ran past its probe bound of " +
+			throw WorkerError(std::string(what) + ": the chunk table of GPU " +
+				std::to_string(sharedTables[i].gpuID) + " ran past its probe bound of " +
 				std::to_string(ELB_DEDUPE_MAX_PROBES) + " entries; the counts are void.");
 
 		out.numChunks += counters[i].numChunks;
@@ -2469,6 +2524,61 @@ int elb_mgr_reduce_stats(elb_mgr* m, uint64_t* outNumChunks, uint64_t* outNumDis
 	*outNumBytes = counters.numBytes;
 	*outNumBytesDistinct = counters.numBytesDistinct;
 	*outNumBytesStored = counters.numBytesStored;
+	return 0;
+}
+
+int elb_mgr_set_cdc_stats(elb_mgr* m, unsigned avgShift)
+{
+	if(!m)
+	{
+		elb_set_last_error("elb_mgr_set_cdc_stats: NULL manager");
+		return -1;
+	}
+
+	try
+	{
+		m->impl->setCdcStats(avgShift);
+	}
+	catch(std::exception& e)
+	{
+		elb_set_last_error(e.what() );
+		return -1;
+	}
+
+	return 0;
+}
+
+int elb_mgr_cdc_stats(elb_mgr* m, uint64_t* outNumChunks, uint64_t* outNumDistinct,
+	uint64_t* outNumBytes, uint64_t* outNumBytesDistinct)
+{
+	if(!m || !outNumChunks || !outNumDistinct || !outNumBytes || !outNumBytesDistinct)
+	{
+		elb_set_last_error("elb_mgr_cdc_stats: NULL argument");
+		return -1;
+	}
+
+	if(!m->impl->shared.cfg.cdcAvgShift)
+	{
+		elb_set_last_error("elb_mgr_cdc_stats: CDC stats are off (elb_mgr_set_cdc_stats)");
+		return -1;
+	}
+
+	elb_reduce_counters counters;
+
+	try
+	{
+		m->impl->getCdcStats(counters);
+	}
+	catch(std::exception& e)
+	{
+		elb_set_last_error(e.what() );
+		return -1;
+	}
+
+	*outNumChunks = counters.numChunks;
+	*outNumDistinct = counters.numDistinct;
+	*outNumBytes = counters.numBytes;
+	*outNumBytesDistinct = counters.numBytesDistinct;
 	return 0;
 }
 

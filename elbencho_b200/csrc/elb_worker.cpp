@@ -826,11 +826,12 @@ void Worker::preparePhase()
  * chunk size, else the batch's own. --compressstats: the chunk size and counters of the stages'
  * LZ4 launch. --reducestats: the table the stages insert into, where the digests come from (as
  * for --dedupestats, or the dedupe launch's own at the same chunk size) and the batches' marks.
- * Runs after the rings are made and at the start of every write and read phase, since a checksum
- * list (elb_mgr_set_checksum_list) or the LZ4 or reduce chunk size (elb_mgr_set_compress_stats,
- * elb_mgr_set_reduce_stats) may be set and the manager may make new tables between phases; a
- * change drops the batch graphs, which hold the launches of the old setup. Without these options
- * it allocates and changes nothing.
+ * --cdcstats: the table the stages insert into and the batches' chunk counts and ends. Runs after
+ * the rings are made and at the start of every write and read phase, since a checksum list
+ * (elb_mgr_set_checksum_list) or the LZ4, reduce or CDC chunk size (elb_mgr_set_compress_stats,
+ * elb_mgr_set_reduce_stats, elb_mgr_set_cdc_stats) may be set and the manager may make new tables
+ * between phases; a change drops the batch graphs, which hold the launches of the old setup.
+ * Without these options it allocates and changes nothing.
  */
 void Worker::setupChecksums()
 {
@@ -882,6 +883,17 @@ void Worker::setupChecksums()
 	const uint64_t reduceSlots = !reduce ? 1 : std::max( (cfg.blockSize +
 		( (uint64_t)1 << cfg.reduceChunkShift) - 1) >> cfg.reduceChunkShift, (uint64_t)1);
 
+	ReduceTable cTable;
+
+	for(const ReduceTable& gpuTable : shared->cdcTables)
+		if(cfg.cdcAvgShift && (gpuTable.gpuID == gpuID) )
+			cTable = gpuTable;
+
+	const bool cdc = (cTable.entries != NULL);
+	const unsigned cdcMinShift = cfg.cdcAvgShift - 2;
+	const uint64_t cdcSlots = !cdc ? 1 : std::max( (cfg.blockSize +
+		( (uint64_t)1 << cdcMinShift) - 1) >> cdcMinShift, (uint64_t)1);
+
 	if(batches.empty() || ( (readChecksum == readStage.checksum) &&
 		(chunkShift == checksumChunkShift) && (slotsPerDesc == checksumSlotsPerDesc) &&
 		(cfg.checksumAlgo == checksumAlgo) && (dedupe == readStage.dedupe) &&
@@ -893,7 +905,9 @@ void Worker::setupChecksums()
 		(rTable.numEntries == reduceTable.numEntries) &&
 		(rTable.counters == reduceTable.counters) && (reduceSlots == reduceSlotsPerDesc) &&
 		( (reduceUsesSums && readChecksum) == reduceUsesReadSums) &&
-		(reduceUsesDedupe == reduceUsesDedupeSums) ) )
+		(reduceUsesDedupe == reduceUsesDedupeSums) && (cdc == readStage.cdc) &&
+		(cTable.entries == cdcTable.entries) && (cTable.numEntries == cdcTable.numEntries) &&
+		(cTable.counters == cdcTable.counters) && (cdcSlots == cdcSlotsPerDesc) ) )
 		return;
 
 	std::shared_lock<std::shared_timed_mutex> allocLock(shared->gpuAllocMutex);
@@ -909,11 +923,16 @@ void Worker::setupChecksums()
 	writeStage.reduce = reduce;
 	readStage.reduce = reduce;
 	verifyBackStage.reduce = false;
-	/* --verifydirect: a write phase's checksums, dedupe, compress and reduce counts are those of
-	   the written bytes, so the read-back takes none, and must not share the read phase's batch
+	writeStage.cdc = cdc;
+	readStage.cdc = cdc;
+	verifyBackStage.cdc = false;
+	/* --verifydirect: a write phase's checksums, dedupe, compress, reduce and CDC counts are those
+	   of the written bytes, so the read-back takes none, and must not share the read phase's batch
 	   graphs then */
 	verifyBackStage.useGraph = readStage.useGraph && !readChecksum && !dedupe && !lz4ChunkShift &&
-		!reduce;
+		!reduce && !cdc;
+	cdcTable = cTable;
+	cdcSlotsPerDesc = cdcSlots;
 	reduceTable = rTable;
 	reduceSlotsPerDesc = reduceSlots;
 	reduceUsesWriteSums = reduceUsesSums && cfg.checksums;
@@ -948,6 +967,10 @@ void Worker::setupChecksums()
 			cudaFree(batch.devReduceSums);
 		if(batch.devReduceMarks)
 			cudaFree(batch.devReduceMarks);
+		if(batch.devCdcCounts)
+			cudaFree(batch.devCdcCounts);
+		if(batch.devCdcEnds)
+			cudaFree(batch.devCdcEnds);
 
 		batch.readGraphExec = NULL;
 		batch.writeGraphExec = NULL;
@@ -956,6 +979,8 @@ void Worker::setupChecksums()
 		batch.devDedupeSums = NULL;
 		batch.devReduceSums = NULL;
 		batch.devReduceMarks = NULL;
+		batch.devCdcCounts = NULL;
+		batch.devCdcEnds = NULL;
 
 		if(dedupeNeedsOwnSums)
 			ELB_CUDA_CHECK(cudaMalloc(&batch.devDedupeSums, elb_checksum_value_bytes(
@@ -968,6 +993,14 @@ void Worker::setupChecksums()
 		if(reduce)
 			ELB_CUDA_CHECK(cudaMalloc( (void**)&batch.devReduceMarks, sizeof(uint64_t) *
 				batchBlocks * reduceSlots), "GPU reduce mark allocation");
+
+		if(cdc)
+		{
+			ELB_CUDA_CHECK(cudaMalloc( (void**)&batch.devCdcCounts, sizeof(uint32_t) * batchBlocks),
+				"GPU CDC count allocation");
+			ELB_CUDA_CHECK(cudaMalloc( (void**)&batch.devCdcEnds, sizeof(uint64_t) * batchBlocks *
+				cdcSlots), "GPU CDC chunk allocation");
+		}
 
 		if(!readChecksum)
 			continue;
@@ -1249,6 +1282,10 @@ void Worker::freeRings() // LocalWorker::cleanup (:1570-1641)
 			cudaFree(batch.devReduceSums);
 		if(batch.devReduceMarks)
 			cudaFree(batch.devReduceMarks);
+		if(batch.devCdcCounts)
+			cudaFree(batch.devCdcCounts);
+		if(batch.devCdcEnds)
+			cudaFree(batch.devCdcEnds);
 		if(batch.hostSums)
 			cudaFreeHost(batch.hostSums);
 	}
@@ -1995,6 +2032,7 @@ void Worker::rwPhase()
 
 	checkDedupeOverflow();
 	checkReduceOverflow();
+	checkCdcOverflow();
 }
 
 /**
@@ -2558,6 +2596,9 @@ void Worker::enqueueStage(Batch& batch, const GpuStage& stage, uint32_t numBlock
 	if(stage.reduce)
 		enqueueReduce(batch, stage, numBlocks);
 
+	if(stage.cdc)
+		enqueueCdc(batch, numBlocks);
+
 	if( (stage.transfer == GpuStage::TRANSFER_COPY) && !stage.isRead)
 		enqueueStageCopies(batch, false, true);
 }
@@ -2651,6 +2692,41 @@ void Worker::checkReduceOverflow()
 			"the counts are void.");
 }
 
+/* --cdcstats: the batch's blocks cut into content-defined chunks, then the chunks' digests into
+ * the CDC table of this worker's GPU. Nothing is copied or waited for: the table is read at the end
+ * of the phase. */
+void Worker::enqueueCdc(Batch& batch, uint32_t numBlocks)
+{
+	if(elb_launch_cdc_cut(batch.hostDescs, numBlocks, cfg.cdcAvgShift, cdcSlotsPerDesc,
+		batch.devCdcCounts, batch.devCdcEnds, batch.stream) )
+		throw WorkerError(std::string("GPU CDC cut failed. ") + elb_last_error() );
+
+	if(elb_launch_cdc_hash_insert(batch.hostDescs, numBlocks, cfg.cdcAvgShift, cdcSlotsPerDesc,
+		batch.devCdcCounts, batch.devCdcEnds, NULL, cdcTable.entries, cdcTable.payloads,
+		cdcTable.numEntries, cdcTable.counters, batch.stream) )
+		throw WorkerError(std::string("GPU CDC insert failed. ") + elb_last_error() );
+}
+
+/* --cdcstats: the phase fails if the table of this worker's GPU ran past its probe bound (a
+ * guard: a table is sized for a load of at most 0.5) */
+void Worker::checkCdcOverflow()
+{
+	if(!readStage.cdc || batches.empty() )
+		return;
+
+	uint32_t overflow = 0;
+
+	ELB_CUDA_CHECK(cudaMemcpyAsync(&overflow, &cdcTable.counters->overflow, sizeof(overflow),
+		cudaMemcpyDeviceToHost, batches[0].stream), "GPU CDC counter read");
+	ELB_CUDA_CHECK(cudaStreamSynchronize(batches[0].stream), "GPU CDC counter read");
+
+	if(overflow)
+		throw WorkerError("CDC stats (--cdcstats): the chunk table of GPU " +
+			std::to_string(gpuID) + " (" + std::to_string(cdcTable.numEntries) + " entries) "
+			"ran past its probe bound of " + std::to_string(ELB_DEDUPE_MAX_PROBES) + " entries; "
+			"the counts are void.");
+}
+
 /**
  * GPU stage of a batch, write (fill + stage-out, LocalWorker.cpp:1249-1265) or read (stage-in +
  * verify, :1311-1319; the reference verifies on the CPU), between the batch's stage events. A
@@ -2696,6 +2772,8 @@ void Worker::gpuLaunchStage(Batch& batch, bool isRead)
 		numKernelLaunches += ( (stage.checksum &&
 			(stage.isRead ? reduceUsesReadSums : reduceUsesWriteSums) ) ||
 			(stage.dedupe && reduceUsesDedupeSums) ) ? 2 : 3;
+	if(numBlocks && stage.cdc) // (the cut and the hash-insert)
+		numKernelLaunches += 2;
 
 	if(stage.transfer != GpuStage::TRANSFER_NONE)
 		(isRead ? numH2DBytes : numD2HBytes) += numBytes;

@@ -62,9 +62,10 @@ struct DedupeTable
 	elb_dedupe_counters* counters{NULL};
 };
 
-/* --reducestats: the reduce table of one GPU (elb_reduce_insert): the keys as in DedupeTable, the
- * payloads after them in the same allocation, and its counters; made and cleared by the manager at
- * the start of every write and read phase, shared by the GPU's workers */
+/* --reducestats, --cdcstats: the reduce table of one GPU (elb_reduce_insert, elb_cdc_hash_insert):
+ * the keys as in DedupeTable, the payloads after them in the same allocation, and its counters;
+ * made and cleared by the manager at the start of every write and read phase, shared by the GPU's
+ * workers */
 struct ReduceTable
 {
 	int gpuID{-1};
@@ -109,6 +110,7 @@ struct Shared
 	uint8_t dedupeZeroDigest[32]{};        // --dedupestats: the BLAKE3 of a chunk of zero bytes
 	std::vector<CompressCounters> compressCounters; // --compressstats: one per GPU
 	std::vector<ReduceTable> reduceTables; // --reducestats: one per GPU, the first worker's first
+	std::vector<ReduceTable> cdcTables;    // --cdcstats: one per GPU, the first worker's first
 
 	/* workers hold this shared while they allocate / free device memory or instantiate graphs;
 	   the live stats reducer holds it exclusively while its collective is in flight, because a
@@ -288,6 +290,8 @@ struct GpuStage
 	bool compress;    // --compressstats: the LZ4 launch over the chunks, into the GPU's counters
 	bool reduce;      // --reducestats: the chunks' digests into the GPU's reduce table, the new
 	                  // ones compressed
+	bool cdc;         // --cdcstats: the blocks cut into content-defined chunks, their digests into
+	                  // the GPU's CDC table
 };
 
 /* a batch: a contiguous slice of the rings plus everything its GPU stage needs */
@@ -325,6 +329,10 @@ struct Batch
 	   and every slot's mark (elb_reduce_insert), 8 bytes per slot (device only) */
 	void* devReduceSums{NULL};
 	uint64_t* devReduceMarks{NULL};
+	/* --cdcstats: every block's chunk count (4 bytes) and its chunks' end offsets, 8 bytes per
+	   slot (device only) */
+	uint32_t* devCdcCounts{NULL};
+	uint64_t* devCdcEnds{NULL};
 
 	// aio state
 	std::vector<struct iocb> iocbs;
@@ -535,6 +543,9 @@ class Worker
 		bool reduceUsesWriteSums{false};
 		bool reduceUsesReadSums{false};
 		bool reduceUsesDedupeSums{false};
+		/* --cdcstats: the table of this worker's GPU and the slots of the chunk ends per block */
+		ReduceTable cdcTable;
+		uint64_t cdcSlotsPerDesc{1};
 
 		// accounting
 		std::atomic<uint64_t> numH2DBytes{0};
@@ -582,6 +593,8 @@ class Worker
 		void checkDedupeOverflow();
 		void enqueueReduce(Batch& batch, const GpuStage& stage, uint32_t numBlocks);
 		void checkReduceOverflow();
+		void enqueueCdc(Batch& batch, uint32_t numBlocks);
+		void checkCdcOverflow();
 		FileID blockFileID(const BlockRef& block) const;
 		uint64_t blockFileSize(const BlockRef& block) const;
 		void gpuLaunchStage(Batch& batch, bool isRead);
@@ -699,6 +712,15 @@ class Manager
 		   bound) */
 		void getReduceStats(elb_reduce_counters& out);
 
+		/* --cdcstats: from the next write or read phase on, the CDC counts of chunks of mean size
+		   2^avgShift bytes (0: off); throws WorkerError for a shift outside 12..18 or a config it
+		   cannot be used with */
+		void setCdcStats(unsigned avgShift);
+		/* --cdcstats: N, B, D and U (also in S) of the last write or read phase over all GPUs
+		   (merges the other GPUs' tables into the first's; throws WorkerError if a table ran past
+		   its probe bound) */
+		void getCdcStats(elb_reduce_counters& out);
+
 		Shared shared;
 		std::vector<std::unique_ptr<Worker> > workers;
 		std::vector<std::thread> threads;
@@ -719,8 +741,11 @@ class Manager
 		void prepareCompressCounters(int benchPhase);
 		void freeCompressCounters();
 		std::vector<std::pair<int, uint64_t> > chunkTableSizes(unsigned chunkShift);
-		void prepareReduceTables(int benchPhase);
-		void freeReduceTables();
+		void prepareReduceTables(std::vector<ReduceTable>& sharedTables, unsigned chunkShift,
+			const char* what, int benchPhase);
+		void freeReduceTables(std::vector<ReduceTable>& sharedTables);
+		void sumReduceTables(std::vector<ReduceTable>& sharedTables, const char* what,
+			elb_reduce_counters& out);
 		std::unique_ptr<LiveStatsReducer> liveStatsReducer; // created on first use
 		std::mutex liveStatsReducerMutex;
 };

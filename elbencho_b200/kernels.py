@@ -575,3 +575,45 @@ def reduce_line(chunk_size, chunks, distinct, bytes_in, distinct_bytes, stored):
     if lib.elb_format_reduce_line(chunk_size, counters, buf, len(buf)) < 0:
         raise KernelError("elb_format_reduce_line failed: %s" % _native.last_error())
     return buf.value.decode()
+
+
+# ---- --cdcstats: content-defined chunks ----
+
+CDC_GEAR_TAG = 0x6A09E667F3BCC908  # gear[i] = splitmix64_mix(CDC_GEAR_TAG + i)
+
+
+def cdc_cut(pinned_descs_ptr, num_descs, avg_shift, slots_per_desc, dev_counts_ptr, dev_ends_ptr,
+            stream=0):
+    """Cut each descriptor's block into content-defined chunks of mean 2^avg_shift bytes
+    (avg_shift 12..18): the uint32 at dev_counts_ptr + 4 * i gets descriptor i's chunk count, the
+    uint64 at dev_ends_ptr + 8 * (i * slots_per_desc + j) the end offset of its chunk j in the
+    block."""
+    _check(_native.load().elb_cdc_cut(pinned_descs_ptr or None, num_descs, avg_shift,
+                                      slots_per_desc, dev_counts_ptr or None, dev_ends_ptr or None,
+                                      stream),
+           "elb_cdc_cut")
+
+
+def cdc_hash_insert(pinned_descs_ptr, num_descs, avg_shift, slots_per_desc, dev_counts_ptr,
+                    dev_ends_ptr, dev_digests_ptr, dev_table_ptr, dev_payloads_ptr, table_entries,
+                    dev_counters_ptr, stream=0):
+    """Hash every chunk of cdc_cut (the same descriptors, slots, counts and ends) with BLAKE3-256
+    and insert its key into a reduce table as reduce_insert does; a new key writes (length,
+    length) to its payload. Adds the chunks and their bytes to the 48-byte counters (see
+    reduce_counters). dev_digests_ptr, if not 0, gets each chunk's digest in its 32-byte slot."""
+    _check(_native.load().elb_cdc_hash_insert(pinned_descs_ptr or None, num_descs, avg_shift,
+                                              slots_per_desc, dev_counts_ptr or None,
+                                              dev_ends_ptr or None, dev_digests_ptr or None,
+                                              dev_table_ptr or None, dev_payloads_ptr or None,
+                                              table_entries, dev_counters_ptr or None, stream),
+           "elb_cdc_hash_insert")
+
+
+def cdc_line(avg_size, chunks, distinct, bytes_in, distinct_bytes):
+    """the console line of --cdcstats for these counts"""
+    counters = (ctypes.c_uint64 * 6)(chunks, bytes_in, distinct, distinct_bytes, distinct_bytes, 0)
+    buf = ctypes.create_string_buffer(384)
+    lib = _native.load()
+    if lib.elb_format_cdc_line(avg_size, counters, buf, len(buf)) < 0:
+        raise KernelError("elb_format_cdc_line failed: %s" % _native.last_error())
+    return buf.value.decode()

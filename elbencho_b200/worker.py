@@ -120,6 +120,7 @@ class WorkerConfig:
     dedupe_chunk: int = 0             # --dedupestats bytes (a power of two 4K..1G; 0 = off)
     compress_chunk: int = 0           # --compressstats bytes (a power of two 4K..1M; 0 = off)
     reduce_chunk: int = 0             # --reducestats bytes (a power of two 4K..1M; 0 = off)
+    cdc_avg: int = 0                  # --cdcstats mean chunk bytes (a power of two 4K..256K; 0 = off)
     serialize_buffered_writes: int = 0  # 0 auto, 1 on, 2 off (--writegate)
     staging_engine: int = 0           # 0 auto, 1 kernels move the data, 2 cudaMemcpyAsync
     no_gpu_numa_binding: bool = False  # --nogpunuma
@@ -306,6 +307,13 @@ class WorkerManager:
                 err = _native.last_error()
                 self.close()
                 raise WorkerError(err)
+        avg = config.cdc_avg
+        if avg:
+            shift = avg.bit_length() - 1 if not avg & (avg - 1) else 0xffffffff
+            if self._lib.elb_mgr_set_cdc_stats(self._h, shift) != 0:
+                err = _native.last_error()
+                self.close()
+                raise WorkerError(err)
 
     def close(self):
         if self._h:
@@ -479,6 +487,14 @@ class WorkerManager:
         compress ratio U / S and the total B / S."""
         vals = [ctypes.c_uint64(0) for _ in range(5)]
         if self._lib.elb_mgr_reduce_stats(self._h, *[ctypes.byref(v) for v in vals]) != 0:
+            raise WorkerError(_native.last_error())
+        return tuple(v.value for v in vals)
+
+    def cdc_stats(self):
+        """--cdcstats: (chunks N, distinct chunks D, bytes B, distinct bytes U) of the last write or
+        read phase, over all workers and GPUs; the dedupe ratio is B / U."""
+        vals = [ctypes.c_uint64(0) for _ in range(4)]
+        if self._lib.elb_mgr_cdc_stats(self._h, *[ctypes.byref(v) for v in vals]) != 0:
             raise WorkerError(_native.last_error())
         return tuple(v.value for v in vals)
 

@@ -468,6 +468,31 @@ int elb_reduce_merge(const void* srcEntries, const void* srcPayloads, uint64_t n
 int elb_reduce_sum(const void* table, const void* payloads, uint64_t tableEntries,
 	elb_reduce_counters* devCounters, void* stream);
 
+/* --cdcstats: cut each descriptor's block into content-defined chunks from its first byte, with
+ * AVG = 2^avgShift (avgShift 12..18), MIN = AVG / 4 and MAX = 4 * AVG: the gear hash
+ * h(p) = sum over k = 0..63 of gear[b[p - k]] << k (mod 2^64), gear[i] =
+ * splitmix64_mix(0x6A09E667F3BCC908 + i); a chunk from c ends at the least l in [MIN, AVG) whose
+ * h(c + l - 1) has its top avgShift + 2 bits zero, else the least l in [AVG, MAX) whose
+ * h(c + l - 1) has its top avgShift - 2 bits zero, else at MAX, and at the block's end.
+ * devCounts[i] gets descriptor i's chunk count and devEnds[i * slotsPerDesc + j] the end offset in
+ * the block of its chunk j (chunk j is [devEnds[.. j - 1] or 0, devEnds[.. j]) ). descs must be
+ * pinned host memory. Fails without launching for NULL pointers, an avgShift outside 12..18 or a
+ * descriptor that can have more chunks (ceil(len / MIN)) than slotsPerDesc. */
+int elb_cdc_cut(const elb_block_desc* descs, uint32_t numDescs, unsigned avgShift,
+	uint64_t slotsPerDesc, uint32_t* devCounts, uint64_t* devEnds, void* stream);
+/* --cdcstats: the BLAKE3-256 digest of every chunk of elb_cdc_cut (the same descriptors, slots,
+ * devCounts and devEnds), its key inserted into a reduce table as elb_reduce_insert inserts one; a
+ * key that takes a new entry writes {length, length} to its payload, so that elb_reduce_sum gives
+ * the distinct chunks and their bytes. Adds every chunk to numChunks and its length to numBytes
+ * of devCounters; sets overflow past the probe bound. devDigests, if not NULL, gets the digest of
+ * chunk j of descriptor i in the 32 bytes of slot i * slotsPerDesc + j. Fails without launching
+ * for a table size that is not a power of two, NULL pointers (but devDigests), an avgShift outside
+ * 12..18 or a descriptor that can have more chunks than slotsPerDesc. */
+int elb_cdc_hash_insert(const elb_block_desc* descs, uint32_t numDescs, unsigned avgShift,
+	uint64_t slotsPerDesc, const uint32_t* devCounts, const uint64_t* devEnds, void* devDigests,
+	void* table, void* payloads, uint64_t tableEntries, elb_reduce_counters* devCounters,
+	void* stream);
+
 int elb_stage_copy(const elb_block_desc* descs, uint32_t numDescs, int hostToDevice,
 	int64_t hostDelta, uint64_t totalBytes, uint64_t maxBlockLen, void* stream);
 /* devResults[0..numDescs) <- {0, ~0} */
@@ -812,6 +837,13 @@ int64_t elb_format_compress_line(uint64_t chunkSize, const elb_compress_counters
  * Returns the text length (text truncated to outBufLen - 1), -1 on error. */
 int64_t elb_format_reduce_line(uint64_t chunkSize, const elb_reduce_counters* counters,
 	char* outBuf, uint64_t outBufLen);
+/* --cdcstats: the console line of a phase's counters (numChunks N, numDistinct D, numBytes B,
+ * numBytesDistinct U) for a mean chunk size of avgSize bytes, "CDC: <N> chunks of <MIN> to <MAX>
+ * bytes, mean <B/N>, <D> distinct: <B> bytes, <U> distinct bytes: <B/U>:1" (the mean an integer, 0
+ * for no chunks; the ratio with two decimals, 1.00 when U is 0). Returns the text length (text
+ * truncated to outBufLen - 1), -1 on error. */
+int64_t elb_format_cdc_line(uint64_t avgSize, const elb_reduce_counters* counters, char* outBuf,
+	uint64_t outBufLen);
 /* UnitTk::numHumanToBytesBinary (toolkits/UnitTk.cpp:18-76): "4k", "1M", "64G"; 0 ok, -1 error */
 int elb_num_human_to_bytes(const char* numHuman, uint64_t* outBytes);
 
@@ -997,6 +1029,20 @@ int elb_mgr_set_reduce_stats(elb_mgr* m, unsigned chunkShift);
  * or a table ran past its probe bound (elb_last_error), else 0. */
 int elb_mgr_reduce_stats(elb_mgr* m, uint64_t* outNumChunks, uint64_t* outNumDistinct,
 	uint64_t* outNumBytes, uint64_t* outNumBytesDistinct, uint64_t* outNumBytesStored);
+/* --cdcstats: from the next write or read phase on, cut every block a phase moves into
+ * content-defined chunks of mean 2^avgShift bytes (12..18; elb_cdc_cut) and count the distinct
+ * ones in a table per GPU (elb_cdc_hash_insert); 0 turns it off. Returns -1 (elb_last_error) for
+ * another avgShift, or if the config has a block size below the largest chunk (4 * 2^avgShift,
+ * after a block larger than the file is reduced to the file size), random or unaligned random
+ * offsets, an infinite loop or rwmix. */
+int elb_mgr_set_cdc_stats(elb_mgr* m, unsigned avgShift);
+/* --cdcstats: of the last write or read phase, the chunks it moved (N), the distinct ones by
+ * BLAKE3-256 (D), the bytes of all (B) and the bytes of the distinct ones each counted once (U),
+ * over all workers and GPUs of the manager (merges the other GPUs' tables into the first's). All 0
+ * before the first such phase. Returns -1 if --cdcstats is off or a table ran past its probe bound
+ * (elb_last_error), else 0. */
+int elb_mgr_cdc_stats(elb_mgr* m, uint64_t* outNumChunks, uint64_t* outNumDistinct,
+	uint64_t* outNumBytes, uint64_t* outNumBytesDistinct);
 
 uint32_t elb_mgr_num_workers(elb_mgr* m);
 elb_worker* elb_mgr_worker(elb_mgr* m, uint32_t localIdx);
