@@ -272,6 +272,9 @@ SIGNATURES = {
     "elb_cdc_cut": (ctypes.c_int, [_VP, c_u32, ctypes.c_uint, c_u64, _VP, _VP, _VP]),
     "elb_cdc_hash_insert": (ctypes.c_int, [_VP, c_u32, ctypes.c_uint, c_u64, _VP, _VP, _VP, _VP,
                                             _VP, c_u64, _VP, _VP]),
+    "elb_cdc_hash_insert_marks": (ctypes.c_int, [_VP, c_u32, ctypes.c_uint, c_u64, _VP, _VP, _VP,
+                                                  _VP, _VP, c_u64, _VP, _VP, _VP]),
+    "elb_cdc_lz4": (ctypes.c_int, [_VP, c_u32, ctypes.c_uint, c_u64, _VP, _VP, _VP, _VP, _VP]),
     "elb_damage_map": (ctypes.c_int, [_VP, c_u32, ctypes.c_int, c_u64, ctypes.c_uint,
                                       ctypes.c_uint, ctypes.c_uint, _VP, c_u64, _VP]),
     "elb_stage_copy": (ctypes.c_int, [_VP, c_u32, ctypes.c_int, ctypes.c_int64, c_u64, c_u64,
@@ -297,6 +300,7 @@ SIGNATURES = {
     "elb_format_compress_line": (ctypes.c_int64, [c_u64, _VP, ctypes.c_char_p, c_u64]),
     "elb_format_reduce_line": (ctypes.c_int64, [c_u64, _VP, ctypes.c_char_p, c_u64]),
     "elb_format_cdc_line": (ctypes.c_int64, [c_u64, _VP, ctypes.c_char_p, c_u64]),
+    "elb_format_cdc_reduce_line": (ctypes.c_int64, [c_u64, _VP, ctypes.c_char_p, c_u64]),
     "elb_simple128_hash": (None, [ctypes.c_char_p, ctypes.c_char_p]),
     "elb_num_human_to_bytes": (ctypes.c_int, [ctypes.c_char_p, ctypes.POINTER(c_u64)]),
     "elb_rate_limiter_create": (_VP, [c_u64]),
@@ -352,6 +356,8 @@ SIGNATURES = {
     "elb_mgr_reduce_stats": (ctypes.c_int, [_VP] + [ctypes.POINTER(c_u64)] * 5),
     "elb_mgr_set_cdc_stats": (ctypes.c_int, [_VP, ctypes.c_uint]),
     "elb_mgr_cdc_stats": (ctypes.c_int, [_VP] + [ctypes.POINTER(c_u64)] * 4),
+    "elb_mgr_set_cdc_reduce_stats": (ctypes.c_int, [_VP, ctypes.c_uint]),
+    "elb_mgr_cdc_reduce_stats": (ctypes.c_int, [_VP] + [ctypes.POINTER(c_u64)] * 5),
     "elb_mgr_num_workers": (c_u32, [_VP]),
     "elb_mgr_worker": (_VP, [_VP, c_u32]),
     "elb_mgr_last_error": (ctypes.c_char_p, [_VP]),

@@ -846,7 +846,7 @@ int elb_reduce_sum(const void* table, const void* payloads, uint64_t tableEntrie
 	return 0;
 }
 
-/* the mean chunk size check of elb_cdc_cut and _hash_insert */
+/* the mean chunk size check of elb_cdc_cut, _hash_insert, _hash_insert_marks and _lz4 */
 static bool cdcAvgShiftValid(const char* what, unsigned avgShift)
 {
 	if( (avgShift < ELB_CDC_MIN_AVG_SHIFT) || (avgShift > ELB_CDC_MAX_AVG_SHIFT) )
@@ -902,7 +902,61 @@ int elb_cdc_hash_insert(const elb_block_desc* descs, uint32_t numDescs, unsigned
 	}
 
 	if(elb_launch_cdc_hash_insert(descs, numDescs, avgShift, slotsPerDesc, devCounts, devEnds,
-		devDigests, table, payloads, tableEntries, devCounters, (cudaStream_t)stream) )
+		devDigests, table, payloads, tableEntries, devCounters, NULL, (cudaStream_t)stream) )
+	{
+		elb_set_last_error(std::string("elb_") + elb_last_error() );
+		return -1;
+	}
+
+	return 0;
+}
+
+int elb_cdc_hash_insert_marks(const elb_block_desc* descs, uint32_t numDescs, unsigned avgShift,
+	uint64_t slotsPerDesc, const uint32_t* devCounts, const uint64_t* devEnds, void* devDigests,
+	void* table, void* payloads, uint64_t tableEntries, elb_reduce_counters* devCounters,
+	uint64_t* devMarks, void* stream)
+{
+	const char* what = "elb_cdc_hash_insert_marks";
+
+	if(!reduceTableArgsValid(what, table, tableEntries, devCounters) ||
+		!cdcAvgShiftValid(what, avgShift) )
+		return -1;
+
+	if(!payloads || (numDescs && (!descs || !devCounts || !devEnds || !devMarks) ) )
+	{
+		elb_set_last_error(std::string(what) +
+			": NULL payloads, descriptor, count, end or mark array");
+		return -1;
+	}
+
+	if(elb_launch_cdc_hash_insert(descs, numDescs, avgShift, slotsPerDesc, devCounts, devEnds,
+		devDigests, table, payloads, tableEntries, devCounters, devMarks, (cudaStream_t)stream) )
+	{
+		elb_set_last_error(std::string("elb_") + elb_last_error() );
+		return -1;
+	}
+
+	return 0;
+}
+
+int elb_cdc_lz4(const elb_block_desc* descs, uint32_t numDescs, unsigned avgShift,
+	uint64_t slotsPerDesc, const uint32_t* devCounts, const uint64_t* devEnds,
+	const uint64_t* devMarks, void* devPayloads, void* stream)
+{
+	const char* what = "elb_cdc_lz4";
+
+	if(!cdcAvgShiftValid(what, avgShift) )
+		return -1;
+
+	if(numDescs && (!descs || !devCounts || !devEnds || !devMarks || !devPayloads) )
+	{
+		elb_set_last_error(std::string(what) +
+			": NULL descriptor, count, end, mark or payload array");
+		return -1;
+	}
+
+	if(elb_launch_cdc_lz4(descs, numDescs, avgShift, slotsPerDesc, devCounts, devEnds, devMarks,
+		devPayloads, (cudaStream_t)stream) )
 	{
 		elb_set_last_error(std::string("elb_") + elb_last_error() );
 		return -1;

@@ -27,12 +27,17 @@
  *     (elb_patterns.cuh). The key goes into the table by the rules of --dedupestats
  *     (elb_dedupe.cuh); the lane that takes a new entry writes {length, length} to its payload, so
  *     that elb_reduce_merge and elb_reduce_sum give D and U. N and B are added once per warp.
+ * --cdcreducestats takes the cut, the hash and insert with marks (the entry a slot newly took, as
+ * elb_reduce_insert writes them) and a third launch: the LZ4 parse of --compressstats (elb_lz4.cuh)
+ * over each slot marked new, one warp per chunk, which writes {length, min(LZ4 size, length)} to
+ * its entry's payload. So each distinct chunk is compressed once, and elb_reduce_sum gives S too.
  */
 #include <algorithm>
 #include <string>
 
 #include "elb_blake3.cuh"
 #include "elb_dedupe.cuh"
+#include "elb_lz4.cuh"
 
 #define ELB_CDC_THREADS 256
 #define ELB_CDC_RUN 256 /* positions a thread hashes per window */
@@ -239,12 +244,13 @@ elb_cdc_cut_kernel(const elb_block_desc* descs, unsigned avgShift, uint64_t slot
 		counts[blockIdx.x] = numChunks;
 }
 
-/* warp w: chunk j = w % slotsUsed of descriptor w / slotsUsed, if the descriptor has it */
-__global__ void __launch_bounds__(ELB_CDC_HASH_WARPS * 32)
-elb_cdc_hash_insert_kernel(const elb_block_desc* descs, uint32_t numDescs, uint64_t slotsPerDesc,
-	uint64_t slotsUsed, const uint32_t* counts, const uint64_t* ends, uint32_t* digests,
-	DedupeKey* table, CdcPayload* payloads, uint64_t mask, uint64_t maxProbes,
-	elb_reduce_counters* counters)
+/* warp w: chunk j = w % slotsUsed of descriptor w / slotsUsed, if the descriptor has it; if MARKS,
+   its slot's mark (the entry it newly took, or ELB_REDUCE_NOT_NEW) to marks */
+template<bool MARKS>
+__device__ __forceinline__ void cdc_hash_insert(const elb_block_desc* descs, uint32_t numDescs,
+	uint64_t slotsPerDesc, uint64_t slotsUsed, const uint32_t* counts, const uint64_t* ends,
+	uint32_t* digests, DedupeKey* table, CdcPayload* payloads, uint64_t mask, uint64_t maxProbes,
+	elb_reduce_counters* counters, uint64_t* marks)
 {
 	__shared__ uint32_t sStack[ELB_CDC_HASH_WARPS][ELB_CDC_STACK][8];
 	__shared__ uint32_t sStackLeaves[ELB_CDC_HASH_WARPS][ELB_CDC_STACK];
@@ -365,9 +371,82 @@ elb_cdc_hash_insert_kernel(const elb_block_desc* descs, uint32_t numDescs, uint6
 		payloads[pos] = CdcPayload{chunkLen, chunkLen};
 	if(res < 0)
 		atomicExch(&counters->overflow, 1u);
+	if(MARKS)
+		marks[slot] = (res > 0) ? pos : ELB_REDUCE_NOT_NEW;
 
 	atomicAdd( (unsigned long long*)&counters->numChunks, 1ULL);
 	atomicAdd( (unsigned long long*)&counters->numBytes, (unsigned long long)chunkLen);
+}
+
+__global__ void __launch_bounds__(ELB_CDC_HASH_WARPS * 32)
+elb_cdc_hash_insert_kernel(const elb_block_desc* descs, uint32_t numDescs, uint64_t slotsPerDesc,
+	uint64_t slotsUsed, const uint32_t* counts, const uint64_t* ends, uint32_t* digests,
+	DedupeKey* table, CdcPayload* payloads, uint64_t mask, uint64_t maxProbes,
+	elb_reduce_counters* counters)
+{
+	cdc_hash_insert<false>(descs, numDescs, slotsPerDesc, slotsUsed, counts, ends, digests, table,
+		payloads, mask, maxProbes, counters, NULL);
+}
+
+/* --cdcreducestats: the hash and insert with the slots' marks for elb_cdc_lz4_kernel */
+__global__ void __launch_bounds__(ELB_CDC_HASH_WARPS * 32)
+elb_cdc_hash_insert_marks_kernel(const elb_block_desc* descs, uint32_t numDescs,
+	uint64_t slotsPerDesc, uint64_t slotsUsed, const uint32_t* counts, const uint64_t* ends,
+	uint32_t* digests, DedupeKey* table, CdcPayload* payloads, uint64_t mask, uint64_t maxProbes,
+	elb_reduce_counters* counters, uint64_t* marks)
+{
+	cdc_hash_insert<true>(descs, numDescs, slotsPerDesc, slotsUsed, counts, ends, digests, table,
+		payloads, mask, maxProbes, counters, marks);
+}
+
+/* --cdcreducestats: warp w takes slots w, w + numWarps, ... of the descriptors' first slotsUsed
+   each, as elb_reduce_lz4_kernel takes chunks, and compresses the chunks of the cut (counts, ends)
+   whose mark is an entry; {length, min(size, length)} to that entry's payload */
+__global__ void __launch_bounds__(ELB_LZ4_WARPS * 32)
+elb_cdc_lz4_kernel(const elb_block_desc* descs, uint32_t numDescs, uint64_t slotsPerDesc,
+	uint64_t slotsUsed, const uint32_t* counts, const uint64_t* ends, const uint64_t* marks,
+	CdcPayload* payloads)
+{
+	__shared__ __align__(16) uint32_t tables[ELB_LZ4_WARPS][ELB_LZ4_HASH_ENTRIES];
+
+	const unsigned lane = threadIdx.x & 31;
+	const unsigned warp = threadIdx.x >> 5;
+	uint32_t* table = tables[warp];
+	const uint64_t numWarps = (uint64_t)gridDim.x * ELB_LZ4_WARPS;
+	const uint64_t numSlots = (uint64_t)numDescs * slotsUsed;
+
+	#pragma unroll 1
+	for(uint64_t c = (uint64_t)blockIdx.x * ELB_LZ4_WARPS + warp; c < numSlots; c += numWarps)
+	{
+		const uint64_t descIdx = c / slotsUsed;
+		const uint64_t j = c - descIdx * slotsUsed;
+
+		if(j >= counts[descIdx])
+			continue;
+
+		const uint64_t slot = descIdx * slotsPerDesc + j;
+		const uint64_t entry = marks[slot];
+
+		if(entry == ELB_REDUCE_NOT_NEW)
+			continue;
+
+		const uint64_t start = j ? ends[slot - 1] : 0; // (past 4 GiB in a block: 64-bit offsets)
+		const uint32_t n = (uint32_t)(ends[slot] - start); // (at most MAX = 1 MiB)
+
+		for(unsigned i = lane; i < ELB_LZ4_HASH_ENTRIES / 4; i += 32)
+			( (uint4*)table)[i] = make_uint4(ELB_LZ4_NO_POS, ELB_LZ4_NO_POS, ELB_LZ4_NO_POS,
+				ELB_LZ4_NO_POS);
+
+		__syncwarp();
+
+		const uint32_t size = lz4_compress_chunk<false>( (const uint8_t*)descs[descIdx].devPtr +
+			start, n, table, NULL, lane);
+
+		__syncwarp();
+
+		if(!lane)
+			payloads[entry] = CdcPayload{n, min(size, n)};
+	}
 }
 
 static int cdcCheckLaunch(const char* what)
@@ -433,11 +512,12 @@ int elb_launch_cdc_cut(const elb_block_desc* descs, uint32_t numDescs, unsigned 
 int elb_launch_cdc_hash_insert(const elb_block_desc* descs, uint32_t numDescs, unsigned avgShift,
 	uint64_t slotsPerDesc, const uint32_t* devCounts, const uint64_t* devEnds, void* devDigests,
 	void* table, void* payloads, uint64_t tableEntries, elb_reduce_counters* devCounters,
-	cudaStream_t stream)
+	uint64_t* devMarks, cudaStream_t stream)
 {
+	const char* what = devMarks ? "cdc_hash_insert_marks" : "cdc_hash_insert";
 	uint64_t slotsUsed;
 
-	if(cdcSlotsUsed("cdc_hash_insert", descs, numDescs, avgShift, slotsPerDesc, slotsUsed) )
+	if(cdcSlotsUsed(what, descs, numDescs, avgShift, slotsPerDesc, slotsUsed) )
 		return -1;
 
 	if(!numDescs || !slotsUsed)
@@ -447,14 +527,44 @@ int elb_launch_cdc_hash_insert(const elb_block_desc* descs, uint32_t numDescs, u
 
 	if(gridSize > 0x7fffffffULL)
 	{
-		elb_set_last_error("cdc_hash_insert: " + std::to_string(gridSize) + " CTAs are too many");
+		elb_set_last_error(std::string(what) + ": " + std::to_string(gridSize) +
+			" CTAs are too many");
 		return -1;
 	}
 
-	elb_cdc_hash_insert_kernel<<<(unsigned)gridSize, ELB_CDC_HASH_WARPS * 32, 0, stream>>>(descs,
-		numDescs, slotsPerDesc, slotsUsed, devCounts, devEnds, (uint32_t*)devDigests,
-		(DedupeKey*)table, (CdcPayload*)payloads, tableEntries - 1,
-		std::min(tableEntries, (uint64_t)ELB_DEDUPE_MAX_PROBES), devCounters);
+	const uint64_t maxProbes = std::min(tableEntries, (uint64_t)ELB_DEDUPE_MAX_PROBES);
 
-	return cdcCheckLaunch("cdc_hash_insert");
+	if(devMarks)
+		elb_cdc_hash_insert_marks_kernel<<<(unsigned)gridSize, ELB_CDC_HASH_WARPS * 32, 0,
+			stream>>>(descs, numDescs, slotsPerDesc, slotsUsed, devCounts, devEnds,
+			(uint32_t*)devDigests, (DedupeKey*)table, (CdcPayload*)payloads, tableEntries - 1,
+			maxProbes, devCounters, devMarks);
+	else
+		elb_cdc_hash_insert_kernel<<<(unsigned)gridSize, ELB_CDC_HASH_WARPS * 32, 0, stream>>>(descs,
+			numDescs, slotsPerDesc, slotsUsed, devCounts, devEnds, (uint32_t*)devDigests,
+			(DedupeKey*)table, (CdcPayload*)payloads, tableEntries - 1, maxProbes, devCounters);
+
+	return cdcCheckLaunch(what);
+}
+
+int elb_launch_cdc_lz4(const elb_block_desc* descs, uint32_t numDescs, unsigned avgShift,
+	uint64_t slotsPerDesc, const uint32_t* devCounts, const uint64_t* devEnds,
+	const uint64_t* devMarks, void* payloads, cudaStream_t stream)
+{
+	uint64_t slotsUsed, gridSize;
+
+	if(cdcSlotsUsed("cdc_lz4", descs, numDescs, avgShift, slotsPerDesc, slotsUsed) )
+		return -1;
+
+	if(!numDescs || !slotsUsed)
+		return 0;
+
+	if(elb_reduce_grid_size("cdc_lz4", numDescs * slotsUsed, ELB_LZ4_WARPS, ELB_LZ4_CTAS_PER_SM,
+		gridSize) )
+		return -1;
+
+	elb_cdc_lz4_kernel<<<(unsigned)gridSize, ELB_LZ4_WARPS * 32, 0, stream>>>(descs, numDescs,
+		slotsPerDesc, slotsUsed, devCounts, devEnds, devMarks, (CdcPayload*)payloads);
+
+	return cdcCheckLaunch("cdc_lz4");
 }

@@ -183,6 +183,18 @@ static const OptDef optDefs[] =
 		"duplicates at any offset. Each block is chunked on its own from its first byte. The block "
 		"size must be at least MAX. Cannot be used with --rand, --norandalign, --infloop, "
 		"--rwmixpct, --rwmixthr or --hosts. [b200]"},
+	{"cdcreducestats", 0, Opt_BYTES, &ProgArgs::cdcReduceStatsAvgSize, Wire_NONE, "Mean chunk "
+		"size of content-defined data reduction statistics: every write and read phase cuts each "
+		"block it moved into content-defined chunks as --cdcstats does (AVG a power of two from 4K "
+		"to 256K, chunks of MIN = AVG/4 to MAX = 4*AVG bytes), finds the distinct chunks by BLAKE3 "
+		"digest and compresses each distinct chunk once into one LZ4 block as --compressstats "
+		"does, all on the GPU. It prints \"CDC reduce: <N> chunks of <MIN> to <MAX> bytes, mean "
+		"<B/N>, <D> distinct: <B> bytes, <U> distinct bytes stored as <S>: dedupe <B/U>:1, compress "
+		"<U/S>:1, total <B/S>:1\", where U counts each distinct chunk once and S stores it as "
+		"min(LZ4 size, length): what a store that cuts by content, deduplicates and compresses, as "
+		"backup tools do, would keep. With --cdcstats at the same AVG, one set of GPU work serves "
+		"both lines. The block size must be at least MAX. Cannot be used with --rand, "
+		"--norandalign, --infloop, --rwmixpct, --rwmixthr or --hosts. [b200]"},
 	{"rwmixpct", 0, Opt_U64, &ProgArgs::rwMixReadPercent, Wire_REF, "Percentage of blocks that "
 		"should be read in a write phase."},
 	{"rwmixthr", 0, Opt_U64, &ProgArgs::numRWMixReadThreads, Wire_REF, "Number of threads that "
@@ -928,6 +940,41 @@ void ProgArgs::detectBenchPathType()
 	}
 }
 
+/* the checks of --cdcstats and --cdcreducestats (option, with a mean chunk size of avgSize) */
+void ProgArgs::checkCdcAvgSize(const std::string& option, uint64_t avgSize)
+{
+	if( (avgSize < (1ULL << ELB_CDC_MIN_AVG_SHIFT) ) ||
+		(avgSize > (1ULL << ELB_CDC_MAX_AVG_SHIFT) ) ||
+		(avgSize & (avgSize - 1) ) )
+		throw ProgError("Option \"" + option + "\" must be a power of two from 4K to 256K");
+
+	// (as the manager: a block reduced to the file size is the whole file)
+	const uint64_t fileBlockSize = (fileSize && (blockSize > fileSize) ) ? fileSize : blockSize;
+
+	if(fileBlockSize < 4 * avgSize)
+		throw ProgError("The block size (" + std::to_string(fileBlockSize) + ") must be at "
+			"least the largest chunk of \"" + option + "\" (" +
+			std::to_string(4 * avgSize) + ")");
+
+	if(useRandomUnaligned)
+		throw ProgError("Option \"" + option + "\" cannot be used together with \"--norandalign\"");
+
+	if(useRandomOffsets)
+		throw ProgError("Option \"" + option + "\" cannot be used together with \"--rand\"");
+
+	if(doInfiniteIOLoop)
+		throw ProgError("Option \"" + option + "\" cannot be used together with \"--infloop\"");
+
+	if(rwMixReadPercent)
+		throw ProgError("Option \"" + option + "\" cannot be used together with \"--rwmixpct\"");
+
+	if(numRWMixReadThreads)
+		throw ProgError("Option \"" + option + "\" cannot be used together with \"--rwmixthr\"");
+
+	if(!hosts.empty() )
+		throw ProgError("Option \"" + option + "\" cannot be used together with \"--hosts\"");
+}
+
 /* ProgArgs.cpp:1229-1462 (the checks that apply to the supported subset) */
 void ProgArgs::checkArgs()
 {
@@ -1165,38 +1212,10 @@ void ProgArgs::checkArgs()
 	}
 
 	if(cdcStatsAvgSize)
-	{
-		if( (cdcStatsAvgSize < (1ULL << ELB_CDC_MIN_AVG_SHIFT) ) ||
-			(cdcStatsAvgSize > (1ULL << ELB_CDC_MAX_AVG_SHIFT) ) ||
-			(cdcStatsAvgSize & (cdcStatsAvgSize - 1) ) )
-			throw ProgError("Option \"--cdcstats\" must be a power of two from 4K to 256K");
+		checkCdcAvgSize("--cdcstats", cdcStatsAvgSize);
 
-		// (as the manager: a block reduced to the file size is the whole file)
-		const uint64_t fileBlockSize = (fileSize && (blockSize > fileSize) ) ? fileSize : blockSize;
-
-		if(fileBlockSize < 4 * cdcStatsAvgSize)
-			throw ProgError("The block size (" + std::to_string(fileBlockSize) + ") must be at "
-				"least the largest chunk of \"--cdcstats\" (" +
-				std::to_string(4 * cdcStatsAvgSize) + ")");
-
-		if(useRandomUnaligned)
-			throw ProgError("Option \"--cdcstats\" cannot be used together with \"--norandalign\"");
-
-		if(useRandomOffsets)
-			throw ProgError("Option \"--cdcstats\" cannot be used together with \"--rand\"");
-
-		if(doInfiniteIOLoop)
-			throw ProgError("Option \"--cdcstats\" cannot be used together with \"--infloop\"");
-
-		if(rwMixReadPercent)
-			throw ProgError("Option \"--cdcstats\" cannot be used together with \"--rwmixpct\"");
-
-		if(numRWMixReadThreads)
-			throw ProgError("Option \"--cdcstats\" cannot be used together with \"--rwmixthr\"");
-
-		if(!hosts.empty() )
-			throw ProgError("Option \"--cdcstats\" cannot be used together with \"--hosts\"");
-	}
+	if(cdcReduceStatsAvgSize)
+		checkCdcAvgSize("--cdcreducestats", cdcReduceStatsAvgSize);
 
 	if(!checksumAlgoName.empty() )
 	{

@@ -98,6 +98,7 @@ class ProgArgs
 		uint64_t compressStatsChunkSize{0}; // --compressstats
 		uint64_t reduceStatsChunkSize{0}; // --reducestats
 		uint64_t cdcStatsAvgSize{0}; // --cdcstats
+		uint64_t cdcReduceStatsAvgSize{0}; // --cdcreducestats
 		std::shared_ptr<const ChecksumList> checksumList; // --checksumverify, parsed by checkArgs
 		uint64_t rwMixReadPercent{0};
 		bool hasUserSetRWMixPercent{false};
@@ -211,6 +212,7 @@ class ProgArgs
 	private:
 		void initImplicitValues(); // ProgArgs.cpp:1041-1195
 		void checkArgs();          // ProgArgs.cpp:1229-1462
+		void checkCdcAvgSize(const std::string& option, uint64_t avgSize);
 		void detectBenchPathType(); // ProgArgs.cpp findBenchPathType
 		void parseHosts();          // ProgArgs.cpp:2221-2340
 };

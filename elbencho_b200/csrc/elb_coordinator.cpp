@@ -78,6 +78,7 @@ class Coordinator
 		void printCompressLine(int benchPhase);
 		void printReduceLine(int benchPhase);
 		void printCdcLine(int benchPhase);
+		void printCdcReduceLine(int benchPhase);
 		void printDryRunInfo();
 };
 
@@ -418,6 +419,43 @@ void Coordinator::printCdcLine(int benchPhase)
 	std::cout << formatCdcLine(progArgs.cdcStatsAvgSize, counters) << std::endl;
 }
 
+/* --cdcreducestats: "CDC reduce: <N> chunks of <MIN> to <MAX> bytes, mean <B/N>, <D> distinct: <B>
+   bytes, <U> distinct bytes stored as <S>: dedupe <B/U>:1, compress <U/S>:1, total <B/S>:1" for a
+   mean chunk size of avgSize */
+static std::string formatCdcReduceLine(uint64_t avgSize, const elb_reduce_counters& counters)
+{
+	return "CDC reduce: " + std::to_string(counters.numChunks) + " chunks of " +
+		std::to_string(avgSize / 4) + " to " + std::to_string(avgSize * 4) + " bytes, mean " +
+		std::to_string(counters.numChunks ? counters.numBytes / counters.numChunks : 0) + ", " +
+		std::to_string(counters.numDistinct) + " distinct: " + std::to_string(counters.numBytes) +
+		" bytes, " + std::to_string(counters.numBytesDistinct) + " distinct bytes stored as " +
+		std::to_string(counters.numBytesStored) + ": dedupe " +
+		formatReduceRatio(counters.numBytes, counters.numBytesDistinct) + ":1, compress " +
+		formatReduceRatio(counters.numBytesDistinct, counters.numBytesStored) + ":1, total " +
+		formatReduceRatio(counters.numBytes, counters.numBytesStored) + ":1";
+}
+
+/* --cdcreducestats: after each write and read phase that succeeded, its counts and their ratios */
+void Coordinator::printCdcReduceLine(int benchPhase)
+{
+	if(!progArgs.cdcReduceStatsAvgSize ||
+		( (benchPhase != ELB_PHASE_CREATEFILES) && (benchPhase != ELB_PHASE_READFILES) ) )
+		return;
+
+	elb_reduce_counters counters;
+
+	try
+	{
+		manager->getCdcReduceStats(counters);
+	}
+	catch(const WorkerError& e)
+	{
+		throw ProgError(e.what() );
+	}
+
+	std::cout << formatCdcReduceLine(progArgs.cdcReduceStatsAvgSize, counters) << std::endl;
+}
+
 /* Coordinator::runBenchmarkPhase (:248-272) + Statistics live loop (:1284-1345) */
 void Coordinator::runBenchmarkPhase(int benchPhase)
 {
@@ -559,6 +597,7 @@ void Coordinator::runBenchmarkPhase(int benchPhase)
 	printCompressLine(benchPhase);
 	printReduceLine(benchPhase);
 	printCdcLine(benchPhase);
+	printCdcReduceLine(benchPhase);
 }
 
 void waitForUserDefinedStartTime(const ProgArgs& progArgs) // Coordinator.cpp:149-158
@@ -696,6 +735,9 @@ int Coordinator::main() // Coordinator.cpp:31-142
 
 		if(progArgs.cdcStatsAvgSize)
 			manager->setCdcStats(__builtin_ctzll(progArgs.cdcStatsAvgSize) );
+
+		if(progArgs.cdcReduceStatsAvgSize)
+			manager->setCdcReduceStats(__builtin_ctzll(progArgs.cdcReduceStatsAvgSize) );
 
 		/* workers on several GPUs: create the NCCL communicators of the statistics reduce now,
 		   while the workers are idle (and before any result output) */
@@ -893,6 +935,27 @@ extern "C" int64_t elb_format_cdc_line(uint64_t avgSize, const elb_reduce_counte
 	}
 
 	const std::string text = elb::formatCdcLine(avgSize, *counters);
+
+	if(outBuf && outBufLen)
+	{
+		const size_t copyLen = std::min( (size_t)(outBufLen - 1), text.size() );
+		memcpy(outBuf, text.data(), copyLen);
+		outBuf[copyLen] = 0;
+	}
+
+	return (int64_t)text.size();
+}
+
+extern "C" int64_t elb_format_cdc_reduce_line(uint64_t avgSize,
+	const elb_reduce_counters* counters, char* outBuf, uint64_t outBufLen)
+{
+	if(!counters)
+	{
+		elb_set_last_error("elb_format_cdc_reduce_line: NULL counters");
+		return -1;
+	}
+
+	const std::string text = elb::formatCdcReduceLine(avgSize, *counters);
 
 	if(outBuf && outBufLen)
 	{

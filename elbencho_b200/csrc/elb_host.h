@@ -1009,6 +1009,7 @@ struct Config
 	unsigned compressChunkShift{0}; // --compressstats (elb_mgr_set_compress_stats): 0 off, 12..20
 	unsigned reduceChunkShift{0}; // --reducestats (elb_mgr_set_reduce_stats): 0 off, 12..20
 	unsigned cdcAvgShift{0}; // --cdcstats (elb_mgr_set_cdc_stats): mean chunk 2^shift, 0 off, 12..18
+	unsigned cdcReduceAvgShift{0}; // --cdcreducestats (elb_mgr_set_cdc_reduce_stats): as cdcAvgShift
 	int serializeBufferedWrites{ELB_WRITEGATE_AUTO};
 	int stagingEngine{ELB_STAGING_AUTO};
 	bool noGPUNumaBinding{false};
@@ -1027,6 +1028,11 @@ struct Config
 
 	/* --dedupepct: percent of the grains that are duplicates of pool grains (elb_patterns.cuh) */
 	unsigned dedupePercent{0};
+
+	/* --cdcstats: the mean chunk shift of its own table and launches; 0 when it is off or when
+	   --cdcreducestats at the same mean serves its line from that option's table */
+	unsigned cdcOwnAvgShift() const
+		{ return (cdcAvgShift == cdcReduceAvgShift) ? 0 : cdcAvgShift; }
 
 	/* @throw WorkerError on invalid combinations */
 	static Config fromABI(const elb_cfg* cfg);

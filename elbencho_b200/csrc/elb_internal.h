@@ -137,9 +137,14 @@ int elb_launch_reduce_merge(const void* srcEntries, const void* srcPayloads,
 	elb_reduce_counters* devCounters, cudaStream_t stream);
 int elb_launch_reduce_sum(const void* table, const void* payloads, uint64_t tableEntries,
 	elb_reduce_counters* devCounters, cudaStream_t stream);
-/* --cdcstats (elb_cdc.cu; elb_cdc_cut, elb_cdc_hash_insert): descs must be host- and
-   device-readable, the host checks them and sizes the grid from their lengths. The table is a
-   reduce table (keys, payloads, counters). */
+/* a grid of at most numSMs * ctasPerSM CTAs of the current device for numItems items of
+   itemsPerCTA each (at least 1); -1 if there is no usable device */
+int elb_reduce_grid_size(const char* what, uint64_t numItems, uint64_t itemsPerCTA,
+	uint64_t ctasPerSM, uint64_t& gridSize);
+/* --cdcstats, --cdcreducestats (elb_cdc.cu; elb_cdc_cut, elb_cdc_hash_insert, _marks,
+   elb_cdc_lz4): descs must be host- and device-readable, the host checks them and sizes the grid
+   from their lengths. The table is a reduce table (keys, payloads, counters). devMarks NULL: the
+   hash and insert of --cdcstats, which writes no marks. */
 #define ELB_CDC_GEAR_TAG 0x6A09E667F3BCC908ULL /* gear[i] = elb_splitmix64_mix(tag + i) */
 #define ELB_CDC_MIN_AVG_SHIFT 12 /* mean chunk sizes of 4 KiB .. 256 KiB */
 #define ELB_CDC_MAX_AVG_SHIFT 18
@@ -148,7 +153,10 @@ int elb_launch_cdc_cut(const elb_block_desc* descs, uint32_t numDescs, unsigned 
 int elb_launch_cdc_hash_insert(const elb_block_desc* descs, uint32_t numDescs, unsigned avgShift,
 	uint64_t slotsPerDesc, const uint32_t* devCounts, const uint64_t* devEnds, void* devDigests,
 	void* table, void* payloads, uint64_t tableEntries, elb_reduce_counters* devCounters,
-	cudaStream_t stream);
+	uint64_t* devMarks, cudaStream_t stream);
+int elb_launch_cdc_lz4(const elb_block_desc* descs, uint32_t numDescs, unsigned avgShift,
+	uint64_t slotsPerDesc, const uint32_t* devCounts, const uint64_t* devEnds,
+	const uint64_t* devMarks, void* payloads, cudaStream_t stream);
 int elb_kernels_warmup();
 uint64_t elb_get_num_kernel_launches();
 void elb_count_kernel_launch(); // (launches of the kernels outside elb_kernels.cu)

@@ -137,6 +137,7 @@ Manager::~Manager()
 	freeCompressCounters();
 	freeReduceTables(shared.reduceTables);
 	freeReduceTables(shared.cdcTables);
+	freeReduceTables(shared.cdcReduceTables);
 	closeBenchPathFDs();
 }
 
@@ -392,8 +393,12 @@ void Manager::startNextPhase(int benchPhase)
 	prepareCompressCounters(benchPhase);
 	prepareReduceTables(shared.reduceTables, shared.cfg.reduceChunkShift,
 		"Reduce stats (--reducestats)", benchPhase);
-	prepareReduceTables(shared.cdcTables, shared.cfg.cdcAvgShift ? shared.cfg.cdcAvgShift - 2 : 0,
+	prepareReduceTables(shared.cdcTables,
+		shared.cfg.cdcOwnAvgShift() ? shared.cfg.cdcOwnAvgShift() - 2 : 0,
 		"CDC stats (--cdcstats)", benchPhase);
+	prepareReduceTables(shared.cdcReduceTables,
+		shared.cfg.cdcReduceAvgShift ? shared.cfg.cdcReduceAvgShift - 2 : 0,
+		"CDC reduce stats (--cdcreducestats)", benchPhase);
 
 	std::unique_lock<std::mutex> lock(shared.mutex);
 
@@ -1321,10 +1326,12 @@ void Manager::setReduceStats(unsigned chunkShift)
 	cfg.reduceChunkShift = chunkShift;
 }
 
-void Manager::setCdcStats(unsigned avgShift)
+/* --cdcstats, --cdcreducestats: throws WorkerError for a mean chunk shift outside 12..18 (0 is
+ * off) or a config it cannot be used with; option ("--cdcstats") names the option and what ("CDC
+ * stats") the counts in messages */
+static void checkCdcAvgShift(const Config& cfg, unsigned avgShift, const std::string& what,
+	const std::string& option)
 {
-	Config& cfg = shared.cfg;
-
 	if(avgShift && ( (avgShift < ELB_CDC_MIN_AVG_SHIFT) || (avgShift > ELB_CDC_MAX_AVG_SHIFT) ) )
 		throw WorkerError("The CDC mean chunk shift (" + std::to_string(avgShift) + ") is not in "
 			"[" + std::to_string(ELB_CDC_MIN_AVG_SHIFT) + ", " +
@@ -1336,30 +1343,42 @@ void Manager::setCdcStats(unsigned avgShift)
 
 	if(avgShift && (fileBlockSize < (4ULL << avgShift) ) )
 		throw WorkerError("The block size (" + std::to_string(fileBlockSize) + ") is below the "
-			"largest CDC chunk (--cdcstats) (" + std::to_string(4ULL << avgShift) + ").");
+			"largest CDC chunk (" + option + ") (" + std::to_string(4ULL << avgShift) + ").");
 
 	if(avgShift && cfg.useRandomOffsets)
-		throw WorkerError("CDC stats (--cdcstats) cannot be used together with random offsets "
+		throw WorkerError(what + " (" + option + ") cannot be used together with random offsets "
 			"(--rand).");
 
 	if(avgShift && cfg.doInfiniteIOLoop)
-		throw WorkerError("CDC stats (--cdcstats) cannot be used together with an infinite I/O "
+		throw WorkerError(what + " (" + option + ") cannot be used together with an infinite I/O "
 			"loop (--infloop).");
 
 	if(avgShift && cfg.useRandomUnaligned)
-		throw WorkerError("CDC stats (--cdcstats) cannot be used together with unaligned random "
+		throw WorkerError(what + " (" + option + ") cannot be used together with unaligned random "
 			"offsets (--norandalign).");
 
 	if(avgShift && (cfg.rwMixReadPercent || cfg.numRWMixReadThreads) )
-		throw WorkerError("CDC stats (--cdcstats) cannot be used together with rwmix (a phase in "
+		throw WorkerError(what + " (" + option + ") cannot be used together with rwmix (a phase in "
 			"both directions).");
+}
 
-	cfg.cdcAvgShift = avgShift;
+void Manager::setCdcStats(unsigned avgShift)
+{
+	checkCdcAvgShift(shared.cfg, avgShift, "CDC stats", "--cdcstats");
+
+	shared.cfg.cdcAvgShift = avgShift;
+}
+
+void Manager::setCdcReduceStats(unsigned avgShift)
+{
+	checkCdcAvgShift(shared.cfg, avgShift, "CDC reduce stats", "--cdcreducestats");
+
+	shared.cfg.cdcReduceAvgShift = avgShift;
 }
 
 /**
- * --reducestats, --cdcstats: before a write or read phase, one reduce table per GPU of
- * chunkTableSizes for chunks of at least 2^chunkShift bytes (0: the option is off) into
+ * --reducestats, --cdcstats, --cdcreducestats: before a write or read phase, one reduce table
+ * per GPU of chunkTableSizes for chunks of at least 2^chunkShift bytes (0: the option is off) into
  * sharedTables, its keys, payloads and counters cleared. Fails before any I/O if the tables need
  * more than half of a GPU's free memory; what names the option in messages.
  */
@@ -1482,14 +1501,24 @@ void Manager::getReduceStats(elb_reduce_counters& out)
 	sumReduceTables(shared.reduceTables, "Reduce stats (--reducestats)", out);
 }
 
-/* --cdcstats: the counts of the CDC tables, summed as the reduce tables are; U is also in S */
+/* --cdcstats: the counts of the CDC tables, summed as the reduce tables are; U is also in S,
+ * unless the tables are those of --cdcreducestats at the same mean */
 void Manager::getCdcStats(elb_reduce_counters& out)
 {
-	sumReduceTables(shared.cdcTables, "CDC stats (--cdcstats)", out);
+	if(shared.cfg.cdcOwnAvgShift() )
+		sumReduceTables(shared.cdcTables, "CDC stats (--cdcstats)", out);
+	else
+		sumReduceTables(shared.cdcReduceTables, "CDC stats (--cdcstats)", out);
 }
 
-/* --reducestats, --cdcstats: N and B of all tables of sharedTables, and D, U and S of the first
- * after the others are merged into it (what names the option in messages) */
+/* --cdcreducestats: the counts of its tables, summed as the reduce tables are */
+void Manager::getCdcReduceStats(elb_reduce_counters& out)
+{
+	sumReduceTables(shared.cdcReduceTables, "CDC reduce stats (--cdcreducestats)", out);
+}
+
+/* --reducestats, --cdcstats, --cdcreducestats: N and B of all tables of sharedTables, and D, U and
+ * S of the first after the others are merged into it (what names the option in messages) */
 void Manager::sumReduceTables(std::vector<ReduceTable>& sharedTables, const char* what,
 	elb_reduce_counters& out)
 {
@@ -2579,6 +2608,64 @@ int elb_mgr_cdc_stats(elb_mgr* m, uint64_t* outNumChunks, uint64_t* outNumDistin
 	*outNumDistinct = counters.numDistinct;
 	*outNumBytes = counters.numBytes;
 	*outNumBytesDistinct = counters.numBytesDistinct;
+	return 0;
+}
+
+int elb_mgr_set_cdc_reduce_stats(elb_mgr* m, unsigned avgShift)
+{
+	if(!m)
+	{
+		elb_set_last_error("elb_mgr_set_cdc_reduce_stats: NULL manager");
+		return -1;
+	}
+
+	try
+	{
+		m->impl->setCdcReduceStats(avgShift);
+	}
+	catch(std::exception& e)
+	{
+		elb_set_last_error(e.what() );
+		return -1;
+	}
+
+	return 0;
+}
+
+int elb_mgr_cdc_reduce_stats(elb_mgr* m, uint64_t* outNumChunks, uint64_t* outNumDistinct,
+	uint64_t* outNumBytes, uint64_t* outNumBytesDistinct, uint64_t* outNumBytesStored)
+{
+	if(!m || !outNumChunks || !outNumDistinct || !outNumBytes || !outNumBytesDistinct ||
+		!outNumBytesStored)
+	{
+		elb_set_last_error("elb_mgr_cdc_reduce_stats: NULL argument");
+		return -1;
+	}
+
+	if(!m->impl->shared.cfg.cdcReduceAvgShift)
+	{
+		elb_set_last_error("elb_mgr_cdc_reduce_stats: CDC reduce stats are off "
+			"(elb_mgr_set_cdc_reduce_stats)");
+		return -1;
+	}
+
+	elb_reduce_counters counters;
+
+	try
+	{
+		m->impl->getCdcReduceStats(counters);
+	}
+	catch(std::exception& e)
+	{
+		elb_set_last_error(e.what() );
+		return -1;
+	}
+
+	*outNumChunks = counters.numChunks;
+	*outNumDistinct = counters.numDistinct;
+	*outNumBytes = counters.numBytes;
+	*outNumBytesDistinct = counters.numBytesDistinct;
+	*outNumBytesStored = counters.numBytesStored;
 	return 0;
 }
 

@@ -259,8 +259,7 @@ static int reduceSlotsUsed(const char* what, const elb_block_desc* descs, uint32
 	return 0;
 }
 
-/* a grid of at most numSMs * ctasPerSM CTAs for numItems items of itemsPerCTA each */
-static int reduceGridSize(const char* what, uint64_t numItems, uint64_t itemsPerCTA,
+int elb_reduce_grid_size(const char* what, uint64_t numItems, uint64_t itemsPerCTA,
 	uint64_t ctasPerSM, uint64_t& gridSize)
 {
 	int dev = 0, numSMs = 0;
@@ -317,7 +316,7 @@ int elb_launch_reduce_lz4(const elb_block_desc* descs, uint32_t numDescs, unsign
 	if(!numDescs || !slotsUsed)
 		return 0;
 
-	if(reduceGridSize("reduce_lz4", numDescs * slotsUsed, ELB_LZ4_WARPS, ELB_LZ4_CTAS_PER_SM,
+	if(elb_reduce_grid_size("reduce_lz4", numDescs * slotsUsed, ELB_LZ4_WARPS, ELB_LZ4_CTAS_PER_SM,
 		gridSize) )
 		return -1;
 
@@ -336,7 +335,7 @@ int elb_launch_reduce_merge(const void* srcEntries, const void* srcPayloads,
 	if(!numSrcEntries)
 		return 0;
 
-	if(reduceGridSize("reduce_merge", numSrcEntries, ELB_DEDUPE_THREADS, 8, gridSize) )
+	if(elb_reduce_grid_size("reduce_merge", numSrcEntries, ELB_DEDUPE_THREADS, 8, gridSize) )
 		return -1;
 
 	elb_reduce_merge_kernel<<<(unsigned)gridSize, ELB_DEDUPE_THREADS, 0, stream>>>(
@@ -355,7 +354,7 @@ int elb_launch_reduce_sum(const void* table, const void* payloads, uint64_t tabl
 	if(!tableEntries)
 		return 0;
 
-	if(reduceGridSize("reduce_sum", tableEntries, ELB_DEDUPE_THREADS, 8, gridSize) )
+	if(elb_reduce_grid_size("reduce_sum", tableEntries, ELB_DEDUPE_THREADS, 8, gridSize) )
 		return -1;
 
 	elb_reduce_sum_kernel<<<(unsigned)gridSize, ELB_DEDUPE_THREADS, 0, stream>>>(

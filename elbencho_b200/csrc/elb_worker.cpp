@@ -826,12 +826,14 @@ void Worker::preparePhase()
  * chunk size, else the batch's own. --compressstats: the chunk size and counters of the stages'
  * LZ4 launch. --reducestats: the table the stages insert into, where the digests come from (as
  * for --dedupestats, or the dedupe launch's own at the same chunk size) and the batches' marks.
- * --cdcstats: the table the stages insert into and the batches' chunk counts and ends. Runs after
- * the rings are made and at the start of every write and read phase, since a checksum list
- * (elb_mgr_set_checksum_list) or the LZ4, reduce or CDC chunk size (elb_mgr_set_compress_stats,
- * elb_mgr_set_reduce_stats, elb_mgr_set_cdc_stats) may be set and the manager may make new tables
- * between phases; a change drops the batch graphs, which hold the launches of the old setup.
- * Without these options it allocates and changes nothing.
+ * --cdcstats: the table the stages insert into and the batches' chunk counts and ends (unless
+ * --cdcreducestats at the same mean serves it). --cdcreducestats: the same, and the batches'
+ * marks. Runs after the rings are made and at the start of every write and read phase, since a
+ * checksum list (elb_mgr_set_checksum_list) or the LZ4, reduce or CDC chunk size
+ * (elb_mgr_set_compress_stats, elb_mgr_set_reduce_stats, elb_mgr_set_cdc_stats,
+ * elb_mgr_set_cdc_reduce_stats) may be set and the manager may make new tables between phases; a
+ * change drops the batch graphs, which hold the launches of the old setup. Without these options
+ * it allocates and changes nothing.
  */
 void Worker::setupChecksums()
 {
@@ -886,13 +888,24 @@ void Worker::setupChecksums()
 	ReduceTable cTable;
 
 	for(const ReduceTable& gpuTable : shared->cdcTables)
-		if(cfg.cdcAvgShift && (gpuTable.gpuID == gpuID) )
+		if(cfg.cdcOwnAvgShift() && (gpuTable.gpuID == gpuID) )
 			cTable = gpuTable;
 
 	const bool cdc = (cTable.entries != NULL);
 	const unsigned cdcMinShift = cfg.cdcAvgShift - 2;
 	const uint64_t cdcSlots = !cdc ? 1 : std::max( (cfg.blockSize +
 		( (uint64_t)1 << cdcMinShift) - 1) >> cdcMinShift, (uint64_t)1);
+
+	ReduceTable crTable;
+
+	for(const ReduceTable& gpuTable : shared->cdcReduceTables)
+		if(cfg.cdcReduceAvgShift && (gpuTable.gpuID == gpuID) )
+			crTable = gpuTable;
+
+	const bool cdcReduce = (crTable.entries != NULL);
+	const unsigned cdcReduceMinShift = cfg.cdcReduceAvgShift - 2;
+	const uint64_t cdcReduceSlots = !cdcReduce ? 1 : std::max( (cfg.blockSize +
+		( (uint64_t)1 << cdcReduceMinShift) - 1) >> cdcReduceMinShift, (uint64_t)1);
 
 	if(batches.empty() || ( (readChecksum == readStage.checksum) &&
 		(chunkShift == checksumChunkShift) && (slotsPerDesc == checksumSlotsPerDesc) &&
@@ -907,7 +920,11 @@ void Worker::setupChecksums()
 		( (reduceUsesSums && readChecksum) == reduceUsesReadSums) &&
 		(reduceUsesDedupe == reduceUsesDedupeSums) && (cdc == readStage.cdc) &&
 		(cTable.entries == cdcTable.entries) && (cTable.numEntries == cdcTable.numEntries) &&
-		(cTable.counters == cdcTable.counters) && (cdcSlots == cdcSlotsPerDesc) ) )
+		(cTable.counters == cdcTable.counters) && (cdcSlots == cdcSlotsPerDesc) &&
+		(cdcReduce == readStage.cdcReduce) && (crTable.entries == cdcReduceTable.entries) &&
+		(crTable.numEntries == cdcReduceTable.numEntries) &&
+		(crTable.counters == cdcReduceTable.counters) &&
+		(cdcReduceSlots == cdcReduceSlotsPerDesc) ) )
 		return;
 
 	std::shared_lock<std::shared_timed_mutex> allocLock(shared->gpuAllocMutex);
@@ -926,13 +943,18 @@ void Worker::setupChecksums()
 	writeStage.cdc = cdc;
 	readStage.cdc = cdc;
 	verifyBackStage.cdc = false;
+	writeStage.cdcReduce = cdcReduce;
+	readStage.cdcReduce = cdcReduce;
+	verifyBackStage.cdcReduce = false;
 	/* --verifydirect: a write phase's checksums, dedupe, compress, reduce and CDC counts are those
 	   of the written bytes, so the read-back takes none, and must not share the read phase's batch
 	   graphs then */
 	verifyBackStage.useGraph = readStage.useGraph && !readChecksum && !dedupe && !lz4ChunkShift &&
-		!reduce && !cdc;
+		!reduce && !cdc && !cdcReduce;
 	cdcTable = cTable;
 	cdcSlotsPerDesc = cdcSlots;
+	cdcReduceTable = crTable;
+	cdcReduceSlotsPerDesc = cdcReduceSlots;
 	reduceTable = rTable;
 	reduceSlotsPerDesc = reduceSlots;
 	reduceUsesWriteSums = reduceUsesSums && cfg.checksums;
@@ -971,6 +993,12 @@ void Worker::setupChecksums()
 			cudaFree(batch.devCdcCounts);
 		if(batch.devCdcEnds)
 			cudaFree(batch.devCdcEnds);
+		if(batch.devCdcReduceCounts)
+			cudaFree(batch.devCdcReduceCounts);
+		if(batch.devCdcReduceEnds)
+			cudaFree(batch.devCdcReduceEnds);
+		if(batch.devCdcReduceMarks)
+			cudaFree(batch.devCdcReduceMarks);
 
 		batch.readGraphExec = NULL;
 		batch.writeGraphExec = NULL;
@@ -981,6 +1009,9 @@ void Worker::setupChecksums()
 		batch.devReduceMarks = NULL;
 		batch.devCdcCounts = NULL;
 		batch.devCdcEnds = NULL;
+		batch.devCdcReduceCounts = NULL;
+		batch.devCdcReduceEnds = NULL;
+		batch.devCdcReduceMarks = NULL;
 
 		if(dedupeNeedsOwnSums)
 			ELB_CUDA_CHECK(cudaMalloc(&batch.devDedupeSums, elb_checksum_value_bytes(
@@ -1000,6 +1031,16 @@ void Worker::setupChecksums()
 				"GPU CDC count allocation");
 			ELB_CUDA_CHECK(cudaMalloc( (void**)&batch.devCdcEnds, sizeof(uint64_t) * batchBlocks *
 				cdcSlots), "GPU CDC chunk allocation");
+		}
+
+		if(cdcReduce)
+		{
+			ELB_CUDA_CHECK(cudaMalloc( (void**)&batch.devCdcReduceCounts, sizeof(uint32_t) *
+				batchBlocks), "GPU CDC count allocation");
+			ELB_CUDA_CHECK(cudaMalloc( (void**)&batch.devCdcReduceEnds, sizeof(uint64_t) *
+				batchBlocks * cdcReduceSlots), "GPU CDC chunk allocation");
+			ELB_CUDA_CHECK(cudaMalloc( (void**)&batch.devCdcReduceMarks, sizeof(uint64_t) *
+				batchBlocks * cdcReduceSlots), "GPU CDC reduce mark allocation");
 		}
 
 		if(!readChecksum)
@@ -1286,6 +1327,12 @@ void Worker::freeRings() // LocalWorker::cleanup (:1570-1641)
 			cudaFree(batch.devCdcCounts);
 		if(batch.devCdcEnds)
 			cudaFree(batch.devCdcEnds);
+		if(batch.devCdcReduceCounts)
+			cudaFree(batch.devCdcReduceCounts);
+		if(batch.devCdcReduceEnds)
+			cudaFree(batch.devCdcReduceEnds);
+		if(batch.devCdcReduceMarks)
+			cudaFree(batch.devCdcReduceMarks);
 		if(batch.hostSums)
 			cudaFreeHost(batch.hostSums);
 	}
@@ -2032,7 +2079,10 @@ void Worker::rwPhase()
 
 	checkDedupeOverflow();
 	checkReduceOverflow();
-	checkCdcOverflow();
+	if(readStage.cdc)
+		checkCdcOverflow(cdcTable, "CDC stats (--cdcstats)");
+	if(readStage.cdcReduce)
+		checkCdcOverflow(cdcReduceTable, "CDC reduce stats (--cdcreducestats)");
 }
 
 /**
@@ -2599,6 +2649,9 @@ void Worker::enqueueStage(Batch& batch, const GpuStage& stage, uint32_t numBlock
 	if(stage.cdc)
 		enqueueCdc(batch, numBlocks);
 
+	if(stage.cdcReduce)
+		enqueueCdcReduce(batch, numBlocks);
+
 	if( (stage.transfer == GpuStage::TRANSFER_COPY) && !stage.isRead)
 		enqueueStageCopies(batch, false, true);
 }
@@ -2703,26 +2756,47 @@ void Worker::enqueueCdc(Batch& batch, uint32_t numBlocks)
 
 	if(elb_launch_cdc_hash_insert(batch.hostDescs, numBlocks, cfg.cdcAvgShift, cdcSlotsPerDesc,
 		batch.devCdcCounts, batch.devCdcEnds, NULL, cdcTable.entries, cdcTable.payloads,
-		cdcTable.numEntries, cdcTable.counters, batch.stream) )
+		cdcTable.numEntries, cdcTable.counters, NULL, batch.stream) )
 		throw WorkerError(std::string("GPU CDC insert failed. ") + elb_last_error() );
 }
 
-/* --cdcstats: the phase fails if the table of this worker's GPU ran past its probe bound (a
- * guard: a table is sized for a load of at most 0.5) */
-void Worker::checkCdcOverflow()
+/* --cdcreducestats: the cut and the hash and insert of --cdcstats into the CDC reduce table of this
+ * worker's GPU, with every slot's mark, then the LZ4 launch over the slots marked new, which writes
+ * their stored sizes to the table's payloads. Nothing is copied or waited for. */
+void Worker::enqueueCdcReduce(Batch& batch, uint32_t numBlocks)
 {
-	if(!readStage.cdc || batches.empty() )
+	if(elb_launch_cdc_cut(batch.hostDescs, numBlocks, cfg.cdcReduceAvgShift, cdcReduceSlotsPerDesc,
+		batch.devCdcReduceCounts, batch.devCdcReduceEnds, batch.stream) )
+		throw WorkerError(std::string("GPU CDC cut failed. ") + elb_last_error() );
+
+	if(elb_launch_cdc_hash_insert(batch.hostDescs, numBlocks, cfg.cdcReduceAvgShift,
+		cdcReduceSlotsPerDesc, batch.devCdcReduceCounts, batch.devCdcReduceEnds, NULL,
+		cdcReduceTable.entries, cdcReduceTable.payloads, cdcReduceTable.numEntries,
+		cdcReduceTable.counters, batch.devCdcReduceMarks, batch.stream) )
+		throw WorkerError(std::string("GPU CDC insert failed. ") + elb_last_error() );
+
+	if(elb_launch_cdc_lz4(batch.hostDescs, numBlocks, cfg.cdcReduceAvgShift, cdcReduceSlotsPerDesc,
+		batch.devCdcReduceCounts, batch.devCdcReduceEnds, batch.devCdcReduceMarks,
+		cdcReduceTable.payloads, batch.stream) )
+		throw WorkerError(std::string("GPU CDC LZ4 failed. ") + elb_last_error() );
+}
+
+/* --cdcstats, --cdcreducestats: the phase fails if the table of this worker's GPU ran past its
+ * probe bound (a guard: a table is sized for a load of at most 0.5); what names the option */
+void Worker::checkCdcOverflow(const ReduceTable& table, const char* what)
+{
+	if(batches.empty() )
 		return;
 
 	uint32_t overflow = 0;
 
-	ELB_CUDA_CHECK(cudaMemcpyAsync(&overflow, &cdcTable.counters->overflow, sizeof(overflow),
+	ELB_CUDA_CHECK(cudaMemcpyAsync(&overflow, &table.counters->overflow, sizeof(overflow),
 		cudaMemcpyDeviceToHost, batches[0].stream), "GPU CDC counter read");
 	ELB_CUDA_CHECK(cudaStreamSynchronize(batches[0].stream), "GPU CDC counter read");
 
 	if(overflow)
-		throw WorkerError("CDC stats (--cdcstats): the chunk table of GPU " +
-			std::to_string(gpuID) + " (" + std::to_string(cdcTable.numEntries) + " entries) "
+		throw WorkerError(std::string(what) + ": the chunk table of GPU " +
+			std::to_string(gpuID) + " (" + std::to_string(table.numEntries) + " entries) "
 			"ran past its probe bound of " + std::to_string(ELB_DEDUPE_MAX_PROBES) + " entries; "
 			"the counts are void.");
 }
@@ -2774,6 +2848,8 @@ void Worker::gpuLaunchStage(Batch& batch, bool isRead)
 			(stage.dedupe && reduceUsesDedupeSums) ) ? 2 : 3;
 	if(numBlocks && stage.cdc) // (the cut and the hash-insert)
 		numKernelLaunches += 2;
+	if(numBlocks && stage.cdcReduce) // (the cut, the hash-insert and the LZ4 launch)
+		numKernelLaunches += 3;
 
 	if(stage.transfer != GpuStage::TRANSFER_NONE)
 		(isRead ? numH2DBytes : numD2HBytes) += numBytes;

@@ -62,10 +62,10 @@ struct DedupeTable
 	elb_dedupe_counters* counters{NULL};
 };
 
-/* --reducestats, --cdcstats: the reduce table of one GPU (elb_reduce_insert, elb_cdc_hash_insert):
- * the keys as in DedupeTable, the payloads after them in the same allocation, and its counters;
- * made and cleared by the manager at the start of every write and read phase, shared by the GPU's
- * workers */
+/* --reducestats, --cdcstats, --cdcreducestats: the reduce table of one GPU (elb_reduce_insert,
+ * elb_cdc_hash_insert): the keys as in DedupeTable, the payloads after them in the same allocation,
+ * and its counters; made and cleared by the manager at the start of every write and read phase,
+ * shared by the GPU's workers */
 struct ReduceTable
 {
 	int gpuID{-1};
@@ -111,6 +111,9 @@ struct Shared
 	std::vector<CompressCounters> compressCounters; // --compressstats: one per GPU
 	std::vector<ReduceTable> reduceTables; // --reducestats: one per GPU, the first worker's first
 	std::vector<ReduceTable> cdcTables;    // --cdcstats: one per GPU, the first worker's first
+	                                       // (none at the mean of --cdcreducestats: Config::
+	                                       // cdcOwnAvgShift)
+	std::vector<ReduceTable> cdcReduceTables; // --cdcreducestats: one per GPU, likewise
 
 	/* workers hold this shared while they allocate / free device memory or instantiate graphs;
 	   the live stats reducer holds it exclusively while its collective is in flight, because a
@@ -292,6 +295,8 @@ struct GpuStage
 	                  // ones compressed
 	bool cdc;         // --cdcstats: the blocks cut into content-defined chunks, their digests into
 	                  // the GPU's CDC table
+	bool cdcReduce;   // --cdcreducestats: as cdc, into the GPU's CDC reduce table, the new chunks
+	                  // compressed
 };
 
 /* a batch: a contiguous slice of the rings plus everything its GPU stage needs */
@@ -333,6 +338,11 @@ struct Batch
 	   slot (device only) */
 	uint32_t* devCdcCounts{NULL};
 	uint64_t* devCdcEnds{NULL};
+	/* --cdcreducestats: the same for its cut, and every slot's mark (elb_cdc_hash_insert_marks),
+	   8 bytes per slot (device only) */
+	uint32_t* devCdcReduceCounts{NULL};
+	uint64_t* devCdcReduceEnds{NULL};
+	uint64_t* devCdcReduceMarks{NULL};
 
 	// aio state
 	std::vector<struct iocb> iocbs;
@@ -546,6 +556,9 @@ class Worker
 		/* --cdcstats: the table of this worker's GPU and the slots of the chunk ends per block */
 		ReduceTable cdcTable;
 		uint64_t cdcSlotsPerDesc{1};
+		/* --cdcreducestats: the same for its table */
+		ReduceTable cdcReduceTable;
+		uint64_t cdcReduceSlotsPerDesc{1};
 
 		// accounting
 		std::atomic<uint64_t> numH2DBytes{0};
@@ -594,7 +607,8 @@ class Worker
 		void enqueueReduce(Batch& batch, const GpuStage& stage, uint32_t numBlocks);
 		void checkReduceOverflow();
 		void enqueueCdc(Batch& batch, uint32_t numBlocks);
-		void checkCdcOverflow();
+		void enqueueCdcReduce(Batch& batch, uint32_t numBlocks);
+		void checkCdcOverflow(const ReduceTable& table, const char* what);
 		FileID blockFileID(const BlockRef& block) const;
 		uint64_t blockFileSize(const BlockRef& block) const;
 		void gpuLaunchStage(Batch& batch, bool isRead);
@@ -720,6 +734,14 @@ class Manager
 		   (merges the other GPUs' tables into the first's; throws WorkerError if a table ran past
 		   its probe bound) */
 		void getCdcStats(elb_reduce_counters& out);
+
+		/* --cdcreducestats: from the next write or read phase on, the CDC reduce counts of chunks of
+		   mean size 2^avgShift bytes (0: off); throws WorkerError as setCdcStats does */
+		void setCdcReduceStats(unsigned avgShift);
+		/* --cdcreducestats: N, B, D, U and S of the last write or read phase over all GPUs (merges
+		   the other GPUs' tables into the first's; throws WorkerError if a table ran past its probe
+		   bound) */
+		void getCdcReduceStats(elb_reduce_counters& out);
 
 		Shared shared;
 		std::vector<std::unique_ptr<Worker> > workers;

@@ -609,6 +609,34 @@ def cdc_hash_insert(pinned_descs_ptr, num_descs, avg_shift, slots_per_desc, dev_
            "elb_cdc_hash_insert")
 
 
+def cdc_hash_insert_marks(pinned_descs_ptr, num_descs, avg_shift, slots_per_desc, dev_counts_ptr,
+                          dev_ends_ptr, dev_digests_ptr, dev_table_ptr, dev_payloads_ptr,
+                          table_entries, dev_counters_ptr, dev_marks_ptr, stream=0):
+    """--cdcreducestats: cdc_hash_insert, and the uint64 mark of every chunk's slot at
+    dev_marks_ptr + 8 * (i * slots_per_desc + j): the entry its key newly took, or
+    REDUCE_NOT_NEW. The slots past a descriptor's count are not written."""
+    _check(_native.load().elb_cdc_hash_insert_marks(pinned_descs_ptr or None, num_descs, avg_shift,
+                                                    slots_per_desc, dev_counts_ptr or None,
+                                                    dev_ends_ptr or None, dev_digests_ptr or None,
+                                                    dev_table_ptr or None,
+                                                    dev_payloads_ptr or None, table_entries,
+                                                    dev_counters_ptr or None,
+                                                    dev_marks_ptr or None, stream),
+           "elb_cdc_hash_insert_marks")
+
+
+def cdc_lz4(pinned_descs_ptr, num_descs, avg_shift, slots_per_desc, dev_counts_ptr, dev_ends_ptr,
+            dev_marks_ptr, dev_payloads_ptr, stream=0):
+    """--cdcreducestats: compress every chunk of cdc_cut (the same descriptors, slots, counts and
+    ends) whose mark (cdc_hash_insert_marks) is an entry e into one LZ4 block by the parse of
+    lz4_chunks, and write (length, min(block size, length)) to payload e."""
+    _check(_native.load().elb_cdc_lz4(pinned_descs_ptr or None, num_descs, avg_shift,
+                                      slots_per_desc, dev_counts_ptr or None,
+                                      dev_ends_ptr or None, dev_marks_ptr or None,
+                                      dev_payloads_ptr or None, stream),
+           "elb_cdc_lz4")
+
+
 def cdc_line(avg_size, chunks, distinct, bytes_in, distinct_bytes):
     """the console line of --cdcstats for these counts"""
     counters = (ctypes.c_uint64 * 6)(chunks, bytes_in, distinct, distinct_bytes, distinct_bytes, 0)
@@ -616,4 +644,14 @@ def cdc_line(avg_size, chunks, distinct, bytes_in, distinct_bytes):
     lib = _native.load()
     if lib.elb_format_cdc_line(avg_size, counters, buf, len(buf)) < 0:
         raise KernelError("elb_format_cdc_line failed: %s" % _native.last_error())
+    return buf.value.decode()
+
+
+def cdc_reduce_line(avg_size, chunks, distinct, bytes_in, distinct_bytes, stored):
+    """the console line of --cdcreducestats for these counts"""
+    counters = (ctypes.c_uint64 * 6)(chunks, bytes_in, distinct, distinct_bytes, stored, 0)
+    buf = ctypes.create_string_buffer(384)
+    lib = _native.load()
+    if lib.elb_format_cdc_reduce_line(avg_size, counters, buf, len(buf)) < 0:
+        raise KernelError("elb_format_cdc_reduce_line failed: %s" % _native.last_error())
     return buf.value.decode()

@@ -121,6 +121,7 @@ class WorkerConfig:
     compress_chunk: int = 0           # --compressstats bytes (a power of two 4K..1M; 0 = off)
     reduce_chunk: int = 0             # --reducestats bytes (a power of two 4K..1M; 0 = off)
     cdc_avg: int = 0                  # --cdcstats mean chunk bytes (a power of two 4K..256K; 0 = off)
+    cdc_reduce_avg: int = 0           # --cdcreducestats mean chunk bytes (as cdc_avg)
     serialize_buffered_writes: int = 0  # 0 auto, 1 on, 2 off (--writegate)
     staging_engine: int = 0           # 0 auto, 1 kernels move the data, 2 cudaMemcpyAsync
     no_gpu_numa_binding: bool = False  # --nogpunuma
@@ -314,6 +315,13 @@ class WorkerManager:
                 err = _native.last_error()
                 self.close()
                 raise WorkerError(err)
+        avg = config.cdc_reduce_avg
+        if avg:
+            shift = avg.bit_length() - 1 if not avg & (avg - 1) else 0xffffffff
+            if self._lib.elb_mgr_set_cdc_reduce_stats(self._h, shift) != 0:
+                err = _native.last_error()
+                self.close()
+                raise WorkerError(err)
 
     def close(self):
         if self._h:
@@ -495,6 +503,15 @@ class WorkerManager:
         read phase, over all workers and GPUs; the dedupe ratio is B / U."""
         vals = [ctypes.c_uint64(0) for _ in range(4)]
         if self._lib.elb_mgr_cdc_stats(self._h, *[ctypes.byref(v) for v in vals]) != 0:
+            raise WorkerError(_native.last_error())
+        return tuple(v.value for v in vals)
+
+    def cdc_reduce_stats(self):
+        """--cdcreducestats: (chunks N, distinct chunks D, bytes B, distinct bytes U, stored bytes
+        S) of the last write or read phase, over all workers and GPUs; S is the sum of min(LZ4
+        size, length) over the distinct chunks, the ratios are B / U, U / S and B / S."""
+        vals = [ctypes.c_uint64(0) for _ in range(5)]
+        if self._lib.elb_mgr_cdc_reduce_stats(self._h, *[ctypes.byref(v) for v in vals]) != 0:
             raise WorkerError(_native.last_error())
         return tuple(v.value for v in vals)
 

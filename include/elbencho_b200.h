@@ -492,6 +492,23 @@ int elb_cdc_hash_insert(const elb_block_desc* descs, uint32_t numDescs, unsigned
 	uint64_t slotsPerDesc, const uint32_t* devCounts, const uint64_t* devEnds, void* devDigests,
 	void* table, void* payloads, uint64_t tableEntries, elb_reduce_counters* devCounters,
 	void* stream);
+/* --cdcreducestats: elb_cdc_hash_insert, and the mark of every chunk's slot (the entry its key
+ * newly took, or ELB_REDUCE_NOT_NEW, as elb_reduce_insert marks) to devMarks[i * slotsPerDesc + j];
+ * the slots past a descriptor's count are not written. Fails as elb_cdc_hash_insert does, and for
+ * NULL devMarks. */
+int elb_cdc_hash_insert_marks(const elb_block_desc* descs, uint32_t numDescs, unsigned avgShift,
+	uint64_t slotsPerDesc, const uint32_t* devCounts, const uint64_t* devEnds, void* devDigests,
+	void* table, void* payloads, uint64_t tableEntries, elb_reduce_counters* devCounters,
+	uint64_t* devMarks, void* stream);
+/* --cdcreducestats: compress every chunk of elb_cdc_cut (the same descriptors, slots, devCounts and
+ * devEnds) whose mark in devMarks (elb_cdc_hash_insert_marks) is an entry e into one LZ4 block by
+ * the parse of elb_lz4_chunks, and write {length, min(block size, length)} to payload e at
+ * devPayloads, so that elb_reduce_sum gives the stored bytes. A chunk marked not new is not
+ * compressed. Fails without launching for NULL pointers, an avgShift outside 12..18 or a
+ * descriptor that can have more chunks than slotsPerDesc. */
+int elb_cdc_lz4(const elb_block_desc* descs, uint32_t numDescs, unsigned avgShift,
+	uint64_t slotsPerDesc, const uint32_t* devCounts, const uint64_t* devEnds,
+	const uint64_t* devMarks, void* devPayloads, void* stream);
 
 int elb_stage_copy(const elb_block_desc* descs, uint32_t numDescs, int hostToDevice,
 	int64_t hostDelta, uint64_t totalBytes, uint64_t maxBlockLen, void* stream);
@@ -844,6 +861,13 @@ int64_t elb_format_reduce_line(uint64_t chunkSize, const elb_reduce_counters* co
  * truncated to outBufLen - 1), -1 on error. */
 int64_t elb_format_cdc_line(uint64_t avgSize, const elb_reduce_counters* counters, char* outBuf,
 	uint64_t outBufLen);
+/* --cdcreducestats: the console line of a phase's counters (N, D, B, U, S) for a mean chunk size
+ * of avgSize bytes, "CDC reduce: <N> chunks of <MIN> to <MAX> bytes, mean <B/N>, <D> distinct: <B>
+ * bytes, <U> distinct bytes stored as <S>: dedupe <B/U>:1, compress <U/S>:1, total <B/S>:1" (the
+ * mean an integer, 0 for no chunks; ratios with two decimals, 1.00 when the denominator is 0).
+ * Returns the text length (text truncated to outBufLen - 1), -1 on error. */
+int64_t elb_format_cdc_reduce_line(uint64_t avgSize, const elb_reduce_counters* counters,
+	char* outBuf, uint64_t outBufLen);
 /* UnitTk::numHumanToBytesBinary (toolkits/UnitTk.cpp:18-76): "4k", "1M", "64G"; 0 ok, -1 error */
 int elb_num_human_to_bytes(const char* numHuman, uint64_t* outBytes);
 
@@ -1043,6 +1067,18 @@ int elb_mgr_set_cdc_stats(elb_mgr* m, unsigned avgShift);
  * (elb_last_error), else 0. */
 int elb_mgr_cdc_stats(elb_mgr* m, uint64_t* outNumChunks, uint64_t* outNumDistinct,
 	uint64_t* outNumBytes, uint64_t* outNumBytesDistinct);
+/* --cdcreducestats: from the next write or read phase on, cut every block a phase moves into
+ * content-defined chunks as --cdcstats does (elb_mgr_set_cdc_stats; avgShift 12..18, the same
+ * config checks), count the distinct ones in a table per GPU and compress each distinct chunk once
+ * (elb_cdc_hash_insert_marks, elb_cdc_lz4); 0 turns it off. With --cdcstats at the same avgShift,
+ * one table and one set of launches serve both. */
+int elb_mgr_set_cdc_reduce_stats(elb_mgr* m, unsigned avgShift);
+/* --cdcreducestats: of the last write or read phase, N, D, B and U as elb_mgr_cdc_stats gives them
+ * and the sum over the distinct chunks of min(LZ4 size, length) (S), over all workers and GPUs of
+ * the manager. All 0 before the first such phase. Returns -1 if --cdcreducestats is off or a table
+ * ran past its probe bound (elb_last_error), else 0. */
+int elb_mgr_cdc_reduce_stats(elb_mgr* m, uint64_t* outNumChunks, uint64_t* outNumDistinct,
+	uint64_t* outNumBytes, uint64_t* outNumBytesDistinct, uint64_t* outNumBytesStored);
 
 uint32_t elb_mgr_num_workers(elb_mgr* m);
 elb_worker* elb_mgr_worker(elb_mgr* m, uint32_t localIdx);
